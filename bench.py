@@ -12,7 +12,7 @@ mapper-style alignments, 3 candidate alleles per locus), processed window by win
 At N GPUs the windows shard across ranks with no data-path collective; each step ends with ONE NCCL gather (variable block sizes) of the
 variant-site call records to rank 0 (weak scaling: per-GPU work is fixed).
 
-    python bench.py [--gpus N --steps K --warmup W]            our arm (CUDA, sm_100a)
+    python bench.py [--gpus N --steps K --warmup W]            our arm (CUDA, sm_90a)
     python bench.py --impl reference [...]                      the CPU arm: the reference's own functions on the host cores, one process per core
     python bench.py --config cfg2-scoring                       round 1's step (scoring only: K1 + read-max + K2a + K3 on pre-enumerated alignments)
 
@@ -44,7 +44,8 @@ CONFIGS = {  # the scoring-only step's configurations: name: (n_loci, depth, rea
     "tiny": (20_000, 30, 150, 4, "cfg2 shape at 20k loci (plumbing)"),
 }
 WHOLE_PATH = {  # the whole-path step: name: (candidate loci per GPU, loci per window, description)
-    "cfg2": (1_000_000, 100_000, "synthetic 30x germline pileup, 150 bp reads, 1M candidate loci (300 bp apart, 3 candidate alleles each): whole path, mapper alignments in, call records out"),
+    # (50k-locus windows: a context's scratch grows with its window, and the end-to-end leg's four contexts must share an 80 GB card)
+    "cfg2": (1_000_000, 50_000, "synthetic 30x germline pileup, 150 bp reads, 1M candidate loci (300 bp apart, 3 candidate alleles each): whole path, mapper alignments in, call records out"),
     "tiny": (20_000, 10_000, "cfg2 shape at 20k loci (plumbing)"),
 }
 
@@ -75,6 +76,32 @@ def run_threads(fns):
         t.join()
     if errs:
         raise errs[0]
+
+
+def _leaves(a: np.ndarray, name: str):
+    if a.dtype.names:
+        for f in a.dtype.names:
+            if f != "pad":
+                yield from _leaves(a[f], f"{name}.{f}")
+    else:
+        yield name, a
+
+
+def dump_outputs(out_dir: str, tables: dict, max_bytes: int = 60 << 20):
+    """tables: name -> array of rows (structured or plain).  Every leaf field goes to out_dir/<name>.<field>.npy as float64 (exact for the
+    int32 / uint32 / float32 / float64 fields of the ABI records).  A table whose rows exceed its share of max_bytes is cut to a fixed seeded
+    sample of rows, whose indices go to out_dir/<name>.rows.npy."""
+    os.makedirs(out_dir, exist_ok=True)
+    share = (max_bytes - (64 << 10)) // len(tables)  # (64 KB for the .npy headers)
+    for name, a in tables.items():
+        leaves = list(_leaves(a, name))
+        row_bytes = 8 * (1 + sum(int(np.prod(x.shape[1:])) for _, x in leaves))
+        if len(a) * row_bytes > share:
+            rows = np.sort(np.random.default_rng(0).choice(len(a), share // row_bytes, replace=False))
+            np.save(os.path.join(out_dir, f"{name}.rows.npy"), rows.astype(np.float64))
+            leaves = [(k, x[rows]) for k, x in leaves]
+        for k, x in leaves:
+            np.save(os.path.join(out_dir, f"{k}.npy"), np.ascontiguousarray(x, dtype=np.float64))
 
 
 def load_synth():
@@ -833,26 +860,19 @@ def scoring_step_main(args):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s"
+        peak = float(peaks.get("hbm_gbs", 3350.0))
+        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 3350 GB/s (H100 SXM data sheet)"
         total_loci = n_loci * world
         value = total_loci * args.steps / dt
         alg_bytes = ab.algorithmic_bytes()
         achieved = alg_bytes / (k1_avg_ms * 1e-3) / 1e9
-        traffic = None  # dram__bytes_read.sum + dram__bytes_write.sum of one K1 launch from the committed ncu --set full capture
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles", "r1_traffic.json")))
-            if cfg_name in tj and n_loci == CONFIGS[cfg_name][0]:
-                t = tj[cfg_name]["k1q_score_kernel"]
-                traffic = t["dram_bytes_read"] + t["dram_bytes_write"]
-        except Exception:
-            pass
+        traffic = None  # measured DRAM bytes of the launch: no capture is stored for this card
         line = {
             "metric": "candidate_loci_per_sec", "value": value, "unit": "loci/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": 1e3 * dt / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f64", "data": "synthetic",
             "config": {"workload": f"{args.config}: {desc}", "loci_per_gpu": n_loci, "depth": depth, "read_len": read_len, "haplotypes": n_haps,
                        "parallelism": f"region-shard x{world}, one NCCL gather of call records per step" if world > 1 else "single GPU",
-                       "l2": "inputs (%.1f GB per GPU) far exceed the 126 MB L2; no flush needed" % (alg_bytes / 1e9), "gen_seconds": round(t_gen, 1)},
+                       "l2": "inputs (%.1f GB per GPU) far exceed the 50 MB L2; no flush needed" % (alg_bytes / 1e9), "gen_seconds": round(t_gen, 1)},
             "gcups": (cells_k1 + cells_k3) * world * args.steps / dt / 1e9,
             "k1_gcups_kernel_only": cells_k1 / (k1_avg_ms * 1e-3) / 1e9,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
@@ -1224,6 +1244,16 @@ def whole_path_main(args):
     dt = dt_dev
     launches = ctx.total_launches() - launches0
     step_totals = totals // args.steps
+    if args.dump_outputs and rank == 0:  # what the last timed step handed its caller: the step's variant-site records and the DP results
+        ga_res = dgb.res.download(A.GA_RESULT_DT, gb.n)
+        ga_cig = dgb.cigar.download(np.uint32, gb.n * gb.max_ops).reshape(gb.n, gb.max_ops)
+        ga_cig[np.arange(gb.max_ops)[None, :] >= np.minimum(ga_res["n_ops"], gb.max_ops)[:, None]] = 0  # (slots past a matrix's ops are not written)
+        # (several GPUs: the step's records gathered from every rank, rank p's block at byte offset gather_off[p]; the DP results are rank 0's)
+        var = d_all.download(A.SITE_CALL_DT, int(gather_off[world]) // A.SITE_CALL_DT.itemsize) if world > 1 else d_var.download(A.SITE_CALL_DT, n_var_step)
+        dump_outputs(args.dump_outputs, {"variant_sites": var, "global_align": ga_res, "global_align_cigar": ga_cig})
+    # the resident windows give their HBM back before the end-to-end leg: an 80 GB card does not hold both legs' buffers at the default size
+    for buf in dws + [d_var_raw, d_var] + ([d_all] if d_all else []) + list(dgb.bufs.values()) + [dgb.res, dgb.cigar]:
+        buf.free()
 
     # end to end: pinned host arrays through the host-array entry, H2D + kernels + D2H inside the timed region.  Two host threads with a context
     # each take the windows alternately (one window's transfers overlap the other's kernels); the DP batch runs on a third.
@@ -1232,7 +1262,6 @@ def whole_path_main(args):
         n_workers = max(1, min(args.e2e_workers, n_tiles))
         # the end-to-end leg keeps n_workers + 1 host threads per rank waiting on the device.  Where the ranks together have more waiting threads
         # than the job has CPUs (8 ranks x 4 on the GPU boxes' 16-CPU quota) spinning waiters exhaust the quota and every rank stalls: they block instead
-        # (measured on one GPU with CPUs to spare: blocking 321.6 vs spinning 329.4 ms per 300k loci, 0.01 vs 0.68 host CPU seconds per step -- so always)
         if host_wait.startswith("spin") and os.environ.get("SX_BLOCKING_WAIT") != "0":
             if lib.sx_set_host_wait_policy(local_rank, 1) == 0:
                 host_wait = "spin for the resident step, blocking for the end-to-end leg"
@@ -1305,8 +1334,8 @@ def whole_path_main(args):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s"
+        peak = float(peaks.get("hbm_gbs", 3350.0))
+        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 3350 GB/s (H100 SXM data sheet)"
         total_loci = n_loci * world
         value = total_loci * args.steps / dt
         per_step = {k: v / args.steps for k, v in stage_ms.items()}
@@ -1319,13 +1348,7 @@ def whole_path_main(args):
         stage_roof = {k: {"ms": per_step[k], "algorithmic_bytes": int(sb[k]), "achieved_gbs": sb[k] / max(per_step[k], 1e-9) / 1e6, "frac": sb[k] / max(per_step[k], 1e-9) / 1e6 / peak}
                       for k in per_step if k in sb}
         dom = max((k for k in stage_roof), key=lambda k: per_step[k])
-        traffic = None
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles", "r2_traffic.json")))
-            if dom in tj and n_loci == WHOLE_PATH[args.config][0]:
-                traffic = tj[dom]["dram_bytes_read"] + tj[dom]["dram_bytes_write"]
-        except Exception:
-            pass
+        traffic = None  # measured DRAM bytes of the stage: no capture is stored for this card
         # cell updates of a step: one per base of every candidate alignment scored (scoreCandidateAlignment walks the read once per alignment)
         # + 3 states x Q x R per haplotype DP matrix
         cells_k1 = int(step_totals[0]) * WW.READ_LEN
@@ -1342,7 +1365,7 @@ def whole_path_main(args):
                        "concurrency": f"{lanes} contexts (own stream + buffers, one host thread each) take the windows in turn; kernel_ms_per_step sums each stage's device time "
                                       "over the contexts, so the stages add up to more than ms_per_step",
                        "parallelism": f"window-shard x{world}, one NCCL gatherv of variant-site records per step" if world > 1 else "single GPU",
-                       "l2": "inputs (%.1f GB per GPU) far exceed the 126 MB L2; no flush needed" % (sum(WW.input_bytes(w) for w in tiles) / 1e9), "gen_seconds": round(t_gen, 1), "host_binding": numa, "host_wait": host_wait},
+                       "l2": "inputs (%.1f GB per GPU) far exceed the 50 MB L2; no flush needed" % (sum(WW.input_bytes(w) for w in tiles) / 1e9), "gen_seconds": round(t_gen, 1), "host_binding": numa, "host_wait": host_wait},
             "roofline": {"bound": "hbm", "achieved": stage_roof[dom]["achieved_gbs"], "peak": peak, "unit": "GB/s", "frac": stage_roof[dom]["frac"], "traffic": traffic,
                          "kernel": f"stage {dom} (the longest of the step)", "algorithmic_bytes_per_step": stage_roof[dom]["algorithmic_bytes"], "kernel_ms_per_step": per_step[dom],
                          "peak_source": peak_src, "whole_step": {"algorithmic_bytes": int(whole_bytes), "achieved_gbs": whole_bytes / (dt / args.steps) / 1e9,
@@ -1377,7 +1400,7 @@ def whole_path_main(args):
                 line["cpu_baseline"] = {"error": str(e)}
         if world == 1:
             if args.legs:
-                for key, cmd in (("scoring_only_step", [sys.executable, os.path.abspath(__file__), "--config", "cfg2-scoring", "--steps", "5", "--warmup", "3", "--no-legs"]),
+                for key, cmd in (("scoring_only_step", [sys.executable, os.path.abspath(__file__), "--config", "cfg2-scoring", "--steps", str(args.steps), "--warmup", str(args.warmup), "--no-legs"]),
                                  ("k2b_somatic_cfg3", [sys.executable, os.path.join(ROOT, "tools", "site_legs.py"), "k2b", str(peak)]),
                                  ("k5_indel_gl", [sys.executable, os.path.join(ROOT, "tools", "site_legs.py"), "k5", str(peak)])):
                     try:
@@ -1402,7 +1425,7 @@ def main():
     ap.add_argument("--loci", type=int, default=0, help="override the number of candidate loci per GPU")
     ap.add_argument("--tile-loci", type=int, default=0, help="candidate loci per window (whole-path step)")
     ap.add_argument("--e2e-workers", type=int, default=3, help="host threads (one context each) of the end-to-end leg")
-    ap.add_argument("--lanes", type=int, default=1, help="contexts that process the windows of a step concurrently (whole-path step); measured on a B200: no gain beyond 1 once the stages were tuned")
+    ap.add_argument("--lanes", type=int, default=1, help="contexts that process the windows of a step concurrently (whole-path step)")
     ap.add_argument("--lane-offset-ms", type=float, default=0.0, help="delay of context i's first window in a step: i x this (with --lanes > 1)")
     ap.add_argument("--seed", type=int, default=1)
     ap.add_argument("--no-e2e", action="store_true")
@@ -1412,7 +1435,13 @@ def main():
     ap.add_argument("--worker-index", type=int, default=0)
     ap.add_argument("--worker-loci", type=int, default=240)
     ap.add_argument("--worker-cpu", type=int, default=-1)
+    ap.add_argument("--dump-outputs", metavar="DIR", default="",
+                    help="after the timed steps, write what the last one computed (the variant-site records gathered from every rank, rank 0's haplotype-DP "
+                         "results) as DIR/<table>.<field>.npy, float64, at most 64 MB; a larger table is cut to a fixed seeded sample of rows whose indices go to "
+                         "DIR/<table>.rows.npy")
     args = ap.parse_args()
+    if args.dump_outputs and (args.config not in WHOLE_PATH or args.impl != "b200"):
+        ap.error("--dump-outputs is implemented for the GPU's whole-path step (--config cfg2 / tiny)")
     if args.impl == "reference-worker":
         return reference_worker(args)
     if args.config in ("cfg2-scoring", "cfg5", "tiny-scoring"):

@@ -1,5 +1,5 @@
 /*
- * strelka_b200.h -- C ABI of the B200-native Strelka2 per-locus scoring hot path.
+ * strelka_b200.h -- C ABI of the GPU-native Strelka2 per-locus scoring hot path.
  *
  * This is the drop-in boundary (SURVEY.md section 8b).  The reference (Illumina/strelka,
  * paths relative to /root/reference/src/c++/lib/) has no FFI of its own; each entry point
@@ -642,7 +642,7 @@ typedef struct sx_enum_opts {
 /* SX_ENUM_F_FAST (the default of sx_default_enum_opts): ordinary reads (<= 11 nested toggles, <= 16 alignments) search in per-lane-interleaved
  * local memory, the others in a global arena; every read is searched ONCE, its alignments appended to a log and gathered into read order
  * after the scan.  flags = 0 selects the first launch plan (per-thread arena, count / scan / write: the search runs twice) -- same results,
- * 6x slower on cfg2-shaped loci (BENCH_r01: 80.9 vs 13.2 ms per 100k loci); kept as a cross-check of the fast plan. */
+ * several times slower on cfg2-shaped loci; kept as a cross-check of the fast plan. */
 #define SX_ENUM_F_FAST 0x1u
 
 typedef struct sx_enum_batch {

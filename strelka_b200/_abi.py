@@ -1,6 +1,6 @@
 """ctypes view of include/strelka_b200.h (the C ABI) and the loader of libstrelka_b200.so.
 
-The shared library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_100a).  There is no CPU
+The shared library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_90a).  There is no CPU
 fallback: if the library is missing, ``load()`` raises, and without a CUDA device ``sx_create`` fails.
 """
 from __future__ import annotations

@@ -1,8 +1,8 @@
 // k1_score4.cu -- K1 fast path: scoreCandidateAlignment for batches in the 4-bit quality wire format (qual_bits == 4).
 //
 // Same contract as k1_score.cu (reference: starling_common/starling_read_align_score.cpp:260-499, one running double per (read,
-// alignment) path, terms added in read order with __dadd_rn, addends from the host-built table), re-organised around what the ncu
-// profile of that kernel showed: it was bound by issue slots and shared-memory wavefronts, not by HBM, and only 40 % of its
+// alignment) path, terms added in read order with __dadd_rn, addends from the host-built table), re-organised around what a
+// profile of that kernel showed: it was bound by issue slots and shared-memory wavefronts, not by HBM, and less than half of its
 // instructions were the per-cell work.  Here
 //   * a read base is ONE byte: quality code << 4 | page << 2 | base (A C G T = 0..3).  The byte is, up to two masks, the address of
 //     its term in a 1 KB table built per CTA from the quality dictionary: tab[page][quality code][mismatch], page 0 = ordinary base

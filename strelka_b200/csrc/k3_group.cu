@@ -4,14 +4,15 @@
 // Same anti-diagonal wavefront as k3_global_align.cu -- each lane owns a strip of consecutive query rows in registers, the scores of
 // the row above / the diagonal cross lanes by __shfl_up (width 8) -- but with strips of T = ceil(Q/8) rows instead of ceil(Q/32):
 // for a 70 x 65 matrix that is 7 fill/drain steps instead of 22, 9 cells of work per shuffle round instead of 3, and 93 % of the
-// lane-rows are real cells instead of 70 %.  Measured: 2.0x over the warp-per-matrix kernel on the bench mix (see DESIGN.md).
+// lane-rows are real cells instead of 70 %.
 //
 // T is a template parameter (1..16), so the batch is bucketed by (T, reference-length class) on the device first and each T gets its
 // own launch over its bucket; the four matrices of a warp therefore share T and have similar R.
 //
 // The 3 x 2-bit back pointers of cell (row, col) are stored at  scratch[warp][(t * T + r) * 32 + lane]  with t = col + lane-in-group
-// the wavefront step, r the row within the lane's strip: every warp store is one coalesced 32-byte sector, and the whole scratch of
-// the resident warps (tens of MB) lives in the 126 MB L2.  The pointer chase of the traceback reads it back by the same mapping;
+// the wavefront step, r the row within the lane's strip: every warp store is one coalesced 32-byte sector.  The scratch of the resident
+// warps is tens of MB; on an H100 (50 MB of L2) the larger buckets' scratch does not all stay in the L2, so part of the traceback reads
+// come from HBM (K3 is still about 1 % of a cfg2 step there, README.md).  The pointer chase of the traceback reads it back by the same mapping;
 // traceback and '='/'X' expansion run on lane 0 of each group (four at a time per warp).
 // Arithmetic, max3 tie rule and candidate order are those of GlobalAligner<int> (alignment/GlobalAlignerImpl.hh:36-228): bit-exact.
 #include "k3_common.cuh"

@@ -1163,7 +1163,7 @@ int sx_k4_run(sx_ctx* ctx, const sx_pileup_reads_batch* d, const sx_pileup_colum
                        (unsigned long long)out->calls_capacity, (unsigned long long)out->t2_capacity);
     // pass 3: thread per read + warp per 32 sites (default), or SX_K4_PLAN=1: one warp per window, reads in turn
     const size_t bc_bytes = (size_t)d->n_reads * Lcap * 2;
-    const bool gather_plan = (getenv("SX_K4_PLAN") && atoi(getenv("SX_K4_PLAN")) == 2) && bc_bytes <= ((size_t)12 << 30); // (opt-in until it has run on a B200)
+    const bool gather_plan = (getenv("SX_K4_PLAN") && atoi(getenv("SX_K4_PLAN")) == 2) && bc_bytes <= ((size_t)12 << 30); // (opt-in: the windowed fill is the default)
     if (d->n_reads && gather_plan)
     {
         k4_rrec* rec = nullptr;

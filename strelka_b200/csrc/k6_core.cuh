@@ -707,7 +707,7 @@ K6_HD k6_view k6_rebased(const k6_view& v, const k6_block_plan& p, unsigned char
 
 #define K6_FAST_A 8
 #define K6_FAST_E 4
-#define K6_MID_A 40 /* second local-memory tier: ncu put 20 % of the kernel's instructions on the strided-arena accessor once most reads had > 8 alignments */
+#define K6_MID_A 40 /* second local-memory tier: a profile put a large share of the kernel's instructions on the strided-arena accessor once most reads had > 8 alignments */
 
 /// read r of a block whose view is `lv` (staged or not): find its region among the block's and run the body with the cheapest
 /// scratch that fits

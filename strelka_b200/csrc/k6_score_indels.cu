@@ -110,7 +110,7 @@ __global__ void __launch_bounds__(K6_THREADS) k6_score_kernel(const k6_view v, c
 }
 
 // the same per-read body over the dense list of reads that have alignments, on the global arrays (no staging): about half of a 30x window's
-// reads never reach the search, and in the block-staged kernel their threads idle (ncu: 10.9 of 32 lanes) while the staged slices hold the
+// reads never reach the search, and in the block-staged kernel their threads idle (about a third of the lanes busy) while the staged slices hold the
 // occupancy at 9 warps per SM
 __global__ void __launch_bounds__(K6_THREADS) k6_score_list_kernel(const k6_view v, const k6_scratch S0, const uint32_t* __restrict__ list, const uint32_t* __restrict__ n_list,
                                                                   int* __restrict__ status)

@@ -201,7 +201,7 @@ __global__ void k7_active_reads_kernel(const uint32_t n_reads, const uint8_t* __
 
 // ---- reads of one shape side by side.  The active list is in read order: a warp's 32 reads are one region's reads at neighbouring positions,
 // and they differ in WHICH of the window's entries they reach -- so their searches have different trees and the warp executes every tree in turn
-// (ncu: 14.5 of 32 lanes active).  A read's shape class = the window entries (first four of its region) its input alignment's range is adjacent
+// (about half of the 32 lanes active).  A read's shape class = the window entries (first four of its region) its input alignment's range is adjacent
 // to (bp_adjacent: what add_indels_in_range will put into indel_order) + which of them the alignment already contains.  The list is regrouped
 // by class with a block-local counting sort; which thread searches which read does not matter (the output is placed by the scan).
 constexpr uint32_t K7_N_CLASS = SX_RG_CLASSES;
@@ -397,7 +397,8 @@ int k7_run_fast(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsig
     if (const char* e = getenv("SX_K7_LOCAL_ALNS")) small_local = atoi(e) <= 16;
     // the same kernel compiled for 16 / 24 / 32 resident blocks per SM (64 / 40 / 32 registers; its state lives in local memory, so the smaller
     // register budgets spill next to nothing): more warps to hide its latency
-    const int min_blocks(getenv("SX_K7_MIN_BLOCKS") ? atoi(getenv("SX_K7_MIN_BLOCKS")) : 24); // measured per 1M loci: 267.6 / 261.5 / 279.0 ms at 16 / 24 / 32
+    // 16 on an H100: K7 103 vs 119 ms per step at 16 vs 24 (bench.py, 300k cfg2 loci, two runs each; H100 80GB HBM3, 400 W power limit)
+    const int min_blocks(getenv("SX_K7_MIN_BLOCKS") ? atoi(getenv("SX_K7_MIN_BLOCKS")) : 16);
     const auto local_kernel(small_local ? k7_search_local_kernel<16, 16>
                             : min_blocks >= 32 ? k7_search_local_kernel<40, 32>
                             : min_blocks >= 24 ? k7_search_local_kernel<40, 24>
@@ -506,7 +507,7 @@ int k7_run_fast(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsig
     k7_scan_finish<<<n_tiles, K7_SCAN_THREADS, 0, st>>>(n, c, sums, n_tiles, totals, *o, ctx->d_status);
     SX_CUDA(ctx, cudaGetLastError());
     const int g1(std::max(1, std::min<int>((int)((n + 127) / 128), ctx->sm_count * 16)));
-    k7_gather_kernel<<<g1, 128, 0, st>>>(n, c, L, *o, totals, nullptr, nullptr); // (every read, in read order: walking the active list instead measured slower, 117 / 126 vs 106 ms per 600k loci in read / class order)
+    k7_gather_kernel<<<g1, 128, 0, st>>>(n, c, L, *o, totals, nullptr, nullptr); // (every read, in read order: walking the active list instead, in read or class order, was slower)
     SX_CUDA(ctx, cudaGetLastError());
     *launches = (two_levels ? 8 : 7) + extra;
     return SX_OK;
@@ -565,7 +566,7 @@ extern "C" void sx_default_enum_opts(sx_enum_opts* o)
     o->n_samples = 1;
     o->sample_id = 0;
     o->max_alns_per_read = 64;
-    o->flags = SX_ENUM_F_FAST; // the default launch plan since its first timing on a B200 (13.2 vs 80.9 ms per 100k cfg2-shaped loci); 0 = the two-pass arena plan
+    o->flags = SX_ENUM_F_FAST; // the default launch plan; 0 = the two-pass arena plan
 }
 
 extern "C" int sx_enumerate_alignments_dev(sx_ctx* ctx, const sx_enum_batch* d, sx_enum_out* out_dev)

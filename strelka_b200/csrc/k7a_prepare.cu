@@ -34,7 +34,7 @@ __global__ void k7a_read_offsets_kernel(const k7a_view v, unsigned long long* __
 }
 
 // The reads the gates turned away (about half of a 30x window's) have no keys: with a gate the two passes below run over the DENSE list of the
-// others (full warps instead of 9 of 32 lanes, ncu), and the first pass leaves a read's first K7A_STAGE keys in a staging row so that the second
+// others (full warps instead of about a quarter of the lanes), and the first pass leaves a read's first K7A_STAGE keys in a staging row so that the second
 // pass copies them instead of walking the read again.
 #define K7A_STAGE 6u
 

@@ -48,7 +48,7 @@ __global__ void k8_size_kernel(const k8_view v, const uint32_t n_alns, const uin
 }
 
 // per region: exclusive offsets of its alignments within the region (in place) and the region's padded totals.  One WARP per region: a region
-// of a 30x window holds a few hundred alignments, and one thread walking them was the whole cost of the link (3.05 of 4.5 ms per 50k loci, ncu)
+// of a 30x window holds a few hundred alignments, and one thread walking them was most of the link's time
 __global__ void k8_region_kernel(const k8_view v, uint32_t* __restrict__ seg_n, uint32_t* __restrict__ ins_n, uint32_t* __restrict__ reg_seg,
                                  uint32_t* __restrict__ reg_ins, uint32_t* __restrict__ reg_zero)
 {

@@ -430,9 +430,9 @@ extern "C" int sx_create(int cuda_device, const sx_params* p, sx_ctx** out)
     if ((e = cudaSetDevice(cuda_device)) != cudaSuccess) return bail("cudaSetDevice", e);
     cudaDeviceProp prop;
     if ((e = cudaGetDeviceProperties(&prop, cuda_device)) != cudaSuccess) return bail("cudaGetDeviceProperties", e);
-    if (prop.major < 10)
+    if (prop.major != 9 || prop.minor != 0) // sm_90a code loads on compute capability 9.0 only
     {
-        g_create_err = "sx_create: this library is built for sm_100a (B200) only";
+        g_create_err = "sx_create: this library is built for sm_90a (H100) only";
         sx_destroy(ctx);
         return SX_ERR_CUDA;
     }

@@ -1,4 +1,4 @@
-// test_host_mirror.cpp -- the C++ host mirror (strelka_b200/host/strelka_b200.hh) on a B200, written the way the reference's own
+// test_host_mirror.cpp -- the C++ host mirror (strelka_b200/host/strelka_b200.hh) on the GPU, written the way the reference's own
 // unit tests read (alignment/test/GlobalAlignerTest.cpp, starling_common/test/starling_read_align_test.cpp):
 //   * GlobalAligner<int>::align on the reference's 22 known-answer cases (CIGAR, beginPos, score)
 //   * ReadAlignBatch::scoreCandidateAlignments on reference-shaped CandidateAlignments, compared bit-for-bit with the reference's

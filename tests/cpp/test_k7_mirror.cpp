@@ -1,4 +1,4 @@
-// tests/cpp/test_k7_mirror.cpp -- the K7 part of the C++ host mirror on a B200: sx::AlignmentSearchBatch through the real library
+// tests/cpp/test_k7_mirror.cpp -- the K7 part of the C++ host mirror on the GPU: sx::AlignmentSearchBatch through the real library
 // against the candidate alignments the reference's getCandidateAlignments returned (tests/golden/k7_cases.tsv).  The same check runs
 // without a GPU in tests/cpp/test_k7_mirror_cpu.cpp.  Build/run: tests/test_zz_gpu_enumerate.py::test_cpp_host_mirror_k7.
 #include "k7_mirror_check.hh"

@@ -278,19 +278,16 @@ def test_device_resident_chain_from_the_mappers_alignments(ctx, case):
 
 @pytest.mark.parametrize("block", range(10))
 def test_chain_equals_the_references_realignAndScoreRead(ctx, block):
-    """K7g -> K7a -> K7 -> K7b -> K1 -> K6 + K9 on the B200 against the reference's own realignAndScoreRead (oracle/_ref, which travels to the
-    GPU box) on 200 seeded batches: is_realigned, rseg.realignment segment for segment -- hard clips included --, getBestAlignment() of the
-    reads that keep the mapper's alignment, and the ReadPathScores score_indels left in the indel buffer.  (tests/test_chain_plumbing.py runs
-    the same function on the CPU mock.)"""
-    if not reflib.have_ref():
-        pytest.skip("oracle/_ref/libstrelka_ref.so not built")
-    from test_chain_plumbing import chain_vs_realign_and_score_read
+    """K7g -> K7a -> K7 -> K7b -> K1 -> K6 + K9 on the GPU against the reference's own realignAndScoreRead (oracle/_ref where it is built,
+    its frozen digests elsewhere) on 200 seeded batches: is_realigned, rseg.realignment segment for segment -- hard clips included --,
+    getBestAlignment() of the reads that keep the mapper's alignment, and the ReadPathScores score_indels left in the indel buffer.
+    (tests/test_chain_plumbing.py runs the same function on the CPU mock.)"""
+    from test_chain_plumbing import chain_case, chain_vs_realign_and_score_read
 
     n_real = n_recs = 0
     for case in range(20 * block, 20 * block + 20):
-        eb = specgen.enum_edge_case(case) if case % 2 else specgen.enum_case(case)
-        gb = B.GateBatch(eb, specgen.raw_alignments_for(eb, 100 + case))
-        a, b, _c = chain_vs_realign_and_score_read(ctx, eb, gb)
+        eb, gb = chain_case(case)
+        a, b, _c = chain_vs_realign_and_score_read(ctx, eb, gb, case)
         n_real += a
         n_recs += b
     assert n_real > 100 and n_recs > 100

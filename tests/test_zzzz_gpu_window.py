@@ -5,10 +5,9 @@ import numpy as np
 import pytest
 
 import reflib
-import specgen
+import refgold
 import window_check as W
-from strelka_b200 import _abi as A
-from strelka_b200 import batch as B
+from window_check import WW
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900, method="thread")]
 
@@ -26,24 +25,12 @@ def ctx():
 def test_window_equals_the_reference(ctx, block):
     """200 seeded batches (plain, clustered / conflicting, phased, dense windows, hard and soft clips, moved starts, over-long deletions,
     reads the gates turn away), each region a window: per read is_realigned / rseg.realignment segment for segment (hard clips included) and
-    score_indels' records; per window the pile-up columns in read-buffer order and the germline site results."""
-    if not reflib.have_ref():
-        pytest.skip("oracle/_ref/libstrelka_ref.so not built")
+    score_indels' records; per window the pile-up columns in read-buffer order and the germline site results -- against the reference where
+    oracle/_ref is built, against its frozen digests elsewhere."""
     tot = {"reads": 0, "realigned": 0, "records": 0, "threw": 0, "calls": 0, "sites": 0}
     for case in range(10 * block, 10 * block + 10):
-        eb = specgen.enum_edge_case(case) if case % 2 else specgen.enum_case(case)
-        raw = specgen.raw_alignments_for(eb, 100 + case)
-        for eb1, gb1 in W.single_region_windows(eb, raw):
-            rng = np.random.default_rng(77000 + case)
-            n = eb1.n_reads
-            # strands, tiers (a few tier2 and sub-mapped reads), mapping qualities and indel error rates vary
-            tier = rng.choice([1, 1, 1, 1, 2, 0], size=n + 1)
-            flags = ((rng.random(n + 1) < 0.5).astype(np.uint8) * A.SX_PRF_FWD) | np.where(tier == 1, A.SX_PRF_TIER1 | A.SX_PRF_TIER1OR2, 0).astype(np.uint8) | np.where(
-                tier == 2, A.SX_PRF_TIER1OR2, 0).astype(np.uint8)
-            eb1.keys["ref_to_indel_lnp"][: eb1.n_keys] = -rng.uniform(5.0, 12.0, eb1.n_keys)
-            eb1.keys["indel_to_ref_lnp"][: eb1.n_keys] = -rng.uniform(5.0, 12.0, eb1.n_keys)
-            mapq = rng.choice([60, 60, 60, 30, 3], size=n + 1).astype(np.uint8)
-            s = W.check_window(ctx, eb1, gb1, read_flags=flags, mapq=mapq)
+        for i, (eb1, gb1, flags, mapq) in enumerate(W.window_case(case)):
+            s = W.check_window(ctx, eb1, gb1, f"{case}.{i}", read_flags=flags, mapq=mapq)
             for k in tot:
                 tot[k] += s[k]
     assert tot["realigned"] > 0 and tot["records"] > 0 and tot["calls"] > 0, tot
@@ -53,25 +40,21 @@ def test_window_equals_the_reference(ctx, block):
 def test_synthetic_cfg2_window_equals_the_reference(ctx, qual_bits, seed):
     """bench.py's workload (tools/synth_window.cpp: a contig tiled by candidate loci at 30x, mapper-style alignments) through the one-call pass
     against the reference's realignAndScoreRead + pileup_read_segment + position_snp_call_pprob_digt on the same arrays: best alignments,
-    score_indels records, columns (in read-buffer order across loci) and site results."""
-    import os
-    import sys
-
-    if not reflib.have_ref():
-        pytest.skip("oracle/_ref/libstrelka_ref.so not built")
-    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tools"))
-    import window_workload as WW
+    score_indels records, columns (in read-buffer order across loci) and site results (or their frozen digests where oracle/_ref is not built)."""
     from strelka_b200.api import DevWindow
 
     w = WW.make_window(WW.load_synth(), 400, seed, tile=seed, qual_bits=qual_bits, ascii_reads=True)
+    entry = refgold.golden()["synthetic"][f"{qual_bits}-{seed}"]
+    assert entry["inputs"] == refgold.synthetic_inputs_digest(w), "the seeded inputs changed: regenerate tests/golden/window_ref_digests.json"
     dw = DevWindow(ctx, w)
     dw.run()
     d = dw.download()
     dw.run()  # a second pass over the same buffers (the region records were rewritten by the first)
     d2 = dw.download()
     dw.free()
-    res, _secs = WW.reference_pass(w)
-    stats = WW.compare_with_reference(w, d, res)
+    got = WW.window_items(w, d)
+    refgold.compare(got, WW.reference_items(w, WW.reference_pass(w)[0]) if reflib.have_ref() else None, entry)
+    stats = WW.window_stats(w, got)
     for k in d:
         assert np.asarray(d[k]).tobytes() == np.asarray(d2[k]).tobytes(), k
     assert stats["realigned"] > 5000 and stats["records"] > 10000 and stats["variant_sites"] > 50, stats

@@ -3,12 +3,20 @@ REFERENCE run stage by stage on the same window through oracle/_ref/libstrelka_r
     realignAndScoreRead per read            (ref_realign_and_score_read_ex: is_realigned, rseg.realignment, the ReadPathScores it left)
     pileup_read_segment per read            (ref_pileup_reads, in read-buffer order, each read through getBestAlignment())
     position_snp_call_pprob_digt per site   (ref_site_gl_germline)
-Where the reference library is absent the CPU oracles stand in for the last two (they are pinned to it, tests/test_oracle_vs_reference.py)."""
+Where the reference library is absent, check_window compares with the reference's frozen digests (tests/refgold.py)."""
+import os
+import sys
+
 import numpy as np
 
 import reflib
+import refgold
+import specgen
 from strelka_b200 import _abi as A
 from strelka_b200 import batch as B
+
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tools"))
+import window_workload as WW  # noqa: E402
 
 K4_CHAR = {0: "M", 1: "I", 3: "S", 4: "H", 5: "D", 6: "N"}
 COL_NAMES = ("site_off", "calls", "t2_off", "t2_calls", "n_spandel", "n_submapped")
@@ -73,6 +81,12 @@ def parse_k4(cig):
     return out
 
 
+def raw_of(gb, r):
+    """the mapper's alignment of read r: ((pos, cigar in K4 letters), [(op, len)])"""
+    raw_path = [(B.AP_CHAR[int(s["kind"])], int(s["len"])) for s in gb.raw_segs[int(gb.seg_off[r]) : int(gb.seg_off[r + 1])]]
+    return (int(gb.raw_pos[r]), "".join(f"{ln}{t}" for t, ln in raw_path).replace("=", "M").replace("X", "M")), raw_path
+
+
 def reference_window(eb, gb, w, quals=None, params=None):
     """the window through the reference, stage by stage: per-read (status, best alignment as (pos, cigar in K4 letters), records), the
     columns and the site results (None when the reference threw on a read: its process would have stopped there)"""
@@ -86,8 +100,7 @@ def reference_window(eb, gb, w, quals=None, params=None):
     exp = {"status": ref_status, "want": want, "recs": r_recs, "n_rec": r_n_rec, "submapped": submapped, "best": [], "cols": None, "gl": None}
     raws = []
     for r in range(n):
-        raw_path = [(B.AP_CHAR[int(s["kind"])], int(s["len"])) for s in gb.raw_segs[int(gb.seg_off[r]) : int(gb.seg_off[r + 1])]]
-        raw = (int(gb.raw_pos[r]), "".join(f"{ln}{t}" for t, ln in raw_path).replace("=", "M").replace("X", "M"))
+        raw, raw_path = raw_of(gb, r)
         raws.append((raw, raw_path))
         if submapped[r] or (ref_status[r] != 2 and want[r] is None):
             exp["best"].append(raw)
@@ -126,52 +139,75 @@ def reference_window(eb, gb, w, quals=None, params=None):
     return exp
 
 
-def check_window(ctx, eb, gb, pools=None, read_flags=None, mapq=None, quals=None, params=None, report=None, dry=False):
-    """one window through sx_process_window_dev and through the reference; returns counters.  `quals`: the per-base qualities as the
-    reference harness takes them (one byte per base, reads back to back) -- None: B.read_pools_of's constant 30.  dry: only the reference side."""
-    pools = pools or B.read_pools_of(eb)
+def window_case(case):
+    """the single-region windows of seeded batch `case`, each as (eb1, gb1, read_flags, mapq): strands, tiers (a few tier2 and sub-mapped
+    reads), mapping qualities and indel error rates vary"""
+    eb = specgen.enum_edge_case(case) if case % 2 else specgen.enum_case(case)
+    raw = specgen.raw_alignments_for(eb, 100 + case)
+    for eb1, gb1 in single_region_windows(eb, raw):
+        rng = np.random.default_rng(77000 + case)
+        n = eb1.n_reads
+        tier = rng.choice([1, 1, 1, 1, 2, 0], size=n + 1)
+        flags = ((rng.random(n + 1) < 0.5).astype(np.uint8) * A.SX_PRF_FWD) | np.where(tier == 1, A.SX_PRF_TIER1 | A.SX_PRF_TIER1OR2, 0).astype(np.uint8) | np.where(
+            tier == 2, A.SX_PRF_TIER1OR2, 0).astype(np.uint8)
+        eb1.keys["ref_to_indel_lnp"][: eb1.n_keys] = -rng.uniform(5.0, 12.0, eb1.n_keys)
+        eb1.keys["indel_to_ref_lnp"][: eb1.n_keys] = -rng.uniform(5.0, 12.0, eb1.n_keys)
+        mapq = rng.choice([60, 60, 60, 30, 3], size=n + 1).astype(np.uint8)
+        yield eb1, gb1, flags, mapq
+
+
+def reference_items(exp, w):
+    """reference_window's answers as the items check_window compares: per read handed to realignAndScoreRead that the reference did not
+    throw on, (read, is_realigned, best alignment, #records, the records' bytes); the columns and site results where it piled up"""
+    ro = w.a["rec_off"]
+    reads = []
+    for r in range(len(exp["status"])):
+        if exp["submapped"][r] or exp["status"][r] == 2:
+            continue
+        o, k = int(ro[r]), int(exp["n_rec"][r])
+        reads.append((r, exp["want"][r] is not None, exp["best"][r], k, exp["recs"][o : o + k].tobytes()))
+    it = {"reads": reads}
+    if exp["cols"] is not None:
+        it.update(zip(COL_NAMES, exp["cols"]))
+        it.update(WW.site_gl_items(exp["gl"]))
+    return it
+
+
+def check_window(ctx, eb, gb, key, read_flags=None, mapq=None):
+    """one window through sx_process_window_dev and through the reference (or its frozen digests under `key`, tests/refgold.py); returns
+    counters.  Qualities: B.read_pools_of's constant 30, as the reference harness gets them."""
     n = eb.n_reads
-    w = B.WindowBatch.from_enum(eb, gb, pools, read_flags=read_flags, mapq=mapq, report=report)
-    exp = reference_window(eb, gb, w, quals, params)
-    stats = {"reads": n, "realigned": 0, "records": 0, "threw": int((exp["status"] == 2).sum()), "calls": 0, "sites": 0, "stage_ms": {}}
-    if dry:
-        return stats
+    w = B.WindowBatch.from_enum(eb, gb, B.read_pools_of(eb), read_flags=read_flags, mapq=mapq)
+    entry = refgold.golden()["window"].get(key)  # (the batches' seeded inputs are checked by the chain comparisons of the same cases)
+    if reflib.have_ref():
+        exp = reference_window(eb, gb, w)
+        want, threw, piled = reference_items(exp, w), [int(r) for r in np.nonzero(exp["status"] == 2)[0]], exp["cols"] is not None
+    else:
+        want, threw, piled = None, entry["threw"], entry["piled"]
+    submapped = (w.a["read_flags"][:n] & A.SX_PRF_TIER1OR2) == 0
     from strelka_b200.api import DevWindow
 
     dw = DevWindow(ctx, w)
-    stats["stage_ms"] = dw.run()
+    stage_ms = dw.run()
     d = dw.download()
     dw.free()
     seg_off, segs = d["best_seg_off"], d["best_segs"]
+    reads = []
     for r in range(n):
         got = (int(d["best_pos"][r]), cigar_of(segs[int(seg_off[r]) : int(seg_off[r]) + int(d["best_n_seg"][r])]))
-        if exp["submapped"][r]:  # align_pos :746: never handed to realignAndScoreRead
-            assert not (int(d["gate"][r]) & A.SX_GATE_REALIGN) and got == exp["raw"][r], (r, got, exp["raw"][r])
+        if submapped[r]:  # align_pos :746: never handed to realignAndScoreRead
+            raw = raw_of(gb, r)[0]
+            assert not (int(d["gate"][r]) & A.SX_GATE_REALIGN) and got == raw, (r, got, raw)
             continue
-        if exp["status"][r] == 2:
+        if r in threw:
             continue
         assert not (int(d["enum_status"][r]) & A.SX_ENUM_ST_LIMIT), (r, "a per-read capacity of the search")
-        realigned = exp["want"][r] is not None
-        assert bool(int(d["realign_status"][r]) & A.SX_REALIGN_ST_REALIGNED) == realigned, (r, int(d["realign_status"][r]), exp["want"][r])
-        assert got == exp["best"][r], (r, got, exp["best"][r])
-        stats["realigned"] += int(realigned)
-        o = int(w.a["rec_off"][r])
-        assert int(d["n_rec"][r]) == int(exp["n_rec"][r]), (r, int(d["n_rec"][r]), int(exp["n_rec"][r]))
-        assert d["recs"][o : o + int(d["n_rec"][r])].tobytes() == exp["recs"][o : o + int(exp["n_rec"][r])].tobytes(), r
-        stats["records"] += int(exp["n_rec"][r])
-    if exp["cols"] is None:
-        return stats  # the reference process would have stopped at the throw: no pile-up to compare
-    got_cols = (d["site_off"], d["calls"], d["t2_off"], d["t2_calls"], d["n_spandel"], d["n_submapped"])
-    for wv, gv, name in zip(exp["cols"], got_cols, COL_NAMES):
-        assert np.array_equal(wv, gv), name
-    stats["calls"] = int(exp["cols"][0][-1])
-    gl, g = exp["gl"], d["site_gl"]
-    for f in ("ref_gt", "is_computed", "n_used_calls", "phredLoghood"):
-        assert np.array_equal(gl[f], g[f]), f
-    assert np.array_equal(gl["lhood"].view(np.uint32), g["lhood"].view(np.uint32)), "lhood"
-    for rs in ("genome", "poly"):
-        for f in ("max_gt", "snp_qphred", "max_gt_qphred"):
-            assert np.array_equal(gl[rs][f], g[rs][f]), (rs, f)
-        assert np.array_equal(np.ascontiguousarray(gl[rs]["ref_pprob"]).view(np.uint64), np.ascontiguousarray(g[rs]["ref_pprob"]).view(np.uint64)), (rs, "ref_pprob")
-    stats["sites"] = w.n_sites
-    return stats
+        o, k = int(w.a["rec_off"][r]), int(d["n_rec"][r])
+        reads.append((r, bool(int(d["realign_status"][r]) & A.SX_REALIGN_ST_REALIGNED), got, k, d["recs"][o : o + k].tobytes()))
+    it = {"reads": reads}
+    if piled:  # (else the reference process would have stopped at the throw: no pile-up to compare)
+        it.update(zip(COL_NAMES, (d["site_off"], d["calls"], d["t2_off"], d["t2_calls"], d["n_spandel"], d["n_submapped"])))
+        it.update(WW.site_gl_items(d["site_gl"]))
+    refgold.compare(it, want, entry)
+    return {"reads": n, "realigned": sum(x[1] for x in reads), "records": sum(x[3] for x in reads), "threw": len(threw),
+            "calls": int(d["site_off"][-1]) if piled else 0, "sites": w.n_sites if piled else 0, "stage_ms": stage_ms}

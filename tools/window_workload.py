@@ -182,42 +182,57 @@ def reference_pass(w: B.WindowBatch, params=None, max_segs: int = 16):
     return res, {"realign": secs.value, "pileup": s_pile.value, "site_gl": s_gl.value, "realign_call": t_realign_call, "pileup_call": t_pileup, "site_gl_call": t_gl}
 
 
-def compare_with_reference(w: B.WindowBatch, d: dict, res: dict):
-    """d: DevWindow.download() of the same window; raises AssertionError at the first difference; returns counters"""
-    n, ns = w.n_reads, w.n_sites
-    assert not (res["status"] == 2).any(), "the reference threw on a synthetic read"
-    realigned = res["status"] == 1
-    assert np.array_equal(realigned, (d["realign_status"] & A.SX_REALIGN_ST_REALIGNED) != 0), "is_realigned"
-    assert not (d["enum_status"] & (A.SX_ENUM_ST_LIMIT | A.SX_ENUM_ST_EXCEPTION)).any(), "reads left to the caller"
-    assert np.array_equal(res["best_pos"], d["best_pos"]), "best alignment position"
-    # paths, pads of the device's slot layout dropped
-    dseg, doff, dn = d["best_segs"], d["best_seg_off"], d["best_n_seg"]
-    keep = np.zeros(len(dseg), bool)
-    idx = np.concatenate([np.arange(int(doff[r]), int(doff[r]) + int(dn[r])) for r in range(n)]) if n else np.zeros(0, np.int64)
-    keep[idx] = True
-    assert np.array_equal(np.diff(res["best_off"].astype(np.int64)), dn.astype(np.int64)), "best alignment segment counts"
-    assert dseg[keep].tobytes() == res["best_segs"].tobytes(), "best alignment paths"
-    assert np.array_equal(res["n_rec"], d["n_rec"]), "score_indels record counts"
-    ro = w.a["rec_off"]
-    rk = np.zeros(len(d["recs"]), bool)
-    ridx = np.concatenate([np.arange(int(ro[r]), int(ro[r]) + int(d["n_rec"][r])) for r in range(n)]) if n else np.zeros(0, np.int64)
-    rk[ridx] = True
-    assert d["recs"][rk].tobytes() == res["recs"][: len(rk)][rk].tobytes(), "score_indels records"
-    for name in ("site_off", "calls", "t2_off", "n_spandel", "n_submapped"):
-        assert np.array_equal(res[name], d[name]), name
-    gl, g = res["site_gl"], d["site_gl"]
-    for f in ("ref_gt", "is_computed", "n_used_calls", "phredLoghood"):
-        assert np.array_equal(gl[f], g[f]), f
-    assert np.array_equal(gl["lhood"].view(np.uint32), g["lhood"].view(np.uint32)), "lhood"
+def site_gl_items(gl) -> dict:
+    """the compared fields of position_snp_call_pprob_digt's results, floats as their bits"""
+    it = {f: np.ascontiguousarray(gl[f]) for f in ("ref_gt", "is_computed", "n_used_calls", "phredLoghood")}
+    it["lhood"] = np.ascontiguousarray(gl["lhood"]).view(np.uint32)
     for rs in ("genome", "poly"):
         for f in ("max_gt", "snp_qphred", "max_gt_qphred"):
-            assert np.array_equal(gl[rs][f], g[rs][f]), (rs, f)
-        assert np.array_equal(np.ascontiguousarray(gl[rs]["ref_pprob"]).view(np.uint64), np.ascontiguousarray(g[rs]["ref_pprob"]).view(np.uint64)), (rs, "ref_pprob")
-    if "variant_sites" in d:  # the compacted call records: the computed non-reference sites in position order, each with its record and depth
+            it[f"{rs}.{f}"] = np.ascontiguousarray(gl[rs][f])
+        it[f"{rs}.ref_pprob"] = np.ascontiguousarray(gl[rs]["ref_pprob"]).view(np.uint64)
+    return it
+
+
+def _packed(arr, off, cnt):
+    """arr[off[r] : off[r] + cnt[r]] of every r, back to back"""
+    n = len(cnt)
+    idx = np.concatenate([np.arange(int(off[r]), int(off[r]) + int(cnt[r])) for r in range(n)]) if n else np.zeros(0, np.int64)
+    return arr[idx.astype(np.int64)]
+
+
+def reference_items(w: B.WindowBatch, res: dict) -> dict:
+    """reference_pass' results as the items a comparison with the device pass compares (tests/refgold.py)"""
+    assert not (res["status"] == 2).any(), "the reference threw on a synthetic read"
+    it = {"is_realigned": res["status"] == 1, "best_pos": res["best_pos"], "best_n_seg": np.diff(res["best_off"].astype(np.int64)), "best_segs": res["best_segs"],
+          "n_rec": res["n_rec"], "recs": _packed(res["recs"], w.a["rec_off"], res["n_rec"])}
+    for name in ("site_off", "calls", "t2_off", "n_spandel", "n_submapped"):
+        it[name] = res[name]
+    it.update(site_gl_items(res["site_gl"]))
+    return it
+
+
+def window_items(w: B.WindowBatch, d: dict) -> dict:
+    """DevWindow.download() of the window as the items reference_items describes (pads of the device's slot layout dropped), after the
+    checks that need no reference: no read left to the caller, and the compacted call records are the computed non-reference sites in
+    position order, each with its record and depth"""
+    n = w.n_reads
+    assert not (d["enum_status"] & (A.SX_ENUM_ST_LIMIT | A.SX_ENUM_ST_EXCEPTION)).any(), "reads left to the caller"
+    g = d["site_gl"]
+    if "variant_sites" in d:
         sel = np.nonzero((g["is_computed"] != 0) & (g["genome"]["max_gt"] != g["ref_gt"]))[0]
         v = d["variant_sites"]
         assert np.array_equal(v["pos"], (w.report_begin + sel).astype(np.int32)), "variant site positions"
         assert v["gl"].tobytes() == g[sel].tobytes(), "variant site records"
         assert np.array_equal(v["n_calls"], np.diff(d["site_off"].astype(np.int64))[sel].astype(np.uint32)), "variant site depths"
-    return {"reads": n, "realigned": int(realigned.sum()), "records": int(res["n_rec"].sum()), "calls": int(res["site_off"][ns]), "sites": ns,
-            "variant_sites": int((gl["genome"]["max_gt"] != gl["ref_gt"]).sum())}
+    it = {"is_realigned": (d["realign_status"][:n] & A.SX_REALIGN_ST_REALIGNED) != 0, "best_pos": d["best_pos"][:n], "best_n_seg": d["best_n_seg"][:n],
+          "best_segs": _packed(d["best_segs"], d["best_seg_off"], d["best_n_seg"][:n]), "n_rec": d["n_rec"][:n], "recs": _packed(d["recs"], w.a["rec_off"], d["n_rec"][:n])}
+    for name in ("site_off", "calls", "t2_off", "n_spandel", "n_submapped"):
+        it[name] = d[name]
+    it.update(site_gl_items(g))
+    return it
+
+
+def window_stats(w: B.WindowBatch, it: dict) -> dict:
+    return {"reads": w.n_reads, "realigned": int(it["is_realigned"].sum()), "records": int(np.asarray(it["n_rec"]).sum()), "calls": int(it["site_off"][w.n_sites]),
+            "sites": w.n_sites, "variant_sites": int((it["genome.max_gt"] != it["ref_gt"]).sum())}
+
