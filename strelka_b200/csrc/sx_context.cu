@@ -446,6 +446,8 @@ extern "C" int sx_create(int cuda_device, const sx_params* p, sx_ctx** out)
     build_tables(*p, ctx->tables);
     if ((e = cudaMalloc(&ctx->d_tables, sizeof(sx_tables))) != cudaSuccess) return bail("cudaMalloc", e);
     if ((e = cudaMemcpy(ctx->d_tables, &ctx->tables, sizeof(sx_tables), cudaMemcpyHostToDevice)) != cudaSuccess) return bail("cudaMemcpy", e);
+    if ((e = sx_k2a_init_tables(ctx->d_tables)) != cudaSuccess) return bail("K2a tables", e);
+    if ((e = cudaMemcpy(&ctx->tables, ctx->d_tables, sizeof(sx_tables), cudaMemcpyDeviceToHost)) != cudaSuccess) return bail("cudaMemcpy", e);
     if ((e = cudaMalloc(&ctx->d_status, sizeof(int))) != cudaSuccess) return bail("cudaMalloc", e);
     cudaMemset(ctx->d_status, 0, sizeof(int));
     *out = ctx;

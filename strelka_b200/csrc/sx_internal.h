@@ -43,6 +43,17 @@ struct sx_tables
     float g_log_one_third, g_min_vexp;
     double g_ssd_no_mismatch, g_ssd_one_mismatch;
     int g_is_dependent_eprob, g_is_min_vexp;
+    // val0 = logf(de) + ln(1/3) of a call (position_snp_call_pprob_digt.cpp:352) wherever de is a function of q alone.  Filled on the
+    // device right after the upload (sx_k2a_init_tables, k2a_germline.cu) with the kernel's own device functions:
+    //   g_val0_plain[q]     de = eprob[q]                (q < 3, or no dependent error model)
+    //   g_val0_min[q]       de = depmin[q]               (ranks at or past the exponent clamp)
+    //   g_val0_clean[k][q]  de = dependent_eprob(eprob[q], vexp_k), k < g_clean_ranks, in a group without a neighbour-mismatch call
+    //                       (its vexp_frac is (float)bsnp_ssd_no_mismatch, so the exponents vexp_k are the same in every such group)
+    // g_clean_ok: the clean-group rows apply (dependent model on, exponent clamp on, clamp reached within SX_K2_CLEAN_RANKS ranks).
+#define SX_K2_CLEAN_RANKS 8
+    float g_val0_plain[SX_MAX_QSCORE + 1], g_val0_min[SX_MAX_QSCORE + 1];
+    float g_val0_clean[SX_K2_CLEAN_RANKS][SX_MAX_QSCORE + 1];
+    int g_clean_ranks, g_clean_ok;
     // somatic site model
     float s_simple[SX_MAX_QSCORE + 1][3];     // val[0..2] of get_diploid_gt_lhood_cached_simple
     float s_het[9][SX_MAX_QSCORE + 1][2];     // val[0..1] of get_high_low_het_ratio_lhood_cached for ratio index 0..8
@@ -67,6 +78,7 @@ struct sx_tables
 
 int sx_upload_pileup(sx_ctx* ctx, const sx_pileup_batch* b, int slot_base, sx_pileup_batch* d, uint32_t* max_site, cudaStream_t st);
 int sx_k2_max_site_dev(sx_ctx* ctx, const uint32_t* site_off_dev, uint32_t n_sites, uint32_t* out);
+cudaError_t sx_k2a_init_tables(sx_tables* d_tables); // fills the g_val0_* rows of the device copy (synchronous)
 
 struct sx_buf
 {

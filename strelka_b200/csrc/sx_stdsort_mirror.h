@@ -112,12 +112,15 @@ template <typename IdxT, typename KeyT> SX_HD void sx_sort_heapsort(IdxT* v, int
     }
 }
 
-template <typename IdxT, typename KeyT> SX_HD void sx_stdsort_desc(IdxT* v, const uint32_t n_, const KeyT& key)
+// StackN bounds the explicit stack: every partition pushes one entry and spends one unit of depth_limit = 2*floor(log2(n)), so
+// 2*floor(log2(n_max)) + 1 entries cover every n <= n_max (64 covers any 32-bit n; 16 covers n < 256).
+// __introsort_loop alone (n > 16).  What std::sort does after it, __final_insertion_sort, is an insertion sort, and an insertion sort is
+// stable: the final order is the stable descending sort of the array this leaves.  A caller that needs only part of that order (the first
+// few positions) can take it from here without the insertion sort.
+template <int StackN = 64, typename IdxT, typename KeyT> SX_HD void sx_introsort_loop_desc(IdxT* v, const int n, const KeyT& key)
 {
-    const int n = (int)n_;
-    if (n == 0) return;
-    // __introsort_loop, recursion on the right part replaced by an explicit stack (depth <= depth_limit <= 62)
-    int stack_first[64], stack_last[64], stack_depth[64];
+    // recursion on the right part replaced by an explicit stack
+    int stack_first[StackN], stack_last[StackN], stack_depth[StackN];
     int sp = 0;
     int lg = 0;
     for (int t = n; t > 1; t >>= 1) ++lg; // std::__lg
@@ -181,14 +184,19 @@ template <typename IdxT, typename KeyT> SX_HD void sx_stdsort_desc(IdxT* v, cons
             last = cut;
         }
     }
-    // __final_insertion_sort
-    if (n > 16)
-    {
-        sx_sort_insertion(v, 0, 16, key);
-        for (int i = 16; i != n; ++i) sx_sort_unguarded_linear_insert(v, i, key);
-    }
-    else
+}
+
+template <int StackN = 64, typename IdxT, typename KeyT> SX_HD void sx_stdsort_desc(IdxT* v, const uint32_t n_, const KeyT& key)
+{
+    const int n = (int)n_;
+    if (n == 0) return;
+    if (n <= 16) // __introsort_loop returns at once; __final_insertion_sort is a plain insertion sort
     {
         sx_sort_insertion(v, 0, n, key);
+        return;
     }
+    sx_introsort_loop_desc<StackN>(v, n, key);
+    // __final_insertion_sort (n > 16)
+    sx_sort_insertion(v, 0, 16, key);
+    for (int i = 16; i != n; ++i) sx_sort_unguarded_linear_insert(v, i, key);
 }
