@@ -77,7 +77,6 @@ struct sx_tables
 };
 
 int sx_upload_pileup(sx_ctx* ctx, const sx_pileup_batch* b, int slot_base, sx_pileup_batch* d, uint32_t* max_site, cudaStream_t st);
-int sx_k2_max_site_dev(sx_ctx* ctx, const uint32_t* site_off_dev, uint32_t n_sites, uint32_t* out);
 cudaError_t sx_k2a_init_tables(sx_tables* d_tables); // fills the g_val0_* rows of the device copy (synchronous)
 
 struct sx_buf

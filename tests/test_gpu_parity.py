@@ -234,14 +234,8 @@ def test_k3_reference_unit_test_goldens(ctx):
             assert int(res["score"][0]) == case["score"], case["name"]
 
 
-@pytest.mark.parametrize("seed,depth", [(0, 8.0), (1, 30.0), (2, 60.0), (3, 150.0)])
-@pytest.mark.parametrize("always", [True, False])
-def test_k2a_site_gl_germline(ctx, seed, depth, always):
-    rng = np.random.default_rng(2000 + seed)
-    pb = specgen.random_pileups(rng, 2000, depth=depth)
-    p = A.default_params()
-    want = reflib.ox_germline(p, pb, always)
-    got = ctx.site_gl_germline(pb, always)
+def _same_germline(want, got):
+    """every field of two sx_digt_result arrays: equal integers, the same bits for the floats and doubles"""
     for f in ("ref_gt", "is_computed", "n_used_calls", "phredLoghood"):
         assert np.array_equal(want[f], got[f]), f
     assert np.array_equal(_bits(want["lhood"]), _bits(got["lhood"]))
@@ -250,6 +244,15 @@ def test_k2a_site_gl_germline(ctx, seed, depth, always):
         for f in ("max_gt", "snp_qphred", "max_gt_qphred"):
             assert np.array_equal(want[rs][f], got[rs][f]), (rs, f)
         assert np.array_equal(_bits(got[rs]["ref_pprob"]), _bits(want[rs]["ref_pprob"])), (rs, "ref_pprob")  # exp / log10 are the libm mirrors (sx_libm_mirror_d.h)
+
+
+@pytest.mark.parametrize("seed,depth", [(0, 8.0), (1, 30.0), (2, 60.0), (3, 150.0)])
+@pytest.mark.parametrize("always", [True, False])
+def test_k2a_site_gl_germline(ctx, seed, depth, always):
+    rng = np.random.default_rng(2000 + seed)
+    pb = specgen.random_pileups(rng, 2000, depth=depth)
+    p = A.default_params()
+    _same_germline(reflib.ox_germline(p, pb, always), ctx.site_gl_germline(pb, always))
     o_off, o_de = reflib.ox_dependent_eprob(p, pb)
     g_off, g_de = ctx.dependent_eprob(pb)
     assert np.array_equal(o_off, g_off)
@@ -293,6 +296,34 @@ def test_k2a_deep_and_empty_sites(ctx):
     want = reflib.ox_germline(p, empty, True)
     got = ctx.site_gl_germline(empty, True)
     assert want.tobytes() == got.tobytes()
+    # sites of <= 256 calls interleaved with sites of 257-3000 calls, more sites than the launch has warps: one launch (and one warp,
+    # site after site) takes sites in its shared-memory tile and in its global-scratch region
+    parts = [specgen.random_pileups(rng, 4400, depth=60.0), specgen.random_pileups(rng, 20, depth=250.0, max_depth=256),
+             specgen.random_pileups(rng, 20, depth=300.0, max_depth=3000), specgen.random_pileups(rng, 20, depth=2000.0, max_depth=3000)]
+    sites = [(pb.calls[pb.site_off[i]:pb.site_off[i + 1]].tolist(), chr(pb.ref_base[i])) for pb in parts for i in range(pb.n_sites)]
+    sites += [([], "A"), ([], "C"), ([], "T")]
+    sites = [sites[i] for i in rng.permutation(len(sites))]
+    n_ref = next(i for i, (c, r) in enumerate(sites) if len(c) > 256 and r != "N")
+    sites[n_ref] = (sites[n_ref][0], "N")
+    ploidy = np.where(rng.random(len(sites)) < 0.1, 1, 2).astype(np.uint8)
+    mixed = B.PileupBatch.from_sites([c for c, _ in sites], "".join(r for _, r in sites), ploidy)
+    depth = np.diff(mixed.site_off.astype(np.int64))
+    assert len(sites) % 16 != 0 and (depth == 0).sum() >= 3 and (depth > 256).sum() > 30 and depth.max() <= 3000
+    assert np.count_nonzero(np.diff((depth > 256).astype(np.int8))) > 30  # interleaved
+    from strelka_b200.api import Context
+
+    p2 = A.SxParams(0.001, 0.0, 0.0, 0, 1, 0.0, 0.0, 1e-4, 5e-10, 0.0, 0.15, 0, 0)  # no dependent error model
+    c2 = Context(0, p2)
+    try:
+        for params, c in ((p, ctx), (p2, c2)):
+            for always in (True, False):
+                _same_germline(reflib.ox_germline(params, mixed, always), c.site_gl_germline(mixed, always))
+            o_off, o_de = reflib.ox_dependent_eprob(params, mixed)
+            g_off, g_de = c.dependent_eprob(mixed)
+            assert np.array_equal(o_off, g_off)
+            assert np.array_equal(_bits(o_de), _bits(g_de))
+    finally:
+        c2.close()
 
 
 def test_k2a_haploid_and_no_dependency(ctx):
