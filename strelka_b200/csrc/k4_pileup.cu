@@ -53,7 +53,6 @@ struct k4_args
     int32_t origin; // position of window 0's first site (= report_begin - W)
     uint32_t W, n_windows, n_sites;
     uint32_t Lcap; // read-length capacity of the per-warp arrays (the batch's longest read, rounded up)
-    uint32_t span_max, shift_max; // the caller's max_ref_span and max_pos_shift (the gather plan's read range rests on them: checked per read)
     sx_pileup_opts opt;
 };
 
@@ -589,453 +588,6 @@ __global__ void __launch_bounds__(K4_WARPS * 32) k4_fill_kernel(k4_args A, const
     }
 }
 
-// ---------------------------------------------------------------------------------------------------------------------
-// pass 3, second plan: the fill as two kernels without a serial chain.
-//   k4_bases_kernel   THREAD per read, two flat loops over the read's bases (every lane of a warp runs the same loop; the read's own
-//                     segment boundaries only move a small per-lane cursor): (1) the mismatch-density map as a prefix-count array in
-//                     shared memory (one 16-bit entry per base: the events in a window are a difference of two entries; interior indels
-//                     are a short event list), (2) the base_call word of every base of the MATCH segments, written to a per-read row of
-//                     a scratch array, four calls per 64-bit store.  Packed bases and qualities arrive a 32-bit word at a time.
-//   k4_gather_kernel  WARP per 32 neighbouring sites, a lane per site: the warp walks the reads whose alignment can reach the block, in
-//                     read-buffer order -- one 32-byte record per read (its MATCH intervals as (first site, length, first read offset)),
-//                     warp-uniform --, a lane the read covers fetches its call from the read's row (neighbouring lanes = neighbouring
-//                     bases) and appends it to its column: the write cursor is a register.
-// The columns are the same bytes in both plans: a column lists its reads in read-buffer order.
-// ---------------------------------------------------------------------------------------------------------------------
-constexpr uint32_t K4_REC_IV = 3; // MATCH intervals a record holds; a read with more keeps its path (the gather walks it)
-struct __align__(16) k4_rrec // what the gather needs of a read (32 bytes)
-{
-    int32_t site_lo[K4_REC_IV]; // first site of interval j   | fallback: site of the alignment start, read_begin | read_end << 16, seg_off
-    uint16_t len[K4_REC_IV];    // its length
-    uint16_t p_lo[K4_REC_IV];   // read offset of its first base
-    uint32_t n_iv;              // intervals (0: no call; K4_REC_IV + 1: fallback) | n_seg << 8 | tier1 << 31
-};
-
-constexpr int K4B_THREADS = 64;
-constexpr uint32_t K4B_MAX_EV = 8; // interior indels kept per thread; a read with more walks its path per base
-
-// a byte array read through its 4-byte-aligned words (device allocations: the base is 256-byte aligned), positions ascending
-struct k4_wstream
-{
-    const uint32_t* w32;
-    uint32_t off; // byte offset of the read's first byte from w32
-    uint32_t cur; // word index held in w
-    uint32_t w;
-    __device__ __forceinline__ void init(const uint8_t* p)
-    {
-        const uintptr_t a = reinterpret_cast<uintptr_t>(p);
-        w32 = reinterpret_cast<const uint32_t*>(a & ~static_cast<uintptr_t>(3));
-        off = static_cast<uint32_t>(a & 3u);
-        cur = 0xffffffffu;
-        w = 0;
-    }
-    __device__ __forceinline__ uint32_t byte_at(uint32_t b)
-    {
-        const uint32_t ob = off + b, wi = ob >> 2;
-        if (wi != cur)
-        {
-            cur = wi;
-            w = __ldg(w32 + wi);
-        }
-        return (w >> (8u * (ob & 3u))) & 0xffu;
-    }
-    __device__ __forceinline__ uint32_t nibble_at(uint32_t i) { return (byte_at(i >> 1) >> ((~i & 1u) << 2)) & 15u; }
-};
-
-// per-lane cursor over a path while the read offset q runs 0, 1, 2, ...: the segment that holds base q
-struct k4_segcur
-{
-    const sx_aln_seg* path;
-    uint32_t as, i;   // segments, next segment to load
-    uint32_t seg_end; // read offset one past the current read-consuming segment
-    uint32_t kind;    // its kind (SX_SEG_*), 0xff before the first
-    uint32_t rf;      // reference offset (from the alignment start) after the segments loaded so far
-    int32_t rfd;      // MATCH: reference offset of base q = q + rfd
-    __device__ __forceinline__ void init(const sx_aln_seg* p, uint32_t n)
-    {
-        path = p;
-        as = n;
-        i = 0;
-        seg_end = 0;
-        kind = 0xffu;
-        rf = 0;
-        rfd = 0;
-    }
-};
-
-__global__ void __launch_bounds__(K4B_THREADS) k4_bases_kernel(k4_args A, k4_rrec* __restrict__ rec, uint16_t* __restrict__ bc, uint32_t Ls,
-                                                               const sx_tables* __restrict__ tables, int* __restrict__ status)
-{
-    extern __shared__ __align__(16) uint16_t k4b_P[]; // per thread Lcap + 2 entries: P[i] = mismatches among bases [0, i)
-    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= A.n_reads) return;
-    uint16_t* P = k4b_P + static_cast<size_t>(threadIdx.x) * (A.Lcap + 2u); // (Lcap % 16 == 0: an odd number of 32-bit words per thread, no bank conflicts)
-    const sx_pileup_read rd = A.reads[r];
-    const uint32_t as = A.reads[r + 1].seg_off - rd.seg_off;
-    const sx_aln_seg* path = A.segs + rd.seg_off;
-    k4_rrec out;
-#pragma unroll
-    for (uint32_t j = 0; j < K4_REC_IV; ++j)
-    {
-        out.site_lo[j] = 0;
-        out.len[j] = 0;
-        out.p_lo[j] = 0;
-    }
-    out.n_iv = 0;
-    bool ok = (rd.flags & SX_PRF_TIER1OR2) && !(rd.flags & SX_PRF_SKIP) && rd.len <= A.Lcap && as <= K4_MAX_SEGS; // (sub-mapped reads only count, limits: pass 1)
-    uint32_t ref_span = 0, first = as, last = as;
-    if (ok)
-    {
-        for (uint32_t i = 0; i < as; ++i)
-        {
-            const uint32_t k = path[i].kind;
-            if (kind_ref(k)) ref_span += path[i].len;
-            if (k == SX_SEG_MATCH)
-            {
-                if (first == as) first = i;
-                last = i;
-            }
-        }
-        if (ref_span > A.W) ok = false; // flagged by pass 1
-        // the gather looks for a site's reads among the buffer positions [P - span_max - shift_max, P + shift_max]
-        const int64_t sh = static_cast<int64_t>(rd.pos) - bpos_of(A, r);
-        if (ref_span > A.span_max || sh > static_cast<int64_t>(A.shift_max) || -sh > static_cast<int64_t>(A.shift_max))
-        {
-            atomicOr(status, ST_ORDER);
-            ok = false;
-        }
-    }
-    const uint8_t* gs = A.seq4 + rd.seq_off;
-    read_window w;
-    w.read_begin = w.read_end = 0;
-    if (ok && !read_preamble(A, rd, ref_span, [&](uint32_t i) { return code_at(gs, i); }, w)) ok = false;
-    if (!ok)
-    {
-        rec[r] = out;
-        return;
-    }
-    const uint32_t read_size = rd.len;
-    const uint32_t rb = w.read_begin, re = min(w.read_end, read_size);
-    const uint32_t fs = A.opt.mismatchDensityFilterFlankSize, fs2 = fs * 2;
-    const bool isDensity = fs > 0;
-    const uint32_t delta_size = max(1u + fs2, read_size) - fs2;
-    const int32_t site0 = static_cast<int32_t>(static_cast<int64_t>(rd.pos) - A.report_begin);
-    const int64_t ref0 = static_cast<int64_t>(rd.pos) - A.ref_begin; // index of the alignment's first reference base in A.ref
-    k4_wstream sq;
-    k4_segcur sc;
-    uint32_t ev[K4B_MAX_EV]; // interior indels: read offset << 16 | length (create_mismatch_filter_map's inc(start, length))
-    uint32_t n_ev = 0;
-    // the path once: the MATCH intervals for the gather, the interior indels for the density map
-    {
-        uint32_t p = 0, rf = 0, n_iv = 0;
-        for (uint32_t i = 0; i < as; ++i)
-        {
-            const uint32_t k = path[i].kind, len = path[i].len;
-            const bool edge = (i < first) || (i > last);
-            if (k == SX_SEG_MATCH)
-            {
-                const uint32_t a = max(p, rb), e = min(p + len, re);
-                if (a < e)
-                {
-                    // clipped to the reportable sites here: the gather asks for sites [0, n_sites) only
-                    int64_t s_lo = static_cast<int64_t>(site0) + rf + (a - p), s_hi = s_lo + (e - a);
-                    uint32_t a2 = a;
-                    if (s_lo < 0)
-                    {
-                        a2 += static_cast<uint32_t>(-s_lo);
-                        s_lo = 0;
-                    }
-                    if (s_hi > static_cast<int64_t>(A.n_sites)) s_hi = A.n_sites;
-                    if (s_lo < s_hi)
-                    {
-                        if (n_iv < K4_REC_IV)
-                        {
-                            out.site_lo[n_iv] = static_cast<int32_t>(s_lo);
-                            out.len[n_iv] = static_cast<uint16_t>(s_hi - s_lo);
-                            out.p_lo[n_iv] = static_cast<uint16_t>(a2);
-                        }
-                        ++n_iv;
-                    }
-                }
-            }
-            if (isDensity)
-            {
-                if (!edge && (k == SX_SEG_INSERT || k == SX_SEG_DELETE))
-                {
-                    if (n_ev < K4B_MAX_EV) ev[n_ev] = (p << 16) | (k == SX_SEG_INSERT ? len : 0u);
-                    ++n_ev;
-                }
-                else if (k == SX_SEG_SKIP) atomicOr(status, ST_KIND); // "Can't handle cigar code" in create_mismatch_filter_map
-            }
-            if (kind_read(k)) p += len;
-            if (kind_ref(k)) rf += len;
-        }
-        if (n_iv > K4_REC_IV)
-        {
-            out.site_lo[0] = site0;
-            out.site_lo[1] = static_cast<int32_t>(rb | (re << 16));
-            out.site_lo[2] = static_cast<int32_t>(rd.seg_off);
-            n_iv = K4_REC_IV + 1;
-        }
-        out.n_iv = n_iv | (as << 8) | ((rd.flags & SX_PRF_TIER1) ? 0x80000000u : 0u);
-    }
-// advance the cursor to the segment that holds base q (q ascends by one): warp-divergent only at a lane's own segment boundaries
-#define K4_SEG_ADVANCE(sc, q)                                                         \
-    while ((q) >= (sc).seg_end && (sc).i < (sc).as)                                   \
-    {                                                                                 \
-        const uint32_t k_ = (sc).path[(sc).i].kind, l_ = (sc).path[(sc).i].len;       \
-        ++(sc).i;                                                                     \
-        if (kind_read(k_))                                                            \
-        {                                                                             \
-            (sc).kind = k_;                                                           \
-            (sc).rfd = static_cast<int32_t>((sc).rf) - static_cast<int32_t>((sc).seg_end); \
-            (sc).seg_end += l_;                                                       \
-        }                                                                             \
-        if (kind_ref(k_)) (sc).rf += l_;                                              \
-    }
-    if (isDensity)
-    {
-        // create_mismatch_filter_map as counts: P[i] = mismatches (not registered candidate SNVs) among the bases before i, over the whole read
-        sq.init(gs);
-        sc.init(path, as);
-        uint32_t c = 0;
-        P[0] = 0;
-        for (uint32_t q = 0; q < read_size; ++q)
-        {
-            K4_SEG_ADVANCE(sc, q)
-            if (sc.kind == SX_SEG_MATCH && q < sc.seg_end && q >= rb && q < re)
-            {
-                const int32_t roff = static_cast<int32_t>(q) + sc.rfd;
-                const int64_t ri = ref0 + roff;
-                const char refc = (ri >= 0 && ri < static_cast<int64_t>(A.ref_len)) ? A.ref[ri] : 'N';
-                const uint32_t code = sq.nibble_at(q);
-                if (char_of_code(code) != refc)
-                {
-                    // CandidateSnvBuffer::isCandidateSnvAnySample: a registered (position, base) is not counted as a mismatch
-                    bool cand = false;
-                    const int id = static_cast<int>(id_of_code(code));
-                    const int32_t rel = site0 + roff;
-                    if (id < 4 && rel >= 0 && rel < (1 << 30))
-                    {
-                        const uint32_t key = (static_cast<uint32_t>(rel) << 2) | static_cast<uint32_t>(id);
-                        uint32_t l2 = 0, h2 = A.n_cand_snv;
-                        while (l2 < h2)
-                        {
-                            const uint32_t mid = (l2 + h2) >> 1;
-                            if (A.cand_snv[mid] < key) l2 = mid + 1;
-                            else h2 = mid;
-                        }
-                        cand = l2 < A.n_cand_snv && A.cand_snv[l2] == key;
-                    }
-                    if (!cand) ++c;
-                }
-            }
-            P[q + 1] = static_cast<uint16_t>(c);
-        }
-    }
-    // the calls
-    const uint32_t adjustedMapq = max(5u, static_cast<uint32_t>(rd.mapq));
-    const bool tier1 = rd.flags & SX_PRF_TIER1;
-    const uint32_t fwd_bit = (rd.flags & SX_PRF_FWD) ? (1u << 10) : 0u;
-    const bool is_mapq_adjust = A.opt.isBasecallQualAdjustedForMapq && adjustedMapq <= 80u;
-    const uint8_t* mqrow = tables->mappedq[min(adjustedMapq, 90u)];
-    // dictionary-coded qualities: the 16 possible results (dictionary value -> MAPQ-adjusted value, 255 = above the table) as two 64-bit literals
-    unsigned long long qlut_lo = 0, qlut_hi = 0;
-    if (A.qual_bits == 4)
-    {
-        for (uint32_t v = 0; v < 16; ++v)
-        {
-            uint32_t q = A.qual_dict[v];
-            if (is_mapq_adjust) q = q > SX_MAX_QSCORE ? 255u : mqrow[q];
-            if (v < 8) qlut_lo |= static_cast<unsigned long long>(q & 0xffu) << (8u * v);
-            else qlut_hi |= static_cast<unsigned long long>(q & 0xffu) << (8u * (v - 8u));
-        }
-    }
-    k4_wstream qq;
-    sq.init(gs);
-    qq.init(A.qual + rd.qual_off);
-    sc.init(path, as);
-    const int max_pass = static_cast<int>(A.opt.mismatchDensityFilterMaxMismatchCount), max_pass2 = A.opt.tier2MismatchDensityFilterMaxMismatchCount;
-    const int min_q = A.opt.minBasecallErrorPhredProb;
-    const bool use_t2 = A.opt.useTier2Evidence != 0;
-    unsigned long long* row = reinterpret_cast<unsigned long long*>(bc + static_cast<size_t>(r) * Ls); // Ls % 16 == 0: 8-byte aligned groups of four calls
-    unsigned long long acc = 0;
-    for (uint32_t q = rb; q < re; ++q)
-    {
-        K4_SEG_ADVANCE(sc, q)
-        uint32_t v16 = 0;
-        const int32_t site = site0 + static_cast<int32_t>(q) + sc.rfd; // (meaningful for a MATCH base)
-        if (sc.kind == SX_SEG_MATCH && q < sc.seg_end && site >= 0 && site < static_cast<int32_t>(A.n_sites)) // is_pos_reportable
-        {
-            const uint32_t call_code = sq.nibble_at(q);
-            const uint32_t call_id = id_of_code(call_code);
-            if (call_id > 4u) atomicOr(status, ST_BASE);
-            uint32_t qscore;
-            if (A.qual_bits == 4)
-            {
-                const uint32_t v = qq.nibble_at(q);
-                qscore = static_cast<uint32_t>(((v < 8u ? qlut_lo : qlut_hi) >> (8u * (v & 7u))) & 0xffu);
-                if (is_mapq_adjust && qscore == 255u)
-                {
-                    atomicOr(status, ST_QUAL);
-                    qscore = 0;
-                }
-            }
-            else
-            {
-                qscore = qq.byte_at(q);
-                if (is_mapq_adjust)
-                {
-                    if (qscore > SX_MAX_QSCORE)
-                    {
-                        atomicOr(status, ST_QUAL);
-                        qscore = 0;
-                    }
-                    else qscore = mqrow[qscore];
-                }
-            }
-            bool is_call_filter = (call_code == 15u) || (static_cast<int>(qscore) < min_q);
-            bool is_tier2_call_filter = is_call_filter, is_neighbor_mismatch = false;
-            if (isDensity)
-            {
-                const uint32_t di = min(delta_size - 1u, max(fs, q) - fs); // ddata::get's index
-                int del = static_cast<int>(P[min(di + fs2, read_size - 1u) + 1u]) - static_cast<int>(P[di]);
-                if (n_ev)
-                {
-                    if (n_ev <= K4B_MAX_EV)
-                    {
-                        for (uint32_t e = 0; e < n_ev; ++e)
-                        {
-                            const uint32_t st = ev[e] >> 16, ln = ev[e] & 0xffffu;
-                            del += (max(fs2, st) - fs2 <= di && di < st + ln) ? 1 : 0;
-                        }
-                    }
-                    else
-                    {
-                        uint32_t p2 = 0;
-                        for (uint32_t j = 0; j < as; ++j)
-                        {
-                            const uint32_t k2 = path[j].kind, l2 = path[j].len;
-                            if (!((j < first) || (j > last)) && (k2 == SX_SEG_INSERT || k2 == SX_SEG_DELETE))
-                            {
-                                const uint32_t ln = k2 == SX_SEG_INSERT ? l2 : 0u;
-                                del += (max(fs2, p2) - fs2 <= di && di < p2 + ln) ? 1 : 0;
-                            }
-                            if (kind_read(k2)) p2 += l2;
-                        }
-                    }
-                }
-                if (!is_call_filter)
-                {
-                    is_call_filter = max_pass < del;
-                    is_tier2_call_filter = use_t2 ? (max_pass2 < del) : is_call_filter;
-                }
-                const int mis = static_cast<int>(P[q + 1]) - static_cast<int>(P[q]);
-                is_neighbor_mismatch = (del - mis) > 0;
-            }
-            const bool current_call_filter = tier1 ? is_call_filter : is_tier2_call_filter;
-            const bool is_tier_specific_filter = tier1 && is_call_filter && !is_tier2_call_filter;
-            v16 = min(qscore, 63u) | (min(call_id, 4u) << 6) | fwd_bit | ((is_neighbor_mismatch ? 1u : 0u) << 11) | ((current_call_filter ? 1u : 0u) << 12) |
-                  ((is_tier_specific_filter ? 1u : 0u) << 13);
-        }
-        // four calls per 64-bit store (positions outside the MATCH segments hold 0: nobody reads them)
-        acc |= static_cast<unsigned long long>(v16) << (16u * (q & 3u));
-        if ((q & 3u) == 3u)
-        {
-            row[q >> 2] = acc;
-            acc = 0;
-        }
-    }
-    if (re > rb && (re & 3u) != 0u) row[(re - 1u) >> 2] = acc;
-    rec[r] = out;
-#undef K4_SEG_ADVANCE
-}
-
-constexpr uint32_t K4G_CHUNK = 8; // 32-site blocks per warp: its read range advances with the blocks
-
-__global__ void __launch_bounds__(128) k4_gather_kernel(k4_args A, const k4_rrec* __restrict__ rec, const uint16_t* __restrict__ bc, uint32_t Ls, uint32_t reach_back,
-                                                        uint32_t reach_fwd, const uint32_t* __restrict__ site_off, const uint32_t* __restrict__ t2_off,
-                                                        uint16_t* __restrict__ calls, uint16_t* __restrict__ t2_calls)
-{
-    const uint32_t lane = threadIdx.x & 31u;
-    const uint32_t gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const uint32_t n_blocks = (A.n_sites + 31u) / 32u;
-    const uint32_t b0 = gw * K4G_CHUNK;
-    if (b0 >= n_blocks) return;
-    const uint32_t b1 = min(b0 + K4G_CHUNK, n_blocks);
-    // a read can reach site position P only if its buffer position lies in [P - reach_back, P + reach_fwd]
-    // (reach_back = longest alignment span + largest |best start - buffer position|, reach_fwd = the latter)
-    uint32_t lo = 0, hi = 0;
-    if (lane == 0) lo = lower_bound_pos(A, static_cast<int64_t>(A.report_begin) + static_cast<int64_t>(b0) * 32 - reach_back);
-    lo = __shfl_sync(FULL, lo, 0);
-    hi = lo;
-    for (uint32_t b = b0; b < b1; ++b)
-    {
-        const int64_t P0 = static_cast<int64_t>(A.report_begin) + static_cast<int64_t>(b) * 32;
-        const int64_t want_lo = P0 - reach_back, want_hi = P0 + 31 + reach_fwd; // buffer positions in [want_lo, want_hi]
-        while (lo < A.n_reads && bpos_of(A, lo) < want_lo) ++lo; // warp-uniform
-        if (hi < lo) hi = lo;
-        while (hi < A.n_reads && bpos_of(A, hi) <= want_hi) ++hi;
-        const uint32_t s = b * 32u + lane;
-        const bool live = s < A.n_sites;
-        uint32_t c1 = live ? site_off[s] : 0u, c2 = live ? t2_off[s] : 0u;
-        const int32_t si = live ? static_cast<int32_t>(s) : -0x40000000;
-        for (uint32_t r = lo; r < hi; ++r)
-        {
-            const uint4* q4 = reinterpret_cast<const uint4*>(rec + r); // warp-uniform loads
-            const uint4 hdr = q4[1];                                   // len[2] | p_lo[0] << 16, p_lo[1] | p_lo[2] << 16, n_iv, padding
-            const uint32_t n_iv = hdr.z & 0xffu;
-            if (n_iv == 0u) continue;
-            const uint4 lo4 = q4[0]; // site_lo[0..2], len[0] | len[1] << 16
-            uint32_t hit = 0xffffffffu;
-            if (n_iv <= K4_REC_IV)
-            {
-                const uint32_t d0 = static_cast<uint32_t>(si - static_cast<int32_t>(lo4.x));
-                if (d0 < (lo4.w & 0xffffu)) hit = (hdr.x >> 16) + d0;
-                if (n_iv > 1u)
-                {
-                    const uint32_t d1 = static_cast<uint32_t>(si - static_cast<int32_t>(lo4.y));
-                    if (d1 < (lo4.w >> 16)) hit = (hdr.y & 0xffffu) + d1;
-                    if (n_iv > 2u)
-                    {
-                        const uint32_t d2 = static_cast<uint32_t>(si - static_cast<int32_t>(lo4.z));
-                        if (d2 < (hdr.x & 0xffffu)) hit = (hdr.y >> 16) + d2;
-                    }
-                }
-            }
-            else
-            {
-                // more MATCH intervals than a record holds: the path itself
-                const uint32_t rw = lo4.y, rbb = rw & 0xffffu, ree = rw >> 16, ns = (hdr.z >> 8) & 0x7fffffu;
-                const sx_aln_seg* path = A.segs + lo4.z;
-                int32_t ref_head = static_cast<int32_t>(lo4.x);
-                uint32_t read_head = 0;
-                for (uint32_t i = 0; i < ns; ++i)
-                {
-                    const uint32_t k = path[i].kind, len = path[i].len;
-                    if (k == SX_SEG_MATCH)
-                    {
-                        const uint32_t a = max(read_head, rbb), e = min(read_head + len, ree);
-                        if (a < e)
-                        {
-                            const uint32_t d = static_cast<uint32_t>(si - (ref_head + static_cast<int32_t>(a - read_head)));
-                            if (d < e - a) hit = a + d;
-                        }
-                    }
-                    if (kind_read(k)) read_head += len;
-                    if (kind_ref(k)) ref_head += static_cast<int32_t>(len);
-                }
-            }
-            if (hit != 0xffffffffu)
-            {
-                const uint16_t v = bc[static_cast<size_t>(r) * Ls + hit];
-                if (hdr.z & 0x80000000u) calls[c1++] = v;
-                else t2_calls[c2++] = v;
-            }
-        }
-    }
-}
-
 int upload(sx_ctx* ctx, int slot, const void* src, size_t bytes, const void** dst, cudaStream_t st)
 {
     void* p = nullptr;
@@ -1095,9 +647,9 @@ int sx_k4_run(sx_ctx* ctx, const sx_pileup_reads_batch* d, const sx_pileup_colum
     A.origin = d->report_begin - static_cast<int32_t>(W);
     A.W = W;
     A.Lcap = Lcap;
-    A.span_max = d->max_ref_span;
-    A.shift_max = shift;
-    A.n_windows = static_cast<uint32_t>((static_cast<int64_t>(d->report_end) - A.origin + W - 1) / W);
+    // the windows cover every buffer position a read reaching the report range can have: its best alignment starts before report_end,
+    // its buffer position is at most `shift` later
+    A.n_windows = static_cast<uint32_t>((static_cast<int64_t>(d->report_end) + shift - A.origin + W - 1) / W);
     A.n_sites = n_sites;
     A.opt = d->opts;
 
@@ -1161,25 +713,8 @@ int sx_k4_run(sx_ctx* ctx, const sx_pileup_reads_batch* d, const sx_pileup_colum
     if (totals[0] > out->calls_capacity || totals[1] > out->t2_capacity)
         return sx_fail(ctx, SX_ERR_NOMEM, "sx_pileup_reads: the columns hold %u + %u calls, capacities are %llu + %llu", totals[0], totals[1],
                        (unsigned long long)out->calls_capacity, (unsigned long long)out->t2_capacity);
-    // pass 3: thread per read + warp per 32 sites (default), or SX_K4_PLAN=1: one warp per window, reads in turn
-    const size_t bc_bytes = (size_t)d->n_reads * Lcap * 2;
-    const bool gather_plan = (getenv("SX_K4_PLAN") && atoi(getenv("SX_K4_PLAN")) == 2) && bc_bytes <= ((size_t)12 << 30); // (opt-in: the windowed fill is the default)
-    if (d->n_reads && gather_plan)
-    {
-        k4_rrec* rec = nullptr;
-        uint16_t* bc = nullptr;
-        if ((rc = sx_ensure(ctx, 30, (size_t)(d->n_reads + 1) * sizeof(k4_rrec) + 64, reinterpret_cast<void**>(&rec)))) return rc;
-        if ((rc = sx_ensure(ctx, 31, bc_bytes + 64, reinterpret_cast<void**>(&bc)))) return rc;
-        const size_t smem = (size_t)K4B_THREADS * (Lcap + 2u) * 2u;
-        if (smem > 48 * 1024) SX_CUDA(ctx, cudaFuncSetAttribute(k4_bases_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(ctx->smem_optin)));
-        k4_bases_kernel<<<(d->n_reads + K4B_THREADS - 1) / K4B_THREADS, K4B_THREADS, smem, st>>>(A, rec, bc, Lcap, ctx->d_tables, ctx->d_status);
-        SX_CUDA(ctx, cudaGetLastError());
-        const uint32_t n_warps = ((n_sites + 31u) / 32u + K4G_CHUNK - 1u) / K4G_CHUNK;
-        k4_gather_kernel<<<(n_warps + 3u) / 4u, 128, 0, st>>>(A, rec, bc, Lcap, d->max_ref_span + shift, shift, out->site_off, out->t2_off, out->calls, out->t2_calls);
-        SX_CUDA(ctx, cudaGetLastError());
-        launches += 2;
-    }
-    else if (d->n_reads)
+    // pass 3: one warp per window walks the window's reads in read-buffer order
+    if (d->n_reads)
     {
         const size_t smem = (size_t)k4_warp_smem(W, Lcap) * K4_WARPS;
         if (smem > 48 * 1024) SX_CUDA(ctx, cudaFuncSetAttribute(k4_fill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(ctx->smem_optin)));

@@ -603,22 +603,10 @@ template <class SC> K6_HD uint32_t k6_score_read(const k6_view& v, const uint32_
     return 0;
 }
 
-
-// ---------------------------------------------------------------------------------------------------------------------------
-// Block staging.  The reads [r0, r1) of one thread block own CONTIGUOUS slices of every CSR array (alignments, segments, alignment
-// keys, scores) and of the window table of the regions they touch.  The block copies those slices into shared memory with
-// coalesced loads and the per-read body then runs on a view whose pointers are rebased into that copy (absolute indices keep
-// working), so its many small dependent loads cost a shared-memory access instead of an L2 / HBM round trip.
-// ---------------------------------------------------------------------------------------------------------------------------
-struct k6_block_plan
-{
-    uint32_t r0, r1, a0, a1, s0, s1, k0, k1, g0, g1, w0, w1;
-    uint32_t o_lnp, o_keys, o_pos, o_segoff, o_keyoff, o_rro, o_rko, o_segs, o_akeys, bytes;
-};
-
+/// the region of read r: the last region whose first read is <= r (the reads of a region are consecutive)
 K6_HD uint32_t k6_region_of(const uint32_t* region_read_off, const uint32_t n_regions, const uint32_t r)
 {
-    uint32_t lo(0), hi(n_regions); // the last region whose first read is <= r
+    uint32_t lo(0), hi(n_regions);
     while (hi - lo > 1)
     {
         const uint32_t mid((lo + hi) >> 1);
@@ -628,103 +616,32 @@ K6_HD uint32_t k6_region_of(const uint32_t* region_read_off, const uint32_t n_re
     return lo;
 }
 
-K6_HD k6_block_plan k6_plan_block(const sx_score_indels_batch& b, const uint32_t r0, const uint32_t r1)
-{
-    k6_block_plan p;
-    p.r0 = r0;
-    p.r1 = r1;
-    p.a0 = b.aln_off[r0];
-    p.a1 = b.aln_off[r1];
-    p.s0 = b.aln_seg_off[p.a0];
-    p.s1 = b.aln_seg_off[p.a1];
-    p.k0 = b.aln_key_off[p.a0];
-    p.k1 = b.aln_key_off[p.a1];
-    p.g0 = k6_region_of(b.region_read_off, b.n_regions, r0);
-    p.g1 = k6_region_of(b.region_read_off, b.n_regions, r1 - 1);
-    p.w0 = b.region_key_off[p.g0];
-    p.w1 = b.region_key_off[p.g1 + 1];
-    const uint32_t nA(p.a1 - p.a0), nG(p.g1 - p.g0 + 1);
-    uint32_t o(0);
-    p.o_lnp = o;
-    o += 8 * nA;
-    p.o_keys = o;
-    o += (uint32_t)sizeof(sx_indel_key) * (p.w1 - p.w0);
-    p.o_pos = o;
-    o += 4 * nA;
-    p.o_segoff = o;
-    o += 4 * (nA + 1);
-    p.o_keyoff = o;
-    o += 4 * (nA + 1);
-    p.o_rro = o;
-    o += 4 * (nG + 1);
-    p.o_rko = o;
-    o += 4 * (nG + 1);
-    p.o_segs = o;
-    o += 4 * (p.s1 - p.s0);
-    p.o_akeys = o;
-    o += 2 * (p.k1 - p.k0);
-    p.bytes = (o + 15u) & ~15u;
-    return p;
-}
-
-template <class T> K6_HD void k6_copy(T* dst, const T* src, const uint32_t n, const uint32_t t, const uint32_t nt)
-{
-    for (uint32_t i = t; i < n; i += nt) dst[i] = src[i];
-}
-
-/// thread t of nt: its share of the copies
-K6_HD void k6_stage(const k6_view& v, const k6_block_plan& p, unsigned char* sm, const uint32_t t, const uint32_t nt)
-{
-    const sx_score_indels_batch& b(v.b);
-    const uint32_t nA(p.a1 - p.a0), nG(p.g1 - p.g0 + 1);
-    k6_copy(reinterpret_cast<double*>(sm + p.o_lnp), v.lnp + p.a0, nA, t, nt);
-    // window entries as 8-byte words (sx_indel_key is 4 of them)
-    k6_copy(reinterpret_cast<uint64_t*>(sm + p.o_keys), reinterpret_cast<const uint64_t*>(b.keys + p.w0), 4 * (p.w1 - p.w0), t, nt);
-    k6_copy(reinterpret_cast<int32_t*>(sm + p.o_pos), b.aln_pos + p.a0, nA, t, nt);
-    k6_copy(reinterpret_cast<uint32_t*>(sm + p.o_segoff), b.aln_seg_off + p.a0, nA + 1, t, nt);
-    k6_copy(reinterpret_cast<uint32_t*>(sm + p.o_keyoff), b.aln_key_off + p.a0, nA + 1, t, nt);
-    k6_copy(reinterpret_cast<uint32_t*>(sm + p.o_rro), b.region_read_off + p.g0, nG + 1, t, nt);
-    k6_copy(reinterpret_cast<uint32_t*>(sm + p.o_rko), b.region_key_off + p.g0, nG + 1, t, nt);
-    k6_copy(reinterpret_cast<sx_aln_seg*>(sm + p.o_segs), b.segs + p.s0, p.s1 - p.s0, t, nt);
-    k6_copy(reinterpret_cast<uint16_t*>(sm + p.o_akeys), b.aln_keys + p.k0, p.k1 - p.k0, t, nt);
-}
-
-/// the view whose staged arrays point into `sm` (rebased so that absolute indices keep working)
-K6_HD k6_view k6_rebased(const k6_view& v, const k6_block_plan& p, unsigned char* sm)
-{
-    k6_view l(v);
-    l.lnp = reinterpret_cast<const double*>(sm + p.o_lnp) - p.a0;
-    l.b.keys = reinterpret_cast<const sx_indel_key*>(sm + p.o_keys) - p.w0;
-    l.b.aln_pos = reinterpret_cast<const int32_t*>(sm + p.o_pos) - p.a0;
-    l.b.aln_seg_off = reinterpret_cast<const uint32_t*>(sm + p.o_segoff) - p.a0;
-    l.b.aln_key_off = reinterpret_cast<const uint32_t*>(sm + p.o_keyoff) - p.a0;
-    l.b.region_read_off = reinterpret_cast<const uint32_t*>(sm + p.o_rro) - p.g0;
-    l.b.region_key_off = reinterpret_cast<const uint32_t*>(sm + p.o_rko) - p.g0;
-    l.b.segs = reinterpret_cast<const sx_aln_seg*>(sm + p.o_segs) - p.s0;
-    l.b.aln_keys = reinterpret_cast<const uint16_t*>(sm + p.o_akeys) - p.k0;
-    return l;
-}
-
 #define K6_FAST_A 8
 #define K6_FAST_E 4
 #define K6_MID_A 40 /* second local-memory tier: a profile put a large share of the kernel's instructions on the strided-arena accessor once most reads had > 8 alignments */
 
-/// read r of a block whose view is `lv` (staged or not): find its region among the block's and run the body with the cheapest
-/// scratch that fits
-K6_HD uint32_t k6_score_read_in_block(const k6_view& lv, const k6_block_plan& p, const uint32_t r, k6_scratch& S)
+/// which scratch the body of read r runs with: 0 = k6_local_scratch<K6_FAST_A, K6_FAST_E>, 1 = k6_local_scratch<K6_MID_A, K6_FAST_E>, 2 = the arena
+K6_HD unsigned k6_scratch_tier(const sx_score_indels_batch& b, const uint32_t r)
 {
-    uint32_t g(p.g0);
-    while (g < p.g1 && lv.b.region_read_off[g + 1] <= r) ++g;
-    const uint32_t n_cal(lv.b.aln_off[r + 1] - lv.b.aln_off[r]), slots(lv.b.rec_off[r + 1] - lv.b.rec_off[r]);
-    if (n_cal <= K6_FAST_A && slots <= K6_FAST_E)
+    const uint32_t n_cal(b.aln_off[r + 1] - b.aln_off[r]), slots(b.rec_off[r + 1] - b.rec_off[r]);
+    if (n_cal <= K6_FAST_A && slots <= K6_FAST_E) return 0;
+    if (n_cal <= K6_MID_A && slots <= K6_FAST_E) return 1; // (whole-path windows: 12 candidate alignments per realigned read on average, a few dozen at most)
+    return 2;
+}
+
+/// read r of `region` with the cheapest scratch that fits (k6_scratch_tier); S is the arena, for reads too deep for local memory
+K6_HD uint32_t k6_score_read_tiered(const k6_view& v, const uint32_t region, const uint32_t r, k6_scratch& S)
+{
+    const unsigned tier(k6_scratch_tier(v.b, r));
+    if (tier == 0)
     {
         k6_local_scratch<K6_FAST_A, K6_FAST_E> L;
-        return k6_score_read(lv, g, r, L);
+        return k6_score_read(v, region, r, L);
     }
-    if (n_cal <= K6_MID_A && slots <= K6_FAST_E) // (whole-path windows: 12 candidate alignments per realigned read on average, a few dozen at most)
+    if (tier == 1)
     {
         k6_local_scratch<K6_MID_A, K6_FAST_E> L;
-        return k6_score_read(lv, g, r, L);
+        return k6_score_read(v, region, r, L);
     }
-    return k6_score_read(lv, g, r, S);
+    return k6_score_read(v, region, r, S);
 }

@@ -6,12 +6,12 @@
 // and consumes K1's scores where K1 wrote them (device memory).
 //
 // Shape of the work: per read a handful of alignments x a handful of indels of integer bookkeeping and a few fp64 adds and
-// compares -- no reuse between reads and nothing GEMM-like; the algorithmic floor is reading every input once.  A thread block
-// takes 128 consecutive reads per iteration (persistent grid: resident blocks x SM count): the reads own contiguous slices of every
-// CSR array, which the block copies into shared memory with coalesced loads (k6_stage); then one thread runs one read on a view
-// rebased into that copy, so the body's many small dependent loads are shared-memory accesses.  Per-read state (sort order,
-// filter flags, per-indel maxima) is local memory for ordinary reads (<= 8 alignments, <= 4 output slots) and a column of an
-// element-major global arena for deep ones.  Output: one 32-byte record per (read, evaluated indel).  The body is k6_core.cuh.
+// compares -- no reuse between reads and nothing GEMM-like; the algorithmic floor is reading every input once.  About half of a
+// window's reads have no candidate alignment: k6_max_kernel lists the reads that have one, the host memsets the outputs of the
+// others, and k6_score_list_kernel (persistent grid: resident blocks x SM count) runs one listed read per thread on the global
+// arrays, the list regrouped by the read's number of alignments so that a warp's reads do similar work.  Per-read state (sort
+// order, filter flags, per-indel maxima) is local memory for ordinary reads (<= 40 alignments, <= 4 output slots) and a column of
+// an element-major global arena for deep ones.  Output: one 32-byte record per (read, evaluated indel).  The body is k6_core.cuh.
 
 #include "k6_core.cuh"
 #include "sx_regroup.cuh"
@@ -25,12 +25,11 @@ namespace
 constexpr int K6_THREADS = 128;
 constexpr int K6_ST_SHIFT = 9; // K6_ST_* bits are reported as ctx status bits 512, 1024, ...
 
-// sizes the launch needs: out[0] = max alignments of a read, out[1] = max output slots of a read, out[2] / out[3] = largest staging
-// footprint (k6_plan_block().bytes) of a 128-read / 32-read block
-// (+ with `list`: the dense list of the reads that HAVE candidate alignments -- out[4] = their count --, in read order within a warp's 32)
+// sizes the launch needs: out[0] = max alignments of a read, out[1] = max output slots of a read; and the dense list of the reads that
+// HAVE candidate alignments -- out[2] = their count --, in read order within a warp's 32
 __global__ void k6_max_kernel(const sx_score_indels_batch b, uint32_t* __restrict__ out, uint32_t* __restrict__ list)
 {
-    uint32_t mA(0), mS(0), m128(0), m32(0);
+    uint32_t mA(0), mS(0);
     const uint32_t tid(blockIdx.x * blockDim.x + threadIdx.x), nthr(gridDim.x * blockDim.x), lane(threadIdx.x & 31u);
     for (uint32_t b0 = tid - lane; b0 < b.n_reads; b0 += nthr)
     {
@@ -41,77 +40,23 @@ __global__ void k6_max_kernel(const sx_score_indels_batch b, uint32_t* __restric
             mA = max(mA, nc);
             mS = max(mS, b.rec_off[r + 1] - b.rec_off[r]);
         }
-        if (list)
-        {
-            const unsigned m(__ballot_sync(0xffffffffu, nc > 0));
-            uint32_t at(0);
-            if (lane == 0 && m) at = atomicAdd(out + 4, (uint32_t)__popc(m));
-            at = __shfl_sync(0xffffffffu, at, 0);
-            if (nc > 0) list[at + __popc(m & ((1u << lane) - 1u))] = r;
-        }
-    }
-    for (uint32_t c = tid; c < (b.n_reads + 31) / 32; c += nthr) // one thread per 32-read block (and per 128-read block)
-    {
-        const uint32_t r(c * 32);
-        m32 = max(m32, k6_plan_block(b, r, min(b.n_reads, r + 32)).bytes);
-        if ((c & 3) == 0) m128 = max(m128, k6_plan_block(b, r, min(b.n_reads, r + 128)).bytes);
+        const unsigned m(__ballot_sync(0xffffffffu, nc > 0));
+        uint32_t at(0);
+        if (lane == 0 && m) at = atomicAdd(out + 2, (uint32_t)__popc(m));
+        at = __shfl_sync(0xffffffffu, at, 0);
+        if (nc > 0) list[at + __popc(m & ((1u << lane) - 1u))] = r;
     }
     mA = __reduce_max_sync(0xffffffffu, mA);
     mS = __reduce_max_sync(0xffffffffu, mS);
-    m128 = __reduce_max_sync(0xffffffffu, m128);
-    m32 = __reduce_max_sync(0xffffffffu, m32);
     if ((threadIdx.x & 31) == 0)
     {
         atomicMax(out, mA);
         atomicMax(out + 1, mS);
-        atomicMax(out + 2, m128);
-        atomicMax(out + 3, m32);
     }
 }
 
-extern __shared__ __align__(16) unsigned char k6_smem[];
-
-// one block = blockDim.x consecutive reads per iteration: stage their slices, one read per thread
-__global__ void __launch_bounds__(K6_THREADS) k6_score_kernel(const k6_view v, const k6_scratch S0, const uint32_t smem_cap, int* __restrict__ status)
-{
-    __shared__ k6_block_plan plan;
-    const uint32_t t(blockIdx.x * blockDim.x + threadIdx.x);
-    k6_scratch S(S0); // this thread's columns of the element-major arena (reads too deep for the local-memory scratch)
-    S.ord.p += t;
-    S.smooth.p += t;
-    S.filt.p += t;
-    S.ev.p += t;
-    S.slot.p += t;
-    S.present.p += t;
-    S.absent.p += t;
-    S.has.p += t;
-    S.alt.p += t;
-    S.pair.p += t;
-    uint32_t st(0);
-    const uint32_t n_chunks((v.b.n_reads + blockDim.x - 1) / blockDim.x);
-    for (uint32_t chunk = blockIdx.x; chunk < n_chunks; chunk += gridDim.x)
-    {
-        const uint32_t r0(chunk * blockDim.x), r1(min(v.b.n_reads, r0 + blockDim.x));
-        if (threadIdx.x == 0) plan = k6_plan_block(v.b, r0, r1);
-        __syncthreads();
-        const k6_block_plan p(plan);
-        k6_view lv(v);
-        if (p.bytes <= smem_cap)
-        {
-            k6_stage(v, p, k6_smem, threadIdx.x, blockDim.x);
-            __syncthreads();
-            lv = k6_rebased(v, p, k6_smem);
-        }
-        const uint32_t r(r0 + threadIdx.x);
-        if (r < r1) st |= k6_score_read_in_block(lv, p, r, S);
-        __syncthreads(); // the next iteration overwrites plan and the staged slices
-    }
-    if (st) atomicOr(status, (int)(st << K6_ST_SHIFT));
-}
-
-// the same per-read body over the dense list of reads that have alignments, on the global arrays (no staging): about half of a 30x window's
-// reads never reach the search, and in the block-staged kernel their threads idle (about a third of the lanes busy) while the staged slices hold the
-// occupancy at 9 warps per SM
+// the per-read body over the dense list of reads that have alignments: about half of a 30x window's reads never reach the search, and a kernel
+// over all reads would idle their lanes
 __global__ void __launch_bounds__(K6_THREADS) k6_score_list_kernel(const k6_view v, const k6_scratch S0, const uint32_t* __restrict__ list, const uint32_t* __restrict__ n_list,
                                                                   int* __restrict__ status)
 {
@@ -129,21 +74,10 @@ __global__ void __launch_bounds__(K6_THREADS) k6_score_list_kernel(const k6_view
     S.pair.p += t;
     uint32_t st(0);
     const uint32_t n(*n_list);
-    k6_block_plan whole;
-    whole.g0 = 0;
-    whole.g1 = v.b.n_regions;
     for (uint32_t i = t; i < n; i += nthr)
     {
         const uint32_t r(list[i]);
-        uint32_t lo(0), hi(v.b.n_regions); // the read's region: reads of a region are consecutive
-        while (lo + 1 < hi)
-        {
-            const uint32_t mid((lo + hi) / 2);
-            if (v.b.region_read_off[mid] <= r) lo = mid;
-            else hi = mid;
-        }
-        whole.g0 = lo;
-        st |= k6_score_read_in_block(v, whole, r, S);
+        st |= k6_score_read_tiered(v, k6_region_of(v.b.region_read_off, v.b.n_regions, r), r, S);
     }
     if (st) atomicOr(status, (int)(st << K6_ST_SHIFT));
 }
@@ -174,29 +108,23 @@ k6_layout k6_plan(const uint32_t maxA, const uint32_t maxE, const size_t T)
 int k6_run(sx_ctx* ctx, const sx_score_indels_batch* d, const double* lnp_dev, const sx_score_indels_out* out_dev, unsigned* launches)
 {
     cudaStream_t st(ctx->s_compute);
-    // sizes of the launch: the deepest read of the batch decides the scratch, the largest block footprint the shared memory
+    // sizes of the launch: the deepest read of the batch decides the scratch
     uint32_t* d_max(nullptr);
     int rc;
     if ((rc = sx_ensure(ctx, 29, 32, reinterpret_cast<void**>(&d_max)))) return rc;
-    SX_CUDA(ctx, cudaMemsetAsync(d_max, 0, 32, st));
-    static const bool use_list(getenv("SX_K6_STAGED") == nullptr); // (SX_K6_STAGED=1: the block-staged kernel, for A/B timing)
+    SX_CUDA(ctx, cudaMemsetAsync(d_max, 0, 12, st));
     uint32_t* list(nullptr);
-    if (use_list && (rc = sx_ensure(ctx, 69, (size_t)d->n_reads * 4 + 16, reinterpret_cast<void**>(&list)))) return rc;
+    if ((rc = sx_ensure(ctx, 69, (size_t)d->n_reads * 4 + 16, reinterpret_cast<void**>(&list)))) return rc;
     const int grid0(std::max(1, std::min<int>((int)((d->n_reads + 255) / 256), ctx->sm_count * 8)));
     k6_max_kernel<<<grid0, 256, 0, st>>>(*d, d_max, list);
     SX_CUDA(ctx, cudaGetLastError());
-    uint32_t h_max[4] = {0, 0, 0, 0};
-    SX_CUDA(ctx, cudaMemcpyAsync(h_max, d_max, 16, cudaMemcpyDeviceToHost, st));
+    uint32_t h_max[2] = {0, 0};
+    SX_CUDA(ctx, cudaMemcpyAsync(h_max, d_max, 8, cudaMemcpyDeviceToHost, st));
     SX_CUDA(ctx, cudaStreamSynchronize(st));
     const uint32_t maxA(std::max(1u, h_max[0])), maxE(std::max(1u, std::min(K6_MAX_EVAL, h_max[1])));
-    // 128 reads per block when their slices fit a modest tile (several blocks per SM), else 32 reads per block; a block whose
-    // slices still do not fit runs on the global arrays
-    const uint32_t smem_limit(48u * 1024u - 512u); // (the kernel also has ~100 bytes of static shared memory: the two together must stay under the 48 KB no-opt-in limit)
-    const int threads(use_list || h_max[2] <= smem_limit ? K6_THREADS : 32);
-    const uint32_t smem_bytes(use_list ? 0u : std::min(smem_limit, threads == K6_THREADS ? h_max[2] : h_max[3]));
+    const int threads(K6_THREADS);
     int per_sm(1);
-    if (use_list) SX_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k6_score_list_kernel, threads, 0));
-    else SX_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k6_score_kernel, threads, smem_bytes));
+    SX_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k6_score_list_kernel, threads, 0));
     per_sm = std::max(1, per_sm);
 
     // threads: one per read, up to the resident blocks of every SM; fewer when a deep batch would make the arena too large
@@ -227,40 +155,32 @@ int k6_run(sx_ctx* ctx, const sx_score_indels_batch* d, const double* lnp_dev, c
     v.n_rec = out_dev->n_rec;
     v.max_aln = out_dev->max_aln;
     v.eval_aln = out_dev->eval_aln;
-    if (use_list)
+    // the reads without alignments answer "no records, no maximum alignment" (what the body writes for them)
+    SX_CUDA(ctx, cudaMemsetAsync(out_dev->n_rec, 0, (size_t)d->n_reads * 4, st));
+    SX_CUDA(ctx, cudaMemsetAsync(out_dev->max_aln, 0xFF, (size_t)d->n_reads * 4, st));
+    SX_CUDA(ctx, cudaMemsetAsync(out_dev->eval_aln, 0xFF, (size_t)d->n_reads * 4, st));
+    unsigned extra(0);
+    if (!getenv("SX_K6_NO_CLASS_SORT"))
     {
-        // the reads without alignments answer "no records, no maximum alignment" (what the body writes for them)
-        SX_CUDA(ctx, cudaMemsetAsync(out_dev->n_rec, 0, (size_t)d->n_reads * 4, st));
-        SX_CUDA(ctx, cudaMemsetAsync(out_dev->max_aln, 0xFF, (size_t)d->n_reads * 4, st));
-        SX_CUDA(ctx, cudaMemsetAsync(out_dev->eval_aln, 0xFF, (size_t)d->n_reads * 4, st));
-        unsigned extra(0);
-        if (!getenv("SX_K6_NO_CLASS_SORT"))
-        {
-            // the list regrouped by class (sx_regroup.cuh) = the read's number of candidate alignments: score_indels loops over the alignments and the
-            // window entries they carry, so warps of reads with equally many alignments stay together
-            uint8_t* cls(nullptr);
-            uint32_t *hist(nullptr), *list2(nullptr);
-            if ((rc = sx_ensure(ctx, 35, (size_t)d->n_reads + 16, reinterpret_cast<void**>(&cls)))) return rc;
-            if ((rc = sx_ensure(ctx, 36, (size_t)SX_RG_CLASSES * 4 + 16, reinterpret_cast<void**>(&hist)))) return rc;
-            if ((rc = sx_ensure(ctx, 37, (size_t)d->n_reads * 4 + 16, reinterpret_cast<void**>(&list2)))) return rc;
-            SX_CUDA(ctx, cudaMemsetAsync(hist, 0, (size_t)SX_RG_CLASSES * 4, st));
-            const int gc(std::max(1, std::min<int>((int)((d->n_reads + SX_RG_THREADS * SX_RG_ITEMS - 1) / (SX_RG_THREADS * SX_RG_ITEMS)), ctx->sm_count * 8)));
-            sx_regroup_class_by_count_kernel<<<gc, SX_RG_THREADS, 0, st>>>(d->aln_off, list, d_max + 4, cls, hist);
-            sx_regroup_scan_kernel<<<1, SX_RG_CLASSES, 0, st>>>(hist);
-            sx_regroup_scatter_kernel<<<gc, SX_RG_THREADS, 0, st>>>(list, d_max + 4, cls, hist, list2);
-            SX_CUDA(ctx, cudaGetLastError());
-            list = list2;
-            extra = 3;
-        }
-        k6_score_list_kernel<<<(unsigned)(T / threads), threads, 0, st>>>(v, S, list, d_max + 4, ctx->d_status);
+        // the list regrouped by class (sx_regroup.cuh) = the read's number of candidate alignments: score_indels loops over the alignments and the
+        // window entries they carry, so warps of reads with equally many alignments stay together
+        uint8_t* cls(nullptr);
+        uint32_t *hist(nullptr), *list2(nullptr);
+        if ((rc = sx_ensure(ctx, 35, (size_t)d->n_reads + 16, reinterpret_cast<void**>(&cls)))) return rc;
+        if ((rc = sx_ensure(ctx, 36, (size_t)SX_RG_CLASSES * 4 + 16, reinterpret_cast<void**>(&hist)))) return rc;
+        if ((rc = sx_ensure(ctx, 37, (size_t)d->n_reads * 4 + 16, reinterpret_cast<void**>(&list2)))) return rc;
+        SX_CUDA(ctx, cudaMemsetAsync(hist, 0, (size_t)SX_RG_CLASSES * 4, st));
+        const int gc(std::max(1, std::min<int>((int)((d->n_reads + SX_RG_THREADS * SX_RG_ITEMS - 1) / (SX_RG_THREADS * SX_RG_ITEMS)), ctx->sm_count * 8)));
+        sx_regroup_class_by_count_kernel<<<gc, SX_RG_THREADS, 0, st>>>(d->aln_off, list, d_max + 2, cls, hist);
+        sx_regroup_scan_kernel<<<1, SX_RG_CLASSES, 0, st>>>(hist);
+        sx_regroup_scatter_kernel<<<gc, SX_RG_THREADS, 0, st>>>(list, d_max + 2, cls, hist, list2);
         SX_CUDA(ctx, cudaGetLastError());
-        *launches = 2 + extra;
-        return SX_OK;
+        list = list2;
+        extra = 3;
     }
-    else
-        k6_score_kernel<<<(unsigned)(T / threads), threads, smem_bytes, st>>>(v, S, smem_bytes, ctx->d_status);
+    k6_score_list_kernel<<<(unsigned)(T / threads), threads, 0, st>>>(v, S, list, d_max + 2, ctx->d_status);
     SX_CUDA(ctx, cudaGetLastError());
-    *launches = 2;
+    *launches = 2 + extra;
     return SX_OK;
 }
 
@@ -374,7 +294,7 @@ extern "C" int sx_score_indels(sx_ctx* ctx, const sx_score_indels_batch* b, cons
     return sx_check_status(ctx, "sx_score_indels");
 }
 
-// launcher for the device-resident pipeline (sx_pipeline.cu): one 16-byte round trip sizes the scratch, the kernel itself is only enqueued
+// launcher for the device-resident pipeline (sx_pipeline.cu): one 8-byte round trip sizes the scratch, the kernel itself is only enqueued
 int sx_k6_run(sx_ctx* ctx, const sx_score_indels_batch* d, const double* lnp_dev, const sx_score_indels_out* out_dev, unsigned* launches)
 {
     if (d->n_reads == 0) return SX_OK;

@@ -89,7 +89,7 @@ struct k7_scratch // one thread's working memory (contiguous per thread)
     uint32_t n;       // alignments in the set
 };
 
-K7_HD size_t k7_scratch_bytes(const uint32_t maxA, const uint32_t maxF = K7_MAX_INDELS + 1)
+K7_HD constexpr size_t k7_scratch_bytes(const uint32_t maxA, const uint32_t maxF = K7_MAX_INDELS + 1)
 {
     size_t b(0);
     b += ((size_t)K7_MAX_INDELS * 2 + 15) & ~(size_t)15;

@@ -139,15 +139,17 @@ __global__ void __launch_bounds__(K7_THREADS) k7_write_kernel(const k7_view v, u
 // records where; after the scan k7_gather_kernel copies every blob to its place in read order -- the output is independent of
 // which thread got which piece of the log.
 // ---------------------------------------------------------------------------------------------------------------------------
-// The local tier comes in two sizes (SX_K7_LOCAL_ALNS=16|40, default 40): local memory a thread never touches costs nothing but address
-// space, while every read the tier passes on is searched a second time from the start in the slower arena.
+// The local tier holds 40 alignments: local memory a thread never touches costs nothing but address space, while every read the tier
+// passes on is searched a second time from the start in the slower arena (DESIGN.md section 6 has the sweep over 16 / 40 alignments
+// and 16 / 24 / 32 resident blocks per SM behind these constants).
+constexpr uint32_t K7_LOCAL_ALNS = 40;
 constexpr uint32_t K7_LOCAL_FRAMES = 12;
+static_assert(K7_LOCAL_FRAMES <= K7_MAX_INDELS + 1, "local tier sizes");
+constexpr uint32_t K7_LOCAL_BYTES = (uint32_t)((k7_scratch_bytes(K7_LOCAL_ALNS, K7_LOCAL_FRAMES) + 255) & ~(size_t)255); // one thread's local scratch
+// 16 resident blocks per SM (64 registers; its state lives in local memory): on an H100, K7 103 vs 119 ms per step at 16 vs 24 (bench.py,
+// 300k cfg2 loci, two runs each; H100 80GB HBM3, 400 W power limit) -- fewer resident threads keep the local scratch closer to the L2's size
+constexpr int K7_LOCAL_MIN_BLOCKS = 16;
 constexpr uint32_t K7_MID_ALNS = 96; // per-read capacity of the first arena tier
-__host__ __device__ constexpr uint32_t k7_local_bytes(const uint32_t alns) // k7_scratch_bytes(alns, K7_LOCAL_FRAMES), as a constant expression (checked in k7_run_fast)
-{
-    return (uint32_t)(((((size_t)K7_MAX_INDELS * 2 + 15) & ~(size_t)15) + ((sizeof(k7_frame) * K7_LOCAL_FRAMES + 15) & ~(size_t)15) +
-                       ((sizeof(k7_cal) * ((size_t)alns + 1) + 15) & ~(size_t)15) + (((size_t)alns * 2 + 15) & ~(size_t)15) + 255) & ~(size_t)255);
-}
 
 struct k7_log
 {
@@ -258,11 +260,10 @@ __global__ void __launch_bounds__(K7_CLS_THREADS) k7_class_count_kernel(const k7
     if (s_cnt[threadIdx.x]) atomicAdd(&hist[threadIdx.x], s_cnt[threadIdx.x]);
 }
 
-template <uint32_t K7_LOCAL_ALNS, int K7_MIN_BLOCKS>
-__global__ void __launch_bounds__(K7_THREADS, K7_MIN_BLOCKS) k7_search_local_kernel(const k7_view v, const uint32_t* __restrict__ read_region, uint8_t* __restrict__ status,
-                                                                     const k7_retry R, const k7_counts c, const k7_log L)
+__global__ void __launch_bounds__(K7_THREADS, K7_LOCAL_MIN_BLOCKS) k7_search_local_kernel(const k7_view v, const uint32_t* __restrict__ read_region, uint8_t* __restrict__ status,
+                                                                           const k7_retry R, const k7_counts c, const k7_log L)
 {
-    __align__(16) unsigned char local[k7_local_bytes(K7_LOCAL_ALNS)];
+    __align__(16) unsigned char local[K7_LOCAL_BYTES];
     k7_scratch S(k7_scratch_at(local, K7_LOCAL_ALNS, K7_LOCAL_FRAMES, K7_ST_RETRY));
     const uint32_t t(blockIdx.x * blockDim.x + threadIdx.x), nthr(gridDim.x * blockDim.x);
     const uint32_t n_work(R.list0 ? R.n[2] : v.b.n_reads); // (with a list: the counts / status of the other reads were zeroed by the host side)
@@ -392,18 +393,6 @@ int k7_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsigned* 
 
 int k7_run_fast(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsigned* launches)
 {
-    static_assert(K7_LOCAL_FRAMES <= K7_MAX_INDELS + 1, "local tier sizes");
-    bool small_local(false);
-    if (const char* e = getenv("SX_K7_LOCAL_ALNS")) small_local = atoi(e) <= 16;
-    // the same kernel compiled for 16 / 24 / 32 resident blocks per SM (64 / 40 / 32 registers; its state lives in local memory, so the smaller
-    // register budgets spill next to nothing): more warps to hide its latency
-    // 16 on an H100: K7 103 vs 119 ms per step at 16 vs 24 (bench.py, 300k cfg2 loci, two runs each; H100 80GB HBM3, 400 W power limit)
-    const int min_blocks(getenv("SX_K7_MIN_BLOCKS") ? atoi(getenv("SX_K7_MIN_BLOCKS")) : 16);
-    const auto local_kernel(small_local ? k7_search_local_kernel<16, 16>
-                            : min_blocks >= 32 ? k7_search_local_kernel<40, 32>
-                            : min_blocks >= 24 ? k7_search_local_kernel<40, 24>
-                                               : k7_search_local_kernel<40, 16>);
-    if (k7_scratch_bytes(small_local ? 16 : 40, K7_LOCAL_FRAMES) > k7_local_bytes(small_local ? 16 : 40)) return sx_fail(ctx, SX_ERR_ARG, "k7: local scratch smaller than its contents");
     cudaStream_t st(ctx->s_compute);
     const uint32_t n(d->n_reads);
     const uint32_t maxA(d->opts.max_alns_per_read ? std::min<uint32_t>(d->opts.max_alns_per_read, 65535u) : 64u);
@@ -415,12 +404,10 @@ int k7_run_fast(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsig
     const size_t per_thread((k7_scratch_bytes(maxA, maxF) + 255) & ~(size_t)255);
     int per_sm(1), per_sm_local(1);
     SX_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k7_search_arena_kernel, K7_THREADS, 0));
-    SX_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_local, local_kernel, K7_THREADS, 0));
+    SX_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_local, k7_search_local_kernel, K7_THREADS, 0));
     per_sm = std::max(1, per_sm);
     per_sm_local = std::max(1, per_sm_local);
     const size_t n_blocks(((size_t)n + K7_THREADS - 1) / K7_THREADS);
-    // (SX_K7_LOCAL_BLOCKS_PER_SM: tuning knob -- fewer resident threads keep the tier's local-memory scratch closer to the L2's size)
-    if (const char* e = getenv("SX_K7_LOCAL_BLOCKS_PER_SM")) per_sm_local = std::max(1, std::min(per_sm_local, atoi(e)));
     const size_t blocks_local(std::min<size_t>(n_blocks, (size_t)ctx->sm_count * per_sm_local));
     // two arena tiers: a modest one (K7_MID_ALNS alignments per read, the whole device) for the reads the local tier passes on, and -- only when the
     // caller allows more per read -- one with the caller's capacity for the few that still do not fit (few threads: its per-thread scratch is large)
@@ -491,7 +478,7 @@ int k7_run_fast(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsig
         R.list0 = list0b;
         extra += 3;
     }
-    local_kernel<<<(unsigned)blocks_local, K7_THREADS, 0, st>>>(v, read_region, o->status, R, c, L);
+    k7_search_local_kernel<<<(unsigned)blocks_local, K7_THREADS, 0, st>>>(v, read_region, o->status, R, c, L);
     SX_CUDA(ctx, cudaGetLastError());
     k7_search_arena_kernel<<<(unsigned)blocks1, K7_THREADS, 0, st>>>(v, arena1, per_thread1, maxA1, maxF, read_region, o->status, R, 1, two_levels ? 1 : 0, c, L);
     SX_CUDA(ctx, cudaGetLastError());

@@ -6,10 +6,15 @@
 #include <algorithm>
 #include <vector>
 
+// list_walk == 0: the plain body, region by region, read by read.
+// list_walk != 0: what k6_run and k6_score_list_kernel do -- the host memsets of n_rec / max_aln / eval_aln for every read, then
+// the body on the dense list of reads that have alignments, walked backwards (the kernel's regrouping makes the order arbitrary), each
+// read with its region from k6_region_of and the scratch k6_score_read_tiered picks.  counts[0] = reads skipped (no alignment),
+// counts[1 + tier] = listed reads per k6_scratch_tier.
 extern "C" int k6core_run(const sx_score_indels_batch* b, const double* lnp, sx_read_indel_score* recs, uint32_t* n_rec, uint32_t* max_aln, uint32_t* eval_aln,
-                          uint32_t* status_out, uint32_t block_reads, uint32_t smem_cap, uint32_t* staged_blocks)
+                          uint32_t* status_out, uint32_t list_walk, uint32_t* counts)
 {
-    *staged_blocks = 0;
+    std::fill(counts, counts + 4, 0u);
     uint32_t maxA(1), maxE(1);
     for (uint32_t r = 0; r < b->n_reads; ++r)
     {
@@ -43,29 +48,27 @@ extern "C" int k6core_run(const sx_score_indels_batch* b, const double* lnp, sx_
     v.max_aln = max_aln;
     v.eval_aln = eval_aln;
     uint32_t status(0);
-    if (block_reads == 0) // the plain body, read by read
+    if (list_walk == 0)
     {
         for (uint32_t region = 0; region < b->n_regions; ++region)
             for (uint32_t r = b->region_read_off[region]; r < b->region_read_off[region + 1]; ++r) status |= k6_score_read(v, region, r, S);
     }
-    else // what a thread block does: plan, stage the block's slices ("threads" t = 0..nt-1 in turn), run the body on the rebased view
+    else
     {
-        std::vector<uint64_t> smem;
-        for (uint32_t r0 = 0; r0 < b->n_reads; r0 += block_reads)
+        std::fill(n_rec, n_rec + b->n_reads, 0u); // k6_run's memsets
+        std::fill(max_aln, max_aln + b->n_reads, 0xFFFFFFFFu);
+        std::fill(eval_aln, eval_aln + b->n_reads, 0xFFFFFFFFu);
+        std::vector<uint32_t> list; // k6_max_kernel's list
+        for (uint32_t r = 0; r < b->n_reads; ++r)
         {
-            const uint32_t r1(std::min(b->n_reads, r0 + block_reads));
-            const k6_block_plan p(k6_plan_block(v.b, r0, r1));
-            const bool staged(p.bytes <= smem_cap);
-            k6_view lv(v);
-            if (staged)
-            {
-                smem.assign(p.bytes / 8 + 2, 0xdeadbeefdeadbeefull);
-                unsigned char* sm(reinterpret_cast<unsigned char*>(smem.data()));
-                for (uint32_t t = 0; t < block_reads; ++t) k6_stage(v, p, sm, t, block_reads);
-                lv = k6_rebased(v, p, sm);
-                ++*staged_blocks;
-            }
-            for (uint32_t r = r0; r < r1; ++r) status |= k6_score_read_in_block(lv, p, r, S);
+            if (b->aln_off[r + 1] > b->aln_off[r]) list.push_back(r);
+            else ++counts[0];
+        }
+        for (auto it = list.rbegin(); it != list.rend(); ++it)
+        {
+            const uint32_t r(*it);
+            ++counts[1 + k6_scratch_tier(v.b, r)];
+            status |= k6_score_read_tiered(v, k6_region_of(b->region_read_off, b->n_regions, r), r, S);
         }
     }
     *status_out = status;

@@ -151,10 +151,22 @@ def test_score_indels_oracle_against_reference_golden():
     assert total > 200
 
 
-def test_k6_device_body_on_the_host(tmp_path):
+def _k6_list_case(case):
+    """A K6 batch with what score_indels_case has none of: reads without a candidate alignment (the list kernel never sees them) and
+    reads with 9 to 40 alignments (the second local-memory scratch tier)."""
+    rng = np.random.default_rng(7000 + case)
+    regions, lnp = specgen.random_score_indels_regions(rng, 8, alns_per_read=(1, 40))
+    for _win, reads in regions:
+        for _ in range(int(rng.integers(1, 3))):
+            reads.insert(int(rng.integers(0, len(reads) + 1)), B.ScoredReadSpec(int(rng.integers(30, 151)), [], fwd=bool(rng.random() < 0.5)))
+    return B.ScoreIndelsBatch(regions), lnp
+
+
+def test_k6_device_body_and_list_walk_on_the_host(tmp_path):
     """strelka_b200/csrc/k6_core.cuh is __host__ __device__: the exact per-read body the kernel runs, compiled with g++
-    (tests/cpp/k6_core_host.cpp) and run read by read on the CPU, against the oracle -- the logic of the CUDA path is checked in the
-    GPU-less container too.  (A test harness only: libstrelka_b200.so has no host execution path.)"""
+    (tests/cpp/k6_core_host.cpp) and run on the CPU against the oracle, read by read and the way k6_score_list_kernel walks its list --
+    the logic of the CUDA path is checked in the GPU-less container too.  (A test harness only: libstrelka_b200.so has no host
+    execution path.)"""
     import subprocess
 
     root = os.path.dirname(HERE)
@@ -162,24 +174,29 @@ def test_k6_device_body_on_the_host(tmp_path):
     subprocess.check_call(["g++", "-std=c++14", "-O2", "-fPIC", "-shared", "-I" + os.path.join(root, "include"), "-I" + os.path.join(root, "strelka_b200", "csrc"),
                            os.path.join(HERE, "cpp", "k6_core_host.cpp"), "-o", so])
     lib = C.CDLL(so)
-    lib.k6core_run.argtypes = [C.POINTER(A.SxScoreIndelsBatch)] + [C.c_void_p] * 6 + [C.c_uint32, C.c_uint32, C.c_void_p]
-    total = staged_total = 0
+    lib.k6core_run.argtypes = [C.POINTER(A.SxScoreIndelsBatch)] + [C.c_void_p] * 6 + [C.c_uint32, C.c_void_p]
+    total = 0
+    walked = np.zeros(4, np.int64)  # list walk: reads skipped (no alignment), reads per scratch tier (8/4 local, 40/4 local, arena)
     for case in range(60):
-        sb, lnp = specgen.score_indels_case(case)
-        want = reflib.ox_score_indels(sb, lnp)
-        # 0: the plain per-read body; otherwise what a thread block of that many reads does (plan, stage its slices into "shared
-        # memory", run the body on the rebased view; blocks whose slices exceed the capacity run on the global view)
-        for block_reads, cap in ((0, 0), (128, 49152), (32, 49152), (7, 4096), (3, 700), (128, 0)):
-            out = B.ScoreIndelsOut(sb)
-            st, staged = np.zeros(1, np.uint32), np.zeros(1, np.uint32)
-            lib.k6core_run(C.byref(sb.c), A.ptr(lnp), A.ptr(out.recs), A.ptr(out.n_rec), A.ptr(out.max_aln), A.ptr(out.eval_aln), A.ptr(st), block_reads, cap,
-                           A.ptr(staged))
-            assert st[0] == 0
-            for w, g in zip(want, out.compact()):
-                assert w.tobytes() == g.tobytes()
-            staged_total += int(staged[0])
-        total += len(want[0])
-    assert total > 1500 and staged_total > 300
+        for extra, (sb, lnp) in enumerate((specgen.score_indels_case(case), _k6_list_case(case))):
+            want = reflib.ox_score_indels(sb, lnp)
+            # 0: the plain per-read body; 1: what the list kernel does (k6_run's memsets, then the listed reads in reverse order, each
+            # with its region from k6_region_of and the scratch tier the kernel picks)
+            for list_walk in (0, 1):
+                out = B.ScoreIndelsOut(sb)
+                for a in (out.n_rec, out.max_aln, out.eval_aln):
+                    a[:] = 0xA5A5A5A5  # a read whose outputs nobody writes shows up
+                st, counts = np.zeros(1, np.uint32), np.zeros(4, np.uint32)
+                lib.k6core_run(C.byref(sb.c), A.ptr(lnp), A.ptr(out.recs), A.ptr(out.n_rec), A.ptr(out.max_aln), A.ptr(out.eval_aln), A.ptr(st), list_walk,
+                               A.ptr(counts))
+                assert st[0] == 0
+                for w, g in zip(want, out.compact()):
+                    assert w.tobytes() == g.tobytes()
+                walked += counts
+            total += 0 if extra else len(want[0])
+    print("k6 list walk: skipped %d, tiers %d / %d / %d" % tuple(walked))
+    assert total > 1500
+    assert walked[0] > 600 and walked[1] > 1000 and walked[2] > 500 and walked[3] > 1200
 
 
 def test_libm_tables_are_this_libms(tmp_path):

@@ -489,10 +489,9 @@ def test_k4_pileup_in_read_buffer_order(ctx, seed, packed):
 
 @pytest.mark.parametrize("mode", ["germline", "somatic", "edge"])
 @pytest.mark.parametrize("packed", [False, True])
-def test_k4_gather_plan(ctx, monkeypatch, mode, packed):
-    """K4's second plan for the fill (SX_K4_PLAN=2: k4_bases_kernel, a thread per read, + k4_gather_kernel, a warp per 32 sites) gives the same
-    columns as the oracle -- option modes, reads whose best alignment moved away from their buffer position, dictionary-coded qualities."""
-    monkeypatch.setenv("SX_K4_PLAN", "2")
+def test_k4_read_buffer_order_option_modes(ctx, mode, packed):
+    """K4 gives the oracle's columns under the somatic and the edge option sets too, for reads whose best alignment moved away from their
+    buffer position, with and without dictionary-coded qualities."""
     opts = {"germline": None, "somatic": A.SxPileupOpts(1, 0, 20, 3, 1, 10, 0, 0), "edge": A.SxPileupOpts(1, 17, 3, 1, 1, 2, 5, 0)}[mode]
     pb = _buffer_order_case(np.random.default_rng(6400 + len(mode)), packed, opts)
     want = reflib.ox_pileup_reads(pb)
