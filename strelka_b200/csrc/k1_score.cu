@@ -142,7 +142,7 @@ __global__ void __launch_bounds__(K1_THREADS) k1_score_kernel(const sx_region* _
     if (L.n_alns == 0) return;
     if (L.total > smem_bytes)
     {
-        if (threadIdx.x == 0) atomicOr(status, 2);
+        if (threadIdx.x == 0) atomicOr(status, SX_ST_TILE);
         return;
     }
     uint64_t* bar = reinterpret_cast<uint64_t*>(smem);
@@ -186,7 +186,7 @@ __global__ void __launch_bounds__(K1_THREADS) k1_score_kernel(const sx_region* _
     const uint32_t tab_saddr = smem_u32(tab); // shared-window address of the term table
     if (tab_saddr + K1_TAB_BYTES > 0xfff0u || (tab_saddr & 15u))
     {
-        if (threadIdx.x == 0) atomicOr(status, 2);
+        if (threadIdx.x == 0) atomicOr(status, SX_ST_TILE);
         return;
     }
     // quality dictionary of the 4-bit wire format lives in the descriptor block's tail (16 bytes after the 16 descriptors)
@@ -266,7 +266,7 @@ __global__ void __launch_bounds__(K1_THREADS) k1_score_kernel(const sx_region* _
     __syncthreads();
     if ((!baseq && (qual_bits == 2 ? (soff_s[L.n_reads] + 1) / 2 : qual_bits == 4 ? soff_s[L.n_reads] : boff_s[L.n_reads]) > L.qual_bytes) || soff_s[L.n_reads] > L.seq_bytes)
     {
-        if (threadIdx.x == 0) atomicOr(status, 2);
+        if (threadIdx.x == 0) atomicOr(status, SX_ST_TILE);
         return;
     }
     // expand each read once: entry = (table row << 4) | one-hot base.  One packed byte (two bases) per lane and iteration; the
@@ -313,12 +313,12 @@ __global__ void __launch_bounds__(K1_THREADS) k1_score_kernel(const sx_region* _
                 }
                 qmax = max(qmax, (d0 >> 16) ? q0 : 0u);
                 qmax = max(qmax, (d1 >> 16) ? q1 : 0u);
-                const uint32_t e0 = (d0 & 0xffffu) + ((min(q0, (uint32_t)SX_MAX_QSCORE) << 4) & (d0 >> 16));
-                const uint32_t e1 = (d1 & 0xffffu) + ((min(q1, (uint32_t)SX_MAX_QSCORE) << 4) & (d1 >> 16));
-                en2[p] = e0 | (e1 << 16);
+                const uint32_t lo = (d0 & 0xffffu) + ((min(q0, (uint32_t)SX_MAX_QSCORE) << 4) & (d0 >> 16));
+                const uint32_t hi = (d1 & 0xffffu) + ((min(q1, (uint32_t)SX_MAX_QSCORE) << 4) & (d1 >> 16));
+                en2[p] = lo | (hi << 16);
             }
         }
-        if (qmax > SX_MAX_QSCORE) atomicOr(status, 1);
+        if (qmax > SX_MAX_QSCORE) atomicOr(status, SX_ST_QUAL);
         if (baseq && exc_off[ri + 1] > exc_off[ri])
         {
             // the bases that are not A/C/G/T: rebuild their entries from the real code (the nibble kept the quality code)
@@ -328,7 +328,7 @@ __global__ void __launch_bounds__(K1_THREADS) k1_score_kernel(const sx_region* _
                 const uint32_t v = exc[i], pos = v & 0xffffffu, d = desc_s[(v >> 24) & 15u];
                 if (pos >= 2u * soff_s[L.n_reads])
                 {
-                    atomicOr(status, 2);
+                    atomicOr(status, SX_ST_TILE);
                     continue;
                 }
                 const uint32_t q = qd_s[(seq_s[pos >> 1] >> ((~pos & 1u) << 2)) & 3u];
@@ -361,7 +361,7 @@ __global__ void __launch_bounds__(K1_THREADS) k1_score_kernel(const sx_region* _
         const uint32_t rl = h.x;
         if (rl >= L.n_reads)
         {
-            atomicOr(status, 2);
+            atomicOr(status, SX_ST_TILE);
             continue;
         }
         const uint16_t* ent = ent_s + 2u * soff_s[rl];
@@ -397,7 +397,7 @@ __global__ void __launch_bounds__(K1_THREADS) k1_score_kernel(const sx_region* _
                 {
                     if (len > read_left)
                     {
-                        atomicOr(status, 8);
+                        atomicOr(status, SX_ST_READ_OVERRUN);
                         done = true;
                         break;
                     }
@@ -441,7 +441,7 @@ __global__ void __launch_bounds__(K1_THREADS) k1_score_kernel(const sx_region* _
                 }
                 else if (kind != SX_SEG_HARDCLIP)
                 {
-                    atomicOr(status, 4);
+                    atomicOr(status, SX_ST_SEG_KIND);
                 }
             }
             if (done) break;
@@ -558,7 +558,7 @@ __global__ void k1_read_max_kernel(const sx_aln* __restrict__ alns, uint32_t n_a
 int k1_smem_need_dev(sx_ctx* ctx, const sx_region* regions_dev, uint32_t begin, uint32_t end, uint32_t need[2], uint32_t fmt)
 {
     uint32_t* d = nullptr;
-    int rc = sx_ensure(ctx, 20, 2 * sizeof(uint32_t), reinterpret_cast<void**>(&d));
+    int rc = sx_take(ctx, SX_SLOT_K1_SMEM_NEED, 2, d, 0);
     if (rc) return rc;
     SX_CUDA(ctx, cudaMemsetAsync(d, 0, 2 * sizeof(uint32_t), ctx->s_compute));
     const uint32_t n = end - begin;
@@ -706,30 +706,28 @@ extern "C" int sx_score_alignments(sx_ctx* ctx, const sx_align_batch* b, double*
     if (rc) return rc;
 
     sx_align_batch d = *b;
-    void* p = nullptr;
     const size_t reg_bytes = (size_t)(b->n_regions + 1) * sizeof(sx_region);
     const size_t aln_sz = (b->format & SX_FMT_ALN8) ? sizeof(sx_aln8) : sizeof(sx_aln), seg_sz = (b->format & SX_FMT_SEG2) ? sizeof(sx_aln_seg2) : sizeof(sx_aln_seg);
     const size_t aln_bytes = (size_t)(b->n_alns + 1) * aln_sz + 16; // + slack: an sx_aln8 slice is staged from a 16-byte boundary
     const size_t seg_bytes = (size_t)b->n_segs * seg_sz + SX_POOL_SLACK;
-#define SX_POOL(slot, field, type, bytes)            \
-    if ((rc = sx_ensure(ctx, slot, (bytes), &p))) return rc; \
-    d.field = static_cast<type>(p);
-    SX_POOL(0, regions, const sx_region*, reg_bytes)
-    SX_POOL(1, read_len, const uint16_t*, (size_t)b->n_reads * 2 + 16)
-    SX_POOL(2, seq4, const uint8_t*, b->seq4_bytes + SX_POOL_SLACK)
-    SX_POOL(3, qual, const uint8_t*, b->qual_bytes + SX_POOL_SLACK)
-    SX_POOL(4, ref, const char*, b->ref_bytes + SX_POOL_SLACK)
-    SX_POOL(5, alns, const sx_aln*, aln_bytes)
-    SX_POOL(6, segs, const sx_aln_seg*, seg_bytes)
-    SX_POOL(7, ins, const char*, b->ins_bytes + SX_POOL_SLACK)
+    void *alns = nullptr, *segs = nullptr;
+    if ((rc = sx_take(ctx, sx_host_slot(0), (size_t)b->n_regions + 1, d.regions, 0))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(1), b->n_reads, d.read_len, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(2), b->seq4_bytes, d.seq4, SX_POOL_SLACK))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(3), b->qual_bytes, d.qual, SX_POOL_SLACK))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(4), b->ref_bytes, d.ref, SX_POOL_SLACK))) return rc;
+    if ((rc = sx_ensure(ctx, sx_host_slot(5), aln_bytes, &alns))) return rc; // (sx_aln or sx_aln8 entries)
+    if ((rc = sx_ensure(ctx, sx_host_slot(6), seg_bytes, &segs))) return rc;
+    d.alns = static_cast<const sx_aln*>(alns);
+    d.segs = static_cast<const sx_aln_seg*>(segs);
+    if ((rc = sx_take(ctx, sx_host_slot(7), b->ins_bytes, d.ins, SX_POOL_SLACK))) return rc;
     if (b->format & SX_FMT_BASEQ)
     {
-        SX_POOL(24, exc_off, const uint32_t*, (size_t)(b->n_regions + 1) * 4)
-        SX_POOL(25, exc, const uint32_t*, (size_t)b->exc_off[b->n_regions] * 4 + 16)
+        if ((rc = sx_take(ctx, sx_host_slot(24), (size_t)b->n_regions + 1, d.exc_off, 0))) return rc;
+        if ((rc = sx_take(ctx, sx_host_slot(25), b->exc_off[b->n_regions], d.exc, 16))) return rc;
     }
-#undef SX_POOL
     double* d_out = nullptr;
-    if ((rc = sx_ensure(ctx, 8, (size_t)b->n_alns * sizeof(double), reinterpret_cast<void**>(&d_out)))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(8), b->n_alns, d_out, 0))) return rc;
 
     int chunks = ctx->params.pipeline_chunks;
     if (chunks <= 0)

@@ -127,7 +127,7 @@ __global__ void __launch_bounds__(KQ_THREADS) k1q_score_kernel(const sx_region* 
     const uint32_t tab_saddr = (sbase + L.tab + 1023u) & ~1023u; // 1 KB-aligned in the shared window: a cell's address is two PRMT'd bytes
     if (L.total > smem_bytes || sbase + L.total > 0xffffu || tab_saddr + 1024u > 0x7f00u || L.n_segs > 0xffffu)
     {
-        if (threadIdx.x == 0) atomicOr(status, 2);
+        if (threadIdx.x == 0) atomicOr(status, SX_ST_TILE);
         return;
     }
     const uint32_t tid = threadIdx.x;
@@ -240,7 +240,7 @@ __global__ void __launch_bounds__(KQ_THREADS) k1q_score_kernel(const sx_region* 
     __syncthreads();
     if (soff_s[L.n_reads] > L.seq_bytes || (!baseq && (qual_bits == 2 ? (soff_s[L.n_reads] + 1) / 2 : soff_s[L.n_reads]) > L.qual_bytes))
     {
-        if (tid == 0) atomicOr(status, 2);
+        if (tid == 0) atomicOr(status, SX_ST_TILE);
         return;
     }
     // ---- expansion: entry byte 2p / 2p+1 <- packed byte p (high nibble first), for the whole region at once
@@ -274,7 +274,7 @@ __global__ void __launch_bounds__(KQ_THREADS) k1q_score_kernel(const sx_region* 
                     const uint32_t v = exc[i], pos = v & 0xffffffu, code = v >> 24;
                     if (pos >= 2u * soff_s[L.n_reads])
                     {
-                        atomicOr(status, 2);
+                        atomicOr(status, SX_ST_TILE);
                         continue;
                     }
                     const uint32_t page = code == 15u ? PAGE_ZERO : code == 0u ? PAGE_EQ : PAGE_NOMATCH;
@@ -309,7 +309,7 @@ __global__ void __launch_bounds__(KQ_THREADS) k1q_score_kernel(const sx_region* 
             acc |= (w0 & (w0 >> 1) & ~(w0 >> 2) & (w0 >> 3)) | (w1 & (w1 >> 1) & ~(w1 >> 2) & (w1 >> 3));
             ent64[w] = make_uint2(w0, w1);
         }
-        if (acc & 0x01010101u) atomicOr(status, 1);
+        if (acc & 0x01010101u) atomicOr(status, SX_ST_QUAL);
         uint32_t* ref32 = reinterpret_cast<uint32_t*>(ref_s);
         if (ref4)
         {
@@ -350,7 +350,7 @@ __global__ void __launch_bounds__(KQ_THREADS) k1q_score_kernel(const sx_region* 
         const uint32_t seg0 = h.z, seg1 = seg_end_of(a);
         if (rl >= L.n_reads || seg1 > L.n_segs || seg0 > seg1)
         {
-            atomicOr(status, 2);
+            atomicOr(status, SX_ST_TILE);
             continue;
         }
         const uint32_t rec0 = recs_s0 + (seg0 + a) * 8u; // this alignment's records: one per segment at most, + END
@@ -372,7 +372,7 @@ __global__ void __launch_bounds__(KQ_THREADS) k1q_score_kernel(const sx_region* 
                 {
                     if (len > read_left)
                     {
-                        atomicOr(status, 8);
+                        atomicOr(status, SX_ST_READ_OVERRUN);
                         break;
                     }
                     read_left -= len;
@@ -402,10 +402,10 @@ __global__ void __launch_bounds__(KQ_THREADS) k1q_score_kernel(const sx_region* 
                     pre = 0;
                     ent += len;
                 }
-                else if (kind != SX_SEG_HARDCLIP) atomicOr(status, 4);
+                else if (kind != SX_SEG_HARDCLIP) atomicOr(status, SX_ST_SEG_KIND);
                 if ((seg >> 24) & SX_SEGF_NONCANDIDATE)
                 {
-                    if (pre == 255u) atomicOr(status, 4);
+                    if (pre == 255u) atomicOr(status, SX_ST_SEG_KIND);
                     else ++pre;
                 }
             }

@@ -263,7 +263,7 @@ __global__ void __launch_bounds__(K2_WARPS * 32) k2a_germline_batch_kernel(const
                     }
                     else
                     {
-                        if (lane == 0) atomicOr(status, 16);
+                        if (lane == 0) atomicOr(status, SX_ST_SITE_DEPTH);
                         n_raw = 0;
                     }
                 }
@@ -570,7 +570,7 @@ __global__ void __launch_bounds__(K2_WARPS * 32, 8) k2a_germline12_kernel(const 
             uint32_t n_raw = c1 - c0;
             if (n_raw > cap) // the host sizes cap from the deepest site
             {
-                if (lane == 0) atomicOr(status, 16);
+                if (lane == 0) atomicOr(status, SX_ST_SITE_DEPTH);
                 n_raw = 0;
             }
             const char rb = ref_base[site];
@@ -1055,7 +1055,7 @@ int germline_run(sx_ctx* ctx, const sx_pileup_batch* d, int is_always_test, sx_d
     // a deeper site: one site per warp, K2_CAP_SMEM calls in shared memory, a deeper site in the warp's K2_CAP_BIG-call region of the scratch
     const int grid = static_cast<int>(std::min<uint32_t>((d->n_sites + K2_WARPS - 1) / K2_WARPS, (uint32_t)ctx->sm_count * 8));
     unsigned char* scratch = nullptr;
-    const int rc = sx_ensure(ctx, 19, (size_t)grid * K2_WARPS * K2_CAP_BIG * 8, reinterpret_cast<void**>(&scratch));
+    const int rc = sx_take(ctx, SX_SLOT_K2A_SCRATCH, (size_t)grid * K2_WARPS * K2_CAP_BIG * 8, scratch, 0);
     if (rc) return rc;
     k2a_germline_batch_kernel<1><<<grid, K2_WARPS * 32, (size_t)K2_WARPS * K2_CAP_SMEM * 8, ctx->s_compute>>>(d->site_off, d->calls, d->ref_base, d->ploidy, d->n_sites,
                                                                                                            is_always_test, ctx->d_tables, out_dev, de_off_dev, de_dev,
@@ -1067,7 +1067,7 @@ int germline_run(sx_ctx* ctx, const sx_pileup_batch* d, int is_always_test, sx_d
 int max_site_dev(sx_ctx* ctx, const uint32_t* site_off_dev, uint32_t n_sites, uint32_t* out)
 {
     uint32_t* d = nullptr;
-    int rc = sx_ensure(ctx, 20, sizeof(uint32_t), reinterpret_cast<void**>(&d));
+    int rc = sx_take(ctx, SX_SLOT_K2A_MAX_SITE, 1, d, 0);
     if (rc) return rc;
     SX_CUDA(ctx, cudaMemsetAsync(d, 0, sizeof(uint32_t), ctx->s_compute));
     k2_max_site_kernel<<<std::min<uint32_t>((n_sites + 255) / 256, 1184), 256, 0, ctx->s_compute>>>(site_off_dev, n_sites, d);
@@ -1103,14 +1103,13 @@ extern "C" int sx_site_gl_germline_dev(sx_ctx* ctx, const sx_pileup_batch* d, in
     return sx_check_status(ctx, "sx_site_gl_germline");
 }
 
-// upload a host pileup batch into ctx arenas (slots base..base+5); returns the device view
-int sx_upload_pileup(sx_ctx* ctx, const sx_pileup_batch* b, int slot_base, sx_pileup_batch* d, uint32_t* max_site, cudaStream_t st)
+// upload a host pileup batch into host slots host_base..host_base+5; returns the device view
+int sx_upload_pileup(sx_ctx* ctx, const sx_pileup_batch* b, int host_base, sx_pileup_batch* d, uint32_t* max_site)
 {
     if (!b->site_off || !b->calls || !b->ref_base) return sx_fail(ctx, SX_ERR_ARG, "pileup batch: NULL array");
     *d = *b;
-    void* p = nullptr;
     int rc;
-    const uint32_t n_calls = b->site_off[b->n_sites];
+    const size_t n(b->n_sites);
     uint32_t m = 0;
     for (uint32_t s = 0; s < b->n_sites; ++s)
     {
@@ -1118,28 +1117,19 @@ int sx_upload_pileup(sx_ctx* ctx, const sx_pileup_batch* b, int slot_base, sx_pi
         m = std::max(m, b->site_off[s + 1] - b->site_off[s]);
     }
     *max_site = m;
-#define SX_UP(slot, field, type, bytes)                                                                      \
-    if ((rc = sx_ensure(ctx, slot_base + slot, (bytes) + 16, &p))) return rc;                                  \
-    SX_CUDA(ctx, cudaMemcpyAsync(p, b->field, (bytes), cudaMemcpyHostToDevice, st));                          \
-    d->field = static_cast<type>(p);
-    SX_UP(0, site_off, const uint32_t*, (size_t)(b->n_sites + 1) * 4)
-    SX_UP(1, calls, const uint16_t*, (size_t)n_calls * 2)
-    SX_UP(2, ref_base, const char*, (size_t)b->n_sites)
-    if (b->ploidy)
-    {
-        SX_UP(3, ploidy, const uint8_t*, (size_t)b->n_sites)
-    }
+    if ((rc = sx_upload(ctx, sx_host_slot(host_base), b->site_off, n + 1, d->site_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(host_base + 1), b->calls, b->site_off[b->n_sites], d->calls, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(host_base + 2), b->ref_base, n, d->ref_base, 16))) return rc;
+    if (b->ploidy && (rc = sx_upload(ctx, sx_host_slot(host_base + 3), b->ploidy, n, d->ploidy, 16))) return rc;
     if (b->t2_off)
     {
         if (!b->t2_calls) return sx_fail(ctx, SX_ERR_ARG, "pileup batch: t2_off without t2_calls");
-        const uint32_t n2 = b->t2_off[b->n_sites];
-        SX_UP(4, t2_off, const uint32_t*, (size_t)(b->n_sites + 1) * 4)
-        SX_UP(5, t2_calls, const uint16_t*, (size_t)n2 * 2)
+        if ((rc = sx_upload(ctx, sx_host_slot(host_base + 4), b->t2_off, n + 1, d->t2_off, 16))) return rc;
+        if ((rc = sx_upload(ctx, sx_host_slot(host_base + 5), b->t2_calls, b->t2_off[b->n_sites], d->t2_calls, 16))) return rc;
         uint32_t m2 = 0;
         for (uint32_t s = 0; s < b->n_sites; ++s) m2 = std::max(m2, b->site_off[s + 1] - b->site_off[s] + b->t2_off[s + 1] - b->t2_off[s]);
         *max_site = std::max(*max_site, m2);
     }
-#undef SX_UP
     return SX_OK;
 }
 
@@ -1152,20 +1142,14 @@ extern "C" int sx_site_gl_germline(sx_ctx* ctx, const sx_pileup_batch* b, int is
     SX_CUDA(ctx, cudaSetDevice(ctx->device));
     sx_pileup_batch d;
     uint32_t max_site = 0;
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_a, ctx->s_compute));
-    int rc = sx_upload_pileup(ctx, b, 9, &d, &max_site, ctx->s_compute);
+    sx_call_timer t(ctx);
+    int rc = sx_upload_pileup(ctx, b, 9, &d, &max_site);
     if (rc) return rc;
     sx_digt_result* d_out = nullptr;
-    if ((rc = sx_ensure(ctx, 15, (size_t)b->n_sites * sizeof(sx_digt_result), reinterpret_cast<void**>(&d_out)))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(15), b->n_sites, d_out, 0))) return rc;
     if ((rc = germline_run(ctx, &d, is_always_test, d_out, nullptr, nullptr, max_site))) return rc;
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host, d_out, (size_t)b->n_sites * sizeof(sx_digt_result), cudaMemcpyDeviceToHost, ctx->s_compute));
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_b, ctx->s_compute));
-    SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
-    float ms = 0;
-    cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b);
-    ctx->timing.kernel_ms = ms;
-    ctx->timing.launches = 1;
-    ctx->total_launches += 1;
+    if ((rc = sx_download(ctx, out_host, d_out, b->n_sites))) return rc;
+    if ((rc = t.finish(1))) return rc; // (the deepest site was found on the host)
     return sx_check_status(ctx, "sx_site_gl_germline");
 }
 
@@ -1190,15 +1174,14 @@ extern "C" int sx_dependent_eprob(sx_ctx* ctx, const sx_pileup_batch* b, uint32_
     out_off_host[b->n_sites] = off;
     sx_pileup_batch d;
     uint32_t max_site = 0;
-    int rc = sx_upload_pileup(ctx, b, 9, &d, &max_site, ctx->s_compute);
+    int rc = sx_upload_pileup(ctx, b, 9, &d, &max_site);
     if (rc) return rc;
     uint32_t* d_off = nullptr;
     float* d_de = nullptr;
-    if ((rc = sx_ensure(ctx, 16, (size_t)(b->n_sites + 1) * 4, reinterpret_cast<void**>(&d_off)))) return rc;
-    if ((rc = sx_ensure(ctx, 17, (size_t)off * 4 + 16, reinterpret_cast<void**>(&d_de)))) return rc;
-    SX_CUDA(ctx, cudaMemcpyAsync(d_off, out_off_host, (size_t)(b->n_sites + 1) * 4, cudaMemcpyHostToDevice, ctx->s_compute));
+    if ((rc = sx_upload(ctx, sx_host_slot(16), out_off_host, (size_t)b->n_sites + 1, d_off, 0))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(17), off, d_de, 16))) return rc;
     if ((rc = germline_run(ctx, &d, 1, nullptr, d_off, d_de, max_site))) return rc;
-    SX_CUDA(ctx, cudaMemcpyAsync(de_host, d_de, (size_t)off * 4, cudaMemcpyDeviceToHost, ctx->s_compute));
+    if ((rc = sx_download(ctx, de_host, d_de, off))) return rc;
     SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
     ctx->timing.launches = 1;
     ctx->total_launches += 1;

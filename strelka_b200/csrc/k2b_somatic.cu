@@ -375,28 +375,17 @@ extern "C" int sx_site_gl_somatic(sx_ctx* ctx, const sx_pileup_batch* n, const s
     if (n->n_sites != t->n_sites) return sx_fail(ctx, SX_ERR_ARG, "sx_site_gl_somatic: normal and tumor batches differ in n_sites");
     if (n->n_sites == 0) return SX_OK;
     SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_a, ctx->s_compute));
+    sx_call_timer tm(ctx);
     sx_pileup_batch dn, dt;
     uint32_t m = 0;
-    int rc = sx_upload_pileup(ctx, n, 9, &dn, &m, ctx->s_compute);
+    int rc = sx_upload_pileup(ctx, n, 9, &dn, &m);
     if (rc) return rc;
-    if ((rc = sx_upload_pileup(ctx, t, 21 - 6, &dt, &m, ctx->s_compute))) return rc; // slots 15..20
-    uint8_t* d_forced = nullptr;
-    if (forced_host)
-    {
-        if ((rc = sx_ensure(ctx, 21, n->n_sites, reinterpret_cast<void**>(&d_forced)))) return rc;
-        SX_CUDA(ctx, cudaMemcpyAsync(d_forced, forced_host, n->n_sites, cudaMemcpyHostToDevice, ctx->s_compute));
-    }
+    if ((rc = sx_upload_pileup(ctx, t, 15, &dt, &m))) return rc;
+    const uint8_t* d_forced = nullptr;
+    if (forced_host && (rc = sx_upload(ctx, sx_host_slot(21), forced_host, n->n_sites, d_forced, 0))) return rc;
     sx_ssnv_result* d_out = nullptr;
-    if ((rc = sx_ensure(ctx, 22, (size_t)n->n_sites * sizeof(sx_ssnv_result), reinterpret_cast<void**>(&d_out)))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(22), n->n_sites, d_out, 0))) return rc;
     if ((rc = somatic_run(ctx, &dn, &dt, d_forced, d_out))) return rc;
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host, d_out, (size_t)n->n_sites * sizeof(sx_ssnv_result), cudaMemcpyDeviceToHost, ctx->s_compute));
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_b, ctx->s_compute));
-    SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
-    float ms = 0;
-    cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b);
-    ctx->timing.kernel_ms = ms;
-    ctx->timing.launches = 1;
-    ctx->total_launches += 1;
-    return SX_OK;
+    if ((rc = sx_download(ctx, out_host, d_out, n->n_sites))) return rc;
+    return tm.finish(1);
 }

@@ -537,34 +537,20 @@ extern "C" int sx_global_align(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_
         const uint32_t Q = b->query_off[i + 1] - b->query_off[i], R = b->ref_off[i + 1] - b->ref_off[i];
         if (Q == 0 || R == 0) return sx_fail(ctx, SX_ERR_ARG, "sx_global_align: empty query or reference in problem %u (asserted at GlobalAlignerImpl.hh:47-48)", i);
     }
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_a, ctx->s_compute));
+    sx_call_timer t(ctx);
     sx_ga_batch d = *b;
-    void* p = nullptr;
     int rc;
-    const size_t qbytes = b->query_off[b->n], rbytes = b->ref_off[b->n];
-#define SX_UP(slot, field, type, bytes)                                                    \
-    if ((rc = sx_ensure(ctx, slot, (bytes) + 16, &p))) return rc;                            \
-    SX_CUDA(ctx, cudaMemcpyAsync(p, b->field, (bytes), cudaMemcpyHostToDevice, ctx->s_compute)); \
-    d.field = static_cast<type>(p);
-    SX_UP(9, query, const char*, qbytes)
-    SX_UP(10, ref, const char*, rbytes)
-    SX_UP(11, query_off, const uint32_t*, (size_t)(b->n + 1) * 4)
-    SX_UP(12, ref_off, const uint32_t*, (size_t)(b->n + 1) * 4)
-#undef SX_UP
+    if ((rc = sx_upload(ctx, sx_host_slot(9), b->query, b->query_off[b->n], d.query, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(10), b->ref, b->ref_off[b->n], d.ref, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(11), b->query_off, (size_t)b->n + 1, d.query_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(12), b->ref_off, (size_t)b->n + 1, d.ref_off, 16))) return rc;
     sx_ga_result* d_res = nullptr;
     uint32_t* d_cig = nullptr;
-    if ((rc = sx_ensure(ctx, 13, (size_t)b->n * sizeof(sx_ga_result), reinterpret_cast<void**>(&d_res)))) return rc;
-    if ((rc = sx_ensure(ctx, 14, (size_t)b->n * b->max_ops * 4 + 16, reinterpret_cast<void**>(&d_cig)))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(13), b->n, d_res, 0))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(14), (size_t)b->n * b->max_ops, d_cig, 16))) return rc;
     SX_CUDA(ctx, cudaMemsetAsync(d_cig, 0, (size_t)b->n * b->max_ops * 4, ctx->s_compute)); // unused cigar slots read as 0
     if ((rc = k3_run(ctx, sc, &d, d_res, d_cig))) return rc;
-    SX_CUDA(ctx, cudaMemcpyAsync(res_host, d_res, (size_t)b->n * sizeof(sx_ga_result), cudaMemcpyDeviceToHost, ctx->s_compute));
-    SX_CUDA(ctx, cudaMemcpyAsync(cigar_host, d_cig, (size_t)b->n * b->max_ops * 4, cudaMemcpyDeviceToHost, ctx->s_compute));
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_b, ctx->s_compute));
-    SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
-    float ms = 0;
-    cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b);
-    ctx->timing.kernel_ms = ms;
-    ctx->timing.launches = 1;
-    ctx->total_launches += 1;
-    return SX_OK;
+    if ((rc = sx_download(ctx, res_host, d_res, b->n))) return rc;
+    if ((rc = sx_download(ctx, cigar_host, d_cig, (size_t)b->n * b->max_ops))) return rc;
+    return t.finish(1);
 }

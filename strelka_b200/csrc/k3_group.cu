@@ -428,7 +428,7 @@ inline int kg_max_ctas_per_sm(int T) { return T >= 10 ? 4 : 8; }
 
 template <int T>
 int kg_launch(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* d, sx_ga_result* res_dev, uint32_t* cigar_dev, const uint32_t* order, uint32_t n, uint32_t max_r,
-              int scratch_slot_id, uint32_t* work_dev)
+              uint32_t* work_dev)
 {
     if (n == 0) return SX_OK;
     const size_t smem = (size_t)kg_warp_smem<T>(max_r) * KG_WARPS;
@@ -441,7 +441,7 @@ int kg_launch(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* d, sx_ga_r
     occ = std::max(1, std::min(occ, kg_max_ctas_per_sm(T)));
     const int grid = static_cast<int>(std::min<uint32_t>((quads + KG_WARPS - 1) / KG_WARPS, (uint32_t)(ctx->sm_count * occ)));
     unsigned char* scratch = nullptr;
-    int rc = sx_ensure(ctx, scratch_slot_id, slot * KG_B * (size_t)grid * KG_WARPS, reinterpret_cast<void**>(&scratch));
+    int rc = sx_take(ctx, SX_SLOT_K3_SCRATCH, slot * KG_B * (size_t)grid * KG_WARPS, scratch, 0);
     if (rc) return rc;
     kg_align_kernel<T><<<grid, KG_WARPS * 32, smem, ctx->s_compute>>>(d->query, d->ref, d->query_off, d->ref_off, order, n, d->max_ops, *sc, res_dev, cigar_dev, max_r, scratch,
                                                                      slot, work_dev);
@@ -457,9 +457,9 @@ int sx_k3_group_run(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* d, s
     uint32_t* d_cursor = nullptr;
     uint32_t* d_order = nullptr;
     int rc;
-    if ((rc = sx_ensure(ctx, 20, sizeof(kg_info), reinterpret_cast<void**>(&d_info)))) return rc;
-    if ((rc = sx_ensure(ctx, 21, sizeof(uint32_t) * KG_BUCKETS, reinterpret_cast<void**>(&d_cursor)))) return rc;
-    if ((rc = sx_ensure(ctx, 22, sizeof(uint32_t) * (size_t)d->n, reinterpret_cast<void**>(&d_order)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K3_INFO, 1, d_info, 0))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K3_CURSOR, KG_BUCKETS, d_cursor, 0))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K3_ORDER, d->n, d_order, 0))) return rc;
     SX_CUDA(ctx, cudaMemsetAsync(d_info, 0, sizeof(kg_info), ctx->s_compute));
     const int cgrid = static_cast<int>(std::min<uint32_t>((d->n + 255) / 256, 1184));
     // the group kernel keeps 64*score in 32 bits: penalties that could overflow it send the whole batch to the warp kernel
@@ -483,7 +483,7 @@ int sx_k3_group_run(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* d, s
 #define KG_CASE(TT)                                                                                                                           \
     {                                                                                                                                         \
         const uint32_t b0 = begin[(TT - 1) * KG_RCLASSES], b1 = begin[TT * KG_RCLASSES];                                                       \
-        if ((rc = kg_launch<TT>(ctx, sc, d, res_dev, cigar_dev, d_order + b0, b1 - b0, info.max_r[TT - 1], 23, &d_info->work[TT - 1]))) return rc; \
+        if ((rc = kg_launch<TT>(ctx, sc, d, res_dev, cigar_dev, d_order + b0, b1 - b0, info.max_r[TT - 1], &d_info->work[TT - 1]))) return rc; \
     }
     // one launch per strip height; launches on one stream reuse the same scratch arena (sized for the largest so far by sx_ensure,
     // which only ever grows between launches after a stream-ordered free would be unsafe -- so size it once for the worst class)
@@ -492,8 +492,8 @@ int sx_k3_group_run(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* d, s
         for (int t = 1; t <= 16; ++t)
             if (begin[t * KG_RCLASSES] > begin[(t - 1) * KG_RCLASSES])
                 worst = std::max(worst, (((size_t)(info.max_r[t - 1] + KG_G) * t * 32 + 255) & ~size_t(255)) * kg_max_ctas_per_sm(t));
-        void* p = nullptr;
-        if (worst && (rc = sx_ensure(ctx, 23, worst * KG_B * (size_t)ctx->sm_count * KG_WARPS, &p))) return rc;
+        unsigned char* p = nullptr;
+        if (worst && (rc = sx_take(ctx, SX_SLOT_K3_SCRATCH, worst * KG_B * (size_t)ctx->sm_count * KG_WARPS, p, 0))) return rc;
     }
     KG_CASE(1) KG_CASE(2) KG_CASE(3) KG_CASE(4) KG_CASE(5) KG_CASE(6) KG_CASE(7) KG_CASE(8)
     KG_CASE(9) KG_CASE(10) KG_CASE(11) KG_CASE(12) KG_CASE(13) KG_CASE(14) KG_CASE(15) KG_CASE(16)

@@ -35,7 +35,6 @@ constexpr uint32_t K4_MAX_W = 2048;    // window size limit (shared memory: 16 b
 constexpr uint32_t K4_MAX_READ = 1024; // read length limit (delta + mismatch arrays)
 constexpr uint32_t K4_MAX_SEGS = 64;   // path segments per read
 constexpr unsigned FULL = 0xffffffffu;
-constexpr int ST_ORDER = 64, ST_BASE = 128, ST_LIMIT = 256, ST_QUAL = 1, ST_KIND = 4;
 
 struct k4_args
 {
@@ -132,13 +131,13 @@ __global__ void k4_count_kernel(k4_args A, int* __restrict__ d1, int* __restrict
     if (r >= A.n_reads) return;
     const sx_pileup_read rd = A.reads[r];
     const int32_t bp = bpos_of(A, r);
-    if (r > 0 && bpos_of(A, r - 1) > bp) atomicOr(status, ST_ORDER);
+    if (r > 0 && bpos_of(A, r - 1) > bp) atomicOr(status, SX_ST_READ_ORDER);
     if (rd.flags & SX_PRF_SKIP) return;
     const sx_aln_seg* path = A.segs + rd.seg_off;
     const uint32_t as = A.reads[r + 1].seg_off - rd.seg_off;
     if (rd.len > A.Lcap || as > K4_MAX_SEGS)
     {
-        atomicOr(status, ST_LIMIT);
+        atomicOr(status, SX_ST_READ_LIMIT);
         return;
     }
     uint32_t ref_span = 0, first = as, last = as;
@@ -151,14 +150,14 @@ __global__ void k4_count_kernel(k4_args A, int* __restrict__ d1, int* __restrict
             if (first == as) first = i;
             last = i;
         }
-        if (k > SX_SEG_SKIP) atomicOr(status, ST_KIND);
+        if (k > SX_SEG_SKIP) atomicOr(status, SX_ST_SEG_KIND);
     }
     const uint8_t* seq = A.seq4 + rd.seq_off;
     read_window w;
     if (!read_preamble(A, rd, ref_span, [&](uint32_t i) { return code_at(seq, i); }, w)) return;
     if (ref_span > A.W || bp < A.origin)
     {
-        atomicOr(status, ST_ORDER);
+        atomicOr(status, SX_ST_READ_ORDER);
         return;
     }
     const bool submapped = !(rd.flags & SX_PRF_TIER1OR2), tier1 = rd.flags & SX_PRF_TIER1;
@@ -169,7 +168,7 @@ __global__ void k4_count_kernel(k4_args A, int* __restrict__ d1, int* __restrict
     // the best alignment must stay within the three windows the fill pass holds cursors for (guaranteed by W >= span + max_pos_shift)
     if (static_cast<int64_t>(rd.pos) < this_win_pos - A.W || static_cast<int64_t>(rd.pos) + ref_span > this_win_pos + 2 * static_cast<int64_t>(A.W))
     {
-        atomicOr(status, ST_ORDER);
+        atomicOr(status, SX_ST_READ_ORDER);
         return;
     }
     int64_t ref_head = rd.pos;
@@ -480,7 +479,7 @@ __global__ void __launch_bounds__(K4_WARPS * 32) k4_fill_kernel(k4_args A, const
                 const bool edge = (i < first) || (i > last);
                 if (k == SX_SEG_INSERT && !edge) inc(seg_rd[i], len);
                 else if (k == SX_SEG_DELETE && !edge) inc(seg_rd[i], 0);
-                else if (k == SX_SEG_SKIP) atomicOr(status, ST_KIND); // "Can't handle cigar code" in create_mismatch_filter_map
+                else if (k == SX_SEG_SKIP) atomicOr(status, SX_ST_SEG_KIND); // "Can't handle cigar code" in create_mismatch_filter_map
             }
             for (uint32_t si = 0; si < as; ++si)
             {
@@ -550,7 +549,7 @@ __global__ void __launch_bounds__(K4_WARPS * 32) k4_fill_kernel(k4_args A, const
             const uint32_t call_id = id_of_code(call_code);
             if (call_id > 4u)
             {
-                atomicOr(status, ST_BASE);
+                atomicOr(status, SX_ST_BASE);
                 continue;
             }
             uint32_t qscore = ql[p];
@@ -558,7 +557,7 @@ __global__ void __launch_bounds__(K4_WARPS * 32) k4_fill_kernel(k4_args A, const
             {
                 if (qscore > SX_MAX_QSCORE)
                 {
-                    atomicOr(status, ST_QUAL);
+                    atomicOr(status, SX_ST_QUAL);
                     continue;
                 }
                 qscore = mqrow[qscore];
@@ -588,15 +587,6 @@ __global__ void __launch_bounds__(K4_WARPS * 32) k4_fill_kernel(k4_args A, const
     }
 }
 
-int upload(sx_ctx* ctx, int slot, const void* src, size_t bytes, const void** dst, cudaStream_t st)
-{
-    void* p = nullptr;
-    int rc = sx_ensure(ctx, slot, bytes + 64, &p);
-    if (rc) return rc;
-    if (bytes) SX_CUDA(ctx, cudaMemcpyAsync(p, src, bytes, cudaMemcpyHostToDevice, st));
-    *dst = p;
-    return SX_OK;
-}
 } // namespace
 
 extern "C" void sx_default_pileup_opts(sx_pileup_opts* o)
@@ -661,11 +651,11 @@ int sx_k4_run(sx_ctx* ctx, const sx_pileup_reads_batch* d, const sx_pileup_colum
     int *s1 = nullptr, *s2 = nullptr, *b1 = nullptr, *b2 = nullptr, *tile_sums = nullptr;
     int rc;
     const uint32_t tiles = (n_sites + 1 + SCAN_TILE - 1) / SCAN_TILE;
-    if ((rc = sx_ensure(ctx, 26, (size_t)(n_sites + 1) * 8 + 64, reinterpret_cast<void**>(&s1)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K4_SCAN_S, (size_t)(n_sites + 1) * 2, s1, 64))) return rc;
     s2 = s1 + (n_sites + 1);
-    if ((rc = sx_ensure(ctx, 64, (size_t)(n_sites + 1) * 8 + 64, reinterpret_cast<void**>(&b1)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K4_SCAN_B, (size_t)(n_sites + 1) * 2, b1, 64))) return rc;
     b2 = b1 + (n_sites + 1);
-    if ((rc = sx_ensure(ctx, 27, (size_t)tiles * 8 * sizeof(int) + 64, reinterpret_cast<void**>(&tile_sums)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K4_TILE_SUMS, (size_t)tiles * 8, tile_sums, 64))) return rc;
     SX_CUDA(ctx, cudaMemsetAsync(d1, 0, (size_t)(n_sites + 1) * 4, st));
     SX_CUDA(ctx, cudaMemsetAsync(d2, 0, (size_t)(n_sites + 1) * 4, st));
     SX_CUDA(ctx, cudaMemsetAsync(dsd, 0, (size_t)n_sites * 4, st));
@@ -753,36 +743,31 @@ extern "C" int sx_pileup_reads(sx_ctx* ctx, const sx_pileup_reads_batch* b, sx_p
     sx_pileup_reads_batch d = *b;
     int rc;
     const sx_pileup_read& end = b->reads[b->n_reads];
-    if ((rc = upload(ctx, 0, b->reads, (size_t)(b->n_reads + 1) * sizeof(sx_pileup_read), reinterpret_cast<const void**>(&d.reads), st))) return rc;
-    if ((rc = upload(ctx, 1, b->seq4, end.seq_off, reinterpret_cast<const void**>(&d.seq4), st))) return rc;
-    if ((rc = upload(ctx, 2, b->qual, end.qual_off, reinterpret_cast<const void**>(&d.qual), st))) return rc;
-    if ((rc = upload(ctx, 3, b->segs, (size_t)b->n_segs * sizeof(sx_aln_seg), reinterpret_cast<const void**>(&d.segs), st))) return rc;
-    if ((rc = upload(ctx, 4, b->ref, b->ref_len, reinterpret_cast<const void**>(&d.ref), st))) return rc;
-    if ((rc = upload(ctx, 5, b->cand_snv, (size_t)b->n_cand_snv * 4, reinterpret_cast<const void**>(&d.cand_snv), st))) return rc;
-    if (b->buffer_pos && (rc = upload(ctx, 9, b->buffer_pos, (size_t)b->n_reads * 4, reinterpret_cast<const void**>(&d.buffer_pos), st))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(0), b->reads, (size_t)(b->n_reads + 1), d.reads, 64))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(1), b->seq4, end.seq_off, d.seq4, 64))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(2), b->qual, end.qual_off, d.qual, 64))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(3), b->segs, b->n_segs, d.segs, 64))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(4), b->ref, b->ref_len, d.ref, 64))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(5), b->cand_snv, b->n_cand_snv, d.cand_snv, 64))) return rc;
+    if (b->buffer_pos && (rc = sx_upload(ctx, sx_host_slot(9), b->buffer_pos, b->n_reads, d.buffer_pos, 64))) return rc;
     sx_pileup_columns dc = *out;
-    void* p = nullptr;
-    if ((rc = sx_ensure(ctx, 6, (size_t)(n_sites + 1) * 4 * 4 + 64, &p))) return rc;
-    dc.site_off = static_cast<uint32_t*>(p);
+    if ((rc = sx_take(ctx, sx_host_slot(6), (size_t)(n_sites + 1) * 4, dc.site_off, 64))) return rc;
     dc.t2_off = dc.site_off + (n_sites + 1);
     dc.n_spandel = dc.t2_off + (n_sites + 1);
     dc.n_submapped = dc.n_spandel + (n_sites + 1);
-    if ((rc = sx_ensure(ctx, 7, (size_t)out->calls_capacity * 2 + 64, &p))) return rc;
-    dc.calls = static_cast<uint16_t*>(p);
-    if ((rc = sx_ensure(ctx, 8, (size_t)out->t2_capacity * 2 + 64, &p))) return rc;
-    dc.t2_calls = static_cast<uint16_t*>(p);
-    rc = sx_pileup_reads_dev(ctx, &d, &dc);
-    if (rc && rc != SX_ERR_NOMEM) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(7), out->calls_capacity, dc.calls, 64))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(8), out->t2_capacity, dc.t2_calls, 64))) return rc;
+    const int rc_dev = sx_pileup_reads_dev(ctx, &d, &dc);
+    if (rc_dev && rc_dev != SX_ERR_NOMEM) return rc_dev;
     // offsets and counts are valid even when a capacity was too small (the caller can size and retry)
-    SX_CUDA(ctx, cudaMemcpyAsync(out->site_off, dc.site_off, (size_t)(n_sites + 1) * 4, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaMemcpyAsync(out->t2_off, dc.t2_off, (size_t)(n_sites + 1) * 4, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaMemcpyAsync(out->n_spandel, dc.n_spandel, (size_t)n_sites * 4, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaMemcpyAsync(out->n_submapped, dc.n_submapped, (size_t)n_sites * 4, cudaMemcpyDeviceToHost, st));
+    if ((rc = sx_download(ctx, out->site_off, dc.site_off, (size_t)n_sites + 1))) return rc;
+    if ((rc = sx_download(ctx, out->t2_off, dc.t2_off, (size_t)n_sites + 1))) return rc;
+    if ((rc = sx_download(ctx, out->n_spandel, dc.n_spandel, n_sites))) return rc;
+    if ((rc = sx_download(ctx, out->n_submapped, dc.n_submapped, n_sites))) return rc;
     SX_CUDA(ctx, cudaStreamSynchronize(st));
-    if (rc) return rc;
-    const uint32_t n1 = out->site_off[n_sites], n2 = out->t2_off[n_sites];
-    if (n1) SX_CUDA(ctx, cudaMemcpyAsync(out->calls, dc.calls, (size_t)n1 * 2, cudaMemcpyDeviceToHost, st));
-    if (n2) SX_CUDA(ctx, cudaMemcpyAsync(out->t2_calls, dc.t2_calls, (size_t)n2 * 2, cudaMemcpyDeviceToHost, st));
+    if (rc_dev) return rc_dev;
+    if ((rc = sx_download(ctx, out->calls, dc.calls, out->site_off[n_sites]))) return rc;
+    if ((rc = sx_download(ctx, out->t2_calls, dc.t2_calls, out->t2_off[n_sites]))) return rc;
     SX_CUDA(ctx, cudaStreamSynchronize(st));
     return SX_OK;
 }

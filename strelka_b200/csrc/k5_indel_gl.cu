@@ -57,7 +57,7 @@ __global__ void __launch_bounds__(K5_WARPS * 32) k5_indel_gl_kernel(const uint32
         const uint32_t pl = ploidy[l];
         if (A < 1 || A > SX_INDEL_MAX_ALLELES || (pl != 1 && pl != 2))
         {
-            if (lane == 0) atomicOr(status, 32);
+            if (lane == 0) atomicOr(status, SX_ST_INDEL_ALLELES);
             continue;
         }
         const uint32_t nfull = A + 1;
@@ -239,36 +239,24 @@ extern "C" int sx_indel_gl(sx_ctx* ctx, const sx_indel_batch* b, sx_indel_result
     if (!b || !out_host || !b->read_off || !b->lnp_off || !b->allele_off || !b->ploidy) return sx_fail(ctx, SX_ERR_ARG, "sx_indel_gl: NULL argument");
     if (b->n_loci == 0) return SX_OK;
     SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_a, ctx->s_compute));
+    sx_call_timer t(ctx);
     sx_indel_batch d = *b;
-    void* p = nullptr;
     int rc;
-    const size_t n_reads = b->read_off[b->n_loci], n_lnp = b->lnp_off[b->n_loci], n_al = b->allele_off[b->n_loci];
-#define SX_UP(slot, field, type, bytes)                                                        \
-    if ((rc = sx_ensure(ctx, slot, (bytes) + 16, &p))) return rc;                                \
-    SX_CUDA(ctx, cudaMemcpyAsync(p, b->field, (bytes), cudaMemcpyHostToDevice, ctx->s_compute)); \
-    d.field = static_cast<type>(p);
-    SX_UP(0, read_off, const uint32_t*, (size_t)(b->n_loci + 1) * 4)
-    SX_UP(1, lnp_off, const uint32_t*, (size_t)(b->n_loci + 1) * 4)
-    SX_UP(2, allele_off, const uint32_t*, (size_t)(b->n_loci + 1) * 4)
-    SX_UP(3, ploidy, const uint8_t*, (size_t)b->n_loci)
-    SX_UP(4, allele_del_len, const uint16_t*, n_al * 2)
-    SX_UP(5, allele_ins_len, const uint16_t*, n_al * 2)
-    SX_UP(6, allele_lnp, const float*, n_lnp * 4)
-    SX_UP(7, read_length, const uint16_t*, n_reads * 2)
-    SX_UP(8, non_ambig, const uint16_t*, n_reads * 2)
-    SX_UP(9, is_fwd, const uint8_t*, n_reads)
-#undef SX_UP
+    const size_t n_loci = b->n_loci, n_reads = b->read_off[b->n_loci], n_lnp = b->lnp_off[b->n_loci], n_al = b->allele_off[b->n_loci];
+    if ((rc = sx_upload(ctx, sx_host_slot(0), b->read_off, n_loci + 1, d.read_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(1), b->lnp_off, n_loci + 1, d.lnp_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(2), b->allele_off, n_loci + 1, d.allele_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(3), b->ploidy, n_loci, d.ploidy, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(4), b->allele_del_len, n_al, d.allele_del_len, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(5), b->allele_ins_len, n_al, d.allele_ins_len, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(6), b->allele_lnp, n_lnp, d.allele_lnp, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(7), b->read_length, n_reads, d.read_length, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(8), b->non_ambig, n_reads, d.non_ambig, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(9), b->is_fwd, n_reads, d.is_fwd, 16))) return rc;
     sx_indel_result* d_out = nullptr;
-    if ((rc = sx_ensure(ctx, 10, (size_t)b->n_loci * sizeof(sx_indel_result), reinterpret_cast<void**>(&d_out)))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(10), n_loci, d_out, 0))) return rc;
     if ((rc = k5_run(ctx, &d, d_out))) return rc;
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host, d_out, (size_t)b->n_loci * sizeof(sx_indel_result), cudaMemcpyDeviceToHost, ctx->s_compute));
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_b, ctx->s_compute));
-    SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
-    float ms = 0;
-    cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b);
-    ctx->timing.kernel_ms = ms;
-    ctx->timing.launches = 1;
-    ctx->total_launches += 1;
+    if ((rc = sx_download(ctx, out_host, d_out, n_loci))) return rc;
+    if ((rc = t.finish(1))) return rc;
     return sx_check_status(ctx, "sx_indel_gl");
 }

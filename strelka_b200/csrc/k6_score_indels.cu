@@ -24,6 +24,9 @@ namespace
 {
 constexpr int K6_THREADS = 128;
 constexpr int K6_ST_SHIFT = 9; // K6_ST_* bits are reported as ctx status bits 512, 1024, ...
+static_assert((K6_ST_SEGKIND << K6_ST_SHIFT) == SX_ST_K6_SEG_KIND && (K6_ST_LIMIT_A << K6_ST_SHIFT) == SX_ST_K6_ALNS && (K6_ST_LIMIT_E << K6_ST_SHIFT) == SX_ST_K6_EVAL &&
+                  (K6_ST_RECCAP << K6_ST_SHIFT) == SX_ST_K6_REC_CAP && (K6_ST_BADKEY << K6_ST_SHIFT) == SX_ST_K6_KEY,
+              "K6's shifted status bits are the context's");
 
 // sizes the launch needs: out[0] = max alignments of a read, out[1] = max output slots of a read; and the dense list of the reads that
 // HAVE candidate alignments -- out[2] = their count --, in read order within a warp's 32
@@ -111,10 +114,10 @@ int k6_run(sx_ctx* ctx, const sx_score_indels_batch* d, const double* lnp_dev, c
     // sizes of the launch: the deepest read of the batch decides the scratch
     uint32_t* d_max(nullptr);
     int rc;
-    if ((rc = sx_ensure(ctx, 29, 32, reinterpret_cast<void**>(&d_max)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K6_MAX, 8, d_max, 0))) return rc;
     SX_CUDA(ctx, cudaMemsetAsync(d_max, 0, 12, st));
     uint32_t* list(nullptr);
-    if ((rc = sx_ensure(ctx, 69, (size_t)d->n_reads * 4 + 16, reinterpret_cast<void**>(&list)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K6_LIST, d->n_reads, list, 16))) return rc;
     const int grid0(std::max(1, std::min<int>((int)((d->n_reads + 255) / 256), ctx->sm_count * 8)));
     k6_max_kernel<<<grid0, 256, 0, st>>>(*d, d_max, list);
     SX_CUDA(ctx, cudaGetLastError());
@@ -134,7 +137,7 @@ int k6_run(sx_ctx* ctx, const sx_score_indels_batch* d, const double* lnp_dev, c
     while (T > (size_t)threads && k6_plan(maxA, maxE, T).bytes > arena_cap) T = ((T / 2 + threads - 1) / threads) * threads;
     const k6_layout L(k6_plan(maxA, maxE, T));
     char* arena(nullptr);
-    if ((rc = sx_ensure(ctx, 28, L.bytes, reinterpret_cast<void**>(&arena)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K6_ARENA, L.bytes, arena, 0))) return rc;
     k6_scratch S;
     S.ord = {reinterpret_cast<uint32_t*>(arena + L.off[0]), T};
     S.smooth = {reinterpret_cast<double*>(arena + L.off[1]), T};
@@ -166,9 +169,9 @@ int k6_run(sx_ctx* ctx, const sx_score_indels_batch* d, const double* lnp_dev, c
         // window entries they carry, so warps of reads with equally many alignments stay together
         uint8_t* cls(nullptr);
         uint32_t *hist(nullptr), *list2(nullptr);
-        if ((rc = sx_ensure(ctx, 35, (size_t)d->n_reads + 16, reinterpret_cast<void**>(&cls)))) return rc;
-        if ((rc = sx_ensure(ctx, 36, (size_t)SX_RG_CLASSES * 4 + 16, reinterpret_cast<void**>(&hist)))) return rc;
-        if ((rc = sx_ensure(ctx, 37, (size_t)d->n_reads * 4 + 16, reinterpret_cast<void**>(&list2)))) return rc;
+        if ((rc = sx_take(ctx, SX_SLOT_K6_CLASS, d->n_reads, cls, 16))) return rc;
+        if ((rc = sx_take(ctx, SX_SLOT_K6_HIST, SX_RG_CLASSES, hist, 16))) return rc;
+        if ((rc = sx_take(ctx, SX_SLOT_K6_LIST_BY_CLASS, d->n_reads, list2, 16))) return rc;
         SX_CUDA(ctx, cudaMemsetAsync(hist, 0, (size_t)SX_RG_CLASSES * 4, st));
         const int gc(std::max(1, std::min<int>((int)((d->n_reads + SX_RG_THREADS * SX_RG_ITEMS - 1) / (SX_RG_THREADS * SX_RG_ITEMS)), ctx->sm_count * 8)));
         sx_regroup_class_by_count_kernel<<<gc, SX_RG_THREADS, 0, st>>>(d->aln_off, list, d_max + 2, cls, hist);
@@ -238,59 +241,39 @@ extern "C" int sx_score_indels(sx_ctx* ctx, const sx_score_indels_batch* b, cons
     for (uint32_t k = 0; k < b->n_keys; ++k)
         if (b->keys[k].type > SX_INDEL_TYPE_MISMATCH) return sx_fail(ctx, SX_ERR_UNSUPPORTED, "sx_score_indels: breakend entries are not supported");
     SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    cudaStream_t st(ctx->s_compute);
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_a, st));
+    sx_call_timer t(ctx);
     sx_score_indels_batch d(*b);
-    void* p(nullptr);
-    const size_t n_segs(b->aln_seg_off[b->n_alns]), n_akeys(b->aln_key_off[b->n_alns]), n_slots(b->rec_off[b->n_reads]);
-#define SX_UP(slot, field, type, bytes)                                                     \
-    if ((rc = sx_ensure(ctx, slot, (size_t)(bytes) + 16, &p))) return rc;                    \
-    if (bytes) SX_CUDA(ctx, cudaMemcpyAsync(p, b->field, (bytes), cudaMemcpyHostToDevice, st)); \
-    d.field = static_cast<type>(p);
-    SX_UP(0, region_read_off, const uint32_t*, (size_t)(b->n_regions + 1) * 4)
-    SX_UP(1, region_key_off, const uint32_t*, (size_t)(b->n_regions + 1) * 4)
-    SX_UP(2, keys, const sx_indel_key*, (size_t)b->n_keys * sizeof(sx_indel_key))
-    SX_UP(3, aln_off, const uint32_t*, (size_t)(b->n_reads + 1) * 4)
-    SX_UP(4, aln_pos, const int32_t*, (size_t)b->n_alns * 4)
-    SX_UP(5, aln_seg_off, const uint32_t*, (size_t)(b->n_alns + 1) * 4)
-    SX_UP(6, segs, const sx_aln_seg*, n_segs * sizeof(sx_aln_seg))
-    SX_UP(7, aln_key_off, const uint32_t*, (size_t)(b->n_alns + 1) * 4)
-    SX_UP(8, aln_keys, const uint16_t*, n_akeys * 2)
-    SX_UP(9, read_len, const uint16_t*, (size_t)b->n_reads * 2)
-    SX_UP(10, non_ambig, const uint16_t*, (size_t)b->n_reads * 2)
-    SX_UP(11, read_flags, const uint8_t*, (size_t)b->n_reads)
-    SX_UP(12, rec_off, const uint32_t*, (size_t)(b->n_reads + 1) * 4)
-    if (b->full_len)
-    {
-        SX_UP(13, full_len, const uint16_t*, (size_t)b->n_reads * 2)
-    }
-    if (b->full_off)
-    {
-        SX_UP(14, full_off, const uint16_t*, (size_t)b->n_reads * 2)
-    }
-#undef SX_UP
-    double* d_lnp(nullptr);
-    if ((rc = sx_ensure(ctx, 15, (size_t)b->n_alns * 8 + 16, reinterpret_cast<void**>(&d_lnp)))) return rc;
-    SX_CUDA(ctx, cudaMemcpyAsync(d_lnp, lnp_host, (size_t)b->n_alns * 8, cudaMemcpyHostToDevice, st));
+    const size_t n(b->n_reads), n_segs(b->aln_seg_off[b->n_alns]), n_akeys(b->aln_key_off[b->n_alns]), n_slots(b->rec_off[b->n_reads]);
+    if ((rc = sx_upload(ctx, sx_host_slot(0), b->region_read_off, (size_t)b->n_regions + 1, d.region_read_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(1), b->region_key_off, (size_t)b->n_regions + 1, d.region_key_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(2), b->keys, b->n_keys, d.keys, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(3), b->aln_off, n + 1, d.aln_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(4), b->aln_pos, b->n_alns, d.aln_pos, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(5), b->aln_seg_off, (size_t)b->n_alns + 1, d.aln_seg_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(6), b->segs, n_segs, d.segs, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(7), b->aln_key_off, (size_t)b->n_alns + 1, d.aln_key_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(8), b->aln_keys, n_akeys, d.aln_keys, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(9), b->read_len, n, d.read_len, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(10), b->non_ambig, n, d.non_ambig, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(11), b->read_flags, n, d.read_flags, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(12), b->rec_off, n + 1, d.rec_off, 16))) return rc;
+    if (b->full_len && (rc = sx_upload(ctx, sx_host_slot(13), b->full_len, n, d.full_len, 16))) return rc;
+    if (b->full_off && (rc = sx_upload(ctx, sx_host_slot(14), b->full_off, n, d.full_off, 16))) return rc;
+    const double* d_lnp(nullptr);
+    if ((rc = sx_upload(ctx, sx_host_slot(15), lnp_host, b->n_alns, d_lnp, 16))) return rc;
     sx_score_indels_out o;
-    if ((rc = sx_ensure(ctx, 16, (n_slots + 1) * sizeof(sx_read_indel_score), reinterpret_cast<void**>(&o.recs)))) return rc;
-    if ((rc = sx_ensure(ctx, 17, (size_t)b->n_reads * 4, reinterpret_cast<void**>(&o.n_rec)))) return rc;
-    if ((rc = sx_ensure(ctx, 18, (size_t)b->n_reads * 4, reinterpret_cast<void**>(&o.max_aln)))) return rc;
-    if ((rc = sx_ensure(ctx, 19, (size_t)b->n_reads * 4, reinterpret_cast<void**>(&o.eval_aln)))) return rc;
-    SX_CUDA(ctx, cudaMemsetAsync(o.recs, 0, (n_slots + 1) * sizeof(sx_read_indel_score), st)); // unused slots read back as zeros
+    if ((rc = sx_take(ctx, sx_host_slot(16), n_slots + 1, o.recs, 0))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(17), n, o.n_rec, 0))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(18), n, o.max_aln, 0))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(19), n, o.eval_aln, 0))) return rc;
+    SX_CUDA(ctx, cudaMemsetAsync(o.recs, 0, (n_slots + 1) * sizeof(sx_read_indel_score), ctx->s_compute)); // unused slots read back as zeros
     unsigned launches(0);
     if ((rc = k6_run(ctx, &d, d_lnp, &o, &launches))) return rc;
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host->recs, o.recs, n_slots * sizeof(sx_read_indel_score), cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host->n_rec, o.n_rec, (size_t)b->n_reads * 4, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host->max_aln, o.max_aln, (size_t)b->n_reads * 4, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host->eval_aln, o.eval_aln, (size_t)b->n_reads * 4, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_b, st));
-    SX_CUDA(ctx, cudaStreamSynchronize(st));
-    float ms(0);
-    cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b);
-    ctx->timing.kernel_ms = ms;
-    ctx->timing.launches = launches;
-    ctx->total_launches += launches;
+    if ((rc = sx_download(ctx, out_host->recs, o.recs, n_slots))) return rc;
+    if ((rc = sx_download(ctx, out_host->n_rec, o.n_rec, n))) return rc;
+    if ((rc = sx_download(ctx, out_host->max_aln, o.max_aln, n))) return rc;
+    if ((rc = sx_download(ctx, out_host->eval_aln, o.eval_aln, n))) return rc;
+    if ((rc = t.finish(launches))) return rc;
     return sx_check_status(ctx, "sx_score_indels");
 }
 

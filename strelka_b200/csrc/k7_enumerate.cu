@@ -28,7 +28,6 @@
 namespace
 {
 constexpr int K7_THREADS = 64;
-constexpr int K7_ST_SHIFT = 14; // device status bit 16384: an output capacity is too small (reported as SX_ERR_CAPACITY by the host)
 
 struct k7_counts // per read, then (after the scan) its exclusive offsets
 {
@@ -106,7 +105,7 @@ __global__ void __launch_bounds__(K7_SCAN_THREADS) k7_scan_finish(const uint32_t
         o.totals[0] = totals[0];
         o.totals[1] = totals[1];
         o.totals[2] = totals[2];
-        if (totals[0] > o.cap_alns || totals[1] > o.cap_segs || totals[2] > o.cap_keys) atomicOr(status, 1 << K7_ST_SHIFT);
+        if (totals[0] > o.cap_alns || totals[1] > o.cap_segs || totals[2] > o.cap_keys) atomicOr(status, SX_ST_K7_CAP);
         else
         {
             o.aln_seg_off[totals[0]] = totals[1];
@@ -354,7 +353,7 @@ int k7_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsigned* 
     const uint32_t maxA(d->opts.max_alns_per_read ? std::min<uint32_t>(d->opts.max_alns_per_read, 65535u) : 64u);
     int rc;
     uint32_t* read_region(nullptr);
-    if ((rc = sx_ensure(ctx, 41, (size_t)n * 4 + 32, reinterpret_cast<void**>(&read_region)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7_READ_REGION, n, read_region, 32))) return rc;
     uint32_t maxF(K7_MAX_INDELS + 1);
     if ((rc = k7_frames_needed(ctx, d, read_region, read_region + n + 1, &maxF))) return rc; // (also fills read_region)
     const size_t per_thread((k7_scratch_bytes(maxA, maxF) + 255) & ~(size_t)255);
@@ -365,14 +364,14 @@ int k7_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsigned* 
     const size_t arena_cap((size_t)4 << 30);
     while (blocks > 1 && blocks * K7_THREADS * per_thread > arena_cap) blocks = (blocks + 1) / 2;
     unsigned char* arena(nullptr);
-    if ((rc = sx_ensure(ctx, 40, blocks * K7_THREADS * per_thread, reinterpret_cast<void**>(&arena)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7_ARENA, blocks * K7_THREADS * per_thread, arena, 0))) return rc;
     k7_counts c;
-    if ((rc = sx_ensure(ctx, 42, (size_t)n * 4 + 16, reinterpret_cast<void**>(&c.aln)))) return rc;
-    if ((rc = sx_ensure(ctx, 43, (size_t)n * 4 + 16, reinterpret_cast<void**>(&c.seg)))) return rc;
-    if ((rc = sx_ensure(ctx, 44, (size_t)n * 4 + 16, reinterpret_cast<void**>(&c.key)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7_CNT_ALN, n, c.aln, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7_CNT_SEG, n, c.seg, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7_CNT_KEY, n, c.key, 16))) return rc;
     const uint32_t tile(K7_SCAN_THREADS * K7_SCAN_ITEMS), n_tiles((n + tile - 1) / tile);
     uint32_t* sums(nullptr);
-    if ((rc = sx_ensure(ctx, 45, ((size_t)3 * n_tiles + 4) * 4, reinterpret_cast<void**>(&sums)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7_SUMS, (size_t)3 * n_tiles + 4, sums, 0))) return rc;
     uint32_t* totals(sums + (size_t)3 * n_tiles);
 
     k7_view v;
@@ -398,7 +397,7 @@ int k7_run_fast(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsig
     const uint32_t maxA(d->opts.max_alns_per_read ? std::min<uint32_t>(d->opts.max_alns_per_read, 65535u) : 64u);
     int rc;
     uint32_t* read_region(nullptr);
-    if ((rc = sx_ensure(ctx, 41, (size_t)n * 4 + 32, reinterpret_cast<void**>(&read_region)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7_READ_REGION, n, read_region, 32))) return rc;
     uint32_t maxF(K7_MAX_INDELS + 1);
     if ((rc = k7_frames_needed(ctx, d, read_region, read_region + n + 1, &maxF))) return rc; // (also fills read_region)
     const size_t per_thread((k7_scratch_bytes(maxA, maxF) + 255) & ~(size_t)255);
@@ -420,34 +419,34 @@ int k7_run_fast(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsig
     size_t blocks(std::min<size_t>(n_blocks, std::max<size_t>(1, (size_t)ctx->sm_count * per_sm / 4)));
     while (blocks > 1 && blocks * K7_THREADS * per_thread > arena_cap) blocks = (blocks + 1) / 2;
     unsigned char *arena(nullptr), *arena1(nullptr);
-    if ((rc = sx_ensure(ctx, 40, blocks1 * K7_THREADS * per_thread1, reinterpret_cast<void**>(&arena1)))) return rc;
-    if (two_levels && (rc = sx_ensure(ctx, 65, blocks * K7_THREADS * per_thread, reinterpret_cast<void**>(&arena)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7_ARENA, blocks1 * K7_THREADS * per_thread1, arena1, 0))) return rc;
+    if (two_levels && (rc = sx_take(ctx, SX_SLOT_K7_ARENA_DEEP, blocks * K7_THREADS * per_thread, arena, 0))) return rc;
     k7_counts c;
-    if ((rc = sx_ensure(ctx, 42, (size_t)n * 4 + 16, reinterpret_cast<void**>(&c.aln)))) return rc;
-    if ((rc = sx_ensure(ctx, 43, (size_t)n * 4 + 16, reinterpret_cast<void**>(&c.seg)))) return rc;
-    if ((rc = sx_ensure(ctx, 44, (size_t)n * 4 + 16, reinterpret_cast<void**>(&c.key)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7_CNT_ALN, n, c.aln, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7_CNT_SEG, n, c.seg, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7_CNT_KEY, n, c.key, 16))) return rc;
     const uint32_t tile(K7_SCAN_THREADS * K7_SCAN_ITEMS), n_tiles((n + tile - 1) / tile);
     uint32_t* sums(nullptr);
-    if ((rc = sx_ensure(ctx, 45, ((size_t)3 * n_tiles + 4) * 4, reinterpret_cast<void**>(&sums)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7_SUMS, (size_t)3 * n_tiles + 4, sums, 0))) return rc;
     uint32_t* totals(sums + (size_t)3 * n_tiles);
     // the log holds whatever the output arrays can hold: 3 words + segments + ceil(keys / 2) words per alignment
     const unsigned long long want_words((unsigned long long)o->cap_alns * 4ull + o->cap_segs + (o->cap_keys + 1ull) / 2ull + 16ull);
     k7_log L;
     L.cap = (uint32_t)std::min<unsigned long long>(want_words, 0xFFFFFFF0ull);
     k7_retry R;
-    if ((rc = sx_ensure(ctx, 54, (size_t)L.cap * 4 + 16, reinterpret_cast<void**>(&L.words)))) return rc;
-    if ((rc = sx_ensure(ctx, 55, (size_t)n * 4 + 16, reinterpret_cast<void**>(&L.blob_off)))) return rc;
-    if ((rc = sx_ensure(ctx, 56, 16, reinterpret_cast<void**>(&L.cursor)))) return rc;
-    if ((rc = sx_ensure(ctx, 57, (size_t)n * 4 + 16, reinterpret_cast<void**>(&R.list1)))) return rc;
-    if ((rc = sx_ensure(ctx, 66, (size_t)n * 4 + 16, reinterpret_cast<void**>(&R.list2)))) return rc;
-    if ((rc = sx_ensure(ctx, 67, 16, reinterpret_cast<void**>(&R.n)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7_LOG, L.cap, L.words, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7_LOG_OFF, n, L.blob_off, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7_LOG_CURSOR, 2, L.cursor, 0))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7_RETRY1, n, R.list1, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7_RETRY2, n, R.list2, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7_RETRY_N, 4, R.n, 0))) return rc;
     SX_CUDA(ctx, cudaMemsetAsync(L.cursor, 0, 16, st));
     SX_CUDA(ctx, cudaMemsetAsync(R.n, 0, 16, st));
     R.list0 = nullptr;
     unsigned extra(0);
     if (d->gate)
     {
-        if ((rc = sx_ensure(ctx, 68, (size_t)n * 4 + 16, reinterpret_cast<void**>(&R.list0)))) return rc;
+        if ((rc = sx_take(ctx, SX_SLOT_K7_ACTIVE, n, R.list0, 16))) return rc;
         SX_CUDA(ctx, cudaMemsetAsync(c.aln, 0, (size_t)n * 4, st));
         SX_CUDA(ctx, cudaMemsetAsync(c.seg, 0, (size_t)n * 4, st));
         SX_CUDA(ctx, cudaMemsetAsync(c.key, 0, (size_t)n * 4, st));
@@ -464,9 +463,9 @@ int k7_run_fast(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsig
         // the active list regrouped by shape class (see k7_read_class)
         uint8_t* cls(nullptr);
         uint32_t *hist(nullptr), *list0b(nullptr);
-        if ((rc = sx_ensure(ctx, 32, (size_t)n + 16, reinterpret_cast<void**>(&cls)))) return rc;
-        if ((rc = sx_ensure(ctx, 33, (size_t)K7_N_CLASS * 4 + 16, reinterpret_cast<void**>(&hist)))) return rc;
-        if ((rc = sx_ensure(ctx, 34, (size_t)n * 4 + 16, reinterpret_cast<void**>(&list0b)))) return rc;
+        if ((rc = sx_take(ctx, SX_SLOT_K7_CLASS, n, cls, 16))) return rc;
+        if ((rc = sx_take(ctx, SX_SLOT_K7_HIST, K7_N_CLASS, hist, 16))) return rc;
+        if ((rc = sx_take(ctx, SX_SLOT_K7_ACTIVE_BY_CLASS, n, list0b, 16))) return rc;
         SX_CUDA(ctx, cudaMemsetAsync(hist, 0, (size_t)K7_N_CLASS * 4, st));
         const int gc(std::max(1, std::min<int>((int)((n + K7_CLS_THREADS * K7_CLS_ITEMS - 1) / (K7_CLS_THREADS * K7_CLS_ITEMS)), ctx->sm_count * 8)));
         k7_class_count_kernel<<<gc, K7_CLS_THREADS, 0, st>>>(v, read_region, R.list0, R.n + 2, cls, hist);
@@ -517,21 +516,6 @@ int k7_check_args(sx_ctx* ctx, const sx_enum_batch* b, const sx_enum_out* o, con
     return SX_OK;
 }
 
-int k7_finish(sx_ctx* ctx, const char* what, const uint32_t* totals_host)
-{
-    int st(0);
-    SX_CUDA(ctx, cudaMemcpyAsync(&st, ctx->d_status, sizeof(int), cudaMemcpyDeviceToHost, ctx->s_compute));
-    SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
-    if (st & (1 << K7_ST_SHIFT))
-    {
-        cudaMemsetAsync(ctx->d_status, 0, sizeof(int), ctx->s_compute);
-        if (totals_host)
-            return sx_fail(ctx, SX_ERR_CAPACITY, "%s: output capacity too small: the batch produces %u alignments, %u segments, %u keys", what, totals_host[0],
-                           totals_host[1], totals_host[2]);
-        return sx_fail(ctx, SX_ERR_CAPACITY, "%s: output capacity too small (totals[] holds the needed sizes)", what);
-    }
-    return sx_check_status(ctx, what);
-}
 } // namespace
 
 extern "C" void sx_default_enum_opts(sx_enum_opts* o)
@@ -575,7 +559,7 @@ extern "C" int sx_enumerate_alignments_dev(sx_ctx* ctx, const sx_enum_batch* d, 
     if ((rc = (d->opts.flags & SX_ENUM_F_FAST) ? k7_run_fast(ctx, d, out_dev, &launches) : k7_run(ctx, d, out_dev, &launches))) return rc;
     t.stop(launches);
     if ((rc = t.finish())) return rc;
-    return k7_finish(ctx, "sx_enumerate_alignments", nullptr);
+    return sx_check_status(ctx, "sx_enumerate_alignments", SX_ST_K7_CAP);
 }
 
 extern "C" int sx_enumerate_alignments(sx_ctx* ctx, const sx_enum_batch* b, sx_enum_out* out_host)
@@ -597,76 +581,57 @@ extern "C" int sx_enumerate_alignments(sx_ctx* ctx, const sx_enum_batch* b, sx_e
     for (uint32_t k = 0; k < b->n_keys; ++k)
         if (b->keys[k].type > SX_INDEL_TYPE_MISMATCH) return sx_fail(ctx, SX_ERR_UNSUPPORTED, "sx_enumerate_alignments: breakend entries are not supported");
     SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    cudaStream_t st(ctx->s_compute);
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_a, st));
+    sx_call_timer t(ctx);
     sx_enum_batch d(*b);
-    void* p(nullptr);
-    const size_t n_segs(b->in_seg_off[b->n_reads]), n_ikeys(b->in_key_off[b->n_reads]), n_ukeys(b->use_key_off[b->n_reads]);
-#define SX_UP(slot, field, type, bytes)                                                        \
-    if ((rc = sx_ensure(ctx, slot, (size_t)(bytes) + 16, &p))) return rc;                       \
-    if (bytes) SX_CUDA(ctx, cudaMemcpyAsync(p, b->field, (bytes), cudaMemcpyHostToDevice, st)); \
-    d.field = static_cast<type>(p);
-    SX_UP(0, region_read_off, const uint32_t*, (size_t)(b->n_regions + 1) * 4)
-    SX_UP(1, region_key_off, const uint32_t*, (size_t)(b->n_regions + 1) * 4)
-    SX_UP(2, keys, const sx_indel_key*, (size_t)b->n_keys * sizeof(sx_indel_key))
-    if (b->key_hap)
-    {
-        SX_UP(3, key_hap, const sx_key_hap*, (size_t)b->n_keys * sizeof(sx_key_hap))
-    }
-    SX_UP(4, realign_begin, const int32_t*, (size_t)b->n_regions * 4)
-    SX_UP(5, realign_end, const int32_t*, (size_t)b->n_regions * 4)
-    SX_UP(6, in_pos, const int32_t*, (size_t)b->n_reads * 4)
-    SX_UP(7, in_seg_off, const uint32_t*, (size_t)(b->n_reads + 1) * 4)
-    SX_UP(8, in_segs, const sx_aln_seg*, n_segs * sizeof(sx_aln_seg))
-    SX_UP(9, in_key_off, const uint32_t*, (size_t)(b->n_reads + 1) * 4)
-    SX_UP(10, in_keys, const uint16_t*, n_ikeys * 2)
-    SX_UP(11, use_key_off, const uint32_t*, (size_t)(b->n_reads + 1) * 4)
-    SX_UP(12, use_keys, const uint16_t*, n_ukeys * 2)
-    SX_UP(13, in_lead_key, const uint16_t*, (size_t)b->n_reads * 2)
-    SX_UP(14, in_trail_key, const uint16_t*, (size_t)b->n_reads * 2)
-    SX_UP(15, read_len, const uint16_t*, (size_t)b->n_reads * 2)
-    if (b->gate)
-    {
-        SX_UP(26, gate, const uint8_t*, (size_t)b->n_reads)
-    }
-#undef SX_UP
+    const size_t n(b->n_reads), nr(b->n_regions), n_segs(b->in_seg_off[b->n_reads]), n_ikeys(b->in_key_off[b->n_reads]), n_ukeys(b->use_key_off[b->n_reads]);
+    if ((rc = sx_upload(ctx, sx_host_slot(0), b->region_read_off, nr + 1, d.region_read_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(1), b->region_key_off, nr + 1, d.region_key_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(2), b->keys, b->n_keys, d.keys, 16))) return rc;
+    if (b->key_hap && (rc = sx_upload(ctx, sx_host_slot(3), b->key_hap, b->n_keys, d.key_hap, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(4), b->realign_begin, nr, d.realign_begin, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(5), b->realign_end, nr, d.realign_end, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(6), b->in_pos, n, d.in_pos, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(7), b->in_seg_off, n + 1, d.in_seg_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(8), b->in_segs, n_segs, d.in_segs, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(9), b->in_key_off, n + 1, d.in_key_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(10), b->in_keys, n_ikeys, d.in_keys, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(11), b->use_key_off, n + 1, d.use_key_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(12), b->use_keys, n_ukeys, d.use_keys, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(13), b->in_lead_key, n, d.in_lead_key, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(14), b->in_trail_key, n, d.in_trail_key, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(15), b->read_len, n, d.read_len, 16))) return rc;
+    if (b->gate && (rc = sx_upload(ctx, sx_host_slot(26), b->gate, n, d.gate, 16))) return rc;
     sx_enum_out o(*out_host);
-    if ((rc = sx_ensure(ctx, 16, 16, reinterpret_cast<void**>(&o.totals)))) return rc;
-    if ((rc = sx_ensure(ctx, 17, (size_t)(b->n_reads + 1) * 4, reinterpret_cast<void**>(&o.aln_off)))) return rc;
-    if ((rc = sx_ensure(ctx, 18, (size_t)b->n_reads + 16, reinterpret_cast<void**>(&o.status)))) return rc;
-    if ((rc = sx_ensure(ctx, 19, (size_t)o.cap_alns * 4 + 16, reinterpret_cast<void**>(&o.aln_pos)))) return rc;
-    if ((rc = sx_ensure(ctx, 20, ((size_t)o.cap_alns + 1) * 4 + 16, reinterpret_cast<void**>(&o.aln_seg_off)))) return rc;
-    if ((rc = sx_ensure(ctx, 21, (size_t)o.cap_segs * sizeof(sx_aln_seg) + 16, reinterpret_cast<void**>(&o.segs)))) return rc;
-    if ((rc = sx_ensure(ctx, 22, ((size_t)o.cap_alns + 1) * 4 + 16, reinterpret_cast<void**>(&o.aln_key_off)))) return rc;
-    if ((rc = sx_ensure(ctx, 23, (size_t)o.cap_keys * 2 + 16, reinterpret_cast<void**>(&o.aln_keys)))) return rc;
-    if ((rc = sx_ensure(ctx, 24, (size_t)o.cap_alns * 2 + 16, reinterpret_cast<void**>(&o.aln_lead_key)))) return rc;
-    if ((rc = sx_ensure(ctx, 25, (size_t)o.cap_alns * 2 + 16, reinterpret_cast<void**>(&o.aln_trail_key)))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(16), 4, o.totals, 0))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(17), n + 1, o.aln_off, 0))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(18), n, o.status, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(19), o.cap_alns, o.aln_pos, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(20), (size_t)o.cap_alns + 1, o.aln_seg_off, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(21), o.cap_segs, o.segs, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(22), (size_t)o.cap_alns + 1, o.aln_key_off, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(23), o.cap_keys, o.aln_keys, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(24), o.cap_alns, o.aln_lead_key, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(25), o.cap_alns, o.aln_trail_key, 16))) return rc;
     unsigned launches(0);
     if ((rc = (d.opts.flags & SX_ENUM_F_FAST) ? k7_run_fast(ctx, &d, &o, &launches) : k7_run(ctx, &d, &o, &launches))) return rc;
     // the totals decide how much comes back
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host->totals, o.totals, 12, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host->aln_off, o.aln_off, (size_t)(b->n_reads + 1) * 4, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host->status, o.status, (size_t)b->n_reads, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaStreamSynchronize(st));
+    if ((rc = sx_download(ctx, out_host->totals, o.totals, 3))) return rc;
+    if ((rc = sx_download(ctx, out_host->aln_off, o.aln_off, n + 1))) return rc;
+    if ((rc = sx_download(ctx, out_host->status, o.status, n))) return rc;
+    SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
     const uint32_t nA(out_host->totals[0]), nS(out_host->totals[1]), nK(out_host->totals[2]);
     if (nA <= o.cap_alns && nS <= o.cap_segs && nK <= o.cap_keys)
     {
-        SX_CUDA(ctx, cudaMemcpyAsync(out_host->aln_pos, o.aln_pos, (size_t)nA * 4, cudaMemcpyDeviceToHost, st));
-        SX_CUDA(ctx, cudaMemcpyAsync(out_host->aln_seg_off, o.aln_seg_off, ((size_t)nA + 1) * 4, cudaMemcpyDeviceToHost, st));
-        SX_CUDA(ctx, cudaMemcpyAsync(out_host->segs, o.segs, (size_t)nS * sizeof(sx_aln_seg), cudaMemcpyDeviceToHost, st));
-        SX_CUDA(ctx, cudaMemcpyAsync(out_host->aln_key_off, o.aln_key_off, ((size_t)nA + 1) * 4, cudaMemcpyDeviceToHost, st));
-        SX_CUDA(ctx, cudaMemcpyAsync(out_host->aln_keys, o.aln_keys, (size_t)nK * 2, cudaMemcpyDeviceToHost, st));
-        SX_CUDA(ctx, cudaMemcpyAsync(out_host->aln_lead_key, o.aln_lead_key, (size_t)nA * 2, cudaMemcpyDeviceToHost, st));
-        SX_CUDA(ctx, cudaMemcpyAsync(out_host->aln_trail_key, o.aln_trail_key, (size_t)nA * 2, cudaMemcpyDeviceToHost, st));
+        if ((rc = sx_download(ctx, out_host->aln_pos, o.aln_pos, nA))) return rc;
+        if ((rc = sx_download(ctx, out_host->aln_seg_off, o.aln_seg_off, (size_t)nA + 1))) return rc;
+        if ((rc = sx_download(ctx, out_host->segs, o.segs, nS))) return rc;
+        if ((rc = sx_download(ctx, out_host->aln_key_off, o.aln_key_off, (size_t)nA + 1))) return rc;
+        if ((rc = sx_download(ctx, out_host->aln_keys, o.aln_keys, nK))) return rc;
+        if ((rc = sx_download(ctx, out_host->aln_lead_key, o.aln_lead_key, nA))) return rc;
+        if ((rc = sx_download(ctx, out_host->aln_trail_key, o.aln_trail_key, nA))) return rc;
     }
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_b, st));
-    SX_CUDA(ctx, cudaStreamSynchronize(st));
-    float ms(0);
-    cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b);
-    ctx->timing.kernel_ms = ms;
-    ctx->timing.launches = launches;
-    ctx->total_launches += launches;
-    return k7_finish(ctx, "sx_enumerate_alignments", out_host->totals);
+    if ((rc = t.finish(launches))) return rc;
+    return sx_check_status(ctx, "sx_enumerate_alignments", SX_ST_K7_CAP, out_host->totals);
 }
 
 // asynchronous launcher for the device-resident pipeline (sx_pipeline.cu)

@@ -16,8 +16,6 @@
 
 namespace
 {
-constexpr int K7A_CAP_BIT = 1 << 18;
-
 // byte offset of every read's first packed base: reads of a region are back to back from its seq_off, each on a byte boundary
 __global__ void k7a_read_offsets_kernel(const k7a_view v, unsigned long long* __restrict__ read_byte, uint32_t* __restrict__ read_region)
 {
@@ -89,7 +87,7 @@ __global__ void __launch_bounds__(K7_SCAN_THREADS) k7a_finish_kernel(const uint3
     {
         o.in_key_off[n] = totals[0];
         o.totals[0] = totals[0];
-        if (totals[0] > o.cap_keys) atomicOr(status, K7A_CAP_BIT);
+        if (totals[0] > o.cap_keys) atomicOr(status, SX_ST_K7A_CAP);
     }
 }
 
@@ -140,13 +138,13 @@ int k7a_run(sx_ctx* ctx, const k7a_view& v, const sx_prep_out* o, unsigned* laun
     int rc;
     unsigned long long* read_byte(nullptr);
     uint32_t *read_region(nullptr), *cnt(nullptr), *z1(nullptr), *z2(nullptr), *sums(nullptr);
-    if ((rc = sx_ensure(ctx, 58, (size_t)n * 8 + 16, reinterpret_cast<void**>(&read_byte)))) return rc;
-    if ((rc = sx_ensure(ctx, 59, (size_t)n * 4 + 16, reinterpret_cast<void**>(&read_region)))) return rc;
-    if ((rc = sx_ensure(ctx, 60, (size_t)n * 4 + 16, reinterpret_cast<void**>(&cnt)))) return rc;
-    if ((rc = sx_ensure(ctx, 61, (size_t)n * 4 + 16, reinterpret_cast<void**>(&z1)))) return rc;
-    if ((rc = sx_ensure(ctx, 62, (size_t)n * 4 + 16, reinterpret_cast<void**>(&z2)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_READ_WORD, n, read_byte, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7A_READ_REGION, n, read_region, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_CNT, n, cnt, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_Z1, n, z1, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_Z2, n, z2, 16))) return rc;
     const uint32_t tile(K7_SCAN_THREADS * K7_SCAN_ITEMS), n_tiles((n + tile - 1) / tile);
-    if ((rc = sx_ensure(ctx, 63, ((size_t)3 * n_tiles + 4) * 4, reinterpret_cast<void**>(&sums)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_SUMS, (size_t)3 * n_tiles + 4, sums, 0))) return rc;
     uint32_t* totals(sums + (size_t)3 * n_tiles);
     const int cap(ctx->sm_count * 16);
     const auto grid = [cap](const uint32_t m) { return (unsigned)std::max(1, std::min<int>((int)((m + 127) / 128), cap)); };
@@ -155,10 +153,10 @@ int k7a_run(sx_ctx* ctx, const k7a_view& v, const sx_prep_out* o, unsigned* laun
     uint32_t *list(nullptr), *n_list(nullptr);
     uint16_t* stage(nullptr);
     unsigned extra(0);
-    if ((rc = sx_ensure(ctx, 39, (size_t)n * K7A_STAGE * 2 + 16, reinterpret_cast<void**>(&stage)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7A_STAGE, (size_t)n * K7A_STAGE, stage, 16))) return rc;
     if (v.b.gate)
     {
-        if ((rc = sx_ensure(ctx, 38, ((size_t)n + 4) * 4, reinterpret_cast<void**>(&list)))) return rc;
+        if ((rc = sx_take(ctx, SX_SLOT_K7A_ACTIVE, (size_t)n + 4, list, 0))) return rc;
         n_list = list + n;
         SX_CUDA(ctx, cudaMemsetAsync(n_list, 0, 4, st));
         SX_CUDA(ctx, cudaMemsetAsync(cnt, 0, (size_t)n * 4, st));
@@ -182,20 +180,6 @@ int k7a_run(sx_ctx* ctx, const k7a_view& v, const sx_prep_out* o, unsigned* laun
     SX_CUDA(ctx, cudaGetLastError());
     *launches = 6 + extra;
     return SX_OK;
-}
-
-int k7a_finish(sx_ctx* ctx, const char* what, const uint32_t* totals_host)
-{
-    int st(0);
-    SX_CUDA(ctx, cudaMemcpyAsync(&st, ctx->d_status, sizeof(int), cudaMemcpyDeviceToHost, ctx->s_compute));
-    SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
-    if (st & K7A_CAP_BIT)
-    {
-        cudaMemsetAsync(ctx->d_status, 0, sizeof(int), ctx->s_compute);
-        if (totals_host) return sx_fail(ctx, SX_ERR_CAPACITY, "%s: cap_keys too small: %u keys needed", what, totals_host[0]);
-        return sx_fail(ctx, SX_ERR_CAPACITY, "%s: cap_keys too small (totals[0] holds the needed size)", what);
-    }
-    return sx_check_status(ctx, what);
 }
 
 int k7a_check_args(sx_ctx* ctx, const sx_enum_batch* b, const sx_region* regions, const uint8_t* seq4, const char* ref, const uint32_t* key_ins_off, const char* key_ins,
@@ -251,46 +235,30 @@ extern "C" int sx_realign_gates(sx_ctx* ctx, const sx_gate_batch* b, sx_gate_out
     if ((rc = k7g_check_args(ctx, b, out_host, "sx_realign_gates"))) return rc;
     if (b->n_reads == 0) return SX_OK;
     SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    cudaStream_t st(ctx->s_compute);
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_a, st));
+    sx_call_timer t(ctx);
     sx_gate_batch d(*b);
-    void* p(nullptr);
-    const size_t n_segs(b->seg_off[b->n_reads]), n_win(b->region_key_off[b->n_regions]);
-#define SX_UPX(slot, dst, src, type, bytes)                                                \
-    if ((rc = sx_ensure(ctx, slot, (size_t)(bytes) + 16, &p))) return rc;                   \
-    if (bytes) SX_CUDA(ctx, cudaMemcpyAsync(p, (src), (bytes), cudaMemcpyHostToDevice, st)); \
-    dst = static_cast<type>(p);
-    SX_UPX(0, d.region_read_off, b->region_read_off, const uint32_t*, (size_t)(b->n_regions + 1) * 4)
-    SX_UPX(1, d.region_key_off, b->region_key_off, const uint32_t*, (size_t)(b->n_regions + 1) * 4)
-    SX_UPX(2, d.keys, b->keys, const sx_indel_key*, n_win * sizeof(sx_indel_key))
-    SX_UPX(3, d.realign_begin, b->realign_begin, const int32_t*, (size_t)b->n_regions * 4)
-    SX_UPX(4, d.realign_end, b->realign_end, const int32_t*, (size_t)b->n_regions * 4)
-    SX_UPX(5, d.raw_pos, b->raw_pos, const int32_t*, (size_t)b->n_reads * 4)
-    SX_UPX(6, d.seg_off, b->seg_off, const uint32_t*, (size_t)(b->n_reads + 1) * 4)
-    SX_UPX(7, d.raw_segs, b->raw_segs, const sx_aln_seg*, n_segs * sizeof(sx_aln_seg))
-    SX_UPX(8, d.read_len, b->read_len, const uint16_t*, (size_t)b->n_reads * 2)
-    if (b->pin_flags)
-    {
-        SX_UPX(9, d.pin_flags, b->pin_flags, const uint8_t*, (size_t)b->n_reads)
-    }
-#undef SX_UPX
+    const size_t n(b->n_reads), nr(b->n_regions), n_segs(b->seg_off[b->n_reads]), n_win(b->region_key_off[b->n_regions]);
+    if ((rc = sx_upload(ctx, sx_host_slot(0), b->region_read_off, nr + 1, d.region_read_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(1), b->region_key_off, nr + 1, d.region_key_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(2), b->keys, n_win, d.keys, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(3), b->realign_begin, nr, d.realign_begin, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(4), b->realign_end, nr, d.realign_end, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(5), b->raw_pos, n, d.raw_pos, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(6), b->seg_off, n + 1, d.seg_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(7), b->raw_segs, n_segs, d.raw_segs, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(8), b->read_len, n, d.read_len, 16))) return rc;
+    if (b->pin_flags && (rc = sx_upload(ctx, sx_host_slot(9), b->pin_flags, n, d.pin_flags, 16))) return rc;
     sx_gate_out o;
-    if ((rc = sx_ensure(ctx, 10, (size_t)b->n_reads + 16, reinterpret_cast<void**>(&o.gate)))) return rc;
-    if ((rc = sx_ensure(ctx, 11, (size_t)b->n_reads * 4 + 16, reinterpret_cast<void**>(&o.in_pos)))) return rc;
-    if ((rc = sx_ensure(ctx, 12, n_segs * sizeof(sx_aln_seg) + 16, reinterpret_cast<void**>(&o.in_segs)))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(10), n, o.gate, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(11), n, o.in_pos, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(12), n_segs, o.in_segs, 16))) return rc;
     const unsigned grid((unsigned)std::max(1, std::min<int>((int)((b->n_reads + 127) / 128), ctx->sm_count * 16)));
-    k7g_gates_kernel<<<grid, 128, 0, st>>>(d, o, nullptr);
+    k7g_gates_kernel<<<grid, 128, 0, ctx->s_compute>>>(d, o, nullptr);
     SX_CUDA(ctx, cudaGetLastError());
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host->gate, o.gate, (size_t)b->n_reads, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host->in_pos, o.in_pos, (size_t)b->n_reads * 4, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host->in_segs, o.in_segs, n_segs * sizeof(sx_aln_seg), cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_b, st));
-    SX_CUDA(ctx, cudaStreamSynchronize(st));
-    float ms(0);
-    cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b);
-    ctx->timing.kernel_ms = ms;
-    ctx->timing.launches = 1;
-    ctx->total_launches += 1;
+    if ((rc = sx_download(ctx, out_host->gate, o.gate, n))) return rc;
+    if ((rc = sx_download(ctx, out_host->in_pos, o.in_pos, n))) return rc;
+    if ((rc = sx_download(ctx, out_host->in_segs, o.in_segs, n_segs))) return rc;
+    if ((rc = t.finish(1))) return rc;
     return sx_check_status(ctx, "sx_realign_gates");
 }
 
@@ -321,7 +289,7 @@ extern "C" int sx_alignment_indels_dev(sx_ctx* ctx, const sx_enum_batch* d, cons
     if ((rc = k7a_run(ctx, v, out_dev, &launches))) return rc;
     t.stop(launches);
     if ((rc = t.finish())) return rc;
-    return k7a_finish(ctx, "sx_alignment_indels", nullptr);
+    return sx_check_status(ctx, "sx_alignment_indels", SX_ST_K7A_CAP);
 }
 
 extern "C" int sx_alignment_indels(sx_ctx* ctx, const sx_enum_batch* b, const sx_region* regions, const uint8_t* seq4, const char* ref, const uint32_t* key_ins_off,
@@ -338,57 +306,40 @@ extern "C" int sx_alignment_indels(sx_ctx* ctx, const sx_enum_batch* b, const sx
         return SX_OK;
     }
     SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    cudaStream_t st(ctx->s_compute);
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_a, st));
+    sx_call_timer t(ctx);
     k7a_view v;
     v.b = *b;
-    void* p(nullptr);
-    const size_t n_segs(b->in_seg_off[b->n_reads]);
+    const size_t n(b->n_reads), nr(b->n_regions), n_segs(b->in_seg_off[b->n_reads]);
     const sx_region& end(regions[b->n_regions]); // the sentinel carries the pool sizes
-#define SX_UPX(slot, dst, src, type, bytes)                                                \
-    if ((rc = sx_ensure(ctx, slot, (size_t)(bytes) + 16, &p))) return rc;                   \
-    if (bytes) SX_CUDA(ctx, cudaMemcpyAsync(p, (src), (bytes), cudaMemcpyHostToDevice, st)); \
-    dst = static_cast<type>(p);
-    SX_UPX(0, v.b.region_read_off, b->region_read_off, const uint32_t*, (size_t)(b->n_regions + 1) * 4)
-    SX_UPX(1, v.b.region_key_off, b->region_key_off, const uint32_t*, (size_t)(b->n_regions + 1) * 4)
-    SX_UPX(2, v.b.keys, b->keys, const sx_indel_key*, (size_t)b->n_keys * sizeof(sx_indel_key))
-    SX_UPX(3, v.b.in_pos, b->in_pos, const int32_t*, (size_t)b->n_reads * 4)
-    SX_UPX(4, v.b.in_seg_off, b->in_seg_off, const uint32_t*, (size_t)(b->n_reads + 1) * 4)
-    SX_UPX(5, v.b.in_segs, b->in_segs, const sx_aln_seg*, n_segs * sizeof(sx_aln_seg))
-    SX_UPX(6, v.b.read_len, b->read_len, const uint16_t*, (size_t)b->n_reads * 2)
-    if (b->gate)
-    {
-        SX_UPX(17, v.b.gate, b->gate, const uint8_t*, (size_t)b->n_reads)
-    }
-    SX_UPX(7, v.regions, regions, const sx_region*, ((size_t)b->n_regions + 1) * sizeof(sx_region))
-    SX_UPX(8, v.seq4, seq4, const uint8_t*, (size_t)end.seq_off + SX_POOL_SLACK)
-    SX_UPX(9, v.ref, ref, const char*, (size_t)end.ref_off + SX_POOL_SLACK)
-    const size_t ins_bytes(b->n_keys ? key_ins_off[b->n_keys] : 0);
-    SX_UPX(10, v.key_ins_off, key_ins_off, const uint32_t*, b->n_keys ? ((size_t)b->n_keys + 1) * 4 : 0)
-    SX_UPX(11, v.key_ins, key_ins, const char*, ins_bytes)
-#undef SX_UPX
+    if ((rc = sx_upload(ctx, sx_host_slot(0), b->region_read_off, nr + 1, v.b.region_read_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(1), b->region_key_off, nr + 1, v.b.region_key_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(2), b->keys, b->n_keys, v.b.keys, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(3), b->in_pos, n, v.b.in_pos, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(4), b->in_seg_off, n + 1, v.b.in_seg_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(5), b->in_segs, n_segs, v.b.in_segs, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(6), b->read_len, n, v.b.read_len, 16))) return rc;
+    if (b->gate && (rc = sx_upload(ctx, sx_host_slot(17), b->gate, n, v.b.gate, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(7), regions, nr + 1, v.regions, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(8), seq4, (size_t)end.seq_off + SX_POOL_SLACK, v.seq4, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(9), ref, (size_t)end.ref_off + SX_POOL_SLACK, v.ref, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(10), key_ins_off, b->n_keys ? (size_t)b->n_keys + 1 : 0, v.key_ins_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(11), key_ins, b->n_keys ? key_ins_off[b->n_keys] : 0, v.key_ins, 16))) return rc;
     sx_prep_out o(*out_host);
-    if ((rc = sx_ensure(ctx, 12, 16, reinterpret_cast<void**>(&o.totals)))) return rc;
-    if ((rc = sx_ensure(ctx, 13, (size_t)(b->n_reads + 1) * 4 + 16, reinterpret_cast<void**>(&o.in_key_off)))) return rc;
-    if ((rc = sx_ensure(ctx, 14, (size_t)o.cap_keys * 2 + 16, reinterpret_cast<void**>(&o.in_keys)))) return rc;
-    if ((rc = sx_ensure(ctx, 15, (size_t)b->n_reads * 2 + 16, reinterpret_cast<void**>(&o.in_lead_key)))) return rc;
-    if ((rc = sx_ensure(ctx, 16, (size_t)b->n_reads * 2 + 16, reinterpret_cast<void**>(&o.in_trail_key)))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(12), 4, o.totals, 0))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(13), n + 1, o.in_key_off, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(14), o.cap_keys, o.in_keys, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(15), n, o.in_lead_key, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(16), n, o.in_trail_key, 16))) return rc;
     unsigned launches(0);
     if ((rc = k7a_run(ctx, v, &o, &launches))) return rc;
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host->totals, o.totals, 4, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host->in_key_off, o.in_key_off, (size_t)(b->n_reads + 1) * 4, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host->in_lead_key, o.in_lead_key, (size_t)b->n_reads * 2, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host->in_trail_key, o.in_trail_key, (size_t)b->n_reads * 2, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaStreamSynchronize(st));
-    if (out_host->totals[0] <= o.cap_keys) SX_CUDA(ctx, cudaMemcpyAsync(out_host->in_keys, o.in_keys, (size_t)out_host->totals[0] * 2, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_b, st));
-    SX_CUDA(ctx, cudaStreamSynchronize(st));
-    float ms(0);
-    cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b);
-    ctx->timing.kernel_ms = ms;
-    ctx->timing.launches = launches;
-    ctx->total_launches += launches;
-    return k7a_finish(ctx, "sx_alignment_indels", out_host->totals);
+    if ((rc = sx_download(ctx, out_host->totals, o.totals, 1))) return rc;
+    if ((rc = sx_download(ctx, out_host->in_key_off, o.in_key_off, n + 1))) return rc;
+    if ((rc = sx_download(ctx, out_host->in_lead_key, o.in_lead_key, n))) return rc;
+    if ((rc = sx_download(ctx, out_host->in_trail_key, o.in_trail_key, n))) return rc;
+    SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
+    if (out_host->totals[0] <= o.cap_keys && (rc = sx_download(ctx, out_host->in_keys, o.in_keys, out_host->totals[0]))) return rc;
+    if ((rc = t.finish(launches))) return rc;
+    return sx_check_status(ctx, "sx_alignment_indels", SX_ST_K7A_CAP, out_host->totals);
 }
 
 // ---- asynchronous launchers for the device-resident pipeline (sx_pipeline.cu): everything is enqueued on ctx->s_compute, nothing waits

@@ -17,8 +17,8 @@
 
 namespace
 {
-constexpr int K8_ST_SHIFT = 15;      // device status bits 32768 (no key) / 65536 (segment kind)
-constexpr int K8_CAP_BIT = 1 << 17;  // an output capacity is too small
+constexpr int K8_ST_SHIFT = 15; // K8_ST_* bits are reported as ctx status bits 32768, 65536
+static_assert((K8_ST_NOKEY << K8_ST_SHIFT) == SX_ST_K8_NO_KEY && (K8_ST_KIND << K8_ST_SHIFT) == SX_ST_K8_KIND, "K8's shifted status bits are the context's");
 
 // alignment -> read (K7 lists a read's alignments consecutively)
 __global__ void k8_aln_read_kernel(const uint32_t n_reads, const uint32_t* __restrict__ aln_off, uint32_t* __restrict__ aln_read)
@@ -116,7 +116,7 @@ __global__ void __launch_bounds__(K7_SCAN_THREADS) k8_finish_kernel(const k8_vie
         o.regions[n].seg_begin = totals[0];
         o.regions[n].ins_begin = totals[1];
         o.regions[n].read_begin = v.b.n_reads;
-        if (totals[0] > o.cap_segs || totals[1] > o.cap_ins) atomicOr(status, K8_CAP_BIT);
+        if (totals[0] > o.cap_segs || totals[1] > o.cap_ins) atomicOr(status, SX_ST_K8_CAP);
         else o.alns[n_alns] = sx_aln{v.b.n_reads, 0, totals[0], totals[1]};
     }
 }
@@ -169,15 +169,15 @@ int k8_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* e, const uint
     int rc;
     uint32_t *aln_read(nullptr), *read_region(nullptr), *seg_n(nullptr), *ins_n(nullptr), *reg_seg(nullptr), *reg_ins(nullptr), *reg_zero(nullptr), *sums(nullptr);
     const uint32_t nr(d->n_regions);
-    if ((rc = sx_ensure(ctx, 46, (size_t)n_alns * 4 + 16, reinterpret_cast<void**>(&aln_read)))) return rc;
-    if ((rc = sx_ensure(ctx, 47, (size_t)d->n_reads * 4 + 16, reinterpret_cast<void**>(&read_region)))) return rc;
-    if ((rc = sx_ensure(ctx, 48, (size_t)n_alns * 4 + 16, reinterpret_cast<void**>(&seg_n)))) return rc;
-    if ((rc = sx_ensure(ctx, 49, (size_t)n_alns * 4 + 16, reinterpret_cast<void**>(&ins_n)))) return rc;
-    if ((rc = sx_ensure(ctx, 50, (size_t)nr * 4 + 16, reinterpret_cast<void**>(&reg_seg)))) return rc;
-    if ((rc = sx_ensure(ctx, 51, (size_t)nr * 4 + 16, reinterpret_cast<void**>(&reg_ins)))) return rc;
-    if ((rc = sx_ensure(ctx, 52, (size_t)nr * 4 + 16, reinterpret_cast<void**>(&reg_zero)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K8_ALN_READ, n_alns, aln_read, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K8_READ_REGION, d->n_reads, read_region, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K8_SEG_N, n_alns, seg_n, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K8_INS_N, n_alns, ins_n, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K8_REG_SEG, nr, reg_seg, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K8_REG_INS, nr, reg_ins, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K8_REG_ZERO, nr, reg_zero, 16))) return rc;
     const uint32_t tile(K7_SCAN_THREADS * K7_SCAN_ITEMS), n_tiles((nr + tile - 1) / tile);
-    if ((rc = sx_ensure(ctx, 53, ((size_t)3 * n_tiles + 4) * 4, reinterpret_cast<void**>(&sums)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K8_SUMS, (size_t)3 * n_tiles + 4, sums, 0))) return rc;
     uint32_t* totals(sums + (size_t)3 * n_tiles);
     k8_view v;
     v.b = *d;
@@ -208,23 +208,6 @@ int k8_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* e, const uint
     return SX_OK;
 }
 
-int k8_finish(sx_ctx* ctx, const char* what, const uint32_t* totals_host)
-{
-    int st(0);
-    SX_CUDA(ctx, cudaMemcpyAsync(&st, ctx->d_status, sizeof(int), cudaMemcpyDeviceToHost, ctx->s_compute));
-    SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
-    if (st & (K8_CAP_BIT | (3 << K8_ST_SHIFT)))
-    {
-        cudaMemsetAsync(ctx->d_status, 0, sizeof(int), ctx->s_compute);
-        if (st & (K8_ST_NOKEY << K8_ST_SHIFT))
-            return sx_fail(ctx, SX_ERR_ARG, "%s: a path gap matches no indel key of its alignment (getMatchingIndelKey would assert)", what);
-        if (st & (K8_ST_KIND << K8_ST_SHIFT)) return sx_fail(ctx, SX_ERR_ARG, "%s: can't handle cigar code", what);
-        if (totals_host) return sx_fail(ctx, SX_ERR_CAPACITY, "%s: output capacity too small: %u segments, %u insert bytes needed", what, totals_host[0], totals_host[1]);
-        return sx_fail(ctx, SX_ERR_CAPACITY, "%s: output capacity too small (totals[] holds the needed sizes)", what);
-    }
-    return sx_check_status(ctx, what);
-}
-
 int k8_check_args(sx_ctx* ctx, const sx_enum_batch* b, const sx_enum_out* e, const uint32_t* key_ins_off, const char* key_ins, const sx_link_out* o, const char* what)
 {
     if (!b || !e || !o) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL argument", what);
@@ -250,7 +233,7 @@ extern "C" int sx_link_alignments_dev(sx_ctx* ctx, const sx_enum_batch* d, const
     if ((rc = k8_run(ctx, d, e, n_alns, key_ins_off, key_ins, out_dev, &launches))) return rc;
     t.stop(launches);
     if ((rc = t.finish())) return rc;
-    return k8_finish(ctx, "sx_link_alignments", nullptr);
+    return sx_check_status(ctx, "sx_link_alignments", SX_ST_K8_NO_KEY | SX_ST_K8_KIND | SX_ST_K8_CAP);
 }
 
 extern "C" int sx_link_alignments(sx_ctx* ctx, const sx_enum_batch* b, const sx_enum_out* e, uint32_t n_alns, const uint32_t* key_ins_off, const char* key_ins,
@@ -262,64 +245,47 @@ extern "C" int sx_link_alignments(sx_ctx* ctx, const sx_enum_batch* b, const sx_
     if ((rc = k8_check_args(ctx, b, e, key_ins_off, key_ins, out_host, "sx_link_alignments"))) return rc;
     if (e->aln_off[b->n_reads] != n_alns) return sx_fail(ctx, SX_ERR_ARG, "sx_link_alignments: n_alns is not the enumeration's alignment count");
     SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    cudaStream_t st(ctx->s_compute);
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_a, st));
+    sx_call_timer t(ctx);
     sx_enum_batch d(*b);
     sx_enum_out de(*e);
-    void* p(nullptr);
-    const size_t n_segs(e->aln_seg_off[n_alns]), n_keys(e->aln_key_off[n_alns]);
-#define SX_UPX(slot, dst, src, type, bytes)                                                \
-    if ((rc = sx_ensure(ctx, slot, (size_t)(bytes) + 16, &p))) return rc;                   \
-    if (bytes) SX_CUDA(ctx, cudaMemcpyAsync(p, (src), (bytes), cudaMemcpyHostToDevice, st)); \
-    dst = static_cast<type>(p);
-    SX_UPX(0, d.region_read_off, b->region_read_off, const uint32_t*, (size_t)(b->n_regions + 1) * 4)
-    SX_UPX(1, d.region_key_off, b->region_key_off, const uint32_t*, (size_t)(b->n_regions + 1) * 4)
-    SX_UPX(2, d.keys, b->keys, const sx_indel_key*, (size_t)b->n_keys * sizeof(sx_indel_key))
-    SX_UPX(3, de.aln_off, e->aln_off, uint32_t*, (size_t)(b->n_reads + 1) * 4)
-    SX_UPX(4, de.aln_pos, e->aln_pos, int32_t*, (size_t)n_alns * 4)
-    SX_UPX(5, de.aln_seg_off, e->aln_seg_off, uint32_t*, ((size_t)n_alns + 1) * 4)
-    SX_UPX(6, de.segs, e->segs, sx_aln_seg*, n_segs * sizeof(sx_aln_seg))
-    SX_UPX(7, de.aln_key_off, e->aln_key_off, uint32_t*, ((size_t)n_alns + 1) * 4)
-    SX_UPX(8, de.aln_keys, e->aln_keys, uint16_t*, n_keys * 2)
-    SX_UPX(9, de.aln_lead_key, e->aln_lead_key, uint16_t*, (size_t)n_alns * 2)
-    SX_UPX(10, de.aln_trail_key, e->aln_trail_key, uint16_t*, (size_t)n_alns * 2)
+    const size_t nr(b->n_regions), n_segs(e->aln_seg_off[n_alns]), n_keys(e->aln_key_off[n_alns]);
+    if ((rc = sx_upload(ctx, sx_host_slot(0), b->region_read_off, nr + 1, d.region_read_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(1), b->region_key_off, nr + 1, d.region_key_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(2), b->keys, b->n_keys, d.keys, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(3), e->aln_off, (size_t)b->n_reads + 1, de.aln_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(4), e->aln_pos, n_alns, de.aln_pos, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(5), e->aln_seg_off, (size_t)n_alns + 1, de.aln_seg_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(6), e->segs, n_segs, de.segs, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(7), e->aln_key_off, (size_t)n_alns + 1, de.aln_key_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(8), e->aln_keys, n_keys, de.aln_keys, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(9), e->aln_lead_key, n_alns, de.aln_lead_key, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(10), e->aln_trail_key, n_alns, de.aln_trail_key, 16))) return rc;
     const uint32_t* d_key_ins_off(nullptr);
     const char* d_key_ins(nullptr);
-    const size_t ins_bytes(b->n_keys ? key_ins_off[b->n_keys] : 0);
-    SX_UPX(11, d_key_ins_off, key_ins_off, const uint32_t*, b->n_keys ? ((size_t)b->n_keys + 1) * 4 : 0)
-    SX_UPX(12, d_key_ins, key_ins, const char*, ins_bytes)
+    if ((rc = sx_upload(ctx, sx_host_slot(11), key_ins_off, b->n_keys ? (size_t)b->n_keys + 1 : 0, d_key_ins_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(12), key_ins, b->n_keys ? key_ins_off[b->n_keys] : 0, d_key_ins, 16))) return rc;
     sx_link_out o(*out_host);
-    SX_UPX(13, o.regions, out_host->regions, sx_region*, ((size_t)b->n_regions + 1) * sizeof(sx_region))
-#undef SX_UPX
-    if ((rc = sx_ensure(ctx, 14, 16, reinterpret_cast<void**>(&o.totals)))) return rc;
-    if ((rc = sx_ensure(ctx, 15, ((size_t)n_alns + 1) * sizeof(sx_aln) + 16, reinterpret_cast<void**>(&o.alns)))) return rc;
-    if ((rc = sx_ensure(ctx, 16, (size_t)o.cap_segs * sizeof(sx_aln_seg) + 16, reinterpret_cast<void**>(&o.segs)))) return rc;
-    if ((rc = sx_ensure(ctx, 17, (size_t)o.cap_ins + SX_POOL_SLACK + 16, reinterpret_cast<void**>(&o.ins)))) return rc;
-    if (out_host->k6_segs)
-    {
-        if ((rc = sx_ensure(ctx, 18, n_segs * sizeof(sx_aln_seg) + 16, reinterpret_cast<void**>(&o.k6_segs)))) return rc;
-    }
+    if ((rc = sx_upload(ctx, sx_host_slot(13), out_host->regions, nr + 1, o.regions, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(14), 4, o.totals, 0))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(15), (size_t)n_alns + 1, o.alns, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(16), o.cap_segs, o.segs, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(17), o.cap_ins, o.ins, SX_POOL_SLACK + 16))) return rc;
+    if (out_host->k6_segs && (rc = sx_take(ctx, sx_host_slot(18), n_segs, o.k6_segs, 16))) return rc;
     unsigned launches(0);
     if ((rc = k8_run(ctx, &d, &de, n_alns, d_key_ins_off, d_key_ins, &o, &launches))) return rc;
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host->totals, o.totals, 8, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host->regions, o.regions, ((size_t)b->n_regions + 1) * sizeof(sx_region), cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaStreamSynchronize(st));
+    if ((rc = sx_download(ctx, out_host->totals, o.totals, 2))) return rc;
+    if ((rc = sx_download(ctx, out_host->regions, o.regions, nr + 1))) return rc;
+    SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
     const uint32_t nS(out_host->totals[0]), nI(out_host->totals[1]);
     if (nS <= o.cap_segs && nI <= o.cap_ins)
     {
-        SX_CUDA(ctx, cudaMemcpyAsync(out_host->alns, o.alns, ((size_t)n_alns + 1) * sizeof(sx_aln), cudaMemcpyDeviceToHost, st));
-        SX_CUDA(ctx, cudaMemcpyAsync(out_host->segs, o.segs, (size_t)nS * sizeof(sx_aln_seg), cudaMemcpyDeviceToHost, st));
-        SX_CUDA(ctx, cudaMemcpyAsync(out_host->ins, o.ins, (size_t)nI, cudaMemcpyDeviceToHost, st));
-        if (out_host->k6_segs) SX_CUDA(ctx, cudaMemcpyAsync(out_host->k6_segs, o.k6_segs, n_segs * sizeof(sx_aln_seg), cudaMemcpyDeviceToHost, st));
+        if ((rc = sx_download(ctx, out_host->alns, o.alns, (size_t)n_alns + 1))) return rc;
+        if ((rc = sx_download(ctx, out_host->segs, o.segs, nS))) return rc;
+        if ((rc = sx_download(ctx, out_host->ins, o.ins, nI))) return rc;
+        if (out_host->k6_segs && (rc = sx_download(ctx, out_host->k6_segs, o.k6_segs, n_segs))) return rc;
     }
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_b, st));
-    SX_CUDA(ctx, cudaStreamSynchronize(st));
-    float ms(0);
-    cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b);
-    ctx->timing.kernel_ms = ms;
-    ctx->timing.launches = launches;
-    ctx->total_launches += launches;
-    return k8_finish(ctx, "sx_link_alignments", out_host->totals);
+    if ((rc = t.finish(launches))) return rc;
+    return sx_check_status(ctx, "sx_link_alignments", SX_ST_K8_NO_KEY | SX_ST_K8_KIND | SX_ST_K8_CAP, out_host->totals);
 }
 
 // asynchronous launcher for the device-resident pipeline (sx_pipeline.cu)

@@ -17,8 +17,6 @@
 
 namespace
 {
-constexpr int K9_CAP_BIT = 1 << 19;
-
 __global__ void k9_slots_kernel(const sx_realign_batch b, uint32_t* __restrict__ cnt, uint32_t* __restrict__ z1, uint32_t* __restrict__ z2, uint32_t* __restrict__ read_region)
 {
     for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < b.n_reads; r += gridDim.x * blockDim.x)
@@ -46,7 +44,7 @@ __global__ void __launch_bounds__(K7_SCAN_THREADS) k9_finish_kernel(const uint32
     {
         o.seg_off[n] = totals[0];
         o.totals[0] = totals[0];
-        if (totals[0] > o.cap_segs) atomicOr(status, K9_CAP_BIT);
+        if (totals[0] > o.cap_segs) atomicOr(status, SX_ST_K9_CAP);
     }
 }
 
@@ -79,12 +77,12 @@ int k9_run(sx_ctx* ctx, const sx_realign_batch* d, const double* lnp, const sx_r
     const uint32_t n(d->n_reads);
     int rc;
     uint32_t *cnt(nullptr), *z1(nullptr), *z2(nullptr), *read_region(nullptr), *sums(nullptr);
-    if ((rc = sx_ensure(ctx, 58, (size_t)n * 4 + 16, reinterpret_cast<void**>(&read_region)))) return rc;
-    if ((rc = sx_ensure(ctx, 60, (size_t)n * 4 + 16, reinterpret_cast<void**>(&cnt)))) return rc;
-    if ((rc = sx_ensure(ctx, 61, (size_t)n * 4 + 16, reinterpret_cast<void**>(&z1)))) return rc;
-    if ((rc = sx_ensure(ctx, 62, (size_t)n * 4 + 16, reinterpret_cast<void**>(&z2)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_READ_WORD, n, read_region, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_CNT, n, cnt, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_Z1, n, z1, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_Z2, n, z2, 16))) return rc;
     const uint32_t tile(K7_SCAN_THREADS * K7_SCAN_ITEMS), n_tiles((n + tile - 1) / tile);
-    if ((rc = sx_ensure(ctx, 63, ((size_t)3 * n_tiles + 4) * 4, reinterpret_cast<void**>(&sums)))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_SUMS, (size_t)3 * n_tiles + 4, sums, 0))) return rc;
     uint32_t* totals(sums + (size_t)3 * n_tiles);
     const int cap(ctx->sm_count * 16);
     const auto grid = [cap](const uint32_t m) { return (unsigned)std::max(1, std::min<int>((int)((m + 127) / 128), cap)); };
@@ -103,20 +101,6 @@ int k9_run(sx_ctx* ctx, const sx_realign_batch* d, const double* lnp, const sx_r
     SX_CUDA(ctx, cudaGetLastError());
     *launches = 5;
     return SX_OK;
-}
-
-int k9_finish(sx_ctx* ctx, const char* what, const uint32_t* totals_host)
-{
-    int st(0);
-    SX_CUDA(ctx, cudaMemcpyAsync(&st, ctx->d_status, sizeof(int), cudaMemcpyDeviceToHost, ctx->s_compute));
-    SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
-    if (st & K9_CAP_BIT)
-    {
-        cudaMemsetAsync(ctx->d_status, 0, sizeof(int), ctx->s_compute);
-        if (totals_host) return sx_fail(ctx, SX_ERR_CAPACITY, "%s: cap_segs too small: %u segment slots needed", what, totals_host[0]);
-        return sx_fail(ctx, SX_ERR_CAPACITY, "%s: cap_segs too small (totals[0] holds the needed size)", what);
-    }
-    return sx_check_status(ctx, what);
 }
 
 int k9_check_args(sx_ctx* ctx, const sx_realign_batch* b, const double* lnp, const sx_realign_out* o, const char* what)
@@ -151,7 +135,7 @@ extern "C" int sx_choose_realignment_dev(sx_ctx* ctx, const sx_realign_batch* d,
     if ((rc = k9_run(ctx, d, lnp_dev, out_dev, &launches))) return rc;
     t.stop(launches);
     if ((rc = t.finish())) return rc;
-    return k9_finish(ctx, "sx_choose_realignment", nullptr);
+    return sx_check_status(ctx, "sx_choose_realignment", SX_ST_K9_CAP);
 }
 
 extern "C" int sx_choose_realignment(sx_ctx* ctx, const sx_realign_batch* b, const double* lnp_host, sx_realign_out* out_host)
@@ -168,61 +152,45 @@ extern "C" int sx_choose_realignment(sx_ctx* ctx, const sx_realign_batch* b, con
     }
     if (b->aln_off[b->n_reads] != b->n_alns) return sx_fail(ctx, SX_ERR_ARG, "sx_choose_realignment: aln_off does not end at n_alns");
     SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    cudaStream_t st(ctx->s_compute);
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_a, st));
+    sx_call_timer t(ctx);
     sx_realign_batch d(*b);
-    void* p(nullptr);
-    const size_t n_segs(b->aln_seg_off[b->n_alns]), n_keys(b->aln_key_off[b->n_alns]), n_win(b->region_key_off[b->n_regions]);
-#define SX_UPX(slot, dst, src, type, bytes)                                                \
-    if ((rc = sx_ensure(ctx, slot, (size_t)(bytes) + 16, &p))) return rc;                   \
-    if (bytes) SX_CUDA(ctx, cudaMemcpyAsync(p, (src), (bytes), cudaMemcpyHostToDevice, st)); \
-    dst = static_cast<type>(p);
-    SX_UPX(0, d.region_read_off, b->region_read_off, const uint32_t*, (size_t)(b->n_regions + 1) * 4)
-    SX_UPX(1, d.region_key_off, b->region_key_off, const uint32_t*, (size_t)(b->n_regions + 1) * 4)
-    SX_UPX(2, d.keys, b->keys, const sx_indel_key*, n_win * sizeof(sx_indel_key))
-    SX_UPX(3, d.aln_off, b->aln_off, const uint32_t*, (size_t)(b->n_reads + 1) * 4)
-    SX_UPX(4, d.aln_pos, b->aln_pos, const int32_t*, (size_t)b->n_alns * 4)
-    SX_UPX(5, d.aln_seg_off, b->aln_seg_off, const uint32_t*, ((size_t)b->n_alns + 1) * 4)
-    SX_UPX(6, d.segs, b->segs, const sx_aln_seg*, n_segs * sizeof(sx_aln_seg))
-    SX_UPX(7, d.aln_key_off, b->aln_key_off, const uint32_t*, ((size_t)b->n_alns + 1) * 4)
-    SX_UPX(8, d.aln_keys, b->aln_keys, const uint16_t*, n_keys * 2)
-    SX_UPX(9, d.read_len, b->read_len, const uint16_t*, (size_t)b->n_reads * 2)
-    if (b->pin_flags)
-    {
-        SX_UPX(10, d.pin_flags, b->pin_flags, const uint8_t*, (size_t)b->n_reads)
-    }
+    const size_t n(b->n_reads), n_segs(b->aln_seg_off[b->n_alns]), n_keys(b->aln_key_off[b->n_alns]), n_win(b->region_key_off[b->n_regions]);
+    if ((rc = sx_upload(ctx, sx_host_slot(0), b->region_read_off, (size_t)b->n_regions + 1, d.region_read_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(1), b->region_key_off, (size_t)b->n_regions + 1, d.region_key_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(2), b->keys, n_win, d.keys, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(3), b->aln_off, n + 1, d.aln_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(4), b->aln_pos, b->n_alns, d.aln_pos, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(5), b->aln_seg_off, (size_t)b->n_alns + 1, d.aln_seg_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(6), b->segs, n_segs, d.segs, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(7), b->aln_key_off, (size_t)b->n_alns + 1, d.aln_key_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(8), b->aln_keys, n_keys, d.aln_keys, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(9), b->read_len, n, d.read_len, 16))) return rc;
+    if (b->pin_flags && (rc = sx_upload(ctx, sx_host_slot(10), b->pin_flags, n, d.pin_flags, 16))) return rc;
     const double* d_lnp(nullptr);
-    SX_UPX(11, d_lnp, lnp_host, const double*, (size_t)b->n_alns * 8)
-#undef SX_UPX
+    if ((rc = sx_upload(ctx, sx_host_slot(11), lnp_host, b->n_alns, d_lnp, 16))) return rc;
     sx_realign_out o(*out_host);
-    if ((rc = sx_ensure(ctx, 12, 16, reinterpret_cast<void**>(&o.totals)))) return rc;
-    if ((rc = sx_ensure(ctx, 13, (size_t)(b->n_reads + 1) * 4 + 16, reinterpret_cast<void**>(&o.seg_off)))) return rc;
-    if ((rc = sx_ensure(ctx, 14, (size_t)b->n_reads * 4 + 16, reinterpret_cast<void**>(&o.pos)))) return rc;
-    if ((rc = sx_ensure(ctx, 15, (size_t)b->n_reads * 2 + 16, reinterpret_cast<void**>(&o.n_seg)))) return rc;
-    if ((rc = sx_ensure(ctx, 16, (size_t)b->n_reads + 16, reinterpret_cast<void**>(&o.status)))) return rc;
-    if ((rc = sx_ensure(ctx, 17, (size_t)b->n_reads * 4 + 16, reinterpret_cast<void**>(&o.best_aln)))) return rc;
-    if ((rc = sx_ensure(ctx, 18, (size_t)o.cap_segs * sizeof(sx_aln_seg) + 16, reinterpret_cast<void**>(&o.segs)))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(12), 4, o.totals, 0))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(13), n + 1, o.seg_off, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(14), n, o.pos, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(15), n, o.n_seg, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(16), n, o.status, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(17), n, o.best_aln, 16))) return rc;
+    if ((rc = sx_take(ctx, sx_host_slot(18), o.cap_segs, o.segs, 16))) return rc;
     unsigned launches(0);
     if ((rc = k9_run(ctx, &d, d_lnp, &o, &launches))) return rc;
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host->totals, o.totals, 4, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaMemcpyAsync(out_host->seg_off, o.seg_off, (size_t)(b->n_reads + 1) * 4, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaStreamSynchronize(st));
+    if ((rc = sx_download(ctx, out_host->totals, o.totals, 1))) return rc;
+    if ((rc = sx_download(ctx, out_host->seg_off, o.seg_off, n + 1))) return rc;
+    SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
     if (out_host->totals[0] <= o.cap_segs)
     {
-        SX_CUDA(ctx, cudaMemcpyAsync(out_host->pos, o.pos, (size_t)b->n_reads * 4, cudaMemcpyDeviceToHost, st));
-        SX_CUDA(ctx, cudaMemcpyAsync(out_host->n_seg, o.n_seg, (size_t)b->n_reads * 2, cudaMemcpyDeviceToHost, st));
-        SX_CUDA(ctx, cudaMemcpyAsync(out_host->status, o.status, (size_t)b->n_reads, cudaMemcpyDeviceToHost, st));
-        SX_CUDA(ctx, cudaMemcpyAsync(out_host->best_aln, o.best_aln, (size_t)b->n_reads * 4, cudaMemcpyDeviceToHost, st));
-        SX_CUDA(ctx, cudaMemcpyAsync(out_host->segs, o.segs, (size_t)out_host->totals[0] * sizeof(sx_aln_seg), cudaMemcpyDeviceToHost, st));
+        if ((rc = sx_download(ctx, out_host->pos, o.pos, n))) return rc;
+        if ((rc = sx_download(ctx, out_host->n_seg, o.n_seg, n))) return rc;
+        if ((rc = sx_download(ctx, out_host->status, o.status, n))) return rc;
+        if ((rc = sx_download(ctx, out_host->best_aln, o.best_aln, n))) return rc;
+        if ((rc = sx_download(ctx, out_host->segs, o.segs, out_host->totals[0]))) return rc;
     }
-    SX_CUDA(ctx, cudaEventRecord(ctx->ev_b, st));
-    SX_CUDA(ctx, cudaStreamSynchronize(st));
-    float ms(0);
-    cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b);
-    ctx->timing.kernel_ms = ms;
-    ctx->timing.launches = launches;
-    ctx->total_launches += launches;
-    return k9_finish(ctx, "sx_choose_realignment", out_host->totals);
+    if ((rc = t.finish(launches))) return rc;
+    return sx_check_status(ctx, "sx_choose_realignment", SX_ST_K9_CAP, out_host->totals);
 }
 
 // asynchronous launcher for the device-resident pipeline (sx_pipeline.cu)

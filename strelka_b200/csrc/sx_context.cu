@@ -477,8 +477,9 @@ extern "C" void sx_destroy(sx_ctx* ctx)
     delete ctx;
 }
 
-int sx_ensure(sx_ctx* ctx, int slot, size_t bytes, void** out)
+int sx_ensure(sx_ctx* ctx, sx_slot slot, size_t bytes, void** out)
 {
+    if (slot < 0 || slot >= SX_SLOT_COUNT) return sx_fail(ctx, SX_ERR_ARG, "device buffer slot %d outside the context's %d", (int)slot, (int)SX_SLOT_COUNT);
     sx_buf& b = ctx->buf[slot];
     if (b.cap < bytes)
     {
@@ -498,31 +499,72 @@ int sx_ensure(sx_ctx* ctx, int slot, size_t bytes, void** out)
     return SX_OK;
 }
 
-int sx_check_status(sx_ctx* ctx, const char* what)
+#define SX_STR_(x) #x
+#define SX_STR(x) SX_STR_(x)
+namespace
+{
+// every status bit with its error.  A capacity bit has a second message that quotes the stage's first n_totals totals.
+struct sx_status_entry
+{
+    int bit, code;
+    const char* msg;
+    const char* msg_totals;
+    int n_totals;
+};
+constexpr sx_status_entry k_status[] = {
+    {SX_ST_QUAL, SX_ERR_RANGE, "%s: quality score above " SX_STR(SX_MAX_QSCORE) " (qphred_cache::qscore_check would throw)", nullptr, 0},
+    {SX_ST_TILE, SX_ERR_ARG, "%s: a region does not fit the shared-memory tile the kernel was launched with", nullptr, 0},
+    {SX_ST_SEG_KIND, SX_ERR_ARG, "%s: unknown segment kind", nullptr, 0},
+    {SX_ST_READ_OVERRUN, SX_ERR_ARG, "%s: alignment path consumes more read bases than the read holds", nullptr, 0},
+    {SX_ST_SITE_DEPTH, SX_ERR_UNSUPPORTED, "%s: a site holds more calls than the kernel handles", nullptr, 0},
+    {SX_ST_INDEL_ALLELES, SX_ERR_ARG, "%s: allele count outside 1.." SX_STR(SX_INDEL_MAX_ALLELES) " or ploidy outside {1,2}", nullptr, 0},
+    {SX_ST_READ_ORDER, SX_ERR_ARG, "%s: reads are not in position order, or an alignment spans more reference than max_ref_span", nullptr, 0},
+    {SX_ST_BASE, SX_ERR_ARG, "%s: unknown base code (bam_seq_code_to_id would throw)", nullptr, 0},
+    {SX_ST_READ_LIMIT, SX_ERR_UNSUPPORTED, "%s: a read is longer, or has more path segments, than the kernel handles", nullptr, 0},
+    {SX_ST_K6_SEG_KIND, SX_ERR_UNSUPPORTED, "%s: a path segment kind outside score_indels' domain (SKIP / REFSKIP / unknown)", nullptr, 0},
+    {SX_ST_K6_ALNS, SX_ERR_ARG, "%s: a read has more alignments than the scratch was sized for", nullptr, 0},
+    {SX_ST_K6_EVAL, SX_ERR_UNSUPPORTED, "%s: a read evaluates more than 64 indels", nullptr, 0},
+    {SX_ST_K6_REC_CAP, SX_ERR_NOMEM, "%s: rec_off leaves too few record slots for a read", nullptr, 0},
+    {SX_ST_K6_KEY, SX_ERR_ARG, "%s: an alignment key index outside its region's window, or an unsupported key type", nullptr, 0},
+    {SX_ST_K8_NO_KEY, SX_ERR_ARG, "%s: a path gap matches no indel key of its alignment (getMatchingIndelKey would assert)", nullptr, 0},
+    {SX_ST_K8_KIND, SX_ERR_ARG, "%s: can't handle cigar code", nullptr, 0},
+    {SX_ST_K8_CAP, SX_ERR_CAPACITY, "%s: output capacity too small (totals[] holds the needed sizes)", "%s: output capacity too small: %u segments, %u insert bytes needed", 2},
+    {SX_ST_K7_CAP, SX_ERR_CAPACITY, "%s: output capacity too small (totals[] holds the needed sizes)",
+     "%s: output capacity too small: the batch produces %u alignments, %u segments, %u keys", 3},
+    {SX_ST_K7A_CAP, SX_ERR_CAPACITY, "%s: cap_keys too small (totals[0] holds the needed size)", "%s: cap_keys too small: %u keys needed", 1},
+    {SX_ST_K9_CAP, SX_ERR_CAPACITY, "%s: cap_segs too small (totals[0] holds the needed size)", "%s: cap_segs too small: %u segment slots needed", 1},
+};
+
+constexpr bool status_bits_disjoint()
+{
+    int seen = 0;
+    for (const sx_status_entry& e : k_status)
+    {
+        if (e.bit <= 0 || (e.bit & (e.bit - 1)) || (seen & e.bit)) return false;
+        seen |= e.bit;
+    }
+    return true;
+}
+static_assert(status_bits_disjoint(), "every status bit is one bit, and no two overlap");
+} // namespace
+
+int sx_check_status(sx_ctx* ctx, const char* what, int first, const uint32_t* totals)
 {
     int st = 0;
     SX_CUDA(ctx, cudaMemcpyAsync(&st, ctx->d_status, sizeof(int), cudaMemcpyDeviceToHost, ctx->s_compute));
     SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
-    if (st != 0)
-    {
-        cudaMemsetAsync(ctx->d_status, 0, sizeof(int), ctx->s_compute);
-        if (st & 1) return sx_fail(ctx, SX_ERR_RANGE, "%s: quality score above %d (qphred_cache::qscore_check would throw)", what, SX_MAX_QSCORE);
-        if (st & 2) return sx_fail(ctx, SX_ERR_ARG, "%s: a region does not fit the shared-memory tile the kernel was launched with", what);
-        if (st & 4) return sx_fail(ctx, SX_ERR_ARG, "%s: unknown segment kind", what);
-        if (st & 8) return sx_fail(ctx, SX_ERR_ARG, "%s: alignment path consumes more read bases than the read holds", what);
-        if (st & 16) return sx_fail(ctx, SX_ERR_UNSUPPORTED, "%s: a site holds more calls than the kernel handles", what);
-        if (st & 32) return sx_fail(ctx, SX_ERR_ARG, "%s: allele count outside 1..%d or ploidy outside {1,2}", what, SX_INDEL_MAX_ALLELES);
-        if (st & 64) return sx_fail(ctx, SX_ERR_ARG, "%s: reads are not in position order, or an alignment spans more reference than max_ref_span", what);
-        if (st & 128) return sx_fail(ctx, SX_ERR_ARG, "%s: unknown base code (bam_seq_code_to_id would throw)", what);
-        if (st & 256) return sx_fail(ctx, SX_ERR_UNSUPPORTED, "%s: a read is longer, or has more path segments, than the kernel handles", what);
-        if (st & 512) return sx_fail(ctx, SX_ERR_UNSUPPORTED, "%s: a path segment kind outside score_indels' domain (SKIP / REFSKIP / unknown)", what);
-        if (st & 1024) return sx_fail(ctx, SX_ERR_ARG, "%s: a read has more alignments than the scratch was sized for", what);
-        if (st & 2048) return sx_fail(ctx, SX_ERR_UNSUPPORTED, "%s: a read evaluates more than 64 indels", what);
-        if (st & 4096) return sx_fail(ctx, SX_ERR_NOMEM, "%s: rec_off leaves too few record slots for a read", what);
-        if (st & 8192) return sx_fail(ctx, SX_ERR_ARG, "%s: an alignment key index outside its region's window, or an unsupported key type", what);
-        return sx_fail(ctx, SX_ERR_ARG, "%s: device status %d", what, st);
-    }
-    return SX_OK;
+    if (st == 0) return SX_OK;
+    cudaMemsetAsync(ctx->d_status, 0, sizeof(int), ctx->s_compute);
+    for (const int pass_first : {1, 0})
+        for (const sx_status_entry& e : k_status)
+        {
+            if (!(st & e.bit) || ((first & e.bit) != 0) != (pass_first != 0)) continue;
+            if (!totals || !e.msg_totals || !(first & e.bit)) return sx_fail(ctx, e.code, e.msg, what); // (the totals are the caller's stage's)
+            if (e.n_totals == 1) return sx_fail(ctx, e.code, e.msg_totals, what, totals[0]);
+            if (e.n_totals == 2) return sx_fail(ctx, e.code, e.msg_totals, what, totals[0], totals[1]);
+            return sx_fail(ctx, e.code, e.msg_totals, what, totals[0], totals[1], totals[2]);
+        }
+    return sx_fail(ctx, SX_ERR_ARG, "%s: device status %d", what, st);
 }
 
 extern "C" void* sx_host_alloc(size_t bytes)

@@ -76,8 +76,86 @@ struct sx_tables
     int32_t i_min_flank, i_pad;
 };
 
-int sx_upload_pileup(sx_ctx* ctx, const sx_pileup_batch* b, int slot_base, sx_pileup_batch* d, uint32_t* max_site, cudaStream_t st);
+int sx_upload_pileup(sx_ctx* ctx, const sx_pileup_batch* b, int host_base, sx_pileup_batch* d, uint32_t* max_site); // host slots host_base..+5
 cudaError_t sx_k2a_init_tables(sx_tables* d_tables); // fills the g_val0_* rows of the device copy (synchronous)
+
+// ---------------------------------------------------------------------------------------------------------------
+// device buffers: sx_ctx::buf holds one grow-only buffer per slot.  Every buffer the library allocates has its slot here.
+// ---------------------------------------------------------------------------------------------------------------
+enum sx_slot : int
+{
+    // host staging: what a host-array entry point (sx_score_alignments, sx_site_gl_germline, ...) uploads and downloads, as
+    // sx_host_slot(i).  The running entry owns the whole block; no stage launcher allocates in it.
+    SX_SLOT_HOST = 0,
+    SX_SLOT_HOST_END = SX_SLOT_HOST + 32,
+    // stage scratch, owned by the stage's launcher while its launches run
+    SX_SLOT_K1_SMEM_NEED = SX_SLOT_HOST_END,
+    SX_SLOT_K2A_SCRATCH, SX_SLOT_K2A_MAX_SITE,
+    SX_SLOT_K3_INFO, SX_SLOT_K3_CURSOR, SX_SLOT_K3_ORDER, SX_SLOT_K3_SCRATCH,
+    SX_SLOT_K4_SCAN_S, SX_SLOT_K4_SCAN_B, SX_SLOT_K4_TILE_SUMS,
+    SX_SLOT_K6_MAX, SX_SLOT_K6_LIST, SX_SLOT_K6_ARENA, SX_SLOT_K6_CLASS, SX_SLOT_K6_HIST, SX_SLOT_K6_LIST_BY_CLASS,
+    SX_SLOT_K7_READ_REGION, SX_SLOT_K7_ARENA, SX_SLOT_K7_ARENA_DEEP, SX_SLOT_K7_CNT_ALN, SX_SLOT_K7_CNT_SEG, SX_SLOT_K7_CNT_KEY, SX_SLOT_K7_SUMS,
+    SX_SLOT_K7_LOG, SX_SLOT_K7_LOG_OFF, SX_SLOT_K7_LOG_CURSOR, SX_SLOT_K7_RETRY1, SX_SLOT_K7_RETRY2, SX_SLOT_K7_RETRY_N, SX_SLOT_K7_ACTIVE,
+    SX_SLOT_K7_CLASS, SX_SLOT_K7_HIST, SX_SLOT_K7_ACTIVE_BY_CLASS,
+    SX_SLOT_K7A_READ_REGION, SX_SLOT_K7A_STAGE, SX_SLOT_K7A_ACTIVE,
+    SX_SLOT_K8_ALN_READ, SX_SLOT_K8_READ_REGION, SX_SLOT_K8_SEG_N, SX_SLOT_K8_INS_N, SX_SLOT_K8_REG_SEG, SX_SLOT_K8_REG_INS, SX_SLOT_K8_REG_ZERO, SX_SLOT_K8_SUMS,
+    // per-read scratch shared by K7a and K9: a per-read word (K7a: read byte offset, K9: read region), the per-read counts and their scan.
+    // These are O(reads) and every context that runs the window pass holds them.  Their lifetimes cannot overlap: K7a's are dead once its
+    // write kernel has run, and K9 is enqueued after K7a on the same stream (sx_process_window_dev) or by its own entry point.
+    SX_SLOT_K7A_K9_READ_WORD, SX_SLOT_K7A_K9_CNT, SX_SLOT_K7A_K9_Z1, SX_SLOT_K7A_K9_Z2, SX_SLOT_K7A_K9_SUMS,
+    // window pass: the intermediates of sx_process_window_dev
+    SX_SLOT_WIN_SEQ_OFF, SX_SLOT_WIN_QUAL_OFF, SX_SLOT_WIN_BPOS, SX_SLOT_WIN_NON_AMBIG, SX_SLOT_WIN_PIN, SX_SLOT_WIN_MAXIMA,
+    SX_SLOT_WIN_GATE, SX_SLOT_WIN_IN_POS, SX_SLOT_WIN_IN_SEGS,
+    SX_SLOT_WIN_KEY_TOTALS, SX_SLOT_WIN_IN_KEY_OFF, SX_SLOT_WIN_IN_KEYS, SX_SLOT_WIN_IN_LEAD, SX_SLOT_WIN_IN_TRAIL,
+    SX_SLOT_WIN_ENUM_TOTALS, SX_SLOT_WIN_ALN_OFF, SX_SLOT_WIN_ENUM_STATUS, SX_SLOT_WIN_ALN_POS, SX_SLOT_WIN_ALN_SEG_OFF, SX_SLOT_WIN_SEGS,
+    SX_SLOT_WIN_ALN_KEY_OFF, SX_SLOT_WIN_ALN_KEYS, SX_SLOT_WIN_ALN_LEAD, SX_SLOT_WIN_ALN_TRAIL,
+    SX_SLOT_WIN_LINK_TOTALS, SX_SLOT_WIN_LINK_ALNS, SX_SLOT_WIN_LINK_SEGS, SX_SLOT_WIN_LINK_INS, SX_SLOT_WIN_K6_SEGS, SX_SLOT_WIN_LNP,
+    SX_SLOT_WIN_RECS, SX_SLOT_WIN_N_REC, SX_SLOT_WIN_MAX_ALN, SX_SLOT_WIN_EVAL_ALN,
+    SX_SLOT_WIN_BEST_TOTALS, SX_SLOT_WIN_BEST_SEG_OFF, SX_SLOT_WIN_BEST_POS, SX_SLOT_WIN_BEST_N_SEG, SX_SLOT_WIN_REALIGN_STATUS, SX_SLOT_WIN_BEST_ALN,
+    SX_SLOT_WIN_BEST_SEGS, SX_SLOT_WIN_PILEUP_READS,
+    SX_SLOT_WIN_SITE_OFF, SX_SLOT_WIN_T2_OFF, SX_SLOT_WIN_N_SPANDEL, SX_SLOT_WIN_N_SUBMAPPED, SX_SLOT_WIN_CALLS, SX_SLOT_WIN_T2_CALLS,
+    SX_SLOT_WIN_SITE_GL, SX_SLOT_WIN_VARIANT_CHUNKS,
+    // window pass: what sx_process_window uploads (the window batch's arrays) and the outputs it downloads
+    SX_SLOT_WUP_REGION_READ_OFF, SX_SLOT_WUP_REGION_KEY_OFF, SX_SLOT_WUP_KEYS, SX_SLOT_WUP_KEY_HAP, SX_SLOT_WUP_KEY_INS_OFF, SX_SLOT_WUP_KEY_INS,
+    SX_SLOT_WUP_REALIGN_BEGIN, SX_SLOT_WUP_REALIGN_END, SX_SLOT_WUP_RAW_POS, SX_SLOT_WUP_RAW_SEG_OFF, SX_SLOT_WUP_RAW_SEGS, SX_SLOT_WUP_READ_LEN,
+    SX_SLOT_WUP_READ_FLAGS, SX_SLOT_WUP_MAPQ, SX_SLOT_WUP_USE_KEY_OFF, SX_SLOT_WUP_USE_KEYS, SX_SLOT_WUP_REC_OFF, SX_SLOT_WUP_REGIONS,
+    SX_SLOT_WUP_SEQ4, SX_SLOT_WUP_QUAL, SX_SLOT_WUP_REF, SX_SLOT_WUP_CAND_SNV,
+    SX_SLOT_WDN_GATE, SX_SLOT_WDN_ENUM_STATUS, SX_SLOT_WDN_REALIGN_STATUS, SX_SLOT_WDN_BEST_POS, SX_SLOT_WDN_BEST_SEG_OFF, SX_SLOT_WDN_BEST_N_SEG,
+    SX_SLOT_WDN_BEST_SEGS, SX_SLOT_WDN_RECS, SX_SLOT_WDN_N_REC, SX_SLOT_WDN_SITE_OFF, SX_SLOT_WDN_T2_OFF, SX_SLOT_WDN_N_SPANDEL,
+    SX_SLOT_WDN_N_SUBMAPPED, SX_SLOT_WDN_CALLS, SX_SLOT_WDN_T2_CALLS, SX_SLOT_WDN_SITE_GL, SX_SLOT_WDN_VARIANT_SITES,
+    SX_SLOT_COUNT
+};
+
+// slot i of the host staging block (SX_SLOT_COUNT, which sx_ensure refuses, past its end)
+constexpr sx_slot sx_host_slot(int i) { return i >= 0 && i < SX_SLOT_HOST_END - SX_SLOT_HOST ? sx_slot(SX_SLOT_HOST + i) : SX_SLOT_COUNT; }
+
+// ---------------------------------------------------------------------------------------------------------------
+// device status word (sx_ctx::d_status): the bits the kernels raise.  sx_check_status (sx_context.cu) reports each with its own
+// error code and message, and clears the word.
+// ---------------------------------------------------------------------------------------------------------------
+enum sx_status_bit : int
+{
+    SX_ST_QUAL = 1,              // K1, K4: a quality score above SX_MAX_QSCORE
+    SX_ST_TILE = 2,              // K1: a region does not fit the shared-memory tile of the launch
+    SX_ST_SEG_KIND = 4,          // K1, K4: an unknown segment kind
+    SX_ST_READ_OVERRUN = 8,      // K1: a path consumes more read bases than the read holds
+    SX_ST_SITE_DEPTH = 16,       // K2a: a site deeper than the kernel handles
+    SX_ST_INDEL_ALLELES = 32,    // K5: allele count or ploidy outside the model
+    SX_ST_READ_ORDER = 64,       // K4: reads out of position order, or an alignment wider than max_ref_span
+    SX_ST_BASE = 128,            // K4: an unknown base code
+    SX_ST_READ_LIMIT = 256,      // K4: a read longer, or with more segments, than the kernel handles
+    SX_ST_K6_SEG_KIND = 1 << 9,  // K6 (K6_ST_* of k6_core.cuh, shifted by 9)
+    SX_ST_K6_ALNS = 1 << 10,
+    SX_ST_K6_EVAL = 1 << 11,
+    SX_ST_K6_REC_CAP = 1 << 12,
+    SX_ST_K6_KEY = 1 << 13,
+    SX_ST_K7_CAP = 1 << 14,      // K7: an output capacity is too small
+    SX_ST_K8_NO_KEY = 1 << 15,   // K8 (K8_ST_* of k8_core.cuh, shifted by 15)
+    SX_ST_K8_KIND = 1 << 16,
+    SX_ST_K8_CAP = 1 << 17,      // K8: an output capacity is too small
+    SX_ST_K7A_CAP = 1 << 18,     // K7a: cap_keys is too small
+    SX_ST_K9_CAP = 1 << 19,      // K9: cap_segs is too small
+};
 
 struct sx_buf
 {
@@ -100,7 +178,7 @@ struct sx_ctx
     std::string err;
     sx_timing timing{};
     uint64_t total_launches = 0;
-    sx_buf buf[192];         // grow-only device arenas, one per logical pool (host entries 0..29, K7 family 40..63, K4 64, pipeline 70..)
+    sx_buf buf[SX_SLOT_COUNT]; // grow-only device buffers, one per sx_slot
     void* nccl = nullptr;    // ncclComm_t
     void* nccl_lib = nullptr;
     int rank = 0, world = 1;
@@ -122,8 +200,45 @@ int sx_fail(sx_ctx* ctx, int code, const char* fmt, ...);
         if (e_ != cudaSuccess) return sx_fail((ctx), SX_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
     } while (0)
 
-int sx_ensure(sx_ctx* ctx, int slot, size_t bytes, void** out);
-int sx_check_status(sx_ctx* ctx, const char* what);
+int sx_ensure(sx_ctx* ctx, sx_slot slot, size_t bytes, void** out);
+
+// the slot's buffer as `count` elements of T plus `slack` bytes
+template <typename T> int sx_take(sx_ctx* ctx, sx_slot slot, size_t count, T*& p, size_t slack)
+{
+    void* q(nullptr);
+    const int rc(sx_ensure(ctx, slot, count * sizeof(T) + slack, &q));
+    p = static_cast<T*>(q);
+    return rc;
+}
+
+// host staging of a host-array entry point: `count` elements of `src` into the slot's buffer (sized with `slack` extra bytes) on the
+// compute stream; `dst` is the device copy.  An empty array is allocated but not copied.
+template <typename T> int sx_upload(sx_ctx* ctx, sx_slot slot, const T* src, size_t count, const T*& dst, size_t slack)
+{
+    T* p(nullptr);
+    const int rc(sx_take(ctx, slot, count, p, slack));
+    if (rc) return rc;
+    if (count) SX_CUDA(ctx, cudaMemcpyAsync(p, src, count * sizeof(T), cudaMemcpyHostToDevice, ctx->s_compute));
+    dst = p;
+    return SX_OK;
+}
+template <typename T> int sx_upload(sx_ctx* ctx, sx_slot slot, const T* src, size_t count, T*& dst, size_t slack)
+{
+    const T* p(nullptr);
+    const int rc(sx_upload(ctx, slot, src, count, p, slack));
+    dst = const_cast<T*>(p);
+    return rc;
+}
+// ... and back: `count` elements of `src` into `dst` (nothing for an empty array)
+template <typename T> int sx_download(sx_ctx* ctx, T* dst, const T* src, size_t count)
+{
+    if (count) SX_CUDA(ctx, cudaMemcpyAsync(dst, src, count * sizeof(T), cudaMemcpyDeviceToHost, ctx->s_compute));
+    return SX_OK;
+}
+
+// Reports and clears the device status word: SX_OK when it is 0, else the error of its first set bit.  The bits in `first` (a stage's
+// own) are tested before the others.  `totals`, when the caller has them, are the stage's totals the capacity messages quote.
+int sx_check_status(sx_ctx* ctx, const char* what, int first = 0, const uint32_t* totals = nullptr);
 
 // timing helpers: record kernel time on the compute stream
 struct sx_kernel_timer
@@ -147,6 +262,26 @@ struct sx_kernel_timer
         return SX_OK;
     }
     unsigned pending = 0;
+};
+
+// the host-array counterpart: the whole call on the compute stream, ev_a before the uploads and ev_b after the downloads
+struct sx_call_timer
+{
+    sx_ctx* ctx;
+    cudaError_t start; // (reported by finish)
+    explicit sx_call_timer(sx_ctx* c) : ctx(c), start(cudaEventRecord(c->ev_a, c->s_compute)) {}
+    int finish(unsigned launches)
+    {
+        SX_CUDA(ctx, start);
+        SX_CUDA(ctx, cudaEventRecord(ctx->ev_b, ctx->s_compute));
+        SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
+        float ms = 0;
+        cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b);
+        ctx->timing.kernel_ms = ms;
+        ctx->timing.launches = launches;
+        ctx->total_launches += launches;
+        return SX_OK;
+    }
 };
 
 // kernels' host launchers (each in its own .cu)

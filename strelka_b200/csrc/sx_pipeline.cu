@@ -17,9 +17,6 @@
 
 namespace
 {
-// device status bits the stages raise when one of THEIR capacities is too small (each stage's own file names its bit)
-constexpr int ST_K8_CAP = 1 << 17, ST_K9_CAP = 1 << 19; // (K7: 1 << 14 and K7a: 1 << 18 are handled by their retry loops through the totals)
-
 struct prep_out
 {
     uint32_t* seq_off;   // [n_reads + 1] byte offset of each read's packed bases (reads of a region back to back, each on a byte boundary)
@@ -211,16 +208,11 @@ __global__ void __launch_bounds__(VC_THREADS) sxp_variant_write_kernel(const sx_
     }
 }
 
-template <typename T> int take(sx_ctx* ctx, int slot, size_t count, T*& p)
-{
-    void* q(nullptr);
-    const int rc(sx_ensure(ctx, slot, count * sizeof(T) + 64, &q));
-    p = static_cast<T*>(q);
-    return rc;
-}
+// the window pass's buffers: `count` elements and 64 bytes of slack
+template <typename T> int take(sx_ctx* ctx, sx_slot slot, size_t count, T*& p) { return sx_take(ctx, slot, count, p, 64); }
 
 // the caller's array, or the context's own buffer when the caller passed NULL
-template <typename T> int pick(sx_ctx* ctx, int slot, size_t count, T* user, T*& p)
+template <typename T> int pick(sx_ctx* ctx, sx_slot slot, size_t count, T* user, T*& p)
 {
     if (user)
     {
@@ -286,12 +278,12 @@ extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_w
     // ---------------------------------------------------------------------------------------------------------------- prep
     SX_CUDA(ctx, mark(SX_WIN_ST_PREP));
     prep_out P;
-    if ((rc = take(ctx, 70, (size_t)n + 1, P.seq_off))) return rc;
-    if ((rc = take(ctx, 71, (size_t)n + 1, P.qual_off))) return rc;
-    if ((rc = take(ctx, 72, (size_t)n + 1, P.bpos))) return rc;
-    if ((rc = take(ctx, 73, (size_t)n + 1, P.non_ambig))) return rc;
-    if ((rc = take(ctx, 74, (size_t)n + 1, P.pin))) return rc;
-    if ((rc = take(ctx, 75, 4, P.maxima))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_SEQ_OFF, (size_t)n + 1, P.seq_off))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_QUAL_OFF, (size_t)n + 1, P.qual_off))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_BPOS, (size_t)n + 1, P.bpos))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_NON_AMBIG, (size_t)n + 1, P.non_ambig))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_PIN, (size_t)n + 1, P.pin))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_MAXIMA, 4, P.maxima))) return rc;
     SX_CUDA(ctx, cudaMemsetAsync(P.maxima, 0, 16, st));
     uint32_t n_raw_segs(0);
     if (n)
@@ -307,9 +299,9 @@ extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_w
     uint8_t* gate(nullptr);
     int32_t* in_pos(nullptr);
     sx_aln_seg* in_segs(nullptr);
-    if ((rc = pick(ctx, 76, (size_t)n + 1, out->gate, gate))) return rc;
-    if ((rc = take(ctx, 77, (size_t)n + 1, in_pos))) return rc;
-    if ((rc = take(ctx, 78, (size_t)n_raw_segs + 1, in_segs))) return rc;
+    if ((rc = pick(ctx, SX_SLOT_WIN_GATE, (size_t)n + 1, out->gate, gate))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_IN_POS, (size_t)n + 1, in_pos))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_IN_SEGS, (size_t)n_raw_segs + 1, in_segs))) return rc;
     {
         sx_gate_batch gb;
         memset(&gb, 0, sizeof(gb));
@@ -360,14 +352,14 @@ extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_w
     uint32_t* in_key_off(nullptr);
     uint16_t *in_keys(nullptr), *in_lead(nullptr), *in_trail(nullptr);
     uint32_t cap_in_keys(std::max<uint32_t>(64, 8u * n));
-    if ((rc = take(ctx, 79, 4, po.totals))) return rc;
-    if ((rc = take(ctx, 80, (size_t)n + 1, in_key_off))) return rc;
-    if ((rc = take(ctx, 82, (size_t)n + 1, in_lead))) return rc;
-    if ((rc = take(ctx, 83, (size_t)n + 1, in_trail))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_KEY_TOTALS, 4, po.totals))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_IN_KEY_OFF, (size_t)n + 1, in_key_off))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_IN_LEAD, (size_t)n + 1, in_lead))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_IN_TRAIL, (size_t)n + 1, in_trail))) return rc;
     uint32_t n_in_keys(0);
     for (int attempt = 0; n && attempt < 2; ++attempt)
     {
-        if ((rc = take(ctx, 81, (size_t)cap_in_keys + 1, in_keys))) return rc;
+        if ((rc = take(ctx, SX_SLOT_WIN_IN_KEYS, (size_t)cap_in_keys + 1, in_keys))) return rc;
         po.cap_keys = cap_in_keys;
         po.in_key_off = in_key_off;
         po.in_keys = in_keys;
@@ -379,7 +371,7 @@ extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_w
         if (n_in_keys <= cap_in_keys) break;
         if (attempt == 1) return sx_fail(ctx, SX_ERR_CAPACITY, "sx_process_window_dev: input-alignment keys (%u) exceed the retried capacity", n_in_keys);
         cap_in_keys = n_in_keys + 64; // the count pass has said what is needed: once more with that
-        SX_CUDA(ctx, cudaMemsetAsync(ctx->d_status, 0, sizeof(int), st)); // (clears K7A_CAP_BIT)
+        SX_CUDA(ctx, cudaMemsetAsync(ctx->d_status, 0, sizeof(int), st)); // (clears SX_ST_K7A_CAP)
     }
     eb.in_key_off = in_key_off;
     eb.in_keys = in_keys;
@@ -390,9 +382,9 @@ extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_w
     sx_enum_out eo;
     memset(&eo, 0, sizeof(eo));
     uint8_t* enum_status(nullptr);
-    if ((rc = pick(ctx, 86, (size_t)n + 1, out->enum_status, enum_status))) return rc;
-    if ((rc = take(ctx, 84, 4, eo.totals))) return rc;
-    if ((rc = take(ctx, 85, (size_t)n + 1, eo.aln_off))) return rc;
+    if ((rc = pick(ctx, SX_SLOT_WIN_ENUM_STATUS, (size_t)n + 1, out->enum_status, enum_status))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_ENUM_TOTALS, 4, eo.totals))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_ALN_OFF, (size_t)n + 1, eo.aln_off))) return rc;
     eo.status = enum_status;
     uint32_t capA(std::max<uint32_t>(256, 12u * n)), capS(std::max<uint32_t>(1024, 56u * n)), capK(std::max<uint32_t>(512, 28u * n));
     uint32_t nA(0), nS(0), nK(0);
@@ -402,13 +394,13 @@ extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_w
         eo.cap_alns = capA;
         eo.cap_segs = capS;
         eo.cap_keys = capK;
-        if ((rc = take(ctx, 87, (size_t)capA + 1, eo.aln_pos))) return rc;
-        if ((rc = take(ctx, 88, (size_t)capA + 2, eo.aln_seg_off))) return rc;
-        if ((rc = take(ctx, 89, (size_t)capS + 16, eo.segs))) return rc;
-        if ((rc = take(ctx, 90, (size_t)capA + 2, eo.aln_key_off))) return rc;
-        if ((rc = take(ctx, 91, (size_t)capK + 16, eo.aln_keys))) return rc;
-        if ((rc = take(ctx, 92, (size_t)capA + 1, eo.aln_lead_key))) return rc;
-        if ((rc = take(ctx, 93, (size_t)capA + 1, eo.aln_trail_key))) return rc;
+        if ((rc = take(ctx, SX_SLOT_WIN_ALN_POS, (size_t)capA + 1, eo.aln_pos))) return rc;
+        if ((rc = take(ctx, SX_SLOT_WIN_ALN_SEG_OFF, (size_t)capA + 2, eo.aln_seg_off))) return rc;
+        if ((rc = take(ctx, SX_SLOT_WIN_SEGS, (size_t)capS + 16, eo.segs))) return rc;
+        if ((rc = take(ctx, SX_SLOT_WIN_ALN_KEY_OFF, (size_t)capA + 2, eo.aln_key_off))) return rc;
+        if ((rc = take(ctx, SX_SLOT_WIN_ALN_KEYS, (size_t)capK + 16, eo.aln_keys))) return rc;
+        if ((rc = take(ctx, SX_SLOT_WIN_ALN_LEAD, (size_t)capA + 1, eo.aln_lead_key))) return rc;
+        if ((rc = take(ctx, SX_SLOT_WIN_ALN_TRAIL, (size_t)capA + 1, eo.aln_trail_key))) return rc;
         if ((rc = sx_k7_run(ctx, &eb, &eo, &launches))) return rc;
         uint32_t t3[3] = {0, 0, 0};
         SX_CUDA(ctx, cudaMemcpyAsync(t3, eo.totals, 12, cudaMemcpyDeviceToHost, st));
@@ -422,7 +414,7 @@ extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_w
         capA = std::max(capA, nA + 64); // the search has said what it produces: once more with that
         capS = std::max(capS, nS + 64);
         capK = std::max(capK, nK + 64);
-        SX_CUDA(ctx, cudaMemsetAsync(ctx->d_status, 0, sizeof(int), st)); // (clears the K7 capacity bit)
+        SX_CUDA(ctx, cudaMemsetAsync(ctx->d_status, 0, sizeof(int), st)); // (clears SX_ST_K7_CAP)
     }
     totals[0] = nA;
     totals[1] = nS;
@@ -438,14 +430,14 @@ extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_w
         if (want > 0xFFFFFF00ull) return sx_fail(ctx, SX_ERR_CAPACITY, "sx_process_window_dev: the window's insert pool would exceed 4 GiB; cut it into smaller windows");
         lo.cap_ins = (uint32_t)want;
     }
-    if ((rc = take(ctx, 94, 4, lo.totals))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_LINK_TOTALS, 4, lo.totals))) return rc;
     lo.regions = b->regions;
-    if ((rc = take(ctx, 95, (size_t)nA + 2, lo.alns))) return rc;
-    if ((rc = take(ctx, 96, (size_t)lo.cap_segs + 32, lo.segs))) return rc;
-    if ((rc = take(ctx, 97, (size_t)lo.cap_ins + SX_POOL_SLACK + 16, lo.ins))) return rc;
-    if ((rc = take(ctx, 98, (size_t)nS + 16, lo.k6_segs))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_LINK_ALNS, (size_t)nA + 2, lo.alns))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_LINK_SEGS, (size_t)lo.cap_segs + 32, lo.segs))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_LINK_INS, (size_t)lo.cap_ins + SX_POOL_SLACK + 16, lo.ins))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_K6_SEGS, (size_t)nS + 16, lo.k6_segs))) return rc;
     double* lnp(nullptr);
-    if ((rc = take(ctx, 99, (size_t)nA + 2, lnp))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_LNP, (size_t)nA + 2, lnp))) return rc;
     uint32_t link_totals[2] = {0, 0};
     if (n)
     {
@@ -490,10 +482,10 @@ extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_w
     if (n)
     {
         SX_CUDA(ctx, cudaStreamSynchronize(st));
-        if ((rc = pick(ctx, 100, (size_t)n_rec_slots + 1, out->recs, so.recs))) return rc;
-        if ((rc = pick(ctx, 101, (size_t)n + 1, out->n_rec, so.n_rec))) return rc;
-        if ((rc = take(ctx, 102, (size_t)n + 1, so.max_aln))) return rc;
-        if ((rc = take(ctx, 103, (size_t)n + 1, so.eval_aln))) return rc;
+        if ((rc = pick(ctx, SX_SLOT_WIN_RECS, (size_t)n_rec_slots + 1, out->recs, so.recs))) return rc;
+        if ((rc = pick(ctx, SX_SLOT_WIN_N_REC, (size_t)n + 1, out->n_rec, so.n_rec))) return rc;
+        if ((rc = take(ctx, SX_SLOT_WIN_MAX_ALN, (size_t)n + 1, so.max_aln))) return rc;
+        if ((rc = take(ctx, SX_SLOT_WIN_EVAL_ALN, (size_t)n + 1, so.eval_aln))) return rc;
         sx_score_indels_batch sb;
         memset(&sb, 0, sizeof(sb));
         sb.n_regions = nr;
@@ -522,13 +514,13 @@ extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_w
     memset(&ro, 0, sizeof(ro));
     const uint32_t need_best(nS + 2u * n + n_raw_segs + 64u);
     ro.cap_segs = out->best_segs ? out->cap_best_segs : need_best;
-    if ((rc = take(ctx, 104, 4, ro.totals))) return rc;
-    if ((rc = pick(ctx, 105, (size_t)n + 2, out->best_seg_off, ro.seg_off))) return rc;
-    if ((rc = pick(ctx, 106, (size_t)n + 1, out->best_pos, ro.pos))) return rc;
-    if ((rc = pick(ctx, 107, (size_t)n + 1, out->best_n_seg, ro.n_seg))) return rc;
-    if ((rc = pick(ctx, 108, (size_t)n + 1, out->realign_status, ro.status))) return rc;
-    if ((rc = take(ctx, 109, (size_t)n + 1, ro.best_aln))) return rc;
-    if ((rc = pick(ctx, 110, (size_t)ro.cap_segs + 16, out->best_segs, ro.segs))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_BEST_TOTALS, 4, ro.totals))) return rc;
+    if ((rc = pick(ctx, SX_SLOT_WIN_BEST_SEG_OFF, (size_t)n + 2, out->best_seg_off, ro.seg_off))) return rc;
+    if ((rc = pick(ctx, SX_SLOT_WIN_BEST_POS, (size_t)n + 1, out->best_pos, ro.pos))) return rc;
+    if ((rc = pick(ctx, SX_SLOT_WIN_BEST_N_SEG, (size_t)n + 1, out->best_n_seg, ro.n_seg))) return rc;
+    if ((rc = pick(ctx, SX_SLOT_WIN_REALIGN_STATUS, (size_t)n + 1, out->realign_status, ro.status))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_BEST_ALN, (size_t)n + 1, ro.best_aln))) return rc;
+    if ((rc = pick(ctx, SX_SLOT_WIN_BEST_SEGS, (size_t)ro.cap_segs + 16, out->best_segs, ro.segs))) return rc;
     if (n)
     {
         sx_realign_batch rb;
@@ -558,7 +550,7 @@ extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_w
     // ---------------------------------------------------------------------------------------------------------------- K4 pile-up
     SX_CUDA(ctx, mark(SX_WIN_ST_PILEUP));
     sx_pileup_read* preads(nullptr);
-    if ((rc = take(ctx, 111, (size_t)n + 2, preads))) return rc;
+    if ((rc = take(ctx, SX_SLOT_WIN_PILEUP_READS, (size_t)n + 2, preads))) return rc;
     sx_pileup_columns cols(out->cols);
     uint64_t total_bases(0);
     int st_word(0);
@@ -573,13 +565,13 @@ extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_w
         if ((rc = read_status(ctx, &st_word))) return rc;
         SX_CUDA(ctx, cudaStreamSynchronize(st));
         totals[5] = best_total;
-        if (st_word & ST_K9_CAP)
+        if (st_word & SX_ST_K9_CAP)
         {
             cudaMemsetAsync(ctx->d_status, 0, sizeof(int), st);
             if (totals_host) memcpy(totals_host, totals, sizeof(totals));
             return sx_fail(ctx, SX_ERR_CAPACITY, "sx_process_window_dev: cap_best_segs too small: %u segment slots needed", best_total);
         }
-        if (st_word & ST_K8_CAP)
+        if (st_word & SX_ST_K8_CAP)
         {
             cudaMemsetAsync(ctx->d_status, 0, sizeof(int), st);
             return sx_fail(ctx, SX_ERR_CAPACITY, "sx_process_window_dev: the linked alignments (%u segments, %u insert bytes) exceed their buffers", link_totals[0], link_totals[1]);
@@ -589,12 +581,12 @@ extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_w
         // the columns never hold more calls than the reads have bases
         total_bases = (uint64_t)b->seq4_bytes * 2u + 16u;
         const uint64_t cap_calls(cols.calls ? cols.calls_capacity : total_bases), cap_t2(cols.t2_calls ? cols.t2_capacity : (b->pileup_opts.useTier2Evidence ? total_bases : 64u));
-        if ((rc = pick(ctx, 112, (size_t)n_sites + 2, out->cols.site_off, cols.site_off))) return rc;
-        if ((rc = pick(ctx, 113, (size_t)n_sites + 2, out->cols.t2_off, cols.t2_off))) return rc;
-        if ((rc = pick(ctx, 114, (size_t)n_sites + 2, out->cols.n_spandel, cols.n_spandel))) return rc;
-        if ((rc = pick(ctx, 115, (size_t)n_sites + 2, out->cols.n_submapped, cols.n_submapped))) return rc;
-        if ((rc = pick(ctx, 116, (size_t)cap_calls + 16, out->cols.calls, cols.calls))) return rc;
-        if ((rc = pick(ctx, 117, (size_t)cap_t2 + 16, out->cols.t2_calls, cols.t2_calls))) return rc;
+        if ((rc = pick(ctx, SX_SLOT_WIN_SITE_OFF, (size_t)n_sites + 2, out->cols.site_off, cols.site_off))) return rc;
+        if ((rc = pick(ctx, SX_SLOT_WIN_T2_OFF, (size_t)n_sites + 2, out->cols.t2_off, cols.t2_off))) return rc;
+        if ((rc = pick(ctx, SX_SLOT_WIN_N_SPANDEL, (size_t)n_sites + 2, out->cols.n_spandel, cols.n_spandel))) return rc;
+        if ((rc = pick(ctx, SX_SLOT_WIN_N_SUBMAPPED, (size_t)n_sites + 2, out->cols.n_submapped, cols.n_submapped))) return rc;
+        if ((rc = pick(ctx, SX_SLOT_WIN_CALLS, (size_t)cap_calls + 16, out->cols.calls, cols.calls))) return rc;
+        if ((rc = pick(ctx, SX_SLOT_WIN_T2_CALLS, (size_t)cap_t2 + 16, out->cols.t2_calls, cols.t2_calls))) return rc;
         cols.calls_capacity = cap_calls;
         cols.t2_capacity = cap_t2;
         sx_pileup_reads_batch pb;
@@ -630,7 +622,7 @@ extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_w
     if (b->do_site_gl && n_sites)
     {
         sx_digt_result* gl(nullptr);
-        if ((rc = pick(ctx, 118, (size_t)n_sites + 1, out->site_gl, gl))) return rc;
+        if ((rc = pick(ctx, SX_SLOT_WIN_SITE_GL, (size_t)n_sites + 1, out->site_gl, gl))) return rc;
         sx_pileup_batch k2;
         memset(&k2, 0, sizeof(k2));
         k2.n_sites = n_sites;
@@ -644,7 +636,7 @@ extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_w
         {
             const uint32_t n_chunks((n_sites + VC_CHUNK - 1) / VC_CHUNK);
             uint32_t* chunk_cnt(nullptr);
-            if ((rc = take(ctx, 119, (size_t)n_chunks + 4, chunk_cnt))) return rc;
+            if ((rc = take(ctx, SX_SLOT_WIN_VARIANT_CHUNKS, (size_t)n_chunks + 4, chunk_cnt))) return rc;
             sxp_variant_count_kernel<<<n_chunks, VC_THREADS, 0, st>>>(gl, n_sites, chunk_cnt);
             sxp_variant_scan_kernel<<<1, 1024, 0, st>>>(chunk_cnt, n_chunks, chunk_cnt + n_chunks);
             sxp_variant_write_kernel<<<n_chunks, VC_THREADS, 0, st>>>(gl, cols.site_off, n_sites, b->report_begin, chunk_cnt, out->variant_sites, out->cap_variant_sites);
@@ -696,90 +688,63 @@ extern "C" int sx_process_window(sx_ctx* ctx, const sx_window_batch* b, sx_windo
     const uint32_t n_sites((uint32_t)(b->report_end - b->report_begin));
     sx_window_batch d(*b);
     int rc;
-    int slot(130);
     float h2d_ms(0), d2h_ms(0);
     cudaEvent_t e0(ctx->ev_a), e1(ctx->ev_b);
     SX_CUDA(ctx, cudaEventRecord(e0, st));
-    auto up = [&](const void* src, size_t bytes, const void** dst) -> int {
-        void* p(nullptr);
-        const int r(sx_ensure(ctx, slot++, bytes + 80, &p));
-        if (r) return r;
-        if (bytes && src) SX_CUDA(ctx, cudaMemcpyAsync(p, src, bytes, cudaMemcpyHostToDevice, st));
-        *dst = p;
-        return SX_OK;
-    };
-#define SX_UPW(field, bytes)                                                                 \
-    if ((rc = up(b->field, (size_t)(bytes), reinterpret_cast<const void**>(&d.field)))) return rc;
     const size_t n_raw(n ? b->raw_seg_off[n] : 0), n_use(n ? b->use_key_off[n] : 0), ins_bytes(nk ? b->key_ins_off[nk] : 0);
-    SX_UPW(region_read_off, ((size_t)nr + 1) * 4)
-    SX_UPW(region_key_off, ((size_t)nr + 1) * 4)
-    SX_UPW(keys, (size_t)nk * sizeof(sx_indel_key))
-    if (b->key_hap)
-    {
-        SX_UPW(key_hap, (size_t)nk * sizeof(sx_key_hap))
-    }
-    else ++slot;
-    SX_UPW(key_ins_off, ((size_t)nk + 1) * 4)
-    SX_UPW(key_ins, ins_bytes)
-    SX_UPW(realign_begin, (size_t)nr * 4)
-    SX_UPW(realign_end, (size_t)nr * 4)
-    SX_UPW(raw_pos, (size_t)n * 4)
-    SX_UPW(raw_seg_off, ((size_t)n + 1) * 4)
-    SX_UPW(raw_segs, n_raw * sizeof(sx_aln_seg))
-    SX_UPW(read_len, (size_t)n * 2)
-    SX_UPW(read_flags, (size_t)n)
-    SX_UPW(mapq, (size_t)n)
-    SX_UPW(use_key_off, ((size_t)n + 1) * 4)
-    SX_UPW(use_keys, n_use * 2)
-    SX_UPW(rec_off, ((size_t)n + 1) * 4)
-    {
-        const void* p(nullptr);
-        if ((rc = up(b->regions, ((size_t)nr + 1) * sizeof(sx_region), &p))) return rc;
-        d.regions = static_cast<sx_region*>(const_cast<void*>(p));
-    }
-    SX_UPW(seq4, (size_t)b->seq4_bytes)
-    SX_UPW(qual, (size_t)b->qual_bytes)
-    SX_UPW(ref, (size_t)b->ref_bytes)
-    if (b->cand_snv)
-    {
-        SX_UPW(cand_snv, (size_t)b->n_cand_snv * 4)
-    }
-    else ++slot;
-#undef SX_UPW
+    // An array the caller left NULL (key_ins_off without keys, every array of an empty window) is not copied; its buffer is still passed on.
+    const auto up = [&](sx_slot slot, const auto* src, size_t count, auto& dst) -> int {
+        return src ? sx_upload(ctx, slot, src, count, dst, 80) : sx_take(ctx, slot, count, dst, 80);
+    };
+    if ((rc = up(SX_SLOT_WUP_REGION_READ_OFF, b->region_read_off, (size_t)nr + 1, d.region_read_off))) return rc;
+    if ((rc = up(SX_SLOT_WUP_REGION_KEY_OFF, b->region_key_off, (size_t)nr + 1, d.region_key_off))) return rc;
+    if ((rc = up(SX_SLOT_WUP_KEYS, b->keys, nk, d.keys))) return rc;
+    if (b->key_hap && (rc = up(SX_SLOT_WUP_KEY_HAP, b->key_hap, nk, d.key_hap))) return rc;
+    if ((rc = up(SX_SLOT_WUP_KEY_INS_OFF, b->key_ins_off, (size_t)nk + 1, d.key_ins_off))) return rc;
+    if ((rc = up(SX_SLOT_WUP_KEY_INS, b->key_ins, ins_bytes, d.key_ins))) return rc;
+    if ((rc = up(SX_SLOT_WUP_REALIGN_BEGIN, b->realign_begin, nr, d.realign_begin))) return rc;
+    if ((rc = up(SX_SLOT_WUP_REALIGN_END, b->realign_end, nr, d.realign_end))) return rc;
+    if ((rc = up(SX_SLOT_WUP_RAW_POS, b->raw_pos, n, d.raw_pos))) return rc;
+    if ((rc = up(SX_SLOT_WUP_RAW_SEG_OFF, b->raw_seg_off, (size_t)n + 1, d.raw_seg_off))) return rc;
+    if ((rc = up(SX_SLOT_WUP_RAW_SEGS, b->raw_segs, n_raw, d.raw_segs))) return rc;
+    if ((rc = up(SX_SLOT_WUP_READ_LEN, b->read_len, n, d.read_len))) return rc;
+    if ((rc = up(SX_SLOT_WUP_READ_FLAGS, b->read_flags, n, d.read_flags))) return rc;
+    if ((rc = up(SX_SLOT_WUP_MAPQ, b->mapq, n, d.mapq))) return rc;
+    if ((rc = up(SX_SLOT_WUP_USE_KEY_OFF, b->use_key_off, (size_t)n + 1, d.use_key_off))) return rc;
+    if ((rc = up(SX_SLOT_WUP_USE_KEYS, b->use_keys, n_use, d.use_keys))) return rc;
+    if ((rc = up(SX_SLOT_WUP_REC_OFF, b->rec_off, (size_t)n + 1, d.rec_off))) return rc;
+    if ((rc = up(SX_SLOT_WUP_REGIONS, b->regions, (size_t)nr + 1, d.regions))) return rc;
+    if ((rc = up(SX_SLOT_WUP_SEQ4, b->seq4, b->seq4_bytes, d.seq4))) return rc;
+    if ((rc = up(SX_SLOT_WUP_QUAL, b->qual, b->qual_bytes, d.qual))) return rc;
+    if ((rc = up(SX_SLOT_WUP_REF, b->ref, b->ref_bytes, d.ref))) return rc;
+    if (b->cand_snv && (rc = up(SX_SLOT_WUP_CAND_SNV, b->cand_snv, b->n_cand_snv, d.cand_snv))) return rc;
     SX_CUDA(ctx, cudaEventRecord(e1, st));
     // device outputs for whatever the caller wants back
     sx_window_out o;
     memset(&o, 0, sizeof(o));
     const size_t n_slots(n ? b->rec_off[n] : 0);
-    auto want = [&](const void* host, size_t bytes, void** dev) -> int {
-        *dev = nullptr;
-        if (!host) return SX_OK;
-        return sx_ensure(ctx, slot++, bytes + 80, dev);
-    };
-#define SX_WANT(field, bytes)                                                            \
-    if ((rc = want(out->field, (size_t)(bytes), reinterpret_cast<void**>(&o.field)))) return rc;
-    SX_WANT(gate, n)
-    SX_WANT(enum_status, n)
-    SX_WANT(realign_status, n)
-    SX_WANT(best_pos, (size_t)n * 4)
-    SX_WANT(best_seg_off, ((size_t)n + 1) * 4)
-    SX_WANT(best_n_seg, (size_t)n * 2)
-    SX_WANT(best_segs, (size_t)out->cap_best_segs * sizeof(sx_aln_seg))
+    const auto want = [&](const void* host, sx_slot slot, size_t count, auto*& dev) -> int { return host ? sx_take(ctx, slot, count, dev, 80) : SX_OK; };
+    if ((rc = want(out->gate, SX_SLOT_WDN_GATE, n, o.gate))) return rc;
+    if ((rc = want(out->enum_status, SX_SLOT_WDN_ENUM_STATUS, n, o.enum_status))) return rc;
+    if ((rc = want(out->realign_status, SX_SLOT_WDN_REALIGN_STATUS, n, o.realign_status))) return rc;
+    if ((rc = want(out->best_pos, SX_SLOT_WDN_BEST_POS, n, o.best_pos))) return rc;
+    if ((rc = want(out->best_seg_off, SX_SLOT_WDN_BEST_SEG_OFF, (size_t)n + 1, o.best_seg_off))) return rc;
+    if ((rc = want(out->best_n_seg, SX_SLOT_WDN_BEST_N_SEG, n, o.best_n_seg))) return rc;
+    if ((rc = want(out->best_segs, SX_SLOT_WDN_BEST_SEGS, out->cap_best_segs, o.best_segs))) return rc;
     o.cap_best_segs = out->cap_best_segs;
-    SX_WANT(recs, (n_slots + 1) * sizeof(sx_read_indel_score))
-    SX_WANT(n_rec, (size_t)n * 4)
-    SX_WANT(cols.site_off, ((size_t)n_sites + 1) * 4)
-    SX_WANT(cols.t2_off, ((size_t)n_sites + 1) * 4)
-    SX_WANT(cols.n_spandel, (size_t)n_sites * 4)
-    SX_WANT(cols.n_submapped, (size_t)n_sites * 4)
-    SX_WANT(cols.calls, (size_t)out->cols.calls_capacity * 2)
-    SX_WANT(cols.t2_calls, (size_t)out->cols.t2_capacity * 2)
+    if ((rc = want(out->recs, SX_SLOT_WDN_RECS, n_slots + 1, o.recs))) return rc;
+    if ((rc = want(out->n_rec, SX_SLOT_WDN_N_REC, n, o.n_rec))) return rc;
+    if ((rc = want(out->cols.site_off, SX_SLOT_WDN_SITE_OFF, (size_t)n_sites + 1, o.cols.site_off))) return rc;
+    if ((rc = want(out->cols.t2_off, SX_SLOT_WDN_T2_OFF, (size_t)n_sites + 1, o.cols.t2_off))) return rc;
+    if ((rc = want(out->cols.n_spandel, SX_SLOT_WDN_N_SPANDEL, n_sites, o.cols.n_spandel))) return rc;
+    if ((rc = want(out->cols.n_submapped, SX_SLOT_WDN_N_SUBMAPPED, n_sites, o.cols.n_submapped))) return rc;
+    if ((rc = want(out->cols.calls, SX_SLOT_WDN_CALLS, out->cols.calls_capacity, o.cols.calls))) return rc;
+    if ((rc = want(out->cols.t2_calls, SX_SLOT_WDN_T2_CALLS, out->cols.t2_capacity, o.cols.t2_calls))) return rc;
     o.cols.calls_capacity = out->cols.calls_capacity;
     o.cols.t2_capacity = out->cols.t2_capacity;
-    SX_WANT(site_gl, (size_t)n_sites * sizeof(sx_digt_result))
-    SX_WANT(variant_sites, (size_t)out->cap_variant_sites * sizeof(sx_site_call))
+    if ((rc = want(out->site_gl, SX_SLOT_WDN_SITE_GL, n_sites, o.site_gl))) return rc;
+    if ((rc = want(out->variant_sites, SX_SLOT_WDN_VARIANT_SITES, out->cap_variant_sites, o.variant_sites))) return rc;
     o.cap_variant_sites = out->cap_variant_sites;
-#undef SX_WANT
     uint32_t totals[SX_WIN_TOTALS];
     memset(totals, 0, sizeof(totals));
     rc = sx_process_window_dev(ctx, &d, &o, totals);
@@ -789,27 +754,24 @@ extern "C" int sx_process_window(sx_ctx* ctx, const sx_window_batch* b, sx_windo
     const uint32_t launches(ctx->timing.launches);
     cudaEventElapsedTime(&h2d_ms, e0, e1);
     SX_CUDA(ctx, cudaEventRecord(e0, st));
-    auto down = [&](void* host, const void* dev, size_t bytes) -> int {
-        if (host && dev && bytes) SX_CUDA(ctx, cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, st));
-        return SX_OK;
-    };
+    const auto down = [&](auto* host, const auto* dev, size_t count) -> int { return host ? sx_download(ctx, host, dev, count) : SX_OK; }; // (what the caller asked for)
     if ((rc = down(out->gate, o.gate, n))) return rc;
     if ((rc = down(out->enum_status, o.enum_status, n))) return rc;
     if ((rc = down(out->realign_status, o.realign_status, n))) return rc;
-    if ((rc = down(out->best_pos, o.best_pos, (size_t)n * 4))) return rc;
-    if ((rc = down(out->best_seg_off, o.best_seg_off, ((size_t)n + 1) * 4))) return rc;
-    if ((rc = down(out->best_n_seg, o.best_n_seg, (size_t)n * 2))) return rc;
-    if ((rc = down(out->best_segs, o.best_segs, (size_t)totals[5] * sizeof(sx_aln_seg)))) return rc;
-    if ((rc = down(out->recs, o.recs, n_slots * sizeof(sx_read_indel_score)))) return rc;
-    if ((rc = down(out->n_rec, o.n_rec, (size_t)n * 4))) return rc;
-    if ((rc = down(out->cols.site_off, o.cols.site_off, ((size_t)n_sites + 1) * 4))) return rc;
-    if ((rc = down(out->cols.t2_off, o.cols.t2_off, ((size_t)n_sites + 1) * 4))) return rc;
-    if ((rc = down(out->cols.n_spandel, o.cols.n_spandel, (size_t)n_sites * 4))) return rc;
-    if ((rc = down(out->cols.n_submapped, o.cols.n_submapped, (size_t)n_sites * 4))) return rc;
-    if ((rc = down(out->cols.calls, o.cols.calls, (size_t)totals[6] * 2))) return rc;
-    if ((rc = down(out->cols.t2_calls, o.cols.t2_calls, (size_t)totals[7] * 2))) return rc;
-    if ((rc = down(out->site_gl, o.site_gl, (size_t)n_sites * sizeof(sx_digt_result)))) return rc;
-    if ((rc = down(out->variant_sites, o.variant_sites, (size_t)std::min(totals[8], out->cap_variant_sites) * sizeof(sx_site_call)))) return rc;
+    if ((rc = down(out->best_pos, o.best_pos, n))) return rc;
+    if ((rc = down(out->best_seg_off, o.best_seg_off, (size_t)n + 1))) return rc;
+    if ((rc = down(out->best_n_seg, o.best_n_seg, n))) return rc;
+    if ((rc = down(out->best_segs, o.best_segs, totals[5]))) return rc;
+    if ((rc = down(out->recs, o.recs, n_slots))) return rc;
+    if ((rc = down(out->n_rec, o.n_rec, n))) return rc;
+    if ((rc = down(out->cols.site_off, o.cols.site_off, (size_t)n_sites + 1))) return rc;
+    if ((rc = down(out->cols.t2_off, o.cols.t2_off, (size_t)n_sites + 1))) return rc;
+    if ((rc = down(out->cols.n_spandel, o.cols.n_spandel, n_sites))) return rc;
+    if ((rc = down(out->cols.n_submapped, o.cols.n_submapped, n_sites))) return rc;
+    if ((rc = down(out->cols.calls, o.cols.calls, totals[6]))) return rc;
+    if ((rc = down(out->cols.t2_calls, o.cols.t2_calls, totals[7]))) return rc;
+    if ((rc = down(out->site_gl, o.site_gl, n_sites))) return rc;
+    if ((rc = down(out->variant_sites, o.variant_sites, std::min(totals[8], out->cap_variant_sites)))) return rc;
     if (out->totals) memcpy(out->totals, totals, sizeof(totals));
     SX_CUDA(ctx, cudaEventRecord(e1, st));
     SX_CUDA(ctx, cudaStreamSynchronize(st));

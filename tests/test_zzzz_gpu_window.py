@@ -84,3 +84,73 @@ def test_regrouped_work_lists_change_no_output_byte(ctx, monkeypatch):
     for k in d_on:
         assert np.asarray(d_on[k]).tobytes() == np.asarray(d_off[k]).tobytes(), k
 
+
+
+def _keyless_window():
+    """one region of 40 reads without a window entry (n_keys = 0): every fourth read has a single-base mismatch"""
+    from strelka_b200 import batch as B
+
+    rng = np.random.default_rng(5)
+    ref = "".join(rng.choice(list("ACGT"), 700))
+    rb = 10000
+    reads, raw = [], []
+    for i in range(40):
+        pos = rb + 50 + 12 * i
+        seq = list(ref[pos - rb : pos - rb + 100])
+        if i % 4 == 0:
+            seq[40] = "ACGT"[("ACGT".index(seq[40]) + 1) % 4]
+        reads.append(B.EnumReadSpec("".join(seq), pos, [("M", 100)]))
+        raw.append((pos, [("M", 100)]))
+    eb = B.EnumBatch([(ref, rb, (rb, rb + 700), [], reads)])
+    return B.WindowBatch.from_enum(eb, B.GateBatch(eb, raw), B.read_pools_of(eb))
+
+
+def test_host_window_entry_takes_null_arrays(ctx):
+    """sx_process_window (host arrays in and out) passes on what a caller may leave NULL: the key arrays of a window without window entries
+    (n_keys = 0, key_ins_off / keys / key_ins / use_keys NULL) and the outputs it does not want.  Its outputs equal sx_process_window_dev's
+    on the same window.  An empty window (no regions, no reads, every array NULL) runs and reports nothing."""
+    import ctypes as C
+
+    from strelka_b200 import _abi as A
+    from strelka_b200 import batch as B
+    from strelka_b200.api import DevWindow
+
+    w = _keyless_window()
+    assert w.n_keys == 0 and w.n_reads == 40
+    dw = DevWindow(ctx, w)
+    dw.run()
+    d = dw.download()
+    c = A.SxWindowBatch.from_buffer_copy(dw.c)
+    host = {name: (None if w.a.get(name) is None or name in ("keys", "key_ins_off", "key_ins", "use_keys") else np.ascontiguousarray(w.a[name]))
+            for name in B.WindowBatch.ARRAYS}
+    for name, arr in host.items():
+        setattr(c, name, None if arr is None else arr.ctypes.data)
+    n, ns, cap = w.n_reads, w.n_sites, int(dw.out.cols.calls_capacity)
+    h = {"gate": np.zeros(n, np.uint8), "best_pos": np.zeros(n, np.int32), "best_seg_off": np.zeros(n + 1, np.uint32), "best_n_seg": np.zeros(n, np.uint16),
+         "best_segs": np.zeros(dw.cap_best, A.ALN_SEG_DT), "n_rec": np.zeros(n, np.uint32), "site_off": np.zeros(ns + 1, np.uint32), "t2_off": np.zeros(ns + 1, np.uint32),
+         "n_spandel": np.zeros(ns, np.uint32), "n_submapped": np.zeros(ns, np.uint32), "calls": np.zeros(cap, np.uint16), "t2_calls": np.zeros(cap, np.uint16),
+         "site_gl": np.zeros(ns, A.DIGT_RESULT_DT)}
+    o = A.SxWindowOut()  # enum_status, realign_status, recs, totals and variant_sites stay NULL
+    for k in ("gate", "best_pos", "best_seg_off", "best_n_seg", "best_segs", "n_rec", "site_gl"):
+        setattr(o, k, h[k].ctypes.data)
+    o.cap_best_segs = dw.cap_best
+    o.cols = A.SxPileupColumns(h["site_off"].ctypes.data, h["calls"].ctypes.data, h["t2_off"].ctypes.data, h["t2_calls"].ctypes.data, h["n_spandel"].ctypes.data,
+                               h["n_submapped"].ctypes.data, cap, cap)
+    totals = np.zeros(A.SX_WIN_TOTALS, np.uint32)
+    ctx._chk(ctx.lib.sx_process_window(ctx.h, C.byref(c), C.byref(o), totals.ctypes.data))
+    dw.free()
+    assert totals[6] > 0 and np.array_equal(totals[:8], d["totals"][:8]), (totals, d["totals"])
+    h["best_segs"] = h["best_segs"][: int(h["best_seg_off"][n])]
+    h["calls"], h["t2_calls"] = h["calls"][: int(totals[6])], h["t2_calls"][: int(totals[7])]
+    for k, v in h.items():
+        assert v.tobytes() == np.asarray(d[k]).tobytes(), k
+
+    e = A.SxWindowBatch()
+    ctx.lib.sx_default_window_opts(C.byref(e))
+    e.ref_begin = e.report_begin = e.report_end = 1000
+    site_off = np.full(1, 7, np.uint32)
+    eo = A.SxWindowOut()
+    eo.cols = A.SxPileupColumns(site_off.ctypes.data, None, None, None, None, None, 0, 0)
+    totals[:] = 1
+    ctx._chk(ctx.lib.sx_process_window(ctx.h, C.byref(e), C.byref(eo), totals.ctypes.data))
+    assert not totals.any() and site_off[0] == 0, (totals, site_off)
