@@ -578,6 +578,104 @@ int sx_score_indels(sx_ctx* ctx, const sx_score_indels_batch* batch_host, const 
 int sx_score_indels_dev(sx_ctx* ctx, const sx_score_indels_batch* batch_dev, const double* lnp_dev, sx_score_indels_out* out_dev);
 
 /* ==========================================================================================
+ * K5b  somatic_indel
+ *   replaces _dopt.sicaller_grid().get_somatic_indel(...) of strelka_pos_processor::process_pos_indel_somatic
+ *   (applications/strelka/strelka_pos_processor.cpp:343-348) ->
+ *   somatic_indel_caller_grid::get_somatic_indel      applications/strelka/somatic_indel_grid.cpp:181-361, with
+ *     is_multi_indel_allele :100-175, get_indel_het_grid_lhood :66-90,
+ *     get_indel_digt_lhood / get_high_low_het_ratio_lhood / get_het_observed_allele_ratio
+ *                                                    starling_common/starling_indel_call_pprob_digt.cpp:40-155,240-336,
+ *     get_sum_path_pprob :186-235 with indel_lnp_to_pprob (starling_common/AlleleReportInfoUtil.cpp:220-297),
+ *     is_indel_conflict (starling_common/indel_util.cpp:29-45), calculate_result_set_grid (qscore_calculator.cpp:47-209).
+ *
+ * Per locus: the candidate indel (type INDEL; breakpoints are not accepted), IndelData::isForcedOutput, the index of the
+ * tumor sample's indelToRefErrorProb in the caller's error-rate table, the table of distinct alternate indels the locus's
+ * reads name (only pos, del_len, ins_len and type are read: what is_indel_conflict reads), and per sample (normal, then
+ * tumor) the IndelSampleData::read_path_lnp entries in map order (ascending read id).
+ *
+ * The error-rate table is HOST memory in both entry points (like sx_ga_scores): the library evaluates
+ * std::pow(p, shared_indel_error_factor), std::log and log1p_switch of each entry on the host, in the caller's process, so the
+ * shared-error terms are the reference's own bits, and uploads the resulting float pairs.
+ *
+ * Capacities: at most SX_SINDEL_MAX_ALTS table entries per locus and two alternates per read (ReadPathScores keeps the two best).
+ * A locus over a capacity gets SX_SINDEL_ST_CAP in its status and no result; it is never truncated.  Every result field
+ * is written, so a caller can compare whole records.
+ * ======================================================================================== */
+#define SX_SINDEL_MAX_ALTS 16
+#define SX_SINDEL_ST_CAP 0x100000u /* locus status: over a capacity above, no result */
+
+typedef struct sx_sindel_read { /* one read_path_lnp entry (ReadPathScores, starling_common/IndelData.hh:64-125), 24 bytes */
+    float ref;                 /* ReadPathScores::ref   (score_t = float) */
+    float indel;               /* ReadPathScores::indel */
+    float alt_lnp[2];          /* alt_indel[i].second, in alt_indel order */
+    uint16_t read_length;      /* ReadPathScores::read_length */
+    uint16_t non_ambig;        /* ReadPathScores::nonAmbiguousBasesInRead */
+    uint8_t is_tier1;          /* ReadPathScores::is_tier1_read */
+    uint8_t n_alt;             /* alt_indel.size(), <= 2 */
+    uint8_t alt[2];            /* alt_indel[i].first, as an index into the locus's alternate table */
+} sx_sindel_read;
+
+typedef struct sx_sindel_batch {
+    uint32_t n_loci;
+    uint32_t pad;
+    const sx_indel_key* key;          /* [n_loci] the candidate: del_len, ins_len and type (must be SX_INDEL_TYPE_INDEL) are read */
+    const uint8_t* is_forced_output;  /* [n_loci] IndelData::isForcedOutput */
+    const uint32_t* err_idx;          /* [n_loci] index of the tumor sample's indelToRefErrorProb.getValue() in the error-rate table */
+    const uint32_t* alt_off;          /* [n_loci+1] locus l's alternate table is alts[alt_off[l] .. alt_off[l+1]) */
+    const sx_indel_key* alts;         /* pos, del_len, ins_len, type are read */
+    const uint32_t* read_off;         /* [2*n_loci+1] locus l's normal reads are reads[read_off[2l] .. read_off[2l+1]),
+                                         its tumor reads reads[read_off[2l+1] .. read_off[2l+2]) */
+    const sx_sindel_read* reads;
+} sx_sindel_batch;
+
+typedef struct sx_sindel_opts { /* strelka_options (applications/strelka/strelka_shared.hh:70-151), starling_base_options */
+    double somatic_indel_rate;          /* 1e-6 */
+    double bindel_diploid_theta;        /* 1e-4  (starling_common/starling_base_shared.hh:95) */
+    double indel_contam_tolerance;      /* 0.15 */
+    double shared_indel_error_factor;   /* 1.65 */
+    double randomBaseMatchProb;         /* 0.5   (strelka's noisy-read setting, strelka_shared.hh:74) */
+    double tier2RandomBaseMatchProb;    /* 0.25  (Tier2Options.hh:49; set it to randomBaseMatchProb where
+                                           tier2.isRandomBaseMatchProb is off: starling_base_shared.cpp:44-52) */
+    int32_t useTier2Evidence;           /* 1     (strelka_shared.hh:78) */
+    int32_t min_read_bp_flank[2];       /* [normal, tumor] = 1 (normal_sample_min_read_bp_flank), 5 (default_min_read_bp_flank) */
+    int32_t pad;
+} sx_sindel_opts;
+
+typedef struct sx_sindel_tier { /* indel_result_set (somatic_result_set.hh) of one tier, and the likelihoods handed to the grid */
+    float normal_lhood[21];    /* DIGT_GRID order: STAR_DIINDEL NOINDEL, HOM, HET, then the het grid (low 3..11, high 12..20) */
+    float tumor_lhood[21];
+    int32_t qphred;
+    int32_t from_ntype_qphred;
+    uint32_t ntype;            /* SOMATIC_DIGT */
+    uint32_t max_gt;           /* DDIGT state */
+    uint8_t evaluated;         /* 1: calculate_result_set_grid ran; else only qphred (0) and is_overlap are defined, the rest is 0 */
+    uint8_t is_overlap;
+    uint8_t multi_indel;       /* is_multi_indel_allele rejected the tier (qphred is then 0; with forced output the tier is evaluated) */
+    uint8_t pad;
+} sx_sindel_tier;
+
+typedef struct sx_sindel_result { /* somatic_indel_call */
+    sx_sindel_tier tier[2];
+    uint32_t status;           /* 0, or SX_SINDEL_ST_CAP (nothing else is written) */
+    uint8_t is_output;         /* somatic_indel_call::is_output(); 0: get_somatic_indel returned early, the fields below are 0 */
+    uint8_t sindel_tier;
+    uint8_t sindel_from_ntype_tier;
+    uint8_t is_overlap;        /* rs.is_overlap */
+    uint32_t ntype;            /* NTYPE: REF 0, HOM 1, HET 2, CONFLICT 3.  Forced output with useTier2Evidence off: unspecified
+                                  (the reference compares tier 1's never-assigned ntype, somatic_indel_grid.cpp:322) */
+    uint32_t max_gt;
+    int32_t qphred;            /* QSI */
+    int32_t from_ntype_qphred; /* QSI_NT; unspecified where ntype is */
+} sx_sindel_result;
+
+void sx_default_sindel_opts(sx_sindel_opts* o);
+/* err_prob_host: [n_err] the distinct indelToRefErrorProb values (host memory in both entry points) */
+int sx_somatic_indel(sx_ctx* ctx, const sx_sindel_opts* opts, const sx_sindel_batch* batch_host, const double* err_prob_host, uint32_t n_err,
+                     sx_sindel_result* out_host /*[n_loci]*/);
+int sx_somatic_indel_dev(sx_ctx* ctx, const sx_sindel_opts* opts, const sx_sindel_batch* batch_dev, const double* err_prob_host, uint32_t n_err,
+                         sx_sindel_result* out_dev);
+
+/* ==========================================================================================
  * K7  enumerate_alignments   (SURVEY 8a row a3 / 8f3: the producer of K1's and K6's input)
  *   replaces  getCandidateAlignments           starling_common/starling_read_align.cpp:1816-1994
  *   with      candidate_alignment_search       :857-1277  (the recursive toggle search)

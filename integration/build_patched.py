@@ -1,10 +1,10 @@
 #!/usr/bin/env python
 """integration/build_patched.py -- compiles the shim FOR REAL (SURVEY 8b, VERDICT row g1): makes patched COPIES of three reference translation
 units under oracle/_ref/build/patched/ (git-ignored scratch; the reference tree is read-only and stays untouched, nothing of it enters this
-repository), each edit a single call-site substitution, compiles them with the oracle build's flags and links
+repository), each edit a call-site substitution, compiles them with the oracle build's flags and links
 
     oracle/_ref/bin/starling2_sx   germline caller: computeSampleDiploidSiteGenotype -> sx_site_gl_germline (K2a), haplotype alignment -> sx_global_align (K3)
-    oracle/_ref/bin/strelka2_sx    somatic caller:  position_somatic_snv_call -> sx_site_gl_somatic (K2b)
+    oracle/_ref/bin/strelka2_sx    somatic caller:  position_somatic_snv_call -> sx_site_gl_somatic (K2b), get_somatic_indel -> sx_somatic_indel (K5b)
     oracle/_ref/bin/starling2, strelka2   the unmodified reference binaries (oracle/build_ref.sh --bins)
 
 against strelka_b200/csrc/libstrelka_b200.so.  It also stages the bundled demo inputs (BAMs, reference, model files, expected VCFs) under
@@ -37,7 +37,13 @@ EDITS = [
        r"normal_epi_t2_ptr,\s*tumor_epi_t2_ptr,\s*isComputeNonSomatic,\s*sgtg\);",
        "if (sx_shim::enabled() && !isComputeNonSomatic) sx_shim::site_gl_somatic(_opt, normal_cpi_ptr[0]->rawPileup(), tumor_cpi_ptr[0]->rawPileup(), sgtg);\n"
        "        else _dopt.sscaller_strand_grid().position_somatic_snv_call(normal_cpi_ptr[0]->getExtendedPosInfo(), tumor_cpi_ptr[0]->getExtendedPosInfo(),\n"
-       "                                                                    normal_epi_t2_ptr, tumor_epi_t2_ptr, isComputeNonSomatic, sgtg);")], "#define SX_SHIM_SOMATIC\n"),
+       "                                                                    normal_epi_t2_ptr, tumor_epi_t2_ptr, isComputeNonSomatic, sgtg);"),
+      (r"_dopt\.sicaller_grid\(\)\.get_somatic_indel\(\s*_opt,\s*_dopt,\s*normal_sif\.sampleOptions,\s*tumor_sif\.sampleOptions,\s*indelKey,\s*indelData,\s*NORMAL,\s*TUMOR,\s*"
+       r"is_use_alt_indel,\s*siInfo\.sindel\);",
+       "if (sx_shim::enabled() && is_use_alt_indel) sx_shim::somatic_indel(_opt, _dopt, normal_sif.sampleOptions, tumor_sif.sampleOptions, indelKey, indelData, NORMAL, TUMOR,\n"
+       "                                                                 siInfo.sindel);\n"
+       "            else _dopt.sicaller_grid().get_somatic_indel(_opt, _dopt, normal_sif.sampleOptions, tumor_sif.sampleOptions, indelKey, indelData, NORMAL, TUMOR,\n"
+       "                                                         is_use_alt_indel, siInfo.sindel);")], "#define SX_SHIM_SOMATIC\n"),
 ]
 
 

@@ -34,12 +34,12 @@ inline bool enabled()
 
 struct Counters
 {
-    unsigned long long site_gl_germline = 0, site_gl_somatic = 0, global_align = 0;
+    unsigned long long site_gl_germline = 0, site_gl_somatic = 0, global_align = 0, somatic_indel = 0;
     ~Counters()
     {
         if (std::getenv("SX_SHIM_REPORT"))
-            std::fprintf(stderr, "sx_shim: %llu germline site calls, %llu somatic site calls, %llu haplotype alignments through libstrelka_b200.so\n", site_gl_germline,
-                         site_gl_somatic, global_align);
+            std::fprintf(stderr, "sx_shim: %llu germline site calls, %llu somatic site calls, %llu haplotype alignments through libstrelka_b200.so, %llu somatic indel calls\n",
+                         site_gl_germline, site_gl_somatic, global_align, somatic_indel);
     }
 };
 inline Counters& counters()
@@ -151,14 +151,19 @@ inline void global_align(const AlignmentScores<int>& sc, const std::string& quer
 #ifdef SX_SHIM_SOMATIC
 /// sscaller_strand_grid().position_somatic_snv_call(nepi, tepi, nepi_t2, tepi_t2, isComputeNonSomatic = false, sgtg)
 /// (applications/strelka/strelka_pos_processor.cpp:213-219), from the RAW tumor / normal columns (tier1 + tier2 calls)
-inline void site_gl_somatic(const strelka_options& opt, const snp_pos_info& normal, const snp_pos_info& tumor, somatic_snv_genotype_grid& sgtg)
+inline sx_params somatic_params_of(const strelka_options& opt)
 {
     sx_params p(params_of(opt));
     p.somatic_snv_rate = opt.somatic_snv_rate;
     p.shared_site_error_rate = opt.shared_site_error_rate;
     p.shared_site_error_strand_bias_fraction = opt.shared_site_error_strand_bias_fraction;
     p.ssnv_contam_tolerance = opt.ssnv_contam_tolerance;
-    sx_ctx* ctx(context(p));
+    return p;
+}
+
+inline void site_gl_somatic(const strelka_options& opt, const snp_pos_info& normal, const snp_pos_info& tumor, somatic_snv_genotype_grid& sgtg)
+{
+    sx_ctx* ctx(context(somatic_params_of(opt)));
     const uint16_t none(0);
     const char ref_base(normal.get_ref_base());
     const snp_pos_info* pi[2] = {&normal, &tumor};
@@ -195,6 +200,106 @@ inline void site_gl_somatic(const strelka_options& opt, const snp_pos_info& norm
     sgtg.rs.normal_alt_id = r.normal_alt_id;
     sgtg.rs.tumor_alt_id = r.tumor_alt_id;
     sgtg.rs.strandBias = r.strandBias;
+}
+
+/// _dopt.sicaller_grid().get_somatic_indel(_opt, _dopt, normal_opt, tumor_opt, indelKey, indelData, NORMAL, TUMOR, is_use_alt_indel = true, sindel)
+/// (applications/strelka/strelka_pos_processor.cpp:343-348) as a one-locus sx_somatic_indel batch built from the two samples' read_path_lnp.
+/// A locus the library does not take -- more distinct alternates than SX_SINDEL_MAX_ALTS, a read with more than two, or an alternate that is
+/// neither an indel nor a mismatch -- runs through the reference's own function instead.
+inline void somatic_indel(const strelka_options& opt, const strelka_deriv_options& dopt, const starling_sample_options& normal_opt,
+                          const starling_sample_options& tumor_opt, const IndelKey& indelKey, const IndelData& indelData, const unsigned normalSampleIndex,
+                          const unsigned tumorSampleIndex, somatic_indel_call& sindel)
+{
+    auto cpu = [&]() {
+        dopt.sicaller_grid().get_somatic_indel(opt, dopt, normal_opt, tumor_opt, indelKey, indelData, normalSampleIndex, tumorSampleIndex, true, sindel);
+    };
+    const IndelSampleData* sd[2] = {&indelData.getSampleData(normalSampleIndex), &indelData.getSampleData(tumorSampleIndex)};
+    auto key_of = [](const IndelKey& k, sx_indel_key& o) {
+        std::memset(&o, 0, sizeof(o));
+        o.pos = static_cast<int32_t>(k.pos);
+        o.del_len = static_cast<uint16_t>(k.delete_length());
+        o.ins_len = static_cast<uint16_t>(k.insert_length());
+        o.type = k.isMismatch() ? SX_INDEL_TYPE_MISMATCH : SX_INDEL_TYPE_INDEL;
+    };
+    // the distinct alternates the reads name (get_sum_path_pprob keys them by IndelKey) and the reads in map order
+    std::vector<IndelKey> alt_keys;
+    std::vector<sx_sindel_read> reads;
+    uint32_t read_off[3] = {0u, 0u, 0u};
+    for (unsigned s = 0; s < 2; ++s)
+    {
+        for (const auto& e : sd[s]->read_path_lnp)
+        {
+            const ReadPathScores& rp(e.second);
+            if (rp.alt_indel.size() > 2) return cpu();
+            sx_sindel_read r;
+            std::memset(&r, 0, sizeof(r));
+            r.ref = rp.ref;
+            r.indel = rp.indel;
+            r.read_length = rp.read_length;
+            r.non_ambig = rp.nonAmbiguousBasesInRead;
+            r.is_tier1 = rp.is_tier1_read ? 1 : 0;
+            r.n_alt = static_cast<uint8_t>(rp.alt_indel.size());
+            for (unsigned k = 0; k < rp.alt_indel.size(); ++k)
+            {
+                const IndelKey& ak(rp.alt_indel[k].first);
+                if (ak.type != INDEL::INDEL && ak.type != INDEL::MISMATCH) return cpu();
+                unsigned idx(0);
+                while (idx < alt_keys.size() && !(alt_keys[idx] == ak)) ++idx;
+                if (idx == alt_keys.size())
+                {
+                    if (alt_keys.size() == SX_SINDEL_MAX_ALTS) return cpu();
+                    alt_keys.push_back(ak);
+                }
+                r.alt[k] = static_cast<uint8_t>(idx);
+                r.alt_lnp[k] = rp.alt_indel[k].second;
+            }
+            reads.push_back(r);
+        }
+        read_off[s + 1] = static_cast<uint32_t>(reads.size());
+    }
+    sx_ctx* ctx(context(somatic_params_of(opt)));
+    sx_sindel_opts o;
+    sx_default_sindel_opts(&o);
+    o.somatic_indel_rate = opt.somatic_indel_rate;
+    o.bindel_diploid_theta = opt.bindel_diploid_theta;
+    o.indel_contam_tolerance = opt.indel_contam_tolerance;
+    o.shared_indel_error_factor = opt.shared_indel_error_factor;
+    o.randomBaseMatchProb = opt.randomBaseMatchProb;
+    o.tier2RandomBaseMatchProb = opt.tier2.isRandomBaseMatchProb ? opt.tier2.randomBaseMatchProb : opt.randomBaseMatchProb; // starling_base_shared.cpp:44-52
+    o.useTier2Evidence = opt.useTier2Evidence ? 1 : 0;
+    o.min_read_bp_flank[0] = normal_opt.min_read_bp_flank;
+    o.min_read_bp_flank[1] = tumor_opt.min_read_bp_flank;
+    sx_indel_key key;
+    key_of(indelKey, key);
+    std::vector<sx_indel_key> alts(alt_keys.size() + 1);
+    for (unsigned a = 0; a < alt_keys.size(); ++a) key_of(alt_keys[a], alts[a]);
+    if (reads.empty()) reads.resize(1); // (a valid pointer; read_off says there are none)
+    const uint8_t forced(indelData.isForcedOutput ? 1 : 0);
+    const uint32_t err_idx(0), alt_off[2] = {0u, static_cast<uint32_t>(alt_keys.size())};
+    const double err_prob(sd[1]->getErrorRates().indelToRefErrorProb.getValue());
+    sx_sindel_batch b;
+    std::memset(&b, 0, sizeof(b));
+    b.n_loci = 1;
+    b.key = &key;
+    b.is_forced_output = &forced;
+    b.err_idx = &err_idx;
+    b.alt_off = alt_off;
+    b.alts = alts.data();
+    b.read_off = read_off;
+    b.reads = reads.data();
+    sx_sindel_result r;
+    check(ctx, sx_somatic_indel(ctx, &o, &b, &err_prob, 1, &r));
+    if (r.status != 0) return cpu(); // (SX_SINDEL_ST_CAP; not reached after the checks above)
+    ++counters().somatic_indel;
+    sindel.is_forced_output = indelData.isForcedOutput;
+    if (!r.is_output) return; // the reference returned before the tier choice (somatic_indel_grid.cpp:296-300)
+    sindel.sindel_tier = r.sindel_tier != 0;
+    sindel.sindel_from_ntype_tier = r.sindel_from_ntype_tier != 0;
+    sindel.rs.ntype = r.ntype;
+    sindel.rs.max_gt = r.max_gt;
+    sindel.rs.qphred = r.qphred;
+    sindel.rs.from_ntype_qphred = r.from_ntype_qphred;
+    sindel.rs.is_overlap = r.is_overlap != 0;
 }
 #endif
 } // namespace sx_shim

@@ -99,6 +99,34 @@ class SxIndelBatch(C.Structure):
         "read_off", "lnp_off", "allele_off", "ploidy", "allele_del_len", "allele_ins_len", "allele_lnp", "read_length", "non_ambig", "is_fwd")]
 
 
+# K5b somatic_indel
+SX_SINDEL_MAX_ALTS = 16
+SX_SINDEL_ST_CAP = 0x100000
+SINDEL_READ_DT = np.dtype([("ref", "<f4"), ("indel", "<f4"), ("alt_lnp", "<f4", (2,)), ("read_length", "<u2"), ("non_ambig", "<u2"),
+                           ("is_tier1", "u1"), ("n_alt", "u1"), ("alt", "u1", (2,))])
+SINDEL_TIER_DT = np.dtype([("normal_lhood", "<f4", (21,)), ("tumor_lhood", "<f4", (21,)), ("qphred", "<i4"), ("from_ntype_qphred", "<i4"),
+                           ("ntype", "<u4"), ("max_gt", "<u4"), ("evaluated", "u1"), ("is_overlap", "u1"), ("multi_indel", "u1"), ("pad", "u1")])
+SINDEL_RESULT_DT = np.dtype([("tier", SINDEL_TIER_DT, (2,)), ("status", "<u4"), ("is_output", "u1"), ("sindel_tier", "u1"), ("sindel_from_ntype_tier", "u1"),
+                             ("is_overlap", "u1"), ("ntype", "<u4"), ("max_gt", "<u4"), ("qphred", "<i4"), ("from_ntype_qphred", "<i4")])
+
+
+class SxSindelOpts(C.Structure):
+    _fields_ = [(n, C.c_double) for n in ("somatic_indel_rate", "bindel_diploid_theta", "indel_contam_tolerance", "shared_indel_error_factor",
+                                          "randomBaseMatchProb", "tier2RandomBaseMatchProb")] + [
+        ("useTier2Evidence", C.c_int32), ("min_read_bp_flank", C.c_int32 * 2), ("pad", C.c_int32)]
+
+
+class SxSindelBatch(C.Structure):
+    _fields_ = [("n_loci", C.c_uint32), ("pad", C.c_uint32)] + [(n, C.c_void_p) for n in (
+        "key", "is_forced_output", "err_idx", "alt_off", "alts", "read_off", "reads")]
+
+
+def default_sindel_opts() -> SxSindelOpts:
+    o = SxSindelOpts()
+    load().sx_default_sindel_opts(C.byref(o))
+    return o
+
+
 class SxAlignBatch(C.Structure):
     _fields_ = [
         ("n_regions", C.c_uint32),
@@ -391,6 +419,9 @@ SYMBOLS = [
     ("sx_link_alignments_dev", C.c_int, [_P, C.POINTER(SxEnumBatch), C.POINTER(SxEnumOut), C.c_uint32, _P, _P, C.POINTER(SxLinkOut)]),
     ("sx_indel_gl", C.c_int, [_P, C.POINTER(SxIndelBatch), _P]),
     ("sx_indel_gl_dev", C.c_int, [_P, C.POINTER(SxIndelBatch), _P]),
+    ("sx_default_sindel_opts", None, [C.POINTER(SxSindelOpts)]),
+    ("sx_somatic_indel", C.c_int, [_P, C.POINTER(SxSindelOpts), C.POINTER(SxSindelBatch), _P, C.c_uint32, _P]),
+    ("sx_somatic_indel_dev", C.c_int, [_P, C.POINTER(SxSindelOpts), C.POINTER(SxSindelBatch), _P, C.c_uint32, _P]),
     ("sx_default_pileup_opts", None, [C.POINTER(SxPileupOpts)]),
     ("sx_pileup_reads", C.c_int, [_P, C.POINTER(SxPileupReadsBatch), C.POINTER(SxPileupColumns)]),
     ("sx_pileup_reads_dev", C.c_int, [_P, C.POINTER(SxPileupReadsBatch), C.POINTER(SxPileupColumns)]),

@@ -214,6 +214,40 @@ def _indel_gl(self, ib: "B.IndelBatch", out=None) -> np.ndarray:
 Context.indel_gl = _indel_gl  # K5
 
 
+def _somatic_indel(self, sb: "B.SomaticIndelBatch", opts: Optional[A.SxSindelOpts] = None, out=None) -> np.ndarray:
+    """K5b: get_somatic_indel of every locus (host arrays in, sx_sindel_result records out)."""
+    if out is None:
+        out = np.zeros(sb.n_loci, A.SINDEL_RESULT_DT)
+    o = opts or A.default_sindel_opts()
+    self._chk(self.lib.sx_somatic_indel(self.h, C.byref(o), C.byref(sb.c), A.ptr(sb.err_prob), sb.err_prob.size, out.ctypes.data))
+    return out
+
+
+class DevSomaticIndelBatch:
+    """sx_sindel_batch whose arrays live in HBM, with a device output buffer; the error-rate table stays on the host."""
+
+    _ARRAYS = ("key", "is_forced_output", "err_idx", "alt_off", "alts", "read_off", "reads")
+
+    def __init__(self, ctx: "Context", hb: "B.SomaticIndelBatch"):
+        self.host = hb
+        self.bufs = {n: DeviceArray(ctx, getattr(hb, n).nbytes + 64).upload(getattr(hb, n)) for n in self._ARRAYS}
+        self.c = A.SxSindelBatch(hb.n_loci, 0, *(self.bufs[n].ptr for n in self._ARRAYS))
+        self.out = DeviceArray(ctx, max(1, hb.n_loci) * A.SINDEL_RESULT_DT.itemsize)
+
+    def download(self) -> np.ndarray:
+        return self.out.download(A.SINDEL_RESULT_DT, self.host.n_loci)
+
+
+def _somatic_indel_dev(self, db: DevSomaticIndelBatch, opts: Optional[A.SxSindelOpts] = None) -> None:
+    o = opts or A.default_sindel_opts()
+    hb = db.host
+    self._chk(self.lib.sx_somatic_indel_dev(self.h, C.byref(o), C.byref(db.c), A.ptr(hb.err_prob), hb.err_prob.size, db.out.ptr))
+
+
+Context.somatic_indel = _somatic_indel  # K5b
+Context.somatic_indel_dev = _somatic_indel_dev
+
+
 def _pileup_reads(self, pb: B.PileupReadsBatch):
     """K4: per-position base_call columns of a read batch (host buffers in, host columns out)."""
     out = B.PileupColumns(pb)

@@ -473,6 +473,64 @@ class IndelBatch:
 
 
 # ------------------------------------------------------------------------------------------------------------------
+# K5b somatic_indel
+# ------------------------------------------------------------------------------------------------------------------
+class SomaticIndelBatch:
+    """sx_sindel_batch plus its host error-rate table.  Built from flat arrays (`SomaticIndelBatch(...)`) or from per-locus dicts
+    (`SomaticIndelBatch.from_loci`)."""
+
+    def __init__(self, key, is_forced_output, err_idx, err_prob, alt_off, alts, read_off, reads):
+        self.key = np.ascontiguousarray(key, A.INDEL_KEY_DT)
+        self.n_loci = n = self.key.size
+        self.is_forced_output = np.ascontiguousarray(is_forced_output, np.uint8)
+        self.err_idx = np.ascontiguousarray(err_idx, np.uint32)
+        self.err_prob = np.ascontiguousarray(err_prob, np.float64)
+        self.alt_off = np.ascontiguousarray(alt_off, np.uint32)
+        self.alts = np.ascontiguousarray(alts, A.INDEL_KEY_DT)
+        self.read_off = np.ascontiguousarray(read_off, np.uint32)
+        self.reads = np.ascontiguousarray(reads, A.SINDEL_READ_DT)
+        assert self.is_forced_output.size == n and self.err_idx.size == n and self.alt_off.size == n + 1 and self.read_off.size == 2 * n + 1
+        assert self.alt_off[-1] == self.alts.size and self.read_off[-1] == self.reads.size
+        self._keep = [a if a.size else np.zeros(1, a.dtype) for a in (self.key, self.is_forced_output, self.err_idx, self.alts, self.reads)]
+        k, f, e, al, rd = self._keep
+        self.c = A.SxSindelBatch(n, 0, A.ptr(k), A.ptr(f), A.ptr(e), A.ptr(self.alt_off), A.ptr(al), A.ptr(self.read_off), A.ptr(rd))
+
+    @staticmethod
+    def from_loci(loci) -> "SomaticIndelBatch":
+        """loci: dicts {key: (pos, del_len, ins_len), forced, err_prob, alts: [(pos, del_len, ins_len, ins_id)] (distinct keys),
+        reads: ([normal reads], [tumor reads])}, a read being (ref, indel, read_length, non_ambig, is_tier1, [(alt index, lnp)] <= 2),
+        in read_path_lnp order.  Equal error probabilities share one table entry."""
+        n = len(loci)
+        key = np.zeros(n, A.INDEL_KEY_DT)
+        forced = np.zeros(n, np.uint8)
+        err_idx = np.zeros(n, np.uint32)
+        table: dict = {}
+        alt_off = np.zeros(n + 1, np.uint32)
+        read_off = np.zeros(2 * n + 1, np.uint32)
+        alts, reads = [], []
+        for i, l in enumerate(loci):
+            key[i]["pos"], key[i]["del_len"], key[i]["ins_len"] = l["key"]
+            forced[i] = 1 if l.get("forced") else 0
+            err_idx[i] = table.setdefault(float(l["err_prob"]), len(table))
+            alts.extend(l["alts"])
+            alt_off[i + 1] = alt_off[i] + len(l["alts"])
+            for s in range(2):
+                reads.extend(l["reads"][s])
+                read_off[2 * i + s + 1] = read_off[2 * i + s] + len(l["reads"][s])
+        ak = np.zeros(len(alts), A.INDEL_KEY_DT)
+        for j, (pos, dl, il, ins_id) in enumerate(alts):
+            ak[j]["pos"], ak[j]["del_len"], ak[j]["ins_len"], ak[j]["ins_id"] = pos, dl, il, ins_id
+        rd = np.zeros(len(reads), A.SINDEL_READ_DT)
+        for j, (ref, indel, rlen, nonamb, t1, ra) in enumerate(reads):
+            r = rd[j]
+            r["ref"], r["indel"], r["read_length"], r["non_ambig"], r["is_tier1"], r["n_alt"] = ref, indel, rlen, nonamb, 1 if t1 else 0, len(ra)
+            for k, (a, lnp) in enumerate(ra[:2]):
+                r["alt"][k], r["alt_lnp"][k] = a, lnp
+        err = np.array(sorted(table, key=table.get), np.float64)
+        return SomaticIndelBatch(key, forced, err_idx, err, alt_off, ak, read_off, rd)
+
+
+# ------------------------------------------------------------------------------------------------------------------
 # K4 pileup_reads
 # ------------------------------------------------------------------------------------------------------------------
 _PILEUP_KIND = {"M": A.SX_SEG_MATCH, "I": A.SX_SEG_INSERT, "D": A.SX_SEG_DELETE, "N": A.SX_SEG_SKIP, "S": A.SX_SEG_SOFTCLIP, "H": A.SX_SEG_HARDCLIP}

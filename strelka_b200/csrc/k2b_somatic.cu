@@ -18,6 +18,7 @@
 #include "sx_libm_mirror.h"
 #include "sx_device_util.cuh"
 #include "sx_internal.h"
+#include "sx_result_set_grid.cuh"
 
 #include <algorithm>
 
@@ -137,69 +138,16 @@ __device__ __forceinline__ sample_acc accumulate_sample(const som_tables& T, con
     return o;
 }
 
-// calculate_result_set_grid: all lanes cooperate, all lanes return the same result
-__device__ __forceinline__ void result_set_grid(const som_tables& T, const float* nl, const float* tl, double* scratch, uint32_t lane, tier_rs& rs)
+// calculate_result_set_grid's terms (sx_result_set_grid.cuh): every one is a per-call constant of the context's tables
+struct k2b_terms
 {
-    double log_post_prob[6];
-    double max_log_prob = -INFINITY;
-    rs.max_gt = 0;
-#pragma unroll 1
-    for (uint32_t combo = 0; combo < 6; ++combo)
-    {
-        const uint32_t nt = T.n_terms[combo];
-        double max_log_sum = -INFINITY;
-        // terms in the reference's loop order; two rounds of 32 lanes (nt <= 44)
-        double l0 = -INFINITY, l1 = -INFINITY;
-        if (lane < nt) l0 = d_add(d_add(T.term_lprior[combo][lane], static_cast<double>(nl[T.term_nf[combo][lane]])), static_cast<double>(tl[T.term_tf[combo][lane]]));
-        if (lane + 32 < nt)
-            l1 = d_add(d_add(T.term_lprior[combo][lane + 32], static_cast<double>(nl[T.term_nf[combo][lane + 32]])), static_cast<double>(tl[T.term_tf[combo][lane + 32]]));
-        double m = fmax(l0, l1);
-#pragma unroll
-        for (int d = 16; d; d >>= 1) m = fmax(m, __shfl_xor_sync(FULL, m, d));
-        max_log_sum = m;
-        __syncwarp();
-        if (lane < nt) scratch[lane] = sx_exp(d_sub(l0, max_log_sum));
-        if (lane + 32 < nt) scratch[lane + 32] = sx_exp(d_sub(l1, max_log_sum));
-        __syncwarp();
-        double sum = 0.0;
-        for (uint32_t i = 0; i < nt; ++i) sum = d_add(sum, scratch[i]);
-        const double log_genotype_prior = static_cast<double>(T.geno_prior[combo]);
-        log_post_prob[combo] = d_add(d_add(log_genotype_prior, max_log_sum), sx_log(sum));
-        if (log_post_prob[combo] > max_log_prob)
-        {
-            max_log_prob = log_post_prob[combo];
-            rs.max_gt = combo; // DDIGT::get_state(ngt, tgt) = ngt*2 + tgt
-        }
-    }
-    double sum_prob = 0.0;
-#pragma unroll
-    for (int c = 0; c < 6; ++c) sum_prob = d_add(sum_prob, sx_exp(d_sub(log_post_prob[c], max_log_prob)));
-    const double log_sum_prob = sx_log(sum_prob);
-    double min_not_somfrom_sum = INFINITY;
-    double nonsom_prob = 0.0;
-    rs.ntype = 0;
-    rs.from_ntype_qphred = 0;
-#pragma unroll
-    for (uint32_t ngt = 0; ngt < 3; ++ngt)
-    {
-        double som_prob_given_ngt = 0;
-#pragma unroll
-        for (uint32_t tgt = 0; tgt < 2; ++tgt)
-        {
-            const double pp = sx_exp(d_sub(d_sub(log_post_prob[ngt * 2 + tgt], max_log_prob), log_sum_prob));
-            if (tgt == 0) nonsom_prob = d_add(nonsom_prob, pp);
-            else som_prob_given_ngt = d_add(som_prob_given_ngt, pp);
-        }
-        const double err_som_and_ngt = d_sub(1.0, som_prob_given_ngt);
-        if (err_som_and_ngt < min_not_somfrom_sum)
-        {
-            min_not_somfrom_sum = err_som_and_ngt;
-            rs.from_ntype_qphred = error_prob_to_qphred_d(err_som_and_ngt);
-            rs.ntype = ngt;
-        }
-    }
-    rs.qphred = error_prob_to_qphred_d(nonsom_prob);
-}
+    const som_tables& T;
+    __device__ __forceinline__ uint32_t n_terms(uint32_t combo) const { return T.n_terms[combo]; }
+    __device__ __forceinline__ double lprior(uint32_t combo, uint32_t i) const { return T.term_lprior[combo][i]; }
+    __device__ __forceinline__ uint32_t nf(uint32_t combo, uint32_t i) const { return T.term_nf[combo][i]; }
+    __device__ __forceinline__ uint32_t tf(uint32_t combo, uint32_t i) const { return T.term_tf[combo][i]; }
+    __device__ __forceinline__ float geno_prior(uint32_t combo) const { return T.geno_prior[combo]; }
+};
 
 __global__ void __launch_bounds__(K2B_WARPS * 32) k2b_somatic_kernel(const uint32_t* __restrict__ n_off, const uint16_t* __restrict__ n_calls,
                                                                      const uint32_t* __restrict__ n_t2off, const uint16_t* __restrict__ n_t2calls,
@@ -289,7 +237,7 @@ __global__ void __launch_bounds__(K2B_WARPS * 32) k2b_somatic_kernel(const uint3
             s_nl[warp][tier][lane] = (lane < 21) ? na.lh : 0.f;
             s_tl[warp][tier][lane] = (lane < 30) ? ta.lh : 0.f;
             __syncwarp();
-            result_set_grid(T, s_nl[warp][tier], s_tl[warp][tier], s_scr[warp], lane, trs[tier]);
+            result_set_grid(k2b_terms{T}, s_nl[warp][tier], s_tl[warp][tier], s_scr[warp], lane, trs[tier]);
             // wrapper (strand_grid.cpp:157-226): returns before the strand-bias block when qphred==0 and not forced
             trs[tier].strandBias = 0.f;
             if (forced || trs[tier].qphred != 0)

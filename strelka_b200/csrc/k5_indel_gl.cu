@@ -12,6 +12,7 @@
 // CUDA's double exp/log/log1p (<= 1 ulp each; tested at 1e-10 relative), the integer counts exactly.
 #include "sx_device_util.cuh"
 #include "sx_internal.h"
+#include "sx_log_sum.cuh"
 
 #include <algorithm>
 
@@ -19,21 +20,6 @@ namespace
 {
 constexpr int K5_WARPS = 4;
 constexpr unsigned FULL = 0xffffffffu;
-
-__device__ __forceinline__ double log1p_switch_d(double x) // blt_util/math_util.hh:33-47
-{
-    return (fabs(x) < 0.01) ? sx_log1p(x) : sx_log(d_add(1.0, x)); // (the reference's libm, bit for bit: sx_libm_mirror_d.h)
-}
-__device__ __forceinline__ double get_log_sum(double x1, double x2) // blt_util/logSumUtil.hh:33-41
-{
-    if (x1 < x2)
-    {
-        const double t = x1;
-        x1 = x2;
-        x2 = t;
-    }
-    return d_add(x1, log1p_switch_d(sx_exp(d_sub(x2, x1))));
-}
 
 __global__ void __launch_bounds__(K5_WARPS * 32) k5_indel_gl_kernel(const uint32_t* __restrict__ read_off, const uint32_t* __restrict__ lnp_off,
                                                                     const uint32_t* __restrict__ allele_off, const uint8_t* __restrict__ ploidy,

@@ -25,6 +25,7 @@ static_assert(sizeof(sx_digt_result_set) == 24 && sizeof(sx_digt_result) == 152,
 static_assert(sizeof(sx_ssnv_result) == 288, "K2b POD layout");
 static_assert(sizeof(sx_params) == 104, "sx_params layout");
 static_assert(sizeof(sx_indel_result) == 152, "K5 POD layout");
+static_assert(sizeof(sx_sindel_read) == 24 && sizeof(sx_sindel_opts) == 64 && sizeof(sx_sindel_tier) == 188 && sizeof(sx_sindel_result) == 400, "K5b POD layout");
 
 static thread_local std::string g_create_err;
 
@@ -73,15 +74,15 @@ extern "C" void sx_ga_active_region_scores(sx_ga_scores* s)
 // This translation unit is compiled with -fmad=false equivalents on the host side: nvcc passes it to g++ with
 // -ffp-contract=off (Makefile), so no host FMA contraction can change a table value.
 // --------------------------------------------------------------------------------------------------------------
-namespace
-{
-typedef float blt_float_t;
-
 double log1p_switch(const double x) // blt_util/math_util.hh:33-47 (boost::math::log1p<double> == ::log1p with glibc)
 {
     if (std::abs(x) < 0.01) return ::log1p(x);
     return std::log(1 + x);
 }
+
+namespace
+{
+typedef float blt_float_t;
 
 inline double digt_expect(const int base_id, const int gt) // blt_util/digt.hh:94-113
 {
@@ -533,6 +534,8 @@ constexpr sx_status_entry k_status[] = {
      "%s: output capacity too small: the batch produces %u alignments, %u segments, %u keys", 3},
     {SX_ST_K7A_CAP, SX_ERR_CAPACITY, "%s: cap_keys too small (totals[0] holds the needed size)", "%s: cap_keys too small: %u keys needed", 1},
     {SX_ST_K9_CAP, SX_ERR_CAPACITY, "%s: cap_segs too small (totals[0] holds the needed size)", "%s: cap_segs too small: %u segment slots needed", 1},
+    {SX_ST_SINDEL_CAP, SX_ERR_CAPACITY, "%s: a locus over the alternate-allele caps", nullptr, 0}, // (per-locus status only; listed for the disjointness check)
+    {SX_ST_SINDEL_ARG, SX_ERR_ARG, "%s: a candidate indel that is not of type INDEL, or an error-rate index past the table", nullptr, 0},
 };
 
 constexpr bool status_bits_disjoint()

@@ -76,6 +76,8 @@ struct sx_tables
     int32_t i_min_flank, i_pad;
 };
 
+double log1p_switch(double x); // blt_util/math_util.hh:33-47 with the host libm (sx_context.cu)
+
 int sx_upload_pileup(sx_ctx* ctx, const sx_pileup_batch* b, int host_base, sx_pileup_batch* d, uint32_t* max_site); // host slots host_base..+5
 cudaError_t sx_k2a_init_tables(sx_tables* d_tables); // fills the g_val0_* rows of the device copy (synchronous)
 
@@ -155,7 +157,11 @@ enum sx_status_bit : int
     SX_ST_K8_CAP = 1 << 17,      // K8: an output capacity is too small
     SX_ST_K7A_CAP = 1 << 18,     // K7a: cap_keys is too small
     SX_ST_K9_CAP = 1 << 19,      // K9: cap_segs is too small
+    SX_ST_SINDEL_CAP = 1 << 20,  // K5b: a locus over the alternate caps.  Written to that locus's result status (SX_SINDEL_ST_CAP), never to
+                                 // the device word: the locus gets no result and the call goes on.
+    SX_ST_SINDEL_ARG = 1 << 21,  // K5b: a candidate that is not SX_INDEL_TYPE_INDEL, or an error-rate index past the table
 };
+static_assert(SX_ST_SINDEL_CAP == SX_SINDEL_ST_CAP, "the per-locus capacity status of K5b is its status bit");
 
 struct sx_buf
 {
