@@ -256,11 +256,16 @@ typedef struct sx_ga_result {
     int32_t score;
     int32_t beginPos;
     uint32_t n_ops; /* > max_ops: overflow, cigar truncated */
-    uint32_t status; /* 0 ok; 1 cigar overflow; 2 problem too large for the kernel's shared-memory tile */
+    uint32_t status; /* 0 ok; 1 cigar overflow (the first max_ops ops are stored); 2 no result, score = beginPos = n_ops = 0 and the
+                        cigar row is not written: the problem goes to the warp-per-matrix kernel and its shared-memory slot,
+                        k3_slot_bytes(Q, R) (about (Q+1)*(R+1) pointer bytes plus strips and sequences, k3_common.cuh), exceeds the
+                        device's opt-in shared memory per block (232448 B on an H100: Q = 1023 fits R <= 211).  The device entry also
+                        returns 2 for an empty query or reference; the host entry rejects those with SX_ERR_ARG. */
 } sx_ga_result;
 
+/* Neither limit is enforced anywhere: status 2 above is the only size check. */
 #define SX_GA_MAX_QUERY 1023
-#define SX_GA_MAX_CELLS (200 * 1024) /* (Q+1)*(R+1) pointer bytes must fit one CTA's shared memory */
+#define SX_GA_MAX_CELLS (200 * 1024)
 
 int sx_global_align(sx_ctx* ctx, const sx_ga_scores* scores, const sx_ga_batch* batch_host,
                     sx_ga_result* res_host /*[n]*/, uint32_t* cigar_host /*[n*max_ops]*/);

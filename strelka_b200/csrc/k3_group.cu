@@ -402,7 +402,7 @@ __global__ void __launch_bounds__(KG_WARPS * 32) kg_align_kernel(const char* __r
                     }
                 };
                 if (n_ops <= max_ops) reverse(0, n_ops);
-                else
+                else if (max_ops) // max_ops == 0: push wrote nothing, so there is nothing to put in order
                 {
                     // slot of the forward-first operation is p = (n_ops - 1) mod max_ops; forward[f] = ring[(p - f) mod max_ops]
                     const uint32_t p = (wpos + max_ops - 1) % max_ops, sh = max_ops - 1 - p;
