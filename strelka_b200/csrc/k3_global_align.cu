@@ -20,7 +20,6 @@
 #include "sx_internal.h"
 
 #include <algorithm>
-#include <climits>
 
 namespace
 {
@@ -37,125 +36,129 @@ struct problem_smem
 
 __device__ __forceinline__ problem_smem carve(unsigned char* base, uint32_t Q, uint32_t R)
 {
+    const k3_slot_layout L = k3_slot(Q, R);
     const uint32_t T = (Q + 31) / 32;
     problem_smem p;
-    uint32_t o = 0;
     p.ptr = base;
-    o += pad16u((Q + 1) * (R + 1));
-    p.sM = reinterpret_cast<int*>(base + o);
+    p.sM = reinterpret_cast<int*>(base + L.strips);
     p.sD = p.sM + 32 * T;
     p.sI = p.sD + 32 * T;
-    o += 3u * 32u * T * 4u;
-    p.qs = reinterpret_cast<char*>(base + o);
-    o += pad16u(Q + 8);
-    p.rs = reinterpret_cast<char*>(base + o);
-    o += pad16u(R + 8);
-    p.steps = base + o;
+    p.qs = reinterpret_cast<char*>(base + L.query);
+    p.rs = reinterpret_cast<char*>(base + L.ref);
+    p.steps = base + L.steps;
     return p;
 }
 
-// The wavefront.  STRIP_IN_REGS: T_ rows per lane in registers (T_ == T); otherwise T_ is ignored and the strip lives in shared memory.
-template <int T_, bool STRIP_IN_REGS>
-__device__ __forceinline__ void dp_wavefront(const sx_ga_scores& sc, const problem_smem& S, uint32_t Q, uint32_t R, uint32_t lane, bt_state& colbt)
+// The wavefront with T rows per lane in registers (Q <= 128), written branch-free inside a step: every lane runs all T rows; rows past
+// the query end (only in the last active lane) compute discarded values and skip the pointer store by predicate; DP row 0 (lane 0's
+// "row above") is a select between closed forms instead of a divergent branch.  Leaves the final-column scores in S.sM/sD/sI.
+template <int T>
+__device__ __forceinline__ void dp_register_strip(const sx_ga_scores& sc, const problem_smem& S, uint32_t Q, uint32_t R, uint32_t lane, bt_state& colbt)
 {
-    const uint32_t T = STRIP_IN_REGS ? (uint32_t)T_ : (Q + 31) / 32;
     const uint32_t W = R + 1;
     const uint32_t last_lane = (Q - 1) / T;
     const uint32_t row0 = lane * T; // query index of this lane's first row
-    int rM[T_], rD[T_], rI[T_];
-    char qc[T_];
-    uint32_t prow[T_];
-    if (STRIP_IN_REGS)
-    {
+    int rM[T], rD[T], rI[T];
+    char qc[T];
+    uint32_t prow[T];
 #pragma unroll
-        for (int r = 0; r < T_; ++r)
-        {
-            const uint32_t qi = row0 + r;
-            col0_scores(sc, (int)qi + 1, rM[r], rD[r], rI[r]);
-            qc[r] = qi < Q ? S.qs[qi] : 0;
-            prow[r] = (qi + 1) * W + 1;
-        }
-    }
-    else
+    for (int r = 0; r < T; ++r)
     {
-        for (uint32_t r = 0; r < T; ++r)
-        {
-            int m, d, i;
-            col0_scores(sc, (int)(row0 + r) + 1, m, d, i);
-            S.sM[r * 32 + lane] = m;
-            S.sD[r * 32 + lane] = d;
-            S.sI[r * 32 + lane] = i;
-        }
+        const uint32_t qi = row0 + r;
+        col0_scores(sc, (int)qi + 1, rM[r], rD[r], rI[r]);
+        qc[r] = qi < Q ? S.qs[qi] : 0;
+        prow[r] = (qi + 1) * W + 1;
     }
     int sendM = 0, sendD = 0, sendI = 0;
     int prevRecvM = 0, prevRecvD = 0, prevRecvI = 0;
     const uint32_t n_steps = R + last_lane;
-    if (STRIP_IN_REGS)
+    const int s_match = sc.match, s_mismatch = sc.mismatch, s_open = sc.open, s_extend = sc.extend, s_insdel = sc.insertDelete;
+    const int row0M = sc.isRequireEdgeDeletion ? BAD : 0;
+    const bool req_del = sc.isRequireEdgeDeletion != 0;
+    int c0M, c0D, c0I; // initial column at the DP row above this strip (the diagonal for j == 0)
+    col0_scores(sc, (int)row0, c0M, c0D, c0I);
+    const uint32_t r_last = (Q - 1) - last_lane * T; // strip-relative index of DP row Q in the last lane
+    const bool is_lane0 = lane == 0;
+    for (uint32_t t = 0; t < n_steps; ++t)
     {
-        // Register-strip wavefront, written branch-free inside a step: every lane runs all T_ rows; rows past the query end (only in
-        // the last active lane) compute discarded values and skip the pointer store by predicate; DP row 0 (lane 0's "row above") is
-        // a select between closed forms instead of a divergent branch.
-        const int s_match = sc.match, s_mismatch = sc.mismatch, s_open = sc.open, s_extend = sc.extend, s_insdel = sc.insertDelete;
-        const int row0M = sc.isRequireEdgeDeletion ? BAD : 0;
-        const bool req_del = sc.isRequireEdgeDeletion != 0;
-        int c0M, c0D, c0I; // initial column at the DP row above this strip (the diagonal for j == 0)
-        col0_scores(sc, (int)row0, c0M, c0D, c0I);
-        const uint32_t r_last = (Q - 1) - last_lane * T; // strip-relative index of DP row Q in the last lane
-        const bool is_lane0 = lane == 0;
-        for (uint32_t t = 0; t < n_steps; ++t)
+        const int recvM = __shfl_up_sync(FULL, sendM, 1);
+        const int recvD = __shfl_up_sync(FULL, sendD, 1);
+        const int recvI = __shfl_up_sync(FULL, sendI, 1);
+        const int j = static_cast<int>(t) - static_cast<int>(lane);
+        if (j >= 0 && j < static_cast<int>(R) && lane <= last_lane)
         {
-            const int recvM = __shfl_up_sync(FULL, sendM, 1);
-            const int recvD = __shfl_up_sync(FULL, sendD, 1);
-            const int recvI = __shfl_up_sync(FULL, sendI, 1);
-            const int j = static_cast<int>(t) - static_cast<int>(lane);
-            if (j >= 0 && j < static_cast<int>(R) && lane <= last_lane)
-            {
-                const char rc = S.rs[j];
-                const bool j0 = j == 0;
-                // row above in this column: DP row 0 at matrix column j+1 for lane 0, else what the previous lane sent last step
-                int upM = is_lane0 ? row0M : recvM;
-                int upD = is_lane0 ? (req_del ? s_open + (j + 1) * s_extend : BAD) : recvD;
-                int upI = is_lane0 ? BAD : recvI;
-                // diagonal: initial column for j == 0; else DP row 0 at matrix column j (lane 0) / what arrived one step earlier
-                int dgM = j0 ? c0M : (is_lane0 ? row0M : prevRecvM);
-                int dgD = j0 ? c0D : (is_lane0 ? (req_del ? s_open + j * s_extend : BAD) : prevRecvD);
-                int dgI = j0 ? c0I : (is_lane0 ? BAD : prevRecvI);
-                int mQ = 0;
+            const char rc = S.rs[j];
+            const bool j0 = j == 0;
+            // row above in this column: DP row 0 at matrix column j+1 for lane 0, else what the previous lane sent last step
+            int upM = is_lane0 ? row0M : recvM;
+            int upD = is_lane0 ? (req_del ? s_open + (j + 1) * s_extend : BAD) : recvD;
+            int upI = is_lane0 ? BAD : recvI;
+            // diagonal: initial column for j == 0; else DP row 0 at matrix column j (lane 0) / what arrived one step earlier
+            int dgM = j0 ? c0M : (is_lane0 ? row0M : prevRecvM);
+            int dgD = j0 ? c0D : (is_lane0 ? (req_del ? s_open + j * s_extend : BAD) : prevRecvD);
+            int dgI = j0 ? c0I : (is_lane0 ? BAD : prevRecvI);
+            int mQ = 0;
 #pragma unroll
-                for (int r = 0; r < T_; ++r)
-                {
-                    const int lfM = rM[r], lfD = rD[r], lfI = rI[r];
-                    int m, d, ins;
-                    const uint32_t pm = max3(m, dgM, dgD, dgI);
-                    m += (qc[r] == rc) ? s_match : s_mismatch;
-                    const uint32_t pd = max3(d, lfM + s_open, lfD, lfI + s_insdel);
-                    d = j0 ? BAD : d + s_extend;
-                    const uint32_t pi = max3(ins, upM + s_open, BAD, upI);
-                    ins += s_extend;
-                    if (r == 0) ins = (row0 == 0) ? BAD : ins; // queryIndex 0
-                    if (row0 + r < Q) S.ptr[prow[r] + j] = static_cast<uint8_t>(pm | (pd << 2) | (pi << 4));
-                    dgM = lfM;
-                    dgD = lfD;
-                    dgI = lfI;
-                    upM = m;
-                    upD = d;
-                    upI = ins;
-                    rM[r] = m;
-                    rD[r] = d;
-                    rI[r] = ins;
-                    if ((uint32_t)r == r_last) mQ = m;
-                }
-                sendM = upM;
-                sendD = upD;
-                sendI = upI;
-                if (lane == last_lane && !req_del) update_bt(colbt, mQ, j + 1, Q, ST_MATCH); // :170-175
+            for (int r = 0; r < T; ++r)
+            {
+                const int lfM = rM[r], lfD = rD[r], lfI = rI[r];
+                int m, d, ins;
+                const uint32_t pm = max3(m, dgM, dgD, dgI);
+                m += (qc[r] == rc) ? s_match : s_mismatch;
+                const uint32_t pd = max3(d, lfM + s_open, lfD, lfI + s_insdel);
+                d = j0 ? BAD : d + s_extend;
+                const uint32_t pi = max3(ins, upM + s_open, BAD, upI);
+                ins += s_extend;
+                if (r == 0) ins = (row0 == 0) ? BAD : ins; // queryIndex 0
+                if (row0 + r < Q) S.ptr[prow[r] + j] = static_cast<uint8_t>(pm | (pd << 2) | (pi << 4));
+                dgM = lfM;
+                dgD = lfD;
+                dgI = lfI;
+                upM = m;
+                upD = d;
+                upI = ins;
+                rM[r] = m;
+                rD[r] = d;
+                rI[r] = ins;
+                if ((uint32_t)r == r_last) mQ = m;
             }
-            prevRecvM = recvM;
-            prevRecvD = recvD;
-            prevRecvI = recvI;
+            sendM = upM;
+            sendD = upD;
+            sendI = upI;
+            if (lane == last_lane && !req_del) update_bt(colbt, mQ, j + 1, Q, ST_MATCH); // :170-175
         }
+        prevRecvM = recvM;
+        prevRecvD = recvD;
+        prevRecvI = recvI;
     }
-    else
+#pragma unroll
+    for (int r = 0; r < T; ++r)
+    {
+        S.sM[r * 32 + lane] = rM[r];
+        S.sD[r * 32 + lane] = rD[r];
+        S.sI[r * 32 + lane] = rI[r];
+    }
+    __syncwarp();
+}
+
+// The wavefront with T = ceil(Q/32) > 4 rows per lane (Q > 128): the strip lives in shared memory, at S.sM/sD/sI[r * 32 + lane].
+__device__ __forceinline__ void dp_shared_strip(const sx_ga_scores& sc, const problem_smem& S, uint32_t Q, uint32_t R, uint32_t lane, bt_state& colbt)
+{
+    const uint32_t T = (Q + 31) / 32;
+    const uint32_t W = R + 1;
+    const uint32_t last_lane = (Q - 1) / T;
+    const uint32_t row0 = lane * T; // query index of this lane's first row
+    for (uint32_t r = 0; r < T; ++r)
+    {
+        int m, d, i;
+        col0_scores(sc, (int)(row0 + r) + 1, m, d, i);
+        S.sM[r * 32 + lane] = m;
+        S.sD[r * 32 + lane] = d;
+        S.sI[r * 32 + lane] = i;
+    }
+    int sendM = 0, sendD = 0, sendI = 0;
+    int prevRecvM = 0, prevRecvD = 0, prevRecvI = 0;
+    const uint32_t n_steps = R + last_lane;
     for (uint32_t t = 0; t < n_steps; ++t)
     {
         const int recvM = __shfl_up_sync(FULL, sendM, 1);
@@ -186,63 +189,30 @@ __device__ __forceinline__ void dp_wavefront(const sx_ga_scores& sc, const probl
                 }
             }
             int m = 0, d = 0, ins = 0;
-            if (STRIP_IN_REGS)
+            for (uint32_t r = 0; r < T; ++r)
             {
-#pragma unroll
-                for (int r = 0; r < T_; ++r)
-                {
-                    const uint32_t qi = row0 + r;
-                    if (qi < Q)
-                    {
-                        const int lfM = rM[r], lfD = rD[r], lfI = rI[r];
-                        const uint32_t pm = max3(m, dgM, dgD, dgI);
-                        m += (qc[r] == rc) ? sc.match : sc.mismatch;
-                        const uint32_t pd = max3(d, lfM + sc.open, lfD, lfI + sc.insertDelete);
-                        d += sc.extend;
-                        if (j == 0) d = BAD;
-                        const uint32_t pi = max3(ins, upM + sc.open, BAD, upI);
-                        ins += sc.extend;
-                        if (qi == 0) ins = BAD;
-                        S.ptr[prow[r] + j] = static_cast<uint8_t>(pm | (pd << 2) | (pi << 4));
-                        dgM = lfM;
-                        dgD = lfD;
-                        dgI = lfI;
-                        upM = m;
-                        upD = d;
-                        upI = ins;
-                        rM[r] = m;
-                        rD[r] = d;
-                        rI[r] = ins;
-                    }
-                }
-            }
-            else
-            {
-                for (uint32_t r = 0; r < T; ++r)
-                {
-                    const uint32_t qi = row0 + r;
-                    if (qi >= Q) break;
-                    const uint32_t idx = r * 32 + lane;
-                    const int lfM = S.sM[idx], lfD = S.sD[idx], lfI = S.sI[idx];
-                    const uint32_t pm = max3(m, dgM, dgD, dgI);
-                    m += (S.qs[qi] == rc) ? sc.match : sc.mismatch;
-                    const uint32_t pd = max3(d, lfM + sc.open, lfD, lfI + sc.insertDelete);
-                    d += sc.extend;
-                    if (j == 0) d = BAD;
-                    const uint32_t pi = max3(ins, upM + sc.open, BAD, upI);
-                    ins += sc.extend;
-                    if (qi == 0) ins = BAD;
-                    S.ptr[(qi + 1) * W + (j + 1)] = static_cast<uint8_t>(pm | (pd << 2) | (pi << 4));
-                    dgM = lfM;
-                    dgD = lfD;
-                    dgI = lfI;
-                    upM = m;
-                    upD = d;
-                    upI = ins;
-                    S.sM[idx] = m;
-                    S.sD[idx] = d;
-                    S.sI[idx] = ins;
-                }
+                const uint32_t qi = row0 + r;
+                if (qi >= Q) break;
+                const uint32_t idx = r * 32 + lane;
+                const int lfM = S.sM[idx], lfD = S.sD[idx], lfI = S.sI[idx];
+                const uint32_t pm = max3(m, dgM, dgD, dgI);
+                m += (S.qs[qi] == rc) ? sc.match : sc.mismatch;
+                const uint32_t pd = max3(d, lfM + sc.open, lfD, lfI + sc.insertDelete);
+                d += sc.extend;
+                if (j == 0) d = BAD;
+                const uint32_t pi = max3(ins, upM + sc.open, BAD, upI);
+                ins += sc.extend;
+                if (qi == 0) ins = BAD;
+                S.ptr[(qi + 1) * W + (j + 1)] = static_cast<uint8_t>(pm | (pd << 2) | (pi << 4));
+                dgM = lfM;
+                dgD = lfD;
+                dgI = lfI;
+                upM = m;
+                upD = d;
+                upI = ins;
+                S.sM[idx] = m;
+                S.sD[idx] = d;
+                S.sI[idx] = ins;
             }
             sendM = m;
             sendD = d;
@@ -252,17 +222,6 @@ __device__ __forceinline__ void dp_wavefront(const sx_ga_scores& sc, const probl
         prevRecvM = recvM;
         prevRecvD = recvD;
         prevRecvI = recvI;
-    }
-    if (STRIP_IN_REGS)
-    {
-        // final-column scores of every row, for the backtrace-start scan
-#pragma unroll
-        for (int r = 0; r < T_; ++r)
-        {
-            S.sM[r * 32 + lane] = rM[r];
-            S.sD[r * 32 + lane] = rD[r];
-            S.sI[r * 32 + lane] = rI[r];
-        }
     }
     __syncwarp();
 }
@@ -310,62 +269,14 @@ __global__ void __launch_bounds__(K3_WARPS * 32) k3_global_align_kernel(const ch
         bt_state colbt{0, ST_MATCH, 0, 0, false}; // row-Q match candidates per column (only when !isRequireEdgeDeletion)
         switch (T)
         {
-        case 1: dp_wavefront<1, true>(sc, S, Q, R, lane, colbt); break;
-        case 2: dp_wavefront<2, true>(sc, S, Q, R, lane, colbt); break;
-        case 3: dp_wavefront<3, true>(sc, S, Q, R, lane, colbt); break;
-        case 4: dp_wavefront<4, true>(sc, S, Q, R, lane, colbt); break;
-        default: dp_wavefront<1, false>(sc, S, Q, R, lane, colbt); break;
+        case 1: dp_register_strip<1>(sc, S, Q, R, lane, colbt); break;
+        case 2: dp_register_strip<2>(sc, S, Q, R, lane, colbt); break;
+        case 3: dp_register_strip<3>(sc, S, Q, R, lane, colbt); break;
+        case 4: dp_register_strip<4>(sc, S, Q, R, lane, colbt); break;
+        default: dp_shared_strip(sc, S, Q, R, lane, colbt); break;
         }
         const uint32_t last_lane = (Q - 1) / T;
-
-        // ---- backtrace start selection (:178-209), in the reference's candidate order with strict '>' updates
-        bt_state bt;
-        bt.max = __shfl_sync(FULL, colbt.max, last_lane);
-        bt.refBegin = __shfl_sync(FULL, colbt.refBegin, last_lane);
-        bt.isInit = __shfl_sync(FULL, colbt.isInit ? 1 : 0, last_lane) != 0;
-        bt.queryBegin = Q;
-        bt.state = ST_MATCH;
-        {
-            const uint32_t lastIdx = ((Q - 1) % T) * 32 + last_lane;
-            if (sc.isRequireEdgeDeletion)
-            {
-                update_bt(bt, S.sM[lastIdx], R, Q, ST_MATCH);
-                update_bt(bt, S.sD[lastIdx], R, Q, ST_DELETE);
-            }
-            if (sc.isAllowEdgeInsertion) update_bt(bt, S.sI[lastIdx], R, Q, ST_INSERT);
-            // query falls off the end of the reference: candidates for queryIndex 0..Q-1 in increasing order == the maximum value
-            // with the smallest queryIndex
-            int best = INT_MIN;
-            uint32_t besti = 0xffffffffu;
-            for (uint32_t queryIndex = lane; queryIndex < Q; queryIndex += 32)
-            {
-                int mval;
-                if (queryIndex == 0) mval = sc.isRequireEdgeDeletion ? BAD : 0; // DP row 0 at the last column
-                else
-                {
-                    const uint32_t qi = queryIndex - 1;
-                    mval = S.sM[(qi % T) * 32 + (qi / T)];
-                }
-                const int v = mval + static_cast<int>(Q - queryIndex) * sc.offEdge;
-                if (v > best)
-                {
-                    best = v;
-                    besti = queryIndex;
-                }
-            }
-#pragma unroll
-            for (int d = 16; d; d >>= 1)
-            {
-                const int ov = __shfl_xor_sync(FULL, best, d);
-                const uint32_t oi = __shfl_xor_sync(FULL, besti, d);
-                if (ov > best || (ov == best && oi < besti))
-                {
-                    best = ov;
-                    besti = oi;
-                }
-            }
-            update_bt(bt, best, R, besti, ST_MATCH);
-        }
+        const bt_state bt = backtrace_start<32>(sc, S.sM, S.sD, S.sI, 0, T, Q, R, last_lane, (Q - 1) % T, colbt);
 
         // ---- traceback: pointer chase by lane 0, one step code per move, written in reverse
         uint32_t nsteps = 0, leading_clip = 0, beginPos = 0;

@@ -18,7 +18,6 @@
 #include "k3_common.cuh"
 
 #include <algorithm>
-#include <climits>
 
 namespace
 {
@@ -86,10 +85,17 @@ __global__ void kg_scatter_kernel(const uint32_t* __restrict__ query_off, const 
 constexpr int KG_B = 8; // quads whose DP a warp finishes before it traces back their 4 * KG_B matrices, one per lane
 constexpr uint32_t KG_SAVE_WORDS = 6; // per-matrix state kept from the DP to the traceback
 
-// per-warp shared memory: final-column score strips [3][T][32] ints, per group: query (T*8), reference (max_r); the saved start states
-template <int T> __host__ __device__ constexpr uint32_t kg_warp_smem(uint32_t max_r)
+// per-warp shared memory: final-column score strips [3][T][32] ints at 0; at `groups`, per group: query (qpad bytes), reference (rpad);
+// at `saved`, the saved start states; `bytes` in all
+struct kg_warp_layout
 {
-    return 3u * T * 32u * 4u + 4u * (((T * KG_G + 15u) & ~15u) + ((max_r + 15u) & ~15u)) + KG_SAVE_WORDS * 32u * 4u;
+    uint32_t qpad, rpad, groups, saved, bytes;
+};
+template <int T> __host__ __device__ constexpr kg_warp_layout kg_warp_smem(uint32_t max_r)
+{
+    const uint32_t qpad = (T * KG_G + 15u) & ~15u, rpad = (max_r + 15u) & ~15u;
+    const uint32_t groups = 3u * T * 32u * 4u, saved = groups + 4u * (qpad + rpad);
+    return {qpad, rpad, groups, saved, saved + KG_SAVE_WORDS * 32u * 4u};
 }
 
 // Score keys: 64*score + tag, tag = 21 * (3 - state) = the 2-bit code (3 - state) replicated into three 2-bit fields (match 0b111111,
@@ -114,16 +120,15 @@ __global__ void __launch_bounds__(KG_WARPS * 32) kg_align_kernel(const char* __r
     extern __shared__ __align__(16) unsigned char smem[];
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t grp = lane >> 3, gl = lane & 7u;
-    unsigned char* wsm = smem + (size_t)warp * kg_warp_smem<T>(max_r);
+    const kg_warp_layout L = kg_warp_smem<T>(max_r);
+    unsigned char* wsm = smem + (size_t)warp * L.bytes;
     int* sM = reinterpret_cast<int*>(wsm);
     int* sD = sM + T * 32;
     int* sI = sD + T * 32;
-    const uint32_t qpad = (T * KG_G + 15u) & ~15u, rpad = (max_r + 15u) & ~15u;
-    unsigned char* gsm = wsm + 3u * T * 32u * 4u + grp * (qpad + rpad);
-    char* qs = reinterpret_cast<char*>(gsm);
-    char* rs = qs + qpad;
+    char* qs = reinterpret_cast<char*>(wsm + L.groups + grp * (L.qpad + L.rpad));
+    char* rs = qs + L.qpad;
     // start states of the warp's pending matrices (slot = quad-in-batch * 4 + group): prob, Q, queryBegin, refBegin, state, score
-    uint32_t* sv = reinterpret_cast<uint32_t*>(wsm + 3u * T * 32u * 4u + 4u * (qpad + rpad));
+    uint32_t* sv = reinterpret_cast<uint32_t*>(wsm + L.saved);
     const uint32_t gwarp = blockIdx.x * KG_WARPS + warp;
     unsigned char* const wscratch = scratch + (size_t)gwarp * scratch_slot * KG_B;
 
@@ -268,53 +273,7 @@ __global__ void __launch_bounds__(KG_WARPS * 32) kg_align_kernel(const char* __r
             sI[r * 32 + lane] = rI[r] >> KG_KEY_SHIFT;
         }
         __syncwarp();
-        // ---- backtrace start selection (:178-209)
-        const uint32_t gbase = grp * KG_G;
-        bt_state bt;
-        bt.max = __shfl_sync(FULL, colbt.max, gbase + last_lane);
-        bt.refBegin = __shfl_sync(FULL, colbt.refBegin, gbase + last_lane);
-        bt.isInit = __shfl_sync(FULL, colbt.isInit ? 1 : 0, gbase + last_lane) != 0;
-        bt.queryBegin = Q;
-        bt.state = ST_MATCH;
-        {
-            const uint32_t lastIdx = r_last * 32 + gbase + last_lane;
-            if (req_del)
-            {
-                update_bt(bt, sM[lastIdx], R, Q, ST_MATCH);
-                update_bt(bt, sD[lastIdx], R, Q, ST_DELETE);
-            }
-            if (allow_ins) update_bt(bt, sI[lastIdx], R, Q, ST_INSERT);
-            int best = INT_MIN;
-            uint32_t besti = 0xffffffffu;
-            for (uint32_t queryIndex = gl; queryIndex < Q; queryIndex += KG_G)
-            {
-                int mval;
-                if (queryIndex == 0) mval = row0M; // DP row 0 at the last column
-                else
-                {
-                    const uint32_t qi = queryIndex - 1;
-                    mval = sM[(qi % T) * 32 + gbase + (qi / T)];
-                }
-                const int v = mval + static_cast<int>(Q - queryIndex) * sc.offEdge;
-                if (v > best)
-                {
-                    best = v;
-                    besti = queryIndex;
-                }
-            }
-#pragma unroll
-            for (int d = 4; d; d >>= 1)
-            {
-                const int ov = __shfl_xor_sync(FULL, best, d);
-                const uint32_t oi = __shfl_xor_sync(FULL, besti, d);
-                if (ov > best || (ov == best && oi < besti))
-                {
-                    best = ov;
-                    besti = oi;
-                }
-            }
-            update_bt(bt, best, R, besti, ST_MATCH);
-        }
+        const bt_state bt = backtrace_start<KG_G>(sc, sM, sD, sI, grp * KG_G, T, Q, R, last_lane, r_last, colbt);
         // ---- keep the start state for the batched traceback
         if (is_lane0)
         {
@@ -425,14 +384,16 @@ __global__ void __launch_bounds__(KG_WARPS * 32) kg_align_kernel(const char* __r
 
 // upper bound on resident CTAs per SM used for the grid and for the scratch sizing (strips of 10+ rows need > 100 registers)
 inline int kg_max_ctas_per_sm(int T) { return T >= 10 ? 4 : 8; }
+// scratch bytes of one matrix's back pointers: max_r + KG_G wavefront steps of T rows x 32 lanes
+inline size_t kg_scratch_slot(int T, uint32_t max_r) { return (((size_t)(max_r + KG_G) * T * 32) + 255) & ~size_t(255); }
 
 template <int T>
 int kg_launch(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* d, sx_ga_result* res_dev, uint32_t* cigar_dev, const uint32_t* order, uint32_t n, uint32_t max_r,
               uint32_t* work_dev)
 {
     if (n == 0) return SX_OK;
-    const size_t smem = (size_t)kg_warp_smem<T>(max_r) * KG_WARPS;
-    const size_t slot = (((size_t)(max_r + KG_G) * T * 32) + 255) & ~size_t(255);
+    const size_t smem = (size_t)kg_warp_smem<T>(max_r).bytes * KG_WARPS;
+    const size_t slot = kg_scratch_slot(T, max_r);
     const uint32_t quads = (n + 3) / 4;
     if (smem > 48 * 1024) SX_CUDA(ctx, cudaFuncSetAttribute(kg_align_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(ctx->smem_optin)));
     // persistent grid: as many CTAs per SM as the instantiation's registers / shared memory allow (4 for the tall strips, more below)
@@ -491,7 +452,7 @@ int sx_k3_group_run(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* d, s
         size_t worst = 0;
         for (int t = 1; t <= 16; ++t)
             if (begin[t * KG_RCLASSES] > begin[(t - 1) * KG_RCLASSES])
-                worst = std::max(worst, (((size_t)(info.max_r[t - 1] + KG_G) * t * 32 + 255) & ~size_t(255)) * kg_max_ctas_per_sm(t));
+                worst = std::max(worst, kg_scratch_slot(t, info.max_r[t - 1]) * kg_max_ctas_per_sm(t));
         unsigned char* p = nullptr;
         if (worst && (rc = sx_take(ctx, SX_SLOT_K3_SCRATCH, worst * KG_B * (size_t)ctx->sm_count * KG_WARPS, p, 0))) return rc;
     }

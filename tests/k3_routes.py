@@ -2,8 +2,8 @@
 
 Each DP problem of a batch goes down one of these paths, picked from its shape and from the batch's scores:
   group kernel     kg_align_kernel<T>, T = ceil(Q/8), four reference-length classes   Q <= 128, R <= 255, every score within +-4096
-  warp kernel      register strip dp_wavefront<T, true>, T = ceil(Q/32) <= 4         the other problems with Q <= 128
-                   shared-memory strip, T >= 5                                        Q > 128
+  warp kernel      register strip dp_register_strip<T>, T = ceil(Q/32) <= 4           the other problems with Q <= 128
+                   shared-memory strip dp_shared_strip, T >= 5                        Q > 128
   status 2         no result: k3_slot_bytes(Q, R) exceeds the opt-in shared memory per block, or Q == 0 or R == 0 (device entry)
 and the warp kernel's launch runs 4, 2 or 1 warps per CTA, whichever is the most that fit the batch's largest slot.
 (k3_group.cu: kg_bucket, sx_k3_group_run; k3_global_align.cu: k3_run, k3_global_align_kernel; k3_common.cuh: k3_slot_bytes.)

@@ -38,9 +38,10 @@ def _ga_batch(pairs, max_ops=None):
 # ---------------------------------------------------------------------------------------------------------------------------------
 # CPU: the mirror and the cases
 # ---------------------------------------------------------------------------------------------------------------------------------
-def test_route_constants_match_the_sources():
-    """Every constant tests/k3_routes.py copies, read back out of the kernels: a routing change must update the mirror (and with it
-    the route matrix the other tests check) in the same commit."""
+def test_route_constants_match_the_strip_and_slot_sources():
+    """Every constant tests/k3_routes.py copies, read back out of the kernels -- the routing constants, the four register-strip
+    instantiations and every term of the warp kernel's slot layout: a routing change must update the mirror (and with it the route
+    matrix the other tests check) in the same commit."""
     grp, warp, common = _src("k3_group.cu"), _src("k3_global_align.cu"), _src("k3_common.cuh")
     m = re.search(r"constexpr uint32_t KG_MAX_Q = (\d+), KG_MAX_R = (\d+);", grp)
     assert m and (int(m[1]), int(m[2])) == (K.KG_MAX_Q, K.KG_MAX_R)
@@ -55,8 +56,11 @@ def test_route_constants_match_the_sources():
     assert int(re.search(r"constexpr int K3_WARPS = (\d+);", warp)[1]) == K.K3_WARPS
     assert "while (warps > 1 && slot * warps > ctx->smem_optin) warps >>= 1;" in warp
     assert "if (Q == 0 || R == 0 || k3_slot_bytes(Q, R) > slot_bytes)" in warp
-    assert re.findall(r"case (\d): dp_wavefront<\1, true>", warp) == ["1", "2", "3", "4"]
-    body = re.search(r"uint32_t k3_slot_bytes\(uint32_t Q, uint32_t R\)\s*\{(.*?)\n\}", common, re.S)[1]
+    assert re.findall(r"case (\d): dp_register_strip<\1>\(", warp) == ["1", "2", "3", "4"]
+    assert "default: dp_shared_strip(" in warp
+    assert "uint32_t k3_slot_bytes(uint32_t Q, uint32_t R) { return k3_slot(Q, R).bytes; }" in common
+    body = re.search(r"k3_slot_layout k3_slot\(uint32_t Q, uint32_t R\)\s*\{(.*?)\n\}", common, re.S)[1]
+    assert re.search(r"s\.bytes = o;\s*return s;\s*$", body)
     terms = [re.sub(r"\s+", "", t) for t in re.findall(r"o \+= ([^;]+);", body)]
     assert re.search(r"const uint32_t T = \(Q \+ 31\) / 32;", body)
     assert terms == ["pad16u((Q+1)*(R+1))", "3u*32u*T*4u", "pad16u(Q+8)", "pad16u(R+8)", "pad16u(Q+R+8)"], terms
