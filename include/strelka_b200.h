@@ -681,6 +681,80 @@ int sx_somatic_indel_dev(sx_ctx* ctx, const sx_sindel_opts* opts, const sx_sinde
                          sx_sindel_result* out_dev);
 
 /* ==========================================================================================
+ * K6b  indel_reads   (K6's records -> K5b's per-locus read lists, in device memory)
+ *   replaces the transpose the reference's containers do implicitly:
+ *     the write   read_path_lnp[readId] = ReadPathScores(...)   starling_common/starling_read_align_score_indels.cpp:1071
+ *     the map     IndelSampleData::read_path_lnp                starling_common/IndelData.hh:262
+ *     its readers get_somatic_indel / is_multi_indel_allele     applications/strelka/somatic_indel_grid.cpp:100-175,181-361
+ *                 process_pos_indel_somatic                     applications/strelka/strelka_pos_processor.cpp:305-348
+ *
+ * K6 writes one sx_read_indel_score per (read, evaluated indel), read-major, one record set per sample, keyed by an index into
+ * the window of the read's REGION.  K5b reads locus-major lists that merge the reads of every region and of both samples.  This
+ * stage is that regrouping:
+ *   - Only SX_RIS_SCORED records become entries; SX_RIS_SUBOVERLAP records are not in read_path_lnp (:617-627).
+ *   - A record's key and alt_key[i] are translated to batch-wide ids: key_gid[region_key_off[region of the read] + index].  A
+ *     record whose id is in no loci.gid is skipped.
+ *   - Per locus and sample the entries are in ascending read id (the map's order; K5b's float sums run in it).  Two entries with
+ *     one id in one (locus, sample) set SX_INDEL_READS_ST_DUP_READ (the map would overwrite; a DNA window never does this).
+ *   - A locus's alternate table holds the distinct ids its entries name, normal and tumor together, in ascending id, each copied
+ *     whole from gid_key.  A read's alt[0..n_alt) keep the record's alt_key order (ReadPathScores::alt_indel order), as table
+ *     indices.  More than SX_SINDEL_MAX_ALTS distinct ids set SX_SINDEL_ST_CAP.
+ *   - A flagged locus gets its status and EMPTY lists (no entries, no alternates); nothing is truncated.
+ *   - totals = {entries, alternates} of the unflagged loci.  A capacity below them returns SX_ERR_CAPACITY with totals, status and
+ *     the two offset arrays written, and no entry or table row.
+ *   - Every byte of every entry and table row is written, and the output does not depend on thread scheduling: two runs are
+ *     byte-identical.
+ * The caller guarantees that every read evaluating a listed locus is in the two sample batches: the window contract
+ * report_begin / report_end already imposes on the pile-up.  With the arrays of sx_indel_loci, the output IS an sx_sindel_batch.
+ * ======================================================================================== */
+#define SX_INDEL_READS_ST_DUP_READ 0x400000u /* locus status: one read id twice in one sample's list; no lists */
+
+typedef struct sx_indel_reads_sample { /* one sample's K6 input and output (sx_score_indels_batch / sx_score_indels_out arrays) */
+    uint32_t n_regions, n_reads, n_keys, pad;
+    const uint32_t* region_read_off;   /* [n_regions + 1] as sx_score_indels_batch */
+    const uint32_t* region_key_off;    /* [n_regions + 1] */
+    const uint32_t* key_gid;           /* [n_keys] batch-wide id of each window entry: equal IndelKey <=> equal id, in BOTH samples
+                                          (e.g. the IndelBuffer's iteration index); every id < sx_indel_loci.n_gid */
+    const uint32_t* rec_off;           /* [n_reads + 1] */
+    const sx_read_indel_score* recs;   /* K6's output, untouched */
+    const uint32_t* n_rec;             /* [n_reads] */
+    const uint16_t* read_len;          /* [n_reads] -> ReadPathScores::read_length (rseg.read_size(), :852) */
+    const uint16_t* non_ambig;         /* [n_reads] -> nonAmbiguousBasesInRead */
+    const uint8_t* read_flags;         /* [n_reads] SX_SIF_TIER1 -> is_tier1_read */
+    const uint32_t* read_id;           /* [n_reads] rseg.getReadIndex(); NULL: the read's index in the batch */
+} sx_indel_reads_sample;
+
+typedef struct sx_indel_loci { /* which candidates to call */
+    uint32_t n_loci, n_gid;
+    const uint32_t* gid;               /* [n_loci] strictly ascending, each < n_gid */
+    const sx_indel_key* key;           /* [n_loci] -> sx_sindel_batch.key */
+    const uint8_t* is_forced_output;   /* [n_loci] -> sx_sindel_batch.is_forced_output */
+    const uint32_t* err_idx;           /* [n_loci] -> sx_sindel_batch.err_idx */
+    const sx_indel_key* gid_key;       /* [n_gid] the entry of every id (pos / del_len / ins_len / type are what K5b reads of an alternate) */
+} sx_indel_loci;
+
+typedef struct sx_indel_reads_out { /* caller-allocated */
+    uint32_t* alt_off;                 /* [n_loci + 1] */
+    sx_indel_key* alts;                /* [cap_alts] */
+    uint32_t* read_off;                /* [2 * n_loci + 1] */
+    sx_sindel_read* reads;             /* [cap_reads] */
+    uint32_t* status;                  /* [n_loci] 0, or SX_SINDEL_ST_CAP | SX_INDEL_READS_ST_DUP_READ */
+    uint32_t* totals;                  /* [2] entries, alternates */
+    uint32_t cap_alts, cap_reads;
+} sx_indel_reads_out;
+
+/* Host arrays in and out.  totals_host ([2], may be NULL) receives the totals also when the call returns SX_ERR_CAPACITY. */
+int sx_link_indel_reads(sx_ctx* ctx, const sx_indel_reads_sample* normal, const sx_indel_reads_sample* tumor, const sx_indel_loci* loci,
+                        sx_indel_reads_out* out_host, uint32_t* totals_host);
+/* Device pointers inside every struct (out_dev->totals too); totals_host is host memory. */
+int sx_link_indel_reads_dev(sx_ctx* ctx, const sx_indel_reads_sample* normal_dev, const sx_indel_reads_sample* tumor_dev, const sx_indel_loci* loci_dev,
+                            sx_indel_reads_out* out_dev, uint32_t* totals_host);
+/* The link followed by K5b on the compute stream, the sx_sindel_batch between them in buffers the context owns.  A locus the
+ * link flagged has that status in its sx_sindel_result and no result. */
+int sx_somatic_indel_from_records_dev(sx_ctx* ctx, const sx_sindel_opts* opts, const sx_indel_reads_sample* normal_dev, const sx_indel_reads_sample* tumor_dev,
+                                      const sx_indel_loci* loci_dev, const double* err_prob_host, uint32_t n_err, sx_sindel_result* out_dev /*[n_loci]*/);
+
+/* ==========================================================================================
  * K7  enumerate_alignments   (SURVEY 8a row a3 / 8f3: the producer of K1's and K6's input)
  *   replaces  getCandidateAlignments           starling_common/starling_read_align.cpp:1816-1994
  *   with      candidate_alignment_search       :857-1277  (the recursive toggle search)

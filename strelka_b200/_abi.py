@@ -121,6 +121,23 @@ class SxSindelBatch(C.Structure):
         "key", "is_forced_output", "err_idx", "alt_off", "alts", "read_off", "reads")]
 
 
+# K6b indel_reads
+SX_INDEL_READS_ST_DUP_READ = 0x400000
+
+
+class SxIndelReadsSample(C.Structure):
+    _fields_ = [(n, C.c_uint32) for n in ("n_regions", "n_reads", "n_keys", "pad")] + [(n, C.c_void_p) for n in (
+        "region_read_off", "region_key_off", "key_gid", "rec_off", "recs", "n_rec", "read_len", "non_ambig", "read_flags", "read_id")]
+
+
+class SxIndelLoci(C.Structure):
+    _fields_ = [("n_loci", C.c_uint32), ("n_gid", C.c_uint32)] + [(n, C.c_void_p) for n in ("gid", "key", "is_forced_output", "err_idx", "gid_key")]
+
+
+class SxIndelReadsOut(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("alt_off", "alts", "read_off", "reads", "status", "totals")] + [("cap_alts", C.c_uint32), ("cap_reads", C.c_uint32)]
+
+
 def default_sindel_opts() -> SxSindelOpts:
     o = SxSindelOpts()
     load().sx_default_sindel_opts(C.byref(o))
@@ -422,6 +439,10 @@ SYMBOLS = [
     ("sx_default_sindel_opts", None, [C.POINTER(SxSindelOpts)]),
     ("sx_somatic_indel", C.c_int, [_P, C.POINTER(SxSindelOpts), C.POINTER(SxSindelBatch), _P, C.c_uint32, _P]),
     ("sx_somatic_indel_dev", C.c_int, [_P, C.POINTER(SxSindelOpts), C.POINTER(SxSindelBatch), _P, C.c_uint32, _P]),
+    ("sx_link_indel_reads", C.c_int, [_P, C.POINTER(SxIndelReadsSample), C.POINTER(SxIndelReadsSample), C.POINTER(SxIndelLoci), C.POINTER(SxIndelReadsOut), _P]),
+    ("sx_link_indel_reads_dev", C.c_int, [_P, C.POINTER(SxIndelReadsSample), C.POINTER(SxIndelReadsSample), C.POINTER(SxIndelLoci), C.POINTER(SxIndelReadsOut), _P]),
+    ("sx_somatic_indel_from_records_dev", C.c_int, [_P, C.POINTER(SxSindelOpts), C.POINTER(SxIndelReadsSample), C.POINTER(SxIndelReadsSample), C.POINTER(SxIndelLoci),
+                                                    _P, C.c_uint32, _P]),
     ("sx_default_pileup_opts", None, [C.POINTER(SxPileupOpts)]),
     ("sx_pileup_reads", C.c_int, [_P, C.POINTER(SxPileupReadsBatch), C.POINTER(SxPileupColumns)]),
     ("sx_pileup_reads_dev", C.c_int, [_P, C.POINTER(SxPileupReadsBatch), C.POINTER(SxPileupColumns)]),

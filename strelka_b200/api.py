@@ -304,6 +304,107 @@ Context.score_indels = _score_indels  # K6
 Context.score_indels_dev = _score_indels_dev
 
 
+def _link_caps(normal, tumor, n_loci: int) -> Tuple[int, int]:
+    """Capacities no batch exceeds: an entry per record, two alternates per entry and SX_SINDEL_MAX_ALTS per locus."""
+    cap_reads = sum(int(np.asarray(s.n_rec[: s.n_reads], np.int64).sum()) for s in (normal, tumor))
+    return cap_reads, min(2 * cap_reads, A.SX_SINDEL_MAX_ALTS * n_loci)
+
+
+def _link_indel_reads(self, normal: B.IndelReadsSample, tumor: B.IndelReadsSample, loci: B.IndelLoci, cap_reads=None, cap_alts=None) -> B.IndelReadsOut:
+    """K6b: two samples' K6 records -> K5b's per-locus read lists (host arrays in and out).  SX_ERR_CAPACITY leaves the needed sizes in
+    the SxError's `totals`."""
+    cr, ca = _link_caps(normal, tumor, loci.n_loci)
+    out = B.IndelReadsOut(loci.n_loci, cr if cap_reads is None else cap_reads, ca if cap_alts is None else cap_alts)
+    totals = np.zeros(2, np.uint32)
+    rc = self.lib.sx_link_indel_reads(self.h, C.byref(normal.c), C.byref(tumor.c), C.byref(loci.c), C.byref(out.c), totals.ctypes.data)
+    _chk_totals(self, rc, totals)
+    return out
+
+
+def _chk_totals(self, rc: int, totals: np.ndarray) -> None:
+    try:
+        self._chk(rc)
+    except SxError as e:
+        e.totals = totals.copy()
+        raise
+
+
+class DevIndelReadsSample:
+    """sx_indel_reads_sample in HBM.  `from_score_indels` adopts a DevScoreIndelsBatch: its read arrays and the recs / n_rec arrays K6
+    wrote, which that object owns -- so two samples scored on ONE context stay apart.  A constructor from two DevWindow passes is not
+    built (DESIGN section 8)."""
+
+    def __init__(self, ctx: "Context", hs: B.IndelReadsSample, adopt: Optional[dict] = None):
+        self.host, self.bufs = hs, {}
+        p = dict(adopt or {})
+        for n in B.IndelReadsSample.ARRAYS:
+            a = getattr(hs, n)
+            if n not in p:
+                p[n] = None
+                if a is not None:
+                    self.bufs[n] = DeviceArray(ctx, a.nbytes + 64).upload(a)
+                    p[n] = self.bufs[n].ptr
+        self.c = A.SxIndelReadsSample(hs.n_regions, hs.n_reads, hs.n_keys, 0, *(p[n] for n in B.IndelReadsSample.ARRAYS))
+
+    @staticmethod
+    def from_score_indels(ctx: "Context", db: DevScoreIndelsBatch, key_gid, read_id=None) -> "DevIndelReadsSample":
+        hb = db.host
+        hs = B.IndelReadsSample(hb, np.zeros(hb.n_rec_slots + 1, A.READ_INDEL_SCORE_DT), np.zeros(hb.n_reads + 1, np.uint32), key_gid, read_id)
+        adopt = {n: db.bufs[n].ptr for n in ("region_read_off", "region_key_off", "rec_off", "read_len", "non_ambig", "read_flags")}
+        adopt.update(recs=db.recs.ptr, n_rec=db.n_rec.ptr)
+        self = DevIndelReadsSample(ctx, hs, adopt)
+        self.score = db  # (keeps the adopted buffers alive)
+        return self
+
+
+class DevIndelLoci:
+    def __init__(self, ctx: "Context", hl: B.IndelLoci):
+        self.host = hl
+        self.bufs = {n: DeviceArray(ctx, getattr(hl, n).nbytes + 64).upload(getattr(hl, n)) for n in B.IndelLoci.ARRAYS}
+        self.c = A.SxIndelLoci(hl.n_loci, hl.n_gid, *(self.bufs[n].ptr for n in B.IndelLoci.ARRAYS))
+
+
+def _link_indel_reads_dev(self, normal: DevIndelReadsSample, tumor: DevIndelReadsSample, loci: DevIndelLoci, cap_reads: int, cap_alts: int) -> B.IndelReadsOut:
+    """K6b on device-resident inputs, into device arrays of the given capacities; returns their host copies."""
+    n = loci.host.n_loci
+    out = B.IndelReadsOut(n, cap_reads, cap_alts)
+    d = {k: DeviceArray(self, getattr(out, k).nbytes + 64) for k in ("alt_off", "alts", "read_off", "reads", "status", "totals")}
+    c = A.SxIndelReadsOut(d["alt_off"].ptr, d["alts"].ptr, d["read_off"].ptr, d["reads"].ptr, d["status"].ptr, d["totals"].ptr, cap_alts, cap_reads)
+    totals = np.zeros(2, np.uint32)
+    rc = self.lib.sx_link_indel_reads_dev(self.h, C.byref(normal.c), C.byref(tumor.c), C.byref(loci.c), C.byref(c), totals.ctypes.data)
+    _chk_totals(self, rc, totals)
+    for k in ("alt_off", "read_off", "totals"):
+        getattr(out, k)[:] = d[k].download(np.uint32, getattr(out, k).size)
+    out.status[:n] = d["status"].download(np.uint32, n)
+    out.reads[: int(out.totals[0])] = d["reads"].download(A.SINDEL_READ_DT, int(out.totals[0]))
+    out.alts[: int(out.totals[1])] = d["alts"].download(A.INDEL_KEY_DT, int(out.totals[1]))
+    for x in d.values():
+        x.free()
+    return out
+
+
+Context.link_indel_reads = _link_indel_reads  # K6b
+Context.link_indel_reads_dev = _link_indel_reads_dev
+
+
+class DevSomaticIndelChain:
+    """K6's records of two samples -> somatic indel calls without a host step (sx_somatic_indel_from_records_dev): the link, then K5b on
+    the sx_sindel_batch the link left in the context's buffers.  The samples' recs / n_rec arrays are caller-owned (DevIndelReadsSample)."""
+
+    def __init__(self, ctx: "Context", normal: DevIndelReadsSample, tumor: DevIndelReadsSample, loci: B.IndelLoci):
+        self.ctx, self.normal, self.tumor, self.loci = ctx, normal, tumor, DevIndelLoci(ctx, loci)
+        self.out = DeviceArray(ctx, max(1, loci.n_loci) * A.SINDEL_RESULT_DT.itemsize)
+
+    def run(self, opts: Optional[A.SxSindelOpts] = None) -> None:
+        o = opts or A.default_sindel_opts()
+        hl, ctx = self.loci.host, self.ctx
+        ctx._chk(ctx.lib.sx_somatic_indel_from_records_dev(ctx.h, C.byref(o), C.byref(self.normal.c), C.byref(self.tumor.c), C.byref(self.loci.c),
+                                                           A.ptr(hl.err_prob), hl.err_prob.size, self.out.ptr))
+
+    def download(self) -> np.ndarray:
+        return self.out.download(A.SINDEL_RESULT_DT, self.loci.host.n_loci)
+
+
 class DevEnumBatch:
     """An sx_enum_batch and its sx_enum_out resident in device memory (for sx_enumerate_alignments_dev)."""
 

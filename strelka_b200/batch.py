@@ -531,6 +531,124 @@ class SomaticIndelBatch:
 
 
 # ------------------------------------------------------------------------------------------------------------------
+# K6b indel_reads
+# ------------------------------------------------------------------------------------------------------------------
+class IndelReadsSample:
+    """One sample's side of sx_link_indel_reads: the K6 batch's read arrays, K6's output as it left the device (record slots at rec_off,
+    n_rec of them used per read), the batch-wide id of every window entry and the reads' ids (None: the read's index)."""
+
+    def __init__(self, sb, recs, n_rec, key_gid, read_id=None):
+        n = sb.n_reads
+        self.n_regions, self.n_reads, self.n_keys = sb.n_regions, n, sb.n_keys
+        self.region_read_off, self.region_key_off, self.rec_off = sb.region_read_off, sb.region_key_off, sb.rec_off
+        self.read_len, self.non_ambig, self.read_flags = sb.read_len, sb.non_ambig, sb.read_flags
+        self.recs = np.ascontiguousarray(recs, A.READ_INDEL_SCORE_DT)
+        self.n_rec = np.ascontiguousarray(n_rec, np.uint32)
+        self.key_gid = np.ascontiguousarray(key_gid, np.uint32)
+        self.read_id = None if read_id is None else np.ascontiguousarray(read_id, np.uint32)
+        assert self.recs.size >= int(sb.rec_off[n]) and self.n_rec.size >= n and self.key_gid.size >= sb.n_keys
+        assert self.read_id is None or self.read_id.size >= n
+        self._keep = [a if a.size else np.zeros(1, a.dtype) for a in (self.recs, self.n_rec, self.key_gid)]
+        rc, nr, kg = self._keep
+        self.c = A.SxIndelReadsSample(self.n_regions, n, self.n_keys, 0, A.ptr(self.region_read_off), A.ptr(self.region_key_off), A.ptr(kg), A.ptr(self.rec_off),
+                                      A.ptr(rc), A.ptr(nr), A.ptr(self.read_len), A.ptr(self.non_ambig), A.ptr(self.read_flags), A.ptr(self.read_id))
+
+    ARRAYS = ("region_read_off", "region_key_off", "key_gid", "rec_off", "recs", "n_rec", "read_len", "non_ambig", "read_flags", "read_id")
+
+
+class IndelLoci:
+    """sx_indel_loci: the candidates to call (ascending id) and the table of every id's entry; err_prob is K5b's host error-rate table."""
+
+    def __init__(self, gid, key, is_forced_output, err_idx, gid_key, err_prob):
+        self.gid = np.ascontiguousarray(gid, np.uint32)
+        self.n_loci = n = self.gid.size
+        self.key = np.ascontiguousarray(key, A.INDEL_KEY_DT)
+        self.is_forced_output = np.ascontiguousarray(is_forced_output, np.uint8)
+        self.err_idx = np.ascontiguousarray(err_idx, np.uint32)
+        self.gid_key = np.ascontiguousarray(gid_key, A.INDEL_KEY_DT)
+        self.n_gid = self.gid_key.size
+        self.err_prob = np.ascontiguousarray(err_prob, np.float64)
+        assert self.key.size == n and self.is_forced_output.size == n and self.err_idx.size == n
+        self._keep = [a if a.size else np.zeros(1, a.dtype) for a in (self.gid, self.key, self.is_forced_output, self.err_idx, self.gid_key)]
+        self.c = A.SxIndelLoci(n, self.n_gid, *(A.ptr(a) for a in self._keep))
+
+    ARRAYS = ("gid", "key", "is_forced_output", "err_idx", "gid_key")
+
+
+class IndelReadsOut:
+    """sx_indel_reads_out with capacities; `batch(loci)` is the sx_sindel_batch it forms with the loci."""
+
+    def __init__(self, n_loci, cap_reads, cap_alts):
+        self.n_loci = n_loci
+        self.alt_off = np.zeros(n_loci + 1, np.uint32)
+        self.alts = np.zeros(max(1, cap_alts), A.INDEL_KEY_DT)
+        self.read_off = np.zeros(2 * n_loci + 1, np.uint32)
+        self.reads = np.zeros(max(1, cap_reads), A.SINDEL_READ_DT)
+        self.status = np.zeros(max(1, n_loci), np.uint32)
+        self.totals = np.zeros(2, np.uint32)
+        self.c = A.SxIndelReadsOut(A.ptr(self.alt_off), A.ptr(self.alts), A.ptr(self.read_off), A.ptr(self.reads), A.ptr(self.status), A.ptr(self.totals),
+                                   cap_alts, cap_reads)
+
+    def trimmed(self):
+        """(alt_off, alts, read_off, reads, status, totals) without the unused capacity."""
+        return (self.alt_off, self.alts[: int(self.totals[1])], self.read_off, self.reads[: int(self.totals[0])], self.status[: self.n_loci], self.totals)
+
+    def batch(self, loci: IndelLoci) -> SomaticIndelBatch:
+        alt_off, alts, read_off, reads, _, _ = self.trimmed()
+        return SomaticIndelBatch(loci.key, loci.is_forced_output, loci.err_idx, loci.err_prob, alt_off, alts, read_off, reads)
+
+
+def link_indel_reads(normal: IndelReadsSample, tumor: IndelReadsSample, loci: IndelLoci) -> IndelReadsOut:
+    """Host restatement of sx_link_indel_reads with dicts, the way the reference's containers do it: read_path_lnp[read id] = entry per
+    (locus, sample), walked in key order.  A second check beside the oracle; not a fast path."""
+    locus_of = {int(g): l for l, g in enumerate(loci.gid)}
+    lists = [({}, {}) for _ in range(loci.n_loci)]
+    dup = np.zeros(loci.n_loci, bool)
+    for s, sm in enumerate((normal, tumor)):
+        region = np.repeat(np.arange(sm.n_regions), np.diff(sm.region_read_off[: sm.n_regions + 1]).astype(np.int64))
+        for r in range(sm.n_reads):
+            k0 = int(sm.region_key_off[region[r]]) if sm.n_rec[r] else 0
+            rid = r if sm.read_id is None else int(sm.read_id[r])
+            for rec in sm.recs[int(sm.rec_off[r]) : int(sm.rec_off[r]) + int(sm.n_rec[r])]:
+                if not rec["flags"] & A.SX_RIS_SCORED:
+                    continue
+                l = locus_of.get(int(sm.key_gid[k0 + int(rec["key"])]))
+                if l is None:
+                    continue
+                dup[l] |= rid in lists[l][s]
+                n_alt = int(rec["n_alt"])
+                lists[l][s][rid] = (rec, r, [int(sm.key_gid[k0 + int(rec["alt_key"][a])]) for a in range(n_alt)])
+    alts_of = [sorted({g for d in ls for _, _, ids in d.values() for g in ids}) for ls in lists]
+    status = np.array([(A.SX_INDEL_READS_ST_DUP_READ if dup[l] else 0) | (A.SX_SINDEL_ST_CAP if len(alts_of[l]) > A.SX_SINDEL_MAX_ALTS else 0)
+                       for l in range(loci.n_loci)], np.uint32)
+    n_reads = sum(len(d) for l, ls in enumerate(lists) if not status[l] for d in ls)
+    n_alts = sum(len(a) for l, a in enumerate(alts_of) if not status[l])
+    out = IndelReadsOut(loci.n_loci, n_reads, n_alts)
+    out.status[: loci.n_loci] = status
+    out.totals[:] = (n_reads, n_alts)
+    at = aa = 0
+    for l, ls in enumerate(lists):
+        out.alt_off[l] = aa
+        for s, (sm, d) in enumerate(zip((normal, tumor), ls)):
+            out.read_off[2 * l + s] = at
+            if status[l]:
+                continue
+            for rid in sorted(d):
+                rec, r, ids = d[rid]
+                e = out.reads[at]
+                e["ref"], e["indel"], e["read_length"], e["non_ambig"] = rec["ref_lnp"], rec["indel_lnp"], sm.read_len[r], sm.non_ambig[r]
+                e["is_tier1"], e["n_alt"] = 1 if sm.read_flags[r] & A.SX_SIF_TIER1 else 0, len(ids)
+                for a, g in enumerate(ids):
+                    e["alt"][a], e["alt_lnp"][a] = alts_of[l].index(g), rec["alt_lnp"][a]
+                at += 1
+        if not status[l]:
+            out.alts[aa : aa + len(alts_of[l])] = loci.gid_key[alts_of[l]]
+            aa += len(alts_of[l])
+    out.alt_off[loci.n_loci], out.read_off[2 * loci.n_loci] = aa, at
+    return out
+
+
+# ------------------------------------------------------------------------------------------------------------------
 # K4 pileup_reads
 # ------------------------------------------------------------------------------------------------------------------
 _PILEUP_KIND = {"M": A.SX_SEG_MATCH, "I": A.SX_SEG_INSERT, "D": A.SX_SEG_DELETE, "N": A.SX_SEG_SKIP, "S": A.SX_SEG_SOFTCLIP, "H": A.SX_SEG_HARDCLIP}

@@ -536,6 +536,8 @@ constexpr sx_status_entry k_status[] = {
     {SX_ST_K9_CAP, SX_ERR_CAPACITY, "%s: cap_segs too small (totals[0] holds the needed size)", "%s: cap_segs too small: %u segment slots needed", 1},
     {SX_ST_SINDEL_CAP, SX_ERR_CAPACITY, "%s: a locus over the alternate-allele caps", nullptr, 0}, // (per-locus status only; listed for the disjointness check)
     {SX_ST_SINDEL_ARG, SX_ERR_ARG, "%s: a candidate indel that is not of type INDEL, or an error-rate index past the table", nullptr, 0},
+    {SX_ST_INDEL_READS_DUP, SX_ERR_ARG, "%s: a read id twice in one locus's list", nullptr, 0}, // (per-locus status only; listed for the disjointness check)
+    {SX_ST_K6B_ID, SX_ERR_ARG, "%s: a record's window index outside its region's window, or an indel id at or past n_gid", nullptr, 0},
 };
 
 constexpr bool status_bits_disjoint()

@@ -96,6 +96,11 @@ enum sx_slot : int
     SX_SLOT_K3_INFO, SX_SLOT_K3_CURSOR, SX_SLOT_K3_ORDER, SX_SLOT_K3_SCRATCH,
     SX_SLOT_K4_SCAN_S, SX_SLOT_K4_SCAN_B, SX_SLOT_K4_TILE_SUMS,
     SX_SLOT_K6_MAX, SX_SLOT_K6_LIST, SX_SLOT_K6_ARENA, SX_SLOT_K6_CLASS, SX_SLOT_K6_HIST, SX_SLOT_K6_LIST_BY_CLASS,
+    SX_SLOT_K6B_LOCUS_OF, SX_SLOT_K6B_PAIR_OFF, SX_SLOT_K6B_CURSOR, SX_SLOT_K6B_CNT2, SX_SLOT_K6B_ACNT, SX_SLOT_K6B_SUMS, SX_SLOT_K6B_ALT_IDS,
+    SX_SLOT_K6B_PAIR_ID, SX_SLOT_K6B_PAIR_REC, SX_SLOT_K6B_PAIR_READ, SX_SLOT_K6B_PAIR_ORDER,
+    // K6b's output where the library owns it: the sx_sindel_batch between the link and K5b (sx_somatic_indel_from_records_dev), and the
+    // device side of sx_link_indel_reads
+    SX_SLOT_K6B_OUT_ALT_OFF, SX_SLOT_K6B_OUT_ALTS, SX_SLOT_K6B_OUT_READ_OFF, SX_SLOT_K6B_OUT_READS, SX_SLOT_K6B_OUT_STATUS, SX_SLOT_K6B_OUT_TOTALS,
     SX_SLOT_K7_READ_REGION, SX_SLOT_K7_ARENA, SX_SLOT_K7_ARENA_DEEP, SX_SLOT_K7_CNT_ALN, SX_SLOT_K7_CNT_SEG, SX_SLOT_K7_CNT_KEY, SX_SLOT_K7_SUMS,
     SX_SLOT_K7_LOG, SX_SLOT_K7_LOG_OFF, SX_SLOT_K7_LOG_CURSOR, SX_SLOT_K7_RETRY1, SX_SLOT_K7_RETRY2, SX_SLOT_K7_RETRY_N, SX_SLOT_K7_ACTIVE,
     SX_SLOT_K7_CLASS, SX_SLOT_K7_HIST, SX_SLOT_K7_ACTIVE_BY_CLASS,
@@ -160,6 +165,9 @@ enum sx_status_bit : int
     SX_ST_SINDEL_CAP = 1 << 20,  // K5b: a locus over the alternate caps.  Written to that locus's result status (SX_SINDEL_ST_CAP), never to
                                  // the device word: the locus gets no result and the call goes on.
     SX_ST_SINDEL_ARG = 1 << 21,  // K5b: a candidate that is not SX_INDEL_TYPE_INDEL, or an error-rate index past the table
+    SX_ST_INDEL_READS_DUP = 1 << 22, // K6b: one read id twice in a locus's list.  Like SX_ST_SINDEL_CAP a per-locus status (SX_INDEL_READS_ST_DUP_READ),
+                                     // never in the device word
+    SX_ST_K6B_ID = 1 << 23,      // K6b: a window index past its region's window, or an id at or past n_gid
 };
 static_assert(SX_ST_SINDEL_CAP == SX_SINDEL_ST_CAP, "the per-locus capacity status of K5b is its status bit");
 
@@ -304,6 +312,8 @@ int sx_k8_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* e, uint32_
               unsigned* launches);
 int sx_k1_run_dev(sx_ctx* ctx, const sx_align_batch* d, double* lnp_dev, unsigned* launches);
 int sx_k6_run(sx_ctx* ctx, const sx_score_indels_batch* d, const double* lnp_dev, const sx_score_indels_out* out_dev, unsigned* launches);
+int sx_k6b_run(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* normal, const sx_indel_reads_sample* tumor, const sx_indel_loci* loci, sx_indel_reads_out* out_dev,
+               uint32_t* totals_host, bool own_out, unsigned* launches);
 int sx_k9_run(sx_ctx* ctx, const sx_realign_batch* d, const double* lnp, const sx_realign_out* o, unsigned* launches);
 int sx_k4_run(sx_ctx* ctx, const sx_pileup_reads_batch* d, const sx_pileup_columns* out, unsigned* launches);
 int sx_k2a_run(sx_ctx* ctx, const sx_pileup_batch* d, int is_always_test, sx_digt_result* out_dev, unsigned* launches);
