@@ -14,7 +14,7 @@
 //   1. k4_count_kernel (thread per read): every covered interval is two atomics on difference arrays (tier1 / tier2 column sizes,
 //      the part of each that spills forward into the next window and back into the previous one, spanning deletions, sub-mapped
 //      bases).  Integer, order-free.
-//   2. scans (k4_scan_*): difference arrays -> counts, counts -> CSR offsets.
+//   2. scans (sx_scan): difference arrays -> counts, counts -> CSR offsets.
 //   3. k4_fill_kernel (one WARP per window): walks its reads in order; per read the 32 lanes compute the mismatch-density map
 //      (shared-memory delta array + warp scan) and every base's base_call word, and place it at
 //      site_off[s] + (calls already placed at s).  The running per-site counters live in shared memory for the 3W sites the window's
@@ -204,106 +204,6 @@ __global__ void k4_count_kernel(k4_args A, int* __restrict__ d1, int* __restrict
         }
         if (kind_read(k)) read_head += len;
         if (kind_ref(k)) ref_head += len;
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// pass 2: in-place scans of up to 8 int arrays at once (blockIdx.y picks the array).  Three kernels: tile sums, the scan of the tile
-// sums (one CTA per array), tiles again with their offsets.  exclusive[k] selects the flavour.
-// ---------------------------------------------------------------------------------------------------------------------
-constexpr uint32_t SCAN_TILE = 4096, SCAN_THREADS = 256;
-struct scan_job
-{
-    int* data[8];
-    uint32_t n[8];
-    int exclusive[8];
-};
-
-__device__ __forceinline__ int block_scan_incl(int v, int* warp_sums) // inclusive scan across SCAN_THREADS threads
-{
-    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1)
-    {
-        const int y = __shfl_up_sync(FULL, v, d);
-        if (lane >= (uint32_t)d) v += y;
-    }
-    if (lane == 31) warp_sums[wid] = v;
-    __syncthreads();
-    if (wid == 0)
-    {
-        int s = lane < SCAN_THREADS / 32 ? warp_sums[lane] : 0;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1)
-        {
-            const int y = __shfl_up_sync(FULL, s, d);
-            if (lane >= (uint32_t)d) s += y;
-        }
-        if (lane < SCAN_THREADS / 32) warp_sums[lane] = s;
-    }
-    __syncthreads();
-    if (wid > 0) v += warp_sums[wid - 1];
-    return v;
-}
-
-__global__ void __launch_bounds__(SCAN_THREADS) k4_scan_tile_sums(scan_job J, int* __restrict__ tile_sums, uint32_t tiles_per_array)
-{
-    const uint32_t k = blockIdx.y, tile = blockIdx.x;
-    const uint32_t base = tile * SCAN_TILE;
-    if (base >= J.n[k]) return;
-    int s = 0;
-    for (uint32_t i = base + threadIdx.x; i < min(base + SCAN_TILE, J.n[k]); i += SCAN_THREADS) s += J.data[k][i];
-    __shared__ int ws[SCAN_THREADS / 32];
-    const int incl = block_scan_incl(s, ws);
-    if (threadIdx.x == SCAN_THREADS - 1) tile_sums[k * tiles_per_array + tile] = incl;
-}
-
-__global__ void __launch_bounds__(SCAN_THREADS) k4_scan_of_sums(scan_job J, int* __restrict__ tile_sums, uint32_t tiles_per_array)
-{
-    const uint32_t k = blockIdx.x;
-    const uint32_t nt = (J.n[k] + SCAN_TILE - 1) / SCAN_TILE;
-    __shared__ int ws[SCAN_THREADS / 32];
-    __shared__ int carry_s;
-    if (threadIdx.x == 0) carry_s = 0;
-    __syncthreads();
-    for (uint32_t b = 0; b < nt; b += SCAN_THREADS)
-    {
-        const uint32_t i = b + threadIdx.x;
-        const int v = i < nt ? tile_sums[k * tiles_per_array + i] : 0;
-        const int incl = block_scan_incl(v, ws);
-        const int carry = carry_s;
-        if (i < nt) tile_sums[k * tiles_per_array + i] = carry + incl - v; // exclusive prefix of the tile sums
-        __syncthreads();
-        if (threadIdx.x == SCAN_THREADS - 1) carry_s = carry + incl;
-        __syncthreads();
-    }
-}
-
-__global__ void __launch_bounds__(SCAN_THREADS) k4_scan_tiles(scan_job J, const int* __restrict__ tile_sums, uint32_t tiles_per_array)
-{
-    const uint32_t k = blockIdx.y, tile = blockIdx.x;
-    const uint32_t base = tile * SCAN_TILE, n = J.n[k];
-    if (base >= n) return;
-    __shared__ int ws[SCAN_THREADS / 32];
-    int carry = tile_sums[k * tiles_per_array + tile];
-    constexpr uint32_t PER = SCAN_TILE / SCAN_THREADS; // consecutive elements per thread
-    int v[PER];
-    int s = 0;
-    const uint32_t i0 = base + threadIdx.x * PER;
-#pragma unroll
-    for (uint32_t e = 0; e < PER; ++e)
-    {
-        v[e] = (i0 + e) < n ? J.data[k][i0 + e] : 0;
-        s += v[e];
-    }
-    const int incl = block_scan_incl(s, ws);
-    int run = carry + incl - s;
-#pragma unroll
-    for (uint32_t e = 0; e < PER; ++e)
-    {
-        const int out = J.exclusive[k] ? run : run + v[e];
-        run += v[e];
-        if ((i0 + e) < n) J.data[k][i0 + e] = out;
     }
 }
 
@@ -648,14 +548,12 @@ int sx_k4_run(sx_ctx* ctx, const sx_pileup_reads_batch* d, const sx_pileup_colum
     int* d2 = reinterpret_cast<int*>(out->t2_off);
     int* dsd = reinterpret_cast<int*>(out->n_spandel);
     int* dsm = reinterpret_cast<int*>(out->n_submapped);
-    int *s1 = nullptr, *s2 = nullptr, *b1 = nullptr, *b2 = nullptr, *tile_sums = nullptr;
+    int *s1 = nullptr, *s2 = nullptr, *b1 = nullptr, *b2 = nullptr;
     int rc;
-    const uint32_t tiles = (n_sites + 1 + SCAN_TILE - 1) / SCAN_TILE;
     if ((rc = sx_take(ctx, SX_SLOT_K4_SCAN_S, (size_t)(n_sites + 1) * 2, s1, 64))) return rc;
     s2 = s1 + (n_sites + 1);
     if ((rc = sx_take(ctx, SX_SLOT_K4_SCAN_B, (size_t)(n_sites + 1) * 2, b1, 64))) return rc;
     b2 = b1 + (n_sites + 1);
-    if ((rc = sx_take(ctx, SX_SLOT_K4_TILE_SUMS, (size_t)tiles * 8, tile_sums, 64))) return rc;
     SX_CUDA(ctx, cudaMemsetAsync(d1, 0, (size_t)(n_sites + 1) * 4, st));
     SX_CUDA(ctx, cudaMemsetAsync(d2, 0, (size_t)(n_sites + 1) * 4, st));
     SX_CUDA(ctx, cudaMemsetAsync(dsd, 0, (size_t)n_sites * 4, st));
@@ -669,32 +567,22 @@ int sx_k4_run(sx_ctx* ctx, const sx_pileup_reads_batch* d, const sx_pileup_colum
         SX_CUDA(ctx, cudaGetLastError());
         ++launches;
     }
-    auto run_scans = [&](const scan_job& J, int n_arrays) -> int {
-        const dim3 grid(tiles, n_arrays);
-        k4_scan_tile_sums<<<grid, SCAN_THREADS, 0, st>>>(J, tile_sums, tiles);
-        k4_scan_of_sums<<<n_arrays, SCAN_THREADS, 0, st>>>(J, tile_sums, tiles);
-        k4_scan_tiles<<<grid, SCAN_THREADS, 0, st>>>(J, tile_sums, tiles);
-        SX_CUDA(ctx, cudaGetLastError());
-        launches += 3;
-        return SX_OK;
-    };
     {
-        scan_job J{}; // differences -> counts
-        int* arr[8] = {d1, d2, s1, s2, dsd, dsm, b1, b2};
-        const uint32_t n[8] = {n_sites + 1, n_sites + 1, n_sites, n_sites, n_sites, n_sites, n_sites, n_sites};
-        for (int k = 0; k < 8; ++k)
-        {
-            J.data[k] = arr[k];
-            J.n[k] = n[k];
-            J.exclusive[k] = 0;
-        }
-        if ((rc = run_scans(J, 8))) return rc;
-        scan_job K{}; // counts -> CSR offsets
-        K.data[0] = d1;
-        K.data[1] = d2;
-        K.n[0] = K.n[1] = n_sites + 1;
-        K.exclusive[0] = K.exclusive[1] = 1;
-        if ((rc = run_scans(K, 2))) return rc;
+        // differences -> counts (the int arrays scan as uint32_t: two's-complement sums have the same bits), then counts -> CSR offsets
+        const auto u = [](int* p) { return reinterpret_cast<uint32_t*>(p); };
+        const uint32_t n = n_sites;
+        const sx_scan_set counts = {8,
+                                    {{u(d1), n + 1, 0, nullptr},
+                                     {u(d2), n + 1, 0, nullptr},
+                                     {u(s1), n, 0, nullptr},
+                                     {u(s2), n, 0, nullptr},
+                                     {u(dsd), n, 0, nullptr},
+                                     {u(dsm), n, 0, nullptr},
+                                     {u(b1), n, 0, nullptr},
+                                     {u(b2), n, 0, nullptr}}};
+        if ((rc = sx_scan(ctx, SX_SLOT_K4_TILE_SUMS, counts, &launches))) return rc;
+        const sx_scan_set offsets = {2, {{u(d1), n + 1, SX_SCAN_EXCLUSIVE, nullptr}, {u(d2), n + 1, SX_SCAN_EXCLUSIVE, nullptr}}};
+        if ((rc = sx_scan(ctx, SX_SLOT_K4_TILE_SUMS, offsets, &launches))) return rc;
     }
     uint32_t totals[2] = {0, 0};
     SX_CUDA(ctx, cudaMemcpyAsync(&totals[0], out->site_off + n_sites, 4, cudaMemcpyDeviceToHost, st));

@@ -6,23 +6,24 @@
 //   applications/strelka/strelka_pos_processor.cpp:305-348       process_pos_indel_somatic, its reader
 //
 // Shape of the work: every 32-byte record is read, one in a few becomes a 24-byte entry somewhere else -- no arithmetic, so the floor is
-// the bytes (tools/indel_reads_leg.py counts them).  A CSR producer like K7b and K9: count -> sx_scan3.cuh -> write, with a sort between.
+// the bytes (tools/indel_reads_leg.py counts them).  A CSR producer like K7b and K9: count -> scan (sx_scan) -> write, with a sort between.
 //   k6b_locus_table_kernel  id -> locus as a dense table of n_gid words.  A binary search of loci.gid would cost ~20 dependent loads per
 //                           record, twice (count and scatter), against one load here; the table is an eighth of the gid_key array the
 //                           caller already holds, so an id space too sparse for it is too sparse for the ABI.
 //   k6b_count_kernel        one thread per read of either sample: integer atomics on cnt[2 * locus + sample]
-//   scan                    -> pair_off; one 12-byte round trip sizes the pair scratch (and refuses more than 2^32 - 1 entries)
+//   scan                    -> pair_off, copied to the scatter's cursors; one 12-byte round trip sizes the pair scratch (and refuses more
+//                           than 2^32 - 1 entries)
 //   k6b_scatter_kernel      (read id, record, read) triples at atomic cursors: the order inside a (locus, sample) segment is arbitrary here
 //   k6b_sort_kernel         one warp per locus: each segment sorted by read id (k6b_sort_by_key, in shared memory up to K6B_SMEM_SORT
 //                           entries, in the global scratch itself beyond -- no depth cap), equal neighbours = a duplicate id; the
 //                           alternates' ids gathered into an ascending set of at most 16.  Read ids of an unflagged segment are distinct,
 //                           so the sorted order -- and with it every output byte -- is the same whatever order the atomics ran in.
-//   scan                    of the unflagged loci's counts -> read_off, alt_off, totals; one 8-byte round trip checks the capacities
+//   scan                    of the unflagged loci's counts, in place in read_off and alt_off, -> totals; one 8-byte round trip checks
+//                           the capacities
 //   k6b_write_kernel        one warp per locus: the table rows from gid_key, and every entry (k6b_entry) at its sorted place
 // The body is k6b_core.cuh.
 #include "k6b_core.cuh"
 #include "sx_internal.h"
-#include "sx_scan3.cuh"
 
 #include <algorithm>
 
@@ -71,17 +72,6 @@ __global__ void __launch_bounds__(K6B_THREADS) k6b_count_kernel(const k6b_view v
     if (st) atomicOr(status, SX_ST_K6B_ID);
 }
 
-// adds the tile offsets to the scanned counts: off[i] (and a copy in `cursor`) for i < n, off[n] = the total
-__global__ void __launch_bounds__(K7_SCAN_THREADS) k6b_pair_off_kernel(const uint32_t n, uint32_t* __restrict__ off, uint32_t* __restrict__ cursor, const uint32_t* __restrict__ sums,
-                                                                      const uint32_t* __restrict__ totals)
-{
-    const uint32_t tile(blockIdx.x), base(tile * K7_SCAN_THREADS * K7_SCAN_ITEMS + threadIdx.x * K7_SCAN_ITEMS);
-    const uint32_t add(sums[tile]);
-    for (int i = 0; i < K7_SCAN_ITEMS; ++i)
-        if (base + i < n) cursor[base + i] = off[base + i] = off[base + i] + add;
-    if (blockIdx.x == 0 && threadIdx.x == 0) off[n] = totals[0];
-}
-
 __global__ void __launch_bounds__(K6B_THREADS) k6b_scatter_kernel(const k6b_view v, uint32_t* __restrict__ cursor, const k6b_pairs P)
 {
     const uint32_t n0(v.s[0].n_reads), n(n0 + v.s[1].n_reads);
@@ -99,9 +89,9 @@ __global__ void __launch_bounds__(K6B_THREADS) k6b_scatter_kernel(const k6b_view
 }
 
 // one warp per locus: P.order of both segments, the locus's status, its ascending alternate ids (alt_ids[16 * locus ..]) and the counts
-// the second scan runs over (cnt2[2 * locus + sample], acnt[locus]; 0 for a flagged locus)
-__global__ void __launch_bounds__(K6B_THREADS) k6b_sort_kernel(const k6b_view v, const uint32_t* __restrict__ pair_off, const k6b_pairs P, uint32_t* __restrict__ loc_status,
-                                                              uint32_t* __restrict__ alt_ids, uint32_t* __restrict__ cnt2, uint32_t* __restrict__ acnt, int* __restrict__ status)
+// the second scan runs over (read_off[2 * locus + sample], alt_off[locus]; 0 for a flagged locus)
+__global__ void __launch_bounds__(K6B_THREADS) k6b_sort_kernel(const k6b_view v, const uint32_t* __restrict__ pair_off, const k6b_pairs P, uint32_t* __restrict__ alt_ids,
+                                                              const sx_indel_reads_out o, int* __restrict__ status)
 {
     __shared__ uint32_t s_key[K6B_WARPS][K6B_SMEM_SORT], s_val[K6B_WARPS][K6B_SMEM_SORT];
     __shared__ uint32_t s_set[K6B_WARPS][SX_SINDEL_MAX_ALTS], s_n[K6B_WARPS], s_over[K6B_WARPS];
@@ -163,35 +153,15 @@ __global__ void __launch_bounds__(K6B_THREADS) k6b_sort_kernel(const k6b_view v,
         const uint32_t st((__any_sync(FULL, dup) ? SX_INDEL_READS_ST_DUP_READ : 0u) | (s_over[warp] ? SX_SINDEL_ST_CAP : 0u));
         const uint32_t n_alts(st ? 0u : s_n[warp]);
         if (lane < n_alts) alt_ids[(size_t)SX_SINDEL_MAX_ALTS * l + lane] = s_set[warp][lane];
-        if (lane < 2) cnt2[2 * l + lane] = st ? 0u : pair_off[2 * l + lane + 1] - pair_off[2 * l + lane];
+        if (lane < 2) o.read_off[2 * l + lane] = st ? 0u : pair_off[2 * l + lane + 1] - pair_off[2 * l + lane];
         if (lane == 0)
         {
-            loc_status[l] = st;
-            acnt[l] = n_alts;
+            o.status[l] = st;
+            o.alt_off[l] = n_alts;
         }
         __syncwarp();
     }
     if (bad) atomicOr(status, SX_ST_K6B_ID);
-}
-
-// adds the tile offsets to the second scan: read_off[2 * n_loci + 1], alt_off[n_loci + 1] (acnt is scanned over 2 * n_loci words, the
-// upper half zeros) and the totals
-__global__ void __launch_bounds__(K7_SCAN_THREADS) k6b_out_off_kernel(const uint32_t n_loci, const uint32_t* __restrict__ cnt2, const uint32_t* __restrict__ acnt,
-                                                                     const uint32_t* __restrict__ sums, const uint32_t n_tiles, const uint32_t* __restrict__ totals,
-                                                                     const sx_indel_reads_out o)
-{
-    const uint32_t tile(blockIdx.x), base(tile * K7_SCAN_THREADS * K7_SCAN_ITEMS + threadIdx.x * K7_SCAN_ITEMS);
-    const uint32_t add_r(sums[tile]), add_a(sums[n_tiles + tile]);
-    for (int i = 0; i < K7_SCAN_ITEMS; ++i)
-    {
-        if (base + i < 2 * n_loci) o.read_off[base + i] = cnt2[base + i] + add_r;
-        if (base + i < n_loci) o.alt_off[base + i] = acnt[base + i] + add_a;
-    }
-    if (blockIdx.x == 0 && threadIdx.x == 0)
-    {
-        o.read_off[2 * n_loci] = o.totals[0] = totals[0];
-        o.alt_off[n_loci] = o.totals[1] = totals[1];
-    }
 }
 
 __global__ void __launch_bounds__(K6B_THREADS) k6b_write_kernel(const k6b_view v, const uint32_t* __restrict__ pair_off, const k6b_pairs P, const uint32_t* __restrict__ alt_ids,
@@ -278,17 +248,12 @@ int sx_k6b_run(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* norma
         return SX_OK;
     }
     if (!o->status) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL output array", what);
-    const uint32_t tile(K7_SCAN_THREADS * K7_SCAN_ITEMS), n_tiles((n2 + tile - 1) / tile);
-    uint32_t *locus_of(nullptr), *pair_off(nullptr), *cursor(nullptr), *cnt2(nullptr), *acnt(nullptr), *sums(nullptr), *alt_ids(nullptr);
+    uint32_t *locus_of(nullptr), *pair_off(nullptr), *cursor(nullptr), *alt_ids(nullptr);
     if ((rc = sx_take(ctx, SX_SLOT_K6B_LOCUS_OF, loci->n_gid, locus_of, 16))) return rc;
     if ((rc = sx_take(ctx, SX_SLOT_K6B_PAIR_OFF, (size_t)n2 + 1, pair_off, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K6B_CURSOR, n2, cursor, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K6B_CNT2, n2, cnt2, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K6B_ACNT, n2, acnt, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K6B_SUMS, (size_t)3 * n_tiles + 4 + 2, sums, 0))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K6B_CURSOR, (size_t)n2 + 2, cursor, 0))) return rc;
     if ((rc = sx_take(ctx, SX_SLOT_K6B_ALT_IDS, (size_t)SX_SINDEL_MAX_ALTS * n_loci, alt_ids, 16))) return rc;
-    uint32_t* totals(sums + (size_t)3 * n_tiles);
-    unsigned long long* total64(reinterpret_cast<unsigned long long*>(sums + (((size_t)3 * n_tiles + 4) & ~(size_t)1))); // (8-byte aligned, past totals[0..2])
+    unsigned long long* total64(reinterpret_cast<unsigned long long*>(cursor + n2)); // (past the cursors; n2 is even, so 8-byte aligned)
     const int cap(ctx->sm_count * 16);
     const auto grid = [cap](const uint32_t m, const uint32_t per) { return (unsigned)std::max(1, std::min<int>((int)((m + per - 1) / per), cap)); };
 
@@ -299,22 +264,18 @@ int sx_k6b_run(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* norma
     v.locus_of = locus_of;
     SX_CUDA(ctx, cudaMemsetAsync(locus_of, 0xFF, (size_t)loci->n_gid * 4, st));
     SX_CUDA(ctx, cudaMemsetAsync(pair_off, 0, (size_t)n2 * 4, st));
-    SX_CUDA(ctx, cudaMemsetAsync(cnt2, 0, (size_t)n2 * 4, st)); // (the first scan's idle second and third array)
-    SX_CUDA(ctx, cudaMemsetAsync(acnt, 0, (size_t)n2 * 4, st));
     k6b_locus_table_kernel<<<grid(n_loci, 256), 256, 0, st>>>(*loci, locus_of, ctx->d_status);
     SX_CUDA(ctx, cudaGetLastError());
     SX_CUDA(ctx, cudaMemsetAsync(total64, 0, 8, st));
     k6b_count_kernel<<<grid(n_reads, K6B_THREADS), K6B_THREADS, 0, st>>>(v, pair_off, total64, ctx->d_status);
     SX_CUDA(ctx, cudaGetLastError());
-    k7_scan_tiles<<<n_tiles, K7_SCAN_THREADS, 0, st>>>(n2, pair_off, cnt2, acnt, sums, n_tiles);
-    SX_CUDA(ctx, cudaGetLastError());
-    k7_scan_sums<<<1, K7_SCAN_THREADS, 0, st>>>(sums, n_tiles, totals);
-    SX_CUDA(ctx, cudaGetLastError());
-    k6b_pair_off_kernel<<<n_tiles, K7_SCAN_THREADS, 0, st>>>(n2, pair_off, cursor, sums, totals);
-    SX_CUDA(ctx, cudaGetLastError());
+    *launches += 2;
+    const sx_scan_set pairs = {1, {{pair_off, n2, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, nullptr}}};
+    if ((rc = sx_scan(ctx, SX_SLOT_K6B_SUMS, pairs, launches))) return rc;
+    SX_CUDA(ctx, cudaMemcpyAsync(cursor, pair_off, (size_t)n2 * 4, cudaMemcpyDeviceToDevice, st));
     uint32_t n_pairs(0);
     unsigned long long n_pairs64(0);
-    SX_CUDA(ctx, cudaMemcpyAsync(&n_pairs, totals, 4, cudaMemcpyDeviceToHost, st));
+    SX_CUDA(ctx, cudaMemcpyAsync(&n_pairs, pair_off + n2, 4, cudaMemcpyDeviceToHost, st));
     SX_CUDA(ctx, cudaMemcpyAsync(&n_pairs64, total64, 8, cudaMemcpyDeviceToHost, st));
     SX_CUDA(ctx, cudaStreamSynchronize(st));
     if (n_pairs64 != n_pairs) return sx_fail(ctx, SX_ERR_RANGE, "%s: %llu entries: the offsets are 32-bit", what, n_pairs64);
@@ -326,19 +287,13 @@ int sx_k6b_run(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* norma
     if ((rc = sx_take(ctx, SX_SLOT_K6B_PAIR_ORDER, n_pairs, P.order, 16))) return rc;
     k6b_scatter_kernel<<<grid(n_reads, K6B_THREADS), K6B_THREADS, 0, st>>>(v, cursor, P);
     SX_CUDA(ctx, cudaGetLastError());
-    SX_CUDA(ctx, cudaMemsetAsync(cursor, 0, (size_t)n2 * 4, st)); // (the second scan's idle third array)
-    SX_CUDA(ctx, cudaMemsetAsync(acnt, 0, (size_t)n2 * 4, st));
-    k6b_sort_kernel<<<grid(n_loci, K6B_WARPS), K6B_THREADS, 0, st>>>(v, pair_off, P, o->status, alt_ids, cnt2, acnt, ctx->d_status);
+    k6b_sort_kernel<<<grid(n_loci, K6B_WARPS), K6B_THREADS, 0, st>>>(v, pair_off, P, alt_ids, *o, ctx->d_status);
     SX_CUDA(ctx, cudaGetLastError());
-    k7_scan_tiles<<<n_tiles, K7_SCAN_THREADS, 0, st>>>(n2, cnt2, acnt, cursor, sums, n_tiles);
-    SX_CUDA(ctx, cudaGetLastError());
-    k7_scan_sums<<<1, K7_SCAN_THREADS, 0, st>>>(sums, n_tiles, totals);
-    SX_CUDA(ctx, cudaGetLastError());
-    k6b_out_off_kernel<<<n_tiles, K7_SCAN_THREADS, 0, st>>>(n_loci, cnt2, acnt, sums, n_tiles, totals, *o);
-    SX_CUDA(ctx, cudaGetLastError());
-    SX_CUDA(ctx, cudaMemcpyAsync(h_totals, totals, 8, cudaMemcpyDeviceToHost, st));
+    *launches += 2;
+    const sx_scan_set out = {2, {{o->read_off, n2, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, o->totals}, {o->alt_off, n_loci, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, o->totals + 1}}};
+    if ((rc = sx_scan(ctx, SX_SLOT_K6B_SUMS, out, launches))) return rc;
+    SX_CUDA(ctx, cudaMemcpyAsync(h_totals, o->totals, 8, cudaMemcpyDeviceToHost, st));
     SX_CUDA(ctx, cudaStreamSynchronize(st));
-    *launches += 10;
     if (totals_host)
     {
         totals_host[0] = h_totals[0];

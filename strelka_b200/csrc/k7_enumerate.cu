@@ -12,7 +12,7 @@
 // arena.  The result size is unknown until the search has run, and the output must be a dense CSR in read order (it IS the next
 // kernels' input), so the search runs twice with a scan in between:
 //   k7_count_kernel : search -> per read (alignments, segments, keys) + status
-//   scan            : three exclusive prefix sums over reads (one block per 2048 reads + a single-block pass over the block sums)
+//   scan            : three exclusive prefix sums over reads (sx_scan), the alignment offsets straight into aln_off
 //   k7_write_kernel : search again (deterministic) -> the set, in its order, at the read's offsets
 // Searching twice costs less than a second arena large enough to keep every read's set between the passes, and keeps the output
 // independent of scheduling.  Persistent grid: resident blocks x SM count, a thread strides over reads.
@@ -20,7 +20,6 @@
 #include "k7_core.cuh"
 #include "sx_internal.h"
 #include "sx_regroup.cuh"
-#include "sx_scan3.cuh"
 
 #include <algorithm>
 #include <cstdlib>
@@ -31,7 +30,7 @@ constexpr int K7_THREADS = 64;
 
 struct k7_counts // per read, then (after the scan) its exclusive offsets
 {
-    uint32_t* aln;
+    uint32_t* aln; // the output's aln_off
     uint32_t* seg;
     uint32_t* key;
 };
@@ -83,48 +82,33 @@ int k7_frames_needed(sx_ctx* ctx, const sx_enum_batch* d, uint32_t* read_region,
     return SX_OK;
 }
 
-// phase 2 of the scan + the batch-wide closing entries; flags the capacity overflow
-__global__ void __launch_bounds__(K7_SCAN_THREADS) k7_scan_finish(const uint32_t n, const k7_counts c, const uint32_t* __restrict__ sums, const uint32_t n_tiles,
-                                                                  const uint32_t* __restrict__ totals, const sx_enum_out o, int* __restrict__ status)
+// the scan's totals against the capacities: block 0 raises SX_ST_K7_CAP, or closes the per-alignment offset arrays
+__device__ __forceinline__ bool k7_fits(const sx_enum_out& o, int* __restrict__ status)
 {
-    const uint32_t tile(blockIdx.x);
-    const uint32_t base(tile * K7_SCAN_THREADS * K7_SCAN_ITEMS + threadIdx.x * K7_SCAN_ITEMS);
-    const uint32_t oa(sums[tile]), os(sums[(size_t)n_tiles + tile]), ok(sums[(size_t)2 * n_tiles + tile]);
-    for (int i = 0; i < K7_SCAN_ITEMS; ++i)
-        if (base + i < n)
-        {
-            const uint32_t a(c.aln[base + i] + oa);
-            c.aln[base + i] = a;
-            c.seg[base + i] += os;
-            c.key[base + i] += ok;
-            o.aln_off[base + i] = a;
-        }
+    const bool fits(o.totals[0] <= o.cap_alns && o.totals[1] <= o.cap_segs && o.totals[2] <= o.cap_keys);
     if (blockIdx.x == 0 && threadIdx.x == 0)
     {
-        o.aln_off[n] = totals[0];
-        o.totals[0] = totals[0];
-        o.totals[1] = totals[1];
-        o.totals[2] = totals[2];
-        if (totals[0] > o.cap_alns || totals[1] > o.cap_segs || totals[2] > o.cap_keys) atomicOr(status, SX_ST_K7_CAP);
+        if (!fits) atomicOr(status, SX_ST_K7_CAP);
         else
         {
-            o.aln_seg_off[totals[0]] = totals[1];
-            o.aln_key_off[totals[0]] = totals[2];
+            o.aln_seg_off[o.totals[0]] = o.totals[1];
+            o.aln_key_off[o.totals[0]] = o.totals[2];
         }
     }
+    return fits;
 }
 
 __global__ void __launch_bounds__(K7_THREADS) k7_write_kernel(const k7_view v, unsigned char* __restrict__ arena, const size_t per_thread, const uint32_t maxA,
                                                               const uint32_t maxF, const uint32_t* __restrict__ read_region, const uint8_t* __restrict__ status,
-                                                              const k7_counts c, const sx_enum_out o, const uint32_t* __restrict__ totals)
+                                                              const k7_counts c, const sx_enum_out o, int* __restrict__ d_status)
 {
-    if (totals[0] > o.cap_alns || totals[1] > o.cap_segs || totals[2] > o.cap_keys) return; // reported by k7_scan_finish
+    if (!k7_fits(o, d_status)) return;
     const uint32_t t(blockIdx.x * blockDim.x + threadIdx.x), nthr(gridDim.x * blockDim.x);
     k7_scratch S(k7_scratch_at(arena + (size_t)t * per_thread, maxA, maxF));
     for (uint32_t r = t; r < v.b.n_reads; r += nthr)
     {
         if (status[r] & (SX_ENUM_ST_EXCEPTION | SX_ENUM_ST_LIMIT)) continue;
-        const uint32_t na((r + 1 < v.b.n_reads ? c.aln[r + 1] : totals[0]) - c.aln[r]);
+        const uint32_t na(c.aln[r + 1] - c.aln[r]);
         if (na == 0) continue;
         k7_enumerate_read(v, read_region[r], r, S);
         k7_write(S, o, c.aln[r], c.seg[r], c.key[r]);
@@ -314,16 +298,16 @@ __global__ void __launch_bounds__(K7_THREADS) k7_search_arena_kernel(const k7_vi
     }
 }
 
-__global__ void k7_gather_kernel(const uint32_t n_reads, const k7_counts c, const k7_log L, const sx_enum_out o, const uint32_t* __restrict__ totals,
+__global__ void k7_gather_kernel(const uint32_t n_reads, const k7_counts c, const k7_log L, const sx_enum_out o, int* __restrict__ d_status,
                                  const uint32_t* __restrict__ list, const uint32_t* __restrict__ n_list)
 {
-    if (totals[0] > o.cap_alns || totals[1] > o.cap_segs || totals[2] > o.cap_keys) return; // reported by k7_scan_finish
+    if (!k7_fits(o, d_status)) return;
     // with a list (in read order: the CSR output is written in read order): only the searched reads have a blob
     const uint32_t n_work(list ? *n_list : n_reads);
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_work; i += gridDim.x * blockDim.x)
     {
         const uint32_t r(list ? list[i] : i);
-        const uint32_t na((r + 1 < n_reads ? c.aln[r + 1] : totals[0]) - c.aln[r]);
+        const uint32_t na(c.aln[r + 1] - c.aln[r]);
         if (na == 0 || L.blob_off[r] == UINT32_MAX) continue;
         k7_blob_gather(L.words + L.blob_off[r], na, o, c.aln[r], c.seg[r], c.key[r]);
     }
@@ -346,6 +330,25 @@ unsigned k7_max_candidate_alignment_toggle(const unsigned n_indel, const unsigne
     return n_indel;
 }
 
+// the per-read counts: alignments in the output's aln_off, segments and keys in the stage's scratch
+int k7_take_counts(sx_ctx* ctx, const uint32_t n, const sx_enum_out* o, k7_counts* c)
+{
+    int rc;
+    c->aln = o->aln_off;
+    if ((rc = sx_take(ctx, SX_SLOT_K7_CNT_SEG, n, c->seg, 16))) return rc;
+    return sx_take(ctx, SX_SLOT_K7_CNT_KEY, n, c->key, 16);
+}
+
+// counts -> exclusive offsets, aln_off[n] and the three totals
+int k7_offsets(sx_ctx* ctx, const uint32_t n, const sx_enum_out* o, const k7_counts& c, unsigned* launches)
+{
+    const sx_scan_set J = {3,
+                           {{c.aln, n, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, o->totals},
+                            {c.seg, n, SX_SCAN_EXCLUSIVE, o->totals + 1},
+                            {c.key, n, SX_SCAN_EXCLUSIVE, o->totals + 2}}};
+    return sx_scan(ctx, SX_SLOT_K7_SUMS, J, launches);
+}
+
 int k7_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsigned* launches)
 {
     cudaStream_t st(ctx->s_compute);
@@ -366,27 +369,17 @@ int k7_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsigned* 
     unsigned char* arena(nullptr);
     if ((rc = sx_take(ctx, SX_SLOT_K7_ARENA, blocks * K7_THREADS * per_thread, arena, 0))) return rc;
     k7_counts c;
-    if ((rc = sx_take(ctx, SX_SLOT_K7_CNT_ALN, n, c.aln, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K7_CNT_SEG, n, c.seg, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K7_CNT_KEY, n, c.key, 16))) return rc;
-    const uint32_t tile(K7_SCAN_THREADS * K7_SCAN_ITEMS), n_tiles((n + tile - 1) / tile);
-    uint32_t* sums(nullptr);
-    if ((rc = sx_take(ctx, SX_SLOT_K7_SUMS, (size_t)3 * n_tiles + 4, sums, 0))) return rc;
-    uint32_t* totals(sums + (size_t)3 * n_tiles);
+    if ((rc = k7_take_counts(ctx, n, o, &c))) return rc;
 
     k7_view v;
     v.b = *d;
     k7_count_kernel<<<(unsigned)blocks, K7_THREADS, 0, st>>>(v, arena, per_thread, maxA, maxF, read_region, o->status, c);
     SX_CUDA(ctx, cudaGetLastError());
-    k7_scan_tiles<<<n_tiles, K7_SCAN_THREADS, 0, st>>>(n, c.aln, c.seg, c.key, sums, n_tiles);
+    *launches = 2; // (with the frame count)
+    if ((rc = k7_offsets(ctx, n, o, c, launches))) return rc;
+    k7_write_kernel<<<(unsigned)blocks, K7_THREADS, 0, st>>>(v, arena, per_thread, maxA, maxF, read_region, o->status, c, *o, ctx->d_status);
     SX_CUDA(ctx, cudaGetLastError());
-    k7_scan_sums<<<1, K7_SCAN_THREADS, 0, st>>>(sums, n_tiles, totals);
-    SX_CUDA(ctx, cudaGetLastError());
-    k7_scan_finish<<<n_tiles, K7_SCAN_THREADS, 0, st>>>(n, c, sums, n_tiles, totals, *o, ctx->d_status);
-    SX_CUDA(ctx, cudaGetLastError());
-    k7_write_kernel<<<(unsigned)blocks, K7_THREADS, 0, st>>>(v, arena, per_thread, maxA, maxF, read_region, o->status, c, *o, totals);
-    SX_CUDA(ctx, cudaGetLastError());
-    *launches = 6;
+    *launches += 1;
     return SX_OK;
 }
 
@@ -422,13 +415,7 @@ int k7_run_fast(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsig
     if ((rc = sx_take(ctx, SX_SLOT_K7_ARENA, blocks1 * K7_THREADS * per_thread1, arena1, 0))) return rc;
     if (two_levels && (rc = sx_take(ctx, SX_SLOT_K7_ARENA_DEEP, blocks * K7_THREADS * per_thread, arena, 0))) return rc;
     k7_counts c;
-    if ((rc = sx_take(ctx, SX_SLOT_K7_CNT_ALN, n, c.aln, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K7_CNT_SEG, n, c.seg, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K7_CNT_KEY, n, c.key, 16))) return rc;
-    const uint32_t tile(K7_SCAN_THREADS * K7_SCAN_ITEMS), n_tiles((n + tile - 1) / tile);
-    uint32_t* sums(nullptr);
-    if ((rc = sx_take(ctx, SX_SLOT_K7_SUMS, (size_t)3 * n_tiles + 4, sums, 0))) return rc;
-    uint32_t* totals(sums + (size_t)3 * n_tiles);
+    if ((rc = k7_take_counts(ctx, n, o, &c))) return rc;
     // the log holds whatever the output arrays can hold: 3 words + segments + ceil(keys / 2) words per alignment
     const unsigned long long want_words((unsigned long long)o->cap_alns * 4ull + o->cap_segs + (o->cap_keys + 1ull) / 2ull + 16ull);
     k7_log L;
@@ -451,8 +438,7 @@ int k7_run_fast(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsig
         SX_CUDA(ctx, cudaMemsetAsync(c.seg, 0, (size_t)n * 4, st));
         SX_CUDA(ctx, cudaMemsetAsync(c.key, 0, (size_t)n * 4, st));
         SX_CUDA(ctx, cudaMemsetAsync(o->status, 0, (size_t)n, st));
-        k7_active_reads_kernel<<<std::max(1, std::min<int>((int)((n + 255) / 256), ctx->sm_count * 8)), 256, 0, st>>>(n, d->gate, R.list0, R.n + 2);
-        SX_CUDA(ctx, cudaGetLastError());
+        if ((rc = sx_k7_active_reads(ctx, n, d->gate, R.list0, R.n + 2))) return rc;
         extra = 1;
     }
 
@@ -486,16 +472,12 @@ int k7_run_fast(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsig
         k7_search_arena_kernel<<<(unsigned)blocks, K7_THREADS, 0, st>>>(v, arena, per_thread, maxA, maxF, read_region, o->status, R, 2, 0, c, L);
         SX_CUDA(ctx, cudaGetLastError());
     }
-    k7_scan_tiles<<<n_tiles, K7_SCAN_THREADS, 0, st>>>(n, c.aln, c.seg, c.key, sums, n_tiles);
-    SX_CUDA(ctx, cudaGetLastError());
-    k7_scan_sums<<<1, K7_SCAN_THREADS, 0, st>>>(sums, n_tiles, totals);
-    SX_CUDA(ctx, cudaGetLastError());
-    k7_scan_finish<<<n_tiles, K7_SCAN_THREADS, 0, st>>>(n, c, sums, n_tiles, totals, *o, ctx->d_status);
-    SX_CUDA(ctx, cudaGetLastError());
+    *launches = (two_levels ? 4 : 3) + extra; // (with the frame count)
+    if ((rc = k7_offsets(ctx, n, o, c, launches))) return rc;
     const int g1(std::max(1, std::min<int>((int)((n + 127) / 128), ctx->sm_count * 16)));
-    k7_gather_kernel<<<g1, 128, 0, st>>>(n, c, L, *o, totals, nullptr, nullptr); // (every read, in read order: walking the active list instead, in read or class order, was slower)
+    k7_gather_kernel<<<g1, 128, 0, st>>>(n, c, L, *o, ctx->d_status, nullptr, nullptr); // (every read, in read order: walking the active list instead, in read or class order, was slower)
     SX_CUDA(ctx, cudaGetLastError());
-    *launches = (two_levels ? 8 : 7) + extra;
+    *launches += 1;
     return SX_OK;
 }
 
@@ -517,6 +499,13 @@ int k7_check_args(sx_ctx* ctx, const sx_enum_batch* b, const sx_enum_out* o, con
 }
 
 } // namespace
+
+int sx_k7_active_reads(sx_ctx* ctx, const uint32_t n_reads, const uint8_t* gate, uint32_t* list, uint32_t* count)
+{
+    k7_active_reads_kernel<<<std::max(1, std::min<int>((int)((n_reads + 255) / 256), ctx->sm_count * 8)), 256, 0, ctx->s_compute>>>(n_reads, gate, list, count);
+    SX_CUDA(ctx, cudaGetLastError());
+    return SX_OK;
+}
 
 extern "C" void sx_default_enum_opts(sx_enum_opts* o)
 {

@@ -10,7 +10,6 @@
 
 #include "k7a_core.cuh"
 #include "sx_internal.h"
-#include "sx_scan3.cuh"
 
 #include <algorithm>
 
@@ -36,25 +35,10 @@ __global__ void k7a_read_offsets_kernel(const k7a_view v, unsigned long long* __
 // pass copies them instead of walking the read again.
 #define K7A_STAGE 6u
 
-__global__ void k7a_active_reads_kernel(const uint32_t n_reads, const uint8_t* __restrict__ gate, uint32_t* __restrict__ list, uint32_t* __restrict__ count)
-{
-    const uint32_t lane(threadIdx.x & 31u);
-    for (uint32_t b = (blockIdx.x * blockDim.x + threadIdx.x) - lane; b < n_reads; b += gridDim.x * blockDim.x)
-    {
-        const uint32_t r(b + lane);
-        const bool on(r < n_reads && (gate[r] & SX_GATE_REALIGN));
-        const unsigned m(__ballot_sync(0xffffffffu, on));
-        uint32_t at(0);
-        if (lane == 0 && m) at = atomicAdd(count, (uint32_t)__popc(m));
-        at = __shfl_sync(0xffffffffu, at, 0);
-        if (on) list[at + __popc(m & ((1u << lane) - 1u))] = r;
-    }
-}
-
-// list == NULL: every read (and the per-read defaults are written here); otherwise the listed reads (the defaults were set by the host side)
-__global__ void k7a_count_kernel(const k7a_view v, const unsigned long long* __restrict__ read_byte, const uint32_t* __restrict__ read_region, uint32_t* __restrict__ cnt,
-                                 uint32_t* __restrict__ zero1, uint32_t* __restrict__ zero2, const uint32_t* __restrict__ list, const uint32_t* __restrict__ n_list,
-                                 uint16_t* __restrict__ stage, const sx_prep_out o)
+// list == NULL: every read (and the per-read defaults are written here); otherwise the listed reads (the defaults were set by the host side).
+// The counts go into in_key_off, which the scan turns into the offsets.
+__global__ void k7a_count_kernel(const k7a_view v, const unsigned long long* __restrict__ read_byte, const uint32_t* __restrict__ read_region,
+                                 const uint32_t* __restrict__ list, const uint32_t* __restrict__ n_list, uint16_t* __restrict__ stage, const sx_prep_out o)
 {
     const uint32_t n_work(list ? *n_list : v.b.n_reads);
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_work; i += gridDim.x * blockDim.x)
@@ -62,8 +46,7 @@ __global__ void k7a_count_kernel(const k7a_view v, const unsigned long long* __r
         const uint32_t r(list ? list[i] : i);
         uint16_t keys[K7A_MAX_KEYS], lead, trail;
         const uint32_t n(k7a_read(v, read_region[r], r, read_byte[r], keys, lead, trail));
-        cnt[r] = n;
-        if (!list) zero1[r] = zero2[r] = 0;
+        o.in_key_off[r] = n;
         o.in_lead_key[r] = lead;
         o.in_trail_key[r] = trail;
         if (stage)
@@ -71,36 +54,19 @@ __global__ void k7a_count_kernel(const k7a_view v, const unsigned long long* __r
     }
 }
 
-__global__ void __launch_bounds__(K7_SCAN_THREADS) k7a_finish_kernel(const uint32_t n, uint32_t* __restrict__ cnt, const uint32_t* __restrict__ sums, const uint32_t* __restrict__ totals,
-                                                                    const sx_prep_out o, int* __restrict__ status)
+__global__ void k7a_write_kernel(const k7a_view v, const unsigned long long* __restrict__ read_byte, const uint32_t* __restrict__ read_region, const uint32_t* __restrict__ list,
+                                 const uint32_t* __restrict__ n_list, const uint16_t* __restrict__ stage, const sx_prep_out o, int* __restrict__ status)
 {
-    const uint32_t tile(blockIdx.x), base(tile * K7_SCAN_THREADS * K7_SCAN_ITEMS + threadIdx.x * K7_SCAN_ITEMS);
-    const uint32_t off(sums[tile]);
-    for (int i = 0; i < K7_SCAN_ITEMS; ++i)
-        if (base + i < n)
-        {
-            const uint32_t x(cnt[base + i] + off);
-            cnt[base + i] = x;
-            o.in_key_off[base + i] = x;
-        }
-    if (blockIdx.x == 0 && threadIdx.x == 0)
+    if (o.totals[0] > o.cap_keys)
     {
-        o.in_key_off[n] = totals[0];
-        o.totals[0] = totals[0];
-        if (totals[0] > o.cap_keys) atomicOr(status, SX_ST_K7A_CAP);
+        if (blockIdx.x == 0 && threadIdx.x == 0) atomicOr(status, SX_ST_K7A_CAP);
+        return;
     }
-}
-
-__global__ void k7a_write_kernel(const k7a_view v, const unsigned long long* __restrict__ read_byte, const uint32_t* __restrict__ read_region, const uint32_t* __restrict__ off,
-                                 const uint32_t* __restrict__ totals, const uint32_t* __restrict__ list, const uint32_t* __restrict__ n_list, const uint16_t* __restrict__ stage,
-                                 const sx_prep_out o)
-{
-    if (totals[0] > o.cap_keys) return;
     const uint32_t n_work(list ? *n_list : v.b.n_reads);
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_work; i += gridDim.x * blockDim.x)
     {
         const uint32_t r(list ? list[i] : i);
-        const uint32_t at(off[r]), n_known(o.in_key_off[r + 1] - at);
+        const uint32_t at(o.in_key_off[r]), n_known(o.in_key_off[r + 1] - at);
         if (stage && n_known <= K7A_STAGE)
         {
             for (uint32_t k = 0; k < n_known; ++k) o.in_keys[at + k] = stage[(size_t)r * K7A_STAGE + k];
@@ -137,15 +103,9 @@ int k7a_run(sx_ctx* ctx, const k7a_view& v, const sx_prep_out* o, unsigned* laun
     const uint32_t n(v.b.n_reads);
     int rc;
     unsigned long long* read_byte(nullptr);
-    uint32_t *read_region(nullptr), *cnt(nullptr), *z1(nullptr), *z2(nullptr), *sums(nullptr);
+    uint32_t* read_region(nullptr);
     if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_READ_WORD, n, read_byte, 16))) return rc;
     if ((rc = sx_take(ctx, SX_SLOT_K7A_READ_REGION, n, read_region, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_CNT, n, cnt, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_Z1, n, z1, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_Z2, n, z2, 16))) return rc;
-    const uint32_t tile(K7_SCAN_THREADS * K7_SCAN_ITEMS), n_tiles((n + tile - 1) / tile);
-    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_SUMS, (size_t)3 * n_tiles + 4, sums, 0))) return rc;
-    uint32_t* totals(sums + (size_t)3 * n_tiles);
     const int cap(ctx->sm_count * 16);
     const auto grid = [cap](const uint32_t m) { return (unsigned)std::max(1, std::min<int>((int)((m + 127) / 128), cap)); };
     k7a_read_offsets_kernel<<<grid(v.b.n_regions), 128, 0, st>>>(v, read_byte, read_region);
@@ -159,26 +119,20 @@ int k7a_run(sx_ctx* ctx, const k7a_view& v, const sx_prep_out* o, unsigned* laun
         if ((rc = sx_take(ctx, SX_SLOT_K7A_ACTIVE, (size_t)n + 4, list, 0))) return rc;
         n_list = list + n;
         SX_CUDA(ctx, cudaMemsetAsync(n_list, 0, 4, st));
-        SX_CUDA(ctx, cudaMemsetAsync(cnt, 0, (size_t)n * 4, st));
-        SX_CUDA(ctx, cudaMemsetAsync(z1, 0, (size_t)n * 4, st));
-        SX_CUDA(ctx, cudaMemsetAsync(z2, 0, (size_t)n * 4, st));
+        SX_CUDA(ctx, cudaMemsetAsync(o->in_key_off, 0, (size_t)n * 4, st));
         SX_CUDA(ctx, cudaMemsetAsync(o->in_lead_key, 0xFF, (size_t)n * 2, st)); // SX_NO_KEY
         SX_CUDA(ctx, cudaMemsetAsync(o->in_trail_key, 0xFF, (size_t)n * 2, st));
-        k7a_active_reads_kernel<<<std::max(1, std::min<int>((int)((n + 255) / 256), ctx->sm_count * 8)), 256, 0, st>>>(n, v.b.gate, list, n_list);
-        SX_CUDA(ctx, cudaGetLastError());
+        if ((rc = sx_k7_active_reads(ctx, n, v.b.gate, list, n_list))) return rc;
         extra = 1;
     }
-    k7a_count_kernel<<<grid(n), 128, 0, st>>>(v, read_byte, read_region, cnt, z1, z2, list, n_list, stage, *o);
+    k7a_count_kernel<<<grid(n), 128, 0, st>>>(v, read_byte, read_region, list, n_list, stage, *o);
     SX_CUDA(ctx, cudaGetLastError());
-    k7_scan_tiles<<<n_tiles, K7_SCAN_THREADS, 0, st>>>(n, cnt, z1, z2, sums, n_tiles);
+    *launches = 2 + extra;
+    const sx_scan_set J = {1, {{o->in_key_off, n, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, o->totals}}};
+    if ((rc = sx_scan(ctx, SX_SLOT_K7A_K9_SUMS, J, launches))) return rc;
+    k7a_write_kernel<<<grid(n), 128, 0, st>>>(v, read_byte, read_region, list, n_list, stage, *o, ctx->d_status);
     SX_CUDA(ctx, cudaGetLastError());
-    k7_scan_sums<<<1, K7_SCAN_THREADS, 0, st>>>(sums, n_tiles, totals);
-    SX_CUDA(ctx, cudaGetLastError());
-    k7a_finish_kernel<<<n_tiles, K7_SCAN_THREADS, 0, st>>>(n, cnt, sums, totals, *o, ctx->d_status);
-    SX_CUDA(ctx, cudaGetLastError());
-    k7a_write_kernel<<<grid(n), 128, 0, st>>>(v, read_byte, read_region, cnt, totals, list, n_list, stage, *o);
-    SX_CUDA(ctx, cudaGetLastError());
-    *launches = 6 + extra;
+    *launches += 1;
     return SX_OK;
 }
 

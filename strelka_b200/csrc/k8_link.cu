@@ -7,11 +7,10 @@
 // Shape of the work: a streaming relabel -- every K7 segment is read once, every K1 segment and insert byte written once; the only
 // structure is K1's staging rule (each region's first segment a multiple of 8, its first insert byte a multiple of 16), which turns
 // the offsets into a two-level prefix sum: within a region (one thread per region walks its alignments' sizes) and over regions
-// (sx_scan3.cuh).  Launches: sizes (thread per alignment) -> region sums -> scan -> write (thread per alignment) + region records.
+// (sx_scan).  Launches: sizes (thread per alignment) -> region sums -> scan -> write (thread per alignment) -> pads + region records.
 
 #include "k8_core.cuh"
 #include "sx_internal.h"
-#include "sx_scan3.cuh"
 
 #include <algorithm>
 
@@ -50,7 +49,7 @@ __global__ void k8_size_kernel(const k8_view v, const uint32_t n_alns, const uin
 // per region: exclusive offsets of its alignments within the region (in place) and the region's padded totals.  One WARP per region: a region
 // of a 30x window holds a few hundred alignments, and one thread walking them was most of the link's time
 __global__ void k8_region_kernel(const k8_view v, uint32_t* __restrict__ seg_n, uint32_t* __restrict__ ins_n, uint32_t* __restrict__ reg_seg,
-                                 uint32_t* __restrict__ reg_ins, uint32_t* __restrict__ reg_zero)
+                                 uint32_t* __restrict__ reg_ins)
 {
     const uint32_t lane(threadIdx.x & 31u), wpb(blockDim.x >> 5);
     for (uint32_t g = blockIdx.x * wpb + (threadIdx.x >> 5); g < v.b.n_regions; g += gridDim.x * wpb)
@@ -84,48 +83,17 @@ __global__ void k8_region_kernel(const k8_view v, uint32_t* __restrict__ seg_n, 
         {
             reg_seg[g] = (s + 7u) & ~7u;
             reg_ins[g] = (n + 15u) & ~15u;
-            reg_zero[g] = 0;
         }
     }
 }
 
-// region offsets after the scan; region records; capacity check; sentinels
-__global__ void __launch_bounds__(K7_SCAN_THREADS) k8_finish_kernel(const k8_view v, const uint32_t n_alns, uint32_t* __restrict__ reg_seg, uint32_t* __restrict__ reg_ins,
-                                                                   const uint32_t* __restrict__ sums, const uint32_t n_tiles, const uint32_t* __restrict__ totals,
-                                                                   const sx_link_out o, int* __restrict__ status)
-{
-    const uint32_t n(v.b.n_regions), tile(blockIdx.x);
-    const uint32_t base(tile * K7_SCAN_THREADS * K7_SCAN_ITEMS + threadIdx.x * K7_SCAN_ITEMS);
-    const uint32_t os(sums[tile]), on(sums[(size_t)n_tiles + tile]);
-    for (int i = 0; i < K7_SCAN_ITEMS; ++i)
-        if (base + i < n)
-        {
-            const uint32_t g(base + i);
-            const uint32_t s(reg_seg[g] + os), b(reg_ins[g] + on);
-            reg_seg[g] = s;
-            reg_ins[g] = b;
-            o.regions[g].aln_begin = v.e.aln_off[v.b.region_read_off[g]];
-            o.regions[g].seg_begin = s;
-            o.regions[g].ins_begin = b;
-        }
-    if (blockIdx.x == 0 && threadIdx.x == 0)
-    {
-        o.totals[0] = totals[0];
-        o.totals[1] = totals[1];
-        o.regions[n].aln_begin = n_alns;
-        o.regions[n].seg_begin = totals[0];
-        o.regions[n].ins_begin = totals[1];
-        o.regions[n].read_begin = v.b.n_reads;
-        if (totals[0] > o.cap_segs || totals[1] > o.cap_ins) atomicOr(status, SX_ST_K8_CAP);
-        else o.alns[n_alns] = sx_aln{v.b.n_reads, 0, totals[0], totals[1]};
-    }
-}
+__device__ __forceinline__ bool k8_fits(const sx_link_out& o) { return o.totals[0] <= o.cap_segs && o.totals[1] <= o.cap_ins; }
 
 __global__ void k8_write_kernel(const k8_view v, const uint32_t n_alns, const uint32_t* __restrict__ aln_read, const uint32_t* __restrict__ read_region,
                                 const uint32_t* __restrict__ seg_rel, const uint32_t* __restrict__ ins_rel, const uint32_t* __restrict__ reg_seg,
-                                const uint32_t* __restrict__ reg_ins, const uint32_t* __restrict__ totals, const sx_link_out o)
+                                const uint32_t* __restrict__ reg_ins, const sx_link_out o)
 {
-    if (totals[0] > o.cap_segs || totals[1] > o.cap_ins) return; // reported by k8_finish_kernel
+    if (!k8_fits(o)) return; // reported by k8_pad_kernel
     for (uint32_t a = blockIdx.x * blockDim.x + threadIdx.x; a < n_alns; a += gridDim.x * blockDim.x)
     {
         const uint32_t r(aln_read[a]), g(read_region[r]);
@@ -138,15 +106,31 @@ __global__ void k8_write_kernel(const k8_view v, const uint32_t n_alns, const ui
     }
 }
 
-// the pads between a region's last used segment / insert byte and the next region's first
-__global__ void k8_pad_kernel(const k8_view v, const uint32_t* __restrict__ seg_rel, const uint32_t* __restrict__ ins_rel, const uint32_t* __restrict__ reg_seg,
-                              const uint32_t* __restrict__ reg_ins, const uint32_t* __restrict__ totals, const sx_link_out o)
+// the region records (also when a capacity is too small: they say what each region needs), the sentinels, the capacity check, and the
+// pads between a region's last used segment / insert byte and the next region's first
+__global__ void k8_pad_kernel(const k8_view v, const uint32_t n_alns, const uint32_t* __restrict__ seg_rel, const uint32_t* __restrict__ ins_rel,
+                              const uint32_t* __restrict__ reg_seg, const uint32_t* __restrict__ reg_ins, const sx_link_out o, int* __restrict__ status)
 {
-    if (totals[0] > o.cap_segs || totals[1] > o.cap_ins) return;
-    for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < v.b.n_regions; g += gridDim.x * blockDim.x)
+    const uint32_t nr(v.b.n_regions);
+    const uint32_t* totals(o.totals);
+    const bool fits(k8_fits(o));
+    if (blockIdx.x == 0 && threadIdx.x == 0)
+    {
+        o.regions[nr].aln_begin = n_alns;
+        o.regions[nr].seg_begin = totals[0];
+        o.regions[nr].ins_begin = totals[1];
+        o.regions[nr].read_begin = v.b.n_reads;
+        if (!fits) atomicOr(status, SX_ST_K8_CAP);
+        else o.alns[n_alns] = sx_aln{v.b.n_reads, 0, totals[0], totals[1]};
+    }
+    for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < nr; g += gridDim.x * blockDim.x)
     {
         const uint32_t a0(v.e.aln_off[v.b.region_read_off[g]]), a1(v.e.aln_off[v.b.region_read_off[g + 1]]);
-        const uint32_t seg_end(g + 1 < v.b.n_regions ? reg_seg[g + 1] : totals[0]), ins_end(g + 1 < v.b.n_regions ? reg_ins[g + 1] : totals[1]);
+        o.regions[g].aln_begin = a0;
+        o.regions[g].seg_begin = reg_seg[g];
+        o.regions[g].ins_begin = reg_ins[g];
+        if (!fits) continue;
+        const uint32_t seg_end(g + 1 < nr ? reg_seg[g + 1] : totals[0]), ins_end(g + 1 < nr ? reg_ins[g + 1] : totals[1]);
         uint32_t s(reg_seg[g]), b(reg_ins[g]);
         if (a1 > a0) // the end of the region's last alignment
         {
@@ -158,7 +142,7 @@ __global__ void k8_pad_kernel(const k8_view v, const uint32_t* __restrict__ seg_
         for (; s < seg_end; ++s) o.segs[s] = sx_aln_seg{0, SX_SEG_HARDCLIP, 0};
         for (; b < ins_end; ++b) o.ins[b] = 0;
     }
-    if (blockIdx.x == 0 && threadIdx.x == 0) // K1 loads 16-byte slices: up to 16 no-op segments of slack after the last one, where they fit
+    if (fits && blockIdx.x == 0 && threadIdx.x == 0) // K1 loads 16-byte slices: up to 16 no-op segments of slack after the last one, where they fit
         for (uint32_t s = totals[0]; s < o.cap_segs && s < totals[0] + 16u; ++s) o.segs[s] = sx_aln_seg{0, SX_SEG_HARDCLIP, 0};
 }
 
@@ -167,7 +151,7 @@ int k8_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* e, const uint
 {
     cudaStream_t st(ctx->s_compute);
     int rc;
-    uint32_t *aln_read(nullptr), *read_region(nullptr), *seg_n(nullptr), *ins_n(nullptr), *reg_seg(nullptr), *reg_ins(nullptr), *reg_zero(nullptr), *sums(nullptr);
+    uint32_t *aln_read(nullptr), *read_region(nullptr), *seg_n(nullptr), *ins_n(nullptr), *reg_seg(nullptr), *reg_ins(nullptr);
     const uint32_t nr(d->n_regions);
     if ((rc = sx_take(ctx, SX_SLOT_K8_ALN_READ, n_alns, aln_read, 16))) return rc;
     if ((rc = sx_take(ctx, SX_SLOT_K8_READ_REGION, d->n_reads, read_region, 16))) return rc;
@@ -175,10 +159,6 @@ int k8_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* e, const uint
     if ((rc = sx_take(ctx, SX_SLOT_K8_INS_N, n_alns, ins_n, 16))) return rc;
     if ((rc = sx_take(ctx, SX_SLOT_K8_REG_SEG, nr, reg_seg, 16))) return rc;
     if ((rc = sx_take(ctx, SX_SLOT_K8_REG_INS, nr, reg_ins, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K8_REG_ZERO, nr, reg_zero, 16))) return rc;
-    const uint32_t tile(K7_SCAN_THREADS * K7_SCAN_ITEMS), n_tiles((nr + tile - 1) / tile);
-    if ((rc = sx_take(ctx, SX_SLOT_K8_SUMS, (size_t)3 * n_tiles + 4, sums, 0))) return rc;
-    uint32_t* totals(sums + (size_t)3 * n_tiles);
     k8_view v;
     v.b = *d;
     v.e = *e;
@@ -192,19 +172,16 @@ int k8_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* e, const uint
     SX_CUDA(ctx, cudaGetLastError());
     k8_size_kernel<<<grid(n_alns), 128, 0, st>>>(v, n_alns, aln_read, read_region, seg_n, ins_n, ctx->d_status);
     SX_CUDA(ctx, cudaGetLastError());
-    k8_region_kernel<<<grid((uint32_t)std::min<uint64_t>((uint64_t)nr * 32u, 0xffffff00u)), 128, 0, st>>>(v, seg_n, ins_n, reg_seg, reg_ins, reg_zero);
+    k8_region_kernel<<<grid((uint32_t)std::min<uint64_t>((uint64_t)nr * 32u, 0xffffff00u)), 128, 0, st>>>(v, seg_n, ins_n, reg_seg, reg_ins);
     SX_CUDA(ctx, cudaGetLastError());
-    k7_scan_tiles<<<n_tiles, K7_SCAN_THREADS, 0, st>>>(nr, reg_seg, reg_ins, reg_zero, sums, n_tiles);
+    *launches = 4;
+    const sx_scan_set J = {2, {{reg_seg, nr, SX_SCAN_EXCLUSIVE, o->totals}, {reg_ins, nr, SX_SCAN_EXCLUSIVE, o->totals + 1}}};
+    if ((rc = sx_scan(ctx, SX_SLOT_K8_SUMS, J, launches))) return rc;
+    k8_write_kernel<<<grid(n_alns), 128, 0, st>>>(v, n_alns, aln_read, read_region, seg_n, ins_n, reg_seg, reg_ins, *o);
     SX_CUDA(ctx, cudaGetLastError());
-    k7_scan_sums<<<1, K7_SCAN_THREADS, 0, st>>>(sums, n_tiles, totals);
+    k8_pad_kernel<<<grid(nr), 128, 0, st>>>(v, n_alns, seg_n, ins_n, reg_seg, reg_ins, *o, ctx->d_status);
     SX_CUDA(ctx, cudaGetLastError());
-    k8_finish_kernel<<<n_tiles, K7_SCAN_THREADS, 0, st>>>(v, n_alns, reg_seg, reg_ins, sums, n_tiles, totals, *o, ctx->d_status);
-    SX_CUDA(ctx, cudaGetLastError());
-    k8_write_kernel<<<grid(n_alns), 128, 0, st>>>(v, n_alns, aln_read, read_region, seg_n, ins_n, reg_seg, reg_ins, totals, *o);
-    SX_CUDA(ctx, cudaGetLastError());
-    k8_pad_kernel<<<grid(nr), 128, 0, st>>>(v, seg_n, ins_n, reg_seg, reg_ins, totals, *o);
-    SX_CUDA(ctx, cudaGetLastError());
-    *launches = 9;
+    *launches += 2;
     return SX_OK;
 }
 

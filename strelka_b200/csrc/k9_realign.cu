@@ -11,54 +11,33 @@
 
 #include "k9_core.cuh"
 #include "sx_internal.h"
-#include "sx_scan3.cuh"
 
 #include <algorithm>
 
 namespace
 {
-__global__ void k9_slots_kernel(const sx_realign_batch b, uint32_t* __restrict__ cnt, uint32_t* __restrict__ z1, uint32_t* __restrict__ z2, uint32_t* __restrict__ read_region)
+// the slot counts go into seg_off, which the scan turns into the offsets
+__global__ void k9_slots_kernel(const sx_realign_batch b, uint32_t* __restrict__ cnt, uint32_t* __restrict__ read_region)
 {
-    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < b.n_reads; r += gridDim.x * blockDim.x)
-    {
-        cnt[r] = k9_slots(b, r);
-        z1[r] = z2[r] = 0;
-    }
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < b.n_reads; r += gridDim.x * blockDim.x) cnt[r] = k9_slots(b, r);
     for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < b.n_regions; g += gridDim.x * blockDim.x)
         for (uint32_t r = b.region_read_off[g]; r < b.region_read_off[g + 1]; ++r) read_region[r] = g;
 }
 
-__global__ void __launch_bounds__(K7_SCAN_THREADS) k9_finish_kernel(const uint32_t n, uint32_t* __restrict__ cnt, const uint32_t* __restrict__ sums, const uint32_t* __restrict__ totals,
-                                                                   const sx_realign_out o, int* __restrict__ status)
+__global__ void __launch_bounds__(128) k9_choose_kernel(const k9_view v, const uint32_t* __restrict__ read_region, const sx_realign_out o, int* __restrict__ status)
 {
-    const uint32_t tile(blockIdx.x), base(tile * K7_SCAN_THREADS * K7_SCAN_ITEMS + threadIdx.x * K7_SCAN_ITEMS);
-    const uint32_t off(sums[tile]);
-    for (int i = 0; i < K7_SCAN_ITEMS; ++i)
-        if (base + i < n)
-        {
-            const uint32_t x(cnt[base + i] + off);
-            cnt[base + i] = x;
-            o.seg_off[base + i] = x;
-        }
-    if (blockIdx.x == 0 && threadIdx.x == 0)
+    if (o.totals[0] > o.cap_segs)
     {
-        o.seg_off[n] = totals[0];
-        o.totals[0] = totals[0];
-        if (totals[0] > o.cap_segs) atomicOr(status, SX_ST_K9_CAP);
+        if (blockIdx.x == 0 && threadIdx.x == 0) atomicOr(status, SX_ST_K9_CAP);
+        return;
     }
-}
-
-__global__ void __launch_bounds__(128) k9_choose_kernel(const k9_view v, const uint32_t* __restrict__ read_region, const uint32_t* __restrict__ off, const uint32_t* __restrict__ totals,
-                                                        const sx_realign_out o)
-{
-    if (totals[0] > o.cap_segs) return;
     uint8_t type[K9_MAX_READ];
     int32_t pos[K9_MAX_READ];
     k9_scratch S = {type, pos};
     const uint32_t n(v.b.n_reads);
     for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n; r += gridDim.x * blockDim.x)
     {
-        const uint32_t s0(off[r]), s1(r + 1 < n ? off[r + 1] : totals[0]);
+        const uint32_t s0(o.seg_off[r]), s1(o.seg_off[r + 1]);
         int32_t p;
         uint16_t ns;
         uint32_t best;
@@ -76,30 +55,21 @@ int k9_run(sx_ctx* ctx, const sx_realign_batch* d, const double* lnp, const sx_r
     cudaStream_t st(ctx->s_compute);
     const uint32_t n(d->n_reads);
     int rc;
-    uint32_t *cnt(nullptr), *z1(nullptr), *z2(nullptr), *read_region(nullptr), *sums(nullptr);
+    uint32_t* read_region(nullptr);
     if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_READ_WORD, n, read_region, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_CNT, n, cnt, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_Z1, n, z1, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_Z2, n, z2, 16))) return rc;
-    const uint32_t tile(K7_SCAN_THREADS * K7_SCAN_ITEMS), n_tiles((n + tile - 1) / tile);
-    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_SUMS, (size_t)3 * n_tiles + 4, sums, 0))) return rc;
-    uint32_t* totals(sums + (size_t)3 * n_tiles);
     const int cap(ctx->sm_count * 16);
     const auto grid = [cap](const uint32_t m) { return (unsigned)std::max(1, std::min<int>((int)((m + 127) / 128), cap)); };
-    k9_slots_kernel<<<grid(std::max(n, d->n_regions)), 128, 0, st>>>(*d, cnt, z1, z2, read_region);
+    k9_slots_kernel<<<grid(std::max(n, d->n_regions)), 128, 0, st>>>(*d, o->seg_off, read_region);
     SX_CUDA(ctx, cudaGetLastError());
-    k7_scan_tiles<<<n_tiles, K7_SCAN_THREADS, 0, st>>>(n, cnt, z1, z2, sums, n_tiles);
-    SX_CUDA(ctx, cudaGetLastError());
-    k7_scan_sums<<<1, K7_SCAN_THREADS, 0, st>>>(sums, n_tiles, totals);
-    SX_CUDA(ctx, cudaGetLastError());
-    k9_finish_kernel<<<n_tiles, K7_SCAN_THREADS, 0, st>>>(n, cnt, sums, totals, *o, ctx->d_status);
-    SX_CUDA(ctx, cudaGetLastError());
+    *launches = 1;
+    const sx_scan_set J = {1, {{o->seg_off, n, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, o->totals}}};
+    if ((rc = sx_scan(ctx, SX_SLOT_K7A_K9_SUMS, J, launches))) return rc;
     k9_view v;
     v.b = *d;
     v.lnp = lnp;
-    k9_choose_kernel<<<grid(n), 128, 0, st>>>(v, read_region, cnt, totals, *o);
+    k9_choose_kernel<<<grid(n), 128, 0, st>>>(v, read_region, *o, ctx->d_status);
     SX_CUDA(ctx, cudaGetLastError());
-    *launches = 5;
+    *launches += 1;
     return SX_OK;
 }
 

@@ -96,20 +96,20 @@ enum sx_slot : int
     SX_SLOT_K3_INFO, SX_SLOT_K3_CURSOR, SX_SLOT_K3_ORDER, SX_SLOT_K3_SCRATCH,
     SX_SLOT_K4_SCAN_S, SX_SLOT_K4_SCAN_B, SX_SLOT_K4_TILE_SUMS,
     SX_SLOT_K6_MAX, SX_SLOT_K6_LIST, SX_SLOT_K6_ARENA, SX_SLOT_K6_CLASS, SX_SLOT_K6_HIST, SX_SLOT_K6_LIST_BY_CLASS,
-    SX_SLOT_K6B_LOCUS_OF, SX_SLOT_K6B_PAIR_OFF, SX_SLOT_K6B_CURSOR, SX_SLOT_K6B_CNT2, SX_SLOT_K6B_ACNT, SX_SLOT_K6B_SUMS, SX_SLOT_K6B_ALT_IDS,
+    SX_SLOT_K6B_LOCUS_OF, SX_SLOT_K6B_PAIR_OFF, SX_SLOT_K6B_CURSOR, SX_SLOT_K6B_SUMS, SX_SLOT_K6B_ALT_IDS,
     SX_SLOT_K6B_PAIR_ID, SX_SLOT_K6B_PAIR_REC, SX_SLOT_K6B_PAIR_READ, SX_SLOT_K6B_PAIR_ORDER,
     // K6b's output where the library owns it: the sx_sindel_batch between the link and K5b (sx_somatic_indel_from_records_dev), and the
     // device side of sx_link_indel_reads
     SX_SLOT_K6B_OUT_ALT_OFF, SX_SLOT_K6B_OUT_ALTS, SX_SLOT_K6B_OUT_READ_OFF, SX_SLOT_K6B_OUT_READS, SX_SLOT_K6B_OUT_STATUS, SX_SLOT_K6B_OUT_TOTALS,
-    SX_SLOT_K7_READ_REGION, SX_SLOT_K7_ARENA, SX_SLOT_K7_ARENA_DEEP, SX_SLOT_K7_CNT_ALN, SX_SLOT_K7_CNT_SEG, SX_SLOT_K7_CNT_KEY, SX_SLOT_K7_SUMS,
+    SX_SLOT_K7_READ_REGION, SX_SLOT_K7_ARENA, SX_SLOT_K7_ARENA_DEEP, SX_SLOT_K7_CNT_SEG, SX_SLOT_K7_CNT_KEY, SX_SLOT_K7_SUMS,
     SX_SLOT_K7_LOG, SX_SLOT_K7_LOG_OFF, SX_SLOT_K7_LOG_CURSOR, SX_SLOT_K7_RETRY1, SX_SLOT_K7_RETRY2, SX_SLOT_K7_RETRY_N, SX_SLOT_K7_ACTIVE,
     SX_SLOT_K7_CLASS, SX_SLOT_K7_HIST, SX_SLOT_K7_ACTIVE_BY_CLASS,
     SX_SLOT_K7A_READ_REGION, SX_SLOT_K7A_STAGE, SX_SLOT_K7A_ACTIVE,
-    SX_SLOT_K8_ALN_READ, SX_SLOT_K8_READ_REGION, SX_SLOT_K8_SEG_N, SX_SLOT_K8_INS_N, SX_SLOT_K8_REG_SEG, SX_SLOT_K8_REG_INS, SX_SLOT_K8_REG_ZERO, SX_SLOT_K8_SUMS,
-    // per-read scratch shared by K7a and K9: a per-read word (K7a: read byte offset, K9: read region), the per-read counts and their scan.
+    SX_SLOT_K8_ALN_READ, SX_SLOT_K8_READ_REGION, SX_SLOT_K8_SEG_N, SX_SLOT_K8_INS_N, SX_SLOT_K8_REG_SEG, SX_SLOT_K8_REG_INS, SX_SLOT_K8_SUMS,
+    // per-read scratch shared by K7a and K9: a per-read word (K7a: read byte offset, K9: read region) and the tile sums of their scan.
     // These are O(reads) and every context that runs the window pass holds them.  Their lifetimes cannot overlap: K7a's are dead once its
     // write kernel has run, and K9 is enqueued after K7a on the same stream (sx_process_window_dev) or by its own entry point.
-    SX_SLOT_K7A_K9_READ_WORD, SX_SLOT_K7A_K9_CNT, SX_SLOT_K7A_K9_Z1, SX_SLOT_K7A_K9_Z2, SX_SLOT_K7A_K9_SUMS,
+    SX_SLOT_K7A_K9_READ_WORD, SX_SLOT_K7A_K9_SUMS,
     // window pass: the intermediates of sx_process_window_dev
     SX_SLOT_WIN_SEQ_OFF, SX_SLOT_WIN_QUAL_OFF, SX_SLOT_WIN_BPOS, SX_SLOT_WIN_NON_AMBIG, SX_SLOT_WIN_PIN, SX_SLOT_WIN_MAXIMA,
     SX_SLOT_WIN_GATE, SX_SLOT_WIN_IN_POS, SX_SLOT_WIN_IN_SEGS,
@@ -121,7 +121,7 @@ enum sx_slot : int
     SX_SLOT_WIN_BEST_TOTALS, SX_SLOT_WIN_BEST_SEG_OFF, SX_SLOT_WIN_BEST_POS, SX_SLOT_WIN_BEST_N_SEG, SX_SLOT_WIN_REALIGN_STATUS, SX_SLOT_WIN_BEST_ALN,
     SX_SLOT_WIN_BEST_SEGS, SX_SLOT_WIN_PILEUP_READS,
     SX_SLOT_WIN_SITE_OFF, SX_SLOT_WIN_T2_OFF, SX_SLOT_WIN_N_SPANDEL, SX_SLOT_WIN_N_SUBMAPPED, SX_SLOT_WIN_CALLS, SX_SLOT_WIN_T2_CALLS,
-    SX_SLOT_WIN_SITE_GL, SX_SLOT_WIN_VARIANT_CHUNKS,
+    SX_SLOT_WIN_SITE_GL, SX_SLOT_WIN_VARIANT_CHUNKS, SX_SLOT_WIN_VARIANT_SUMS,
     // window pass: what sx_process_window uploads (the window batch's arrays) and the outputs it downloads
     SX_SLOT_WUP_REGION_READ_OFF, SX_SLOT_WUP_REGION_KEY_OFF, SX_SLOT_WUP_KEYS, SX_SLOT_WUP_KEY_HAP, SX_SLOT_WUP_KEY_INS_OFF, SX_SLOT_WUP_KEY_INS,
     SX_SLOT_WUP_REALIGN_BEGIN, SX_SLOT_WUP_REALIGN_END, SX_SLOT_WUP_RAW_POS, SX_SLOT_WUP_RAW_SEG_OFF, SX_SLOT_WUP_RAW_SEGS, SX_SLOT_WUP_READ_LEN,
@@ -250,6 +250,31 @@ template <typename T> int sx_download(sx_ctx* ctx, T* dst, const T* src, size_t 
     return SX_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// prefix sums (sx_scan.cu): 1..SX_SCAN_MAX uint32 arrays scanned in place, each with its own length and flavour.  One call enqueues
+// three launches on the compute stream and adds them to *launches; `sums_slot` is the calling stage's own buffer for the tile sums.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr uint32_t SX_SCAN_TILE = 4096, SX_SCAN_THREADS = 256;
+constexpr int SX_SCAN_MAX = 8;
+enum sx_scan_flag : uint32_t
+{
+    SX_SCAN_EXCLUSIVE = 1, // data[i] = the sum of the elements before i (else up to and including i)
+    SX_SCAN_CLOSE = 2,     // also data[n] = the sum of all n (the array holds n + 1 words)
+};
+struct sx_scan_array
+{
+    uint32_t* data;
+    uint32_t n;
+    uint32_t flags;  // sx_scan_flag bits
+    uint32_t* total; // device word for the sum of all n, or NULL
+};
+struct sx_scan_set
+{
+    int n_arrays;
+    sx_scan_array a[SX_SCAN_MAX];
+};
+int sx_scan(sx_ctx* ctx, sx_slot sums_slot, const sx_scan_set& job, unsigned* launches);
+
 // Reports and clears the device status word: SX_OK when it is 0, else the error of its first set bit.  The bits in `first` (a stage's
 // own) are tested before the others.  `totals`, when the caller has them, are the stage's totals the capacity messages quote.
 int sx_check_status(sx_ctx* ctx, const char* what, int first = 0, const uint32_t* totals = nullptr);
@@ -308,6 +333,8 @@ int sx_k7g_run(sx_ctx* ctx, const sx_gate_batch* d, const sx_gate_out* o, unsign
 int sx_k7a_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_region* regions, const uint8_t* seq4, const char* ref, const uint32_t* key_ins_off, const char* key_ins,
                const sx_prep_out* o, unsigned* launches);
 int sx_k7_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsigned* launches);
+// K7 and K7a: the reads whose gate lets them into the search (SX_GATE_REALIGN) as a dense list, *count of them (one launch)
+int sx_k7_active_reads(sx_ctx* ctx, uint32_t n_reads, const uint8_t* gate, uint32_t* list, uint32_t* count);
 int sx_k8_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* e, uint32_t n_alns, const uint32_t* key_ins_off, const char* key_ins, const sx_link_out* o,
               unsigned* launches);
 int sx_k1_run_dev(sx_ctx* ctx, const sx_align_batch* d, double* lnp_dev, unsigned* launches);

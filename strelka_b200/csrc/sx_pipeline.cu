@@ -122,7 +122,7 @@ __global__ void sxp_pileup_reads_kernel(const sx_window_batch b, const prep_out 
     if (max_span) atomicMax(&p.maxima[2], max_span);
 }
 
-// ---- variant-site compaction, order-preserving: per 1024-site chunk a count, an exclusive scan over the chunks, ranked writes
+// ---- variant-site compaction, order-preserving: per 1024-site chunk a count, an exclusive scan over the chunks (sx_scan), ranked writes
 constexpr uint32_t VC_CHUNK = 1024, VC_THREADS = 256;
 __device__ __forceinline__ bool is_variant_site(const sx_digt_result& g) { return g.is_computed && g.genome.max_gt != g.ref_gt; }
 
@@ -136,35 +136,6 @@ __global__ void __launch_bounds__(VC_THREADS) sxp_variant_count_kernel(const sx_
         total += __syncthreads_count(s < n_sites && is_variant_site(gl[s]));
     }
     if (threadIdx.x == 0) chunk_cnt[blockIdx.x] = (uint32_t)total;
-}
-
-__global__ void __launch_bounds__(1024) sxp_variant_scan_kernel(uint32_t* __restrict__ chunk_cnt, const uint32_t n_chunks, uint32_t* __restrict__ total_out)
-{
-    __shared__ uint32_t part[1024];
-    const uint32_t per((n_chunks + 1023u) / 1024u), a(threadIdx.x * per), b(min(n_chunks, a + per));
-    uint32_t sum(0);
-    for (uint32_t i = a; i < b; ++i) sum += chunk_cnt[i];
-    part[threadIdx.x] = sum;
-    __syncthreads();
-    if (threadIdx.x == 0)
-    {
-        uint32_t run(0);
-        for (uint32_t i = 0; i < 1024; ++i)
-        {
-            const uint32_t v(part[i]);
-            part[i] = run;
-            run += v;
-        }
-        *total_out = run;
-    }
-    __syncthreads();
-    uint32_t run(part[threadIdx.x]);
-    for (uint32_t i = a; i < b; ++i)
-    {
-        const uint32_t v(chunk_cnt[i]);
-        chunk_cnt[i] = run;
-        run += v;
-    }
 }
 
 __global__ void __launch_bounds__(VC_THREADS) sxp_variant_write_kernel(const sx_digt_result* __restrict__ gl, const uint32_t* __restrict__ site_off, const uint32_t n_sites,
@@ -638,10 +609,12 @@ extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_w
             uint32_t* chunk_cnt(nullptr);
             if ((rc = take(ctx, SX_SLOT_WIN_VARIANT_CHUNKS, (size_t)n_chunks + 4, chunk_cnt))) return rc;
             sxp_variant_count_kernel<<<n_chunks, VC_THREADS, 0, st>>>(gl, n_sites, chunk_cnt);
-            sxp_variant_scan_kernel<<<1, 1024, 0, st>>>(chunk_cnt, n_chunks, chunk_cnt + n_chunks);
+            SX_CUDA(ctx, cudaGetLastError());
+            const sx_scan_set J = {1, {{chunk_cnt, n_chunks, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, nullptr}}};
+            if ((rc = sx_scan(ctx, SX_SLOT_WIN_VARIANT_SUMS, J, &launches))) return rc;
             sxp_variant_write_kernel<<<n_chunks, VC_THREADS, 0, st>>>(gl, cols.site_off, n_sites, b->report_begin, chunk_cnt, out->variant_sites, out->cap_variant_sites);
             SX_CUDA(ctx, cudaGetLastError());
-            launches += 3;
+            launches += 2;
             SX_CUDA(ctx, cudaMemcpyAsync(&totals[8], chunk_cnt + n_chunks, 4, cudaMemcpyDeviceToHost, st));
         }
     }
