@@ -660,15 +660,7 @@ extern "C" int sx_score_alignments_dev(sx_ctx* ctx, const sx_align_batch* d, dou
     ctx->timing = sx_timing{};
     if (!d || !lnp_out_dev) return sx_fail(ctx, SX_ERR_ARG, "sx_score_alignments_dev: NULL argument");
     if (d->n_regions == 0) return SX_OK;
-    SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    sx_kernel_timer t(ctx);
-    uint32_t need[2] = {0, 0};
-    int rc = k1_smem_need_dev(ctx, d->regions, 0, d->n_regions, need, d->format);
-    if (rc) return rc;
-    rc = sx_k1_launch(ctx, d, 0, d->n_regions, lnp_out_dev, need[0], need[1], ctx->s_compute);
-    if (rc) return rc;
-    t.stop(2);
-    rc = t.finish();
+    const int rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k1_run(ctx, d, lnp_out_dev, launches); });
     if (rc) return rc;
     return sx_check_status(ctx, "sx_score_alignments");
 }
@@ -679,16 +671,7 @@ extern "C" int sx_read_max_dev(sx_ctx* ctx, const sx_align_batch* d, const doubl
     ctx->timing = sx_timing{};
     if (!d || !lnp_dev || !max_lnp_dev || !max_aln_dev) return sx_fail(ctx, SX_ERR_ARG, "sx_read_max_dev: NULL argument");
     if (d->n_reads == 0) return SX_OK;
-    SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    sx_kernel_timer t(ctx);
-    if (d->format & SX_FMT_ALN8)
-        k1_read_max8_kernel<<<(d->n_reads + 255) / 256, 256, 0, ctx->s_compute>>>(d->regions, d->n_regions, reinterpret_cast<const sx_aln8*>(d->alns), d->n_reads, lnp_dev,
-                                                                                  max_lnp_dev, max_aln_dev);
-    else
-        k1_read_max_kernel<<<(d->n_reads + 255) / 256, 256, 0, ctx->s_compute>>>(d->alns, d->n_alns, d->n_reads, lnp_dev, max_lnp_dev, max_aln_dev);
-    SX_CUDA(ctx, cudaGetLastError());
-    t.stop(1);
-    return t.finish();
+    return sx_run_timed(ctx, [&](unsigned* launches) { return sx_k1_read_max_run(ctx, d, lnp_dev, max_lnp_dev, max_aln_dev, launches); });
 }
 
 // Host-buffer entry: the batch is cut into chunks of whole regions; chunk k+1's H2D copies overlap chunk k's kernel and chunk
@@ -792,8 +775,8 @@ extern "C" int sx_score_alignments(sx_ctx* ctx, const sx_align_batch* b, double*
     return sx_check_status(ctx, "sx_score_alignments");
 }
 
-// launcher for the device-resident pipeline (sx_pipeline.cu): one 8-byte round trip picks the shared-memory tile, the kernel is only enqueued
-int sx_k1_run_dev(sx_ctx* ctx, const sx_align_batch* d, double* lnp_dev, unsigned* launches)
+// K1's launcher: one 8-byte round trip picks the shared-memory tile, the kernel is only enqueued
+int sx_k1_run(sx_ctx* ctx, const sx_align_batch* d, double* lnp_dev, unsigned* launches)
 {
     if (d->n_regions == 0) return SX_OK;
     uint32_t need[2] = {0, 0};
@@ -802,4 +785,17 @@ int sx_k1_run_dev(sx_ctx* ctx, const sx_align_batch* d, double* lnp_dev, unsigne
     rc = sx_k1_launch(ctx, d, 0, d->n_regions, lnp_dev, need[0], need[1], ctx->s_compute);
     *launches += 2;
     return rc;
+}
+
+// the per-read maximum of K1's scores (one launch)
+int sx_k1_read_max_run(sx_ctx* ctx, const sx_align_batch* d, const double* lnp_dev, double* max_lnp_dev, uint32_t* max_aln_dev, unsigned* launches)
+{
+    if (d->format & SX_FMT_ALN8)
+        k1_read_max8_kernel<<<(d->n_reads + 255) / 256, 256, 0, ctx->s_compute>>>(d->regions, d->n_regions, reinterpret_cast<const sx_aln8*>(d->alns), d->n_reads, lnp_dev,
+                                                                                  max_lnp_dev, max_aln_dev);
+    else
+        k1_read_max_kernel<<<(d->n_reads + 255) / 256, 256, 0, ctx->s_compute>>>(d->alns, d->n_alns, d->n_reads, lnp_dev, max_lnp_dev, max_aln_dev);
+    SX_CUDA(ctx, cudaGetLastError());
+    *launches += 1;
+    return SX_OK;
 }

@@ -1090,15 +1090,7 @@ extern "C" int sx_site_gl_germline_dev(sx_ctx* ctx, const sx_pileup_batch* d, in
     ctx->timing = sx_timing{};
     if (!d || !out_dev || !d->site_off || !d->calls || !d->ref_base) return sx_fail(ctx, SX_ERR_ARG, "sx_site_gl_germline_dev: NULL argument");
     if (d->n_sites == 0) return SX_OK;
-    SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    sx_kernel_timer t(ctx);
-    uint32_t max_site = 0;
-    int rc = max_site_dev(ctx, d->site_off, d->n_sites, &max_site);
-    if (rc) return rc;
-    rc = germline_run(ctx, d, is_always_test, out_dev, nullptr, nullptr, max_site);
-    if (rc) return rc;
-    t.stop(2);
-    rc = t.finish();
+    const int rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k2a_run(ctx, d, is_always_test, out_dev, launches); });
     if (rc) return rc;
     return sx_check_status(ctx, "sx_site_gl_germline");
 }
@@ -1188,7 +1180,7 @@ extern "C" int sx_dependent_eprob(sx_ctx* ctx, const sx_pileup_batch* b, uint32_
     return sx_check_status(ctx, "sx_dependent_eprob");
 }
 
-// launcher for the device-resident pipeline (sx_pipeline.cu): one 4-byte round trip (the deepest column) picks the kernel
+// K2a's launcher: one 4-byte round trip (the deepest column) picks the kernel
 int sx_k2a_run(sx_ctx* ctx, const sx_pileup_batch* d, int is_always_test, sx_digt_result* out_dev, unsigned* launches)
 {
     if (d->n_sites == 0) return SX_OK;

@@ -290,15 +290,17 @@ __global__ void __launch_bounds__(K2B_WARPS * 32) k2b_somatic_kernel(const uint3
     }
 }
 
-int somatic_run(sx_ctx* ctx, const sx_pileup_batch* n, const sx_pileup_batch* t, const uint8_t* forced_dev, sx_ssnv_result* out_dev)
+} // namespace
+
+int sx_k2b_run(sx_ctx* ctx, const sx_pileup_batch* n, const sx_pileup_batch* t, const uint8_t* forced_dev, sx_ssnv_result* out_dev, unsigned* launches)
 {
     const int grid = static_cast<int>(std::min<uint32_t>((n->n_sites + K2B_WARPS - 1) / K2B_WARPS, (uint32_t)ctx->sm_count * 8));
     k2b_somatic_kernel<<<grid, K2B_WARPS * 32, 0, ctx->s_compute>>>(n->site_off, n->calls, n->t2_off, n->t2_calls, t->site_off, t->calls, t->t2_off, t->t2_calls,
                                                                   n->ref_base, forced_dev, n->n_sites, ctx->d_tables, out_dev);
     SX_CUDA(ctx, cudaGetLastError());
+    *launches += 1;
     return SX_OK;
 }
-} // namespace
 
 extern "C" int sx_site_gl_somatic_dev(sx_ctx* ctx, const sx_pileup_batch* n, const sx_pileup_batch* t, const uint8_t* forced_dev, sx_ssnv_result* out_dev)
 {
@@ -307,12 +309,7 @@ extern "C" int sx_site_gl_somatic_dev(sx_ctx* ctx, const sx_pileup_batch* n, con
     if (!n || !t || !out_dev) return sx_fail(ctx, SX_ERR_ARG, "sx_site_gl_somatic_dev: NULL argument");
     if (n->n_sites != t->n_sites) return sx_fail(ctx, SX_ERR_ARG, "sx_site_gl_somatic_dev: normal and tumor batches differ in n_sites");
     if (n->n_sites == 0) return SX_OK;
-    SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    sx_kernel_timer tm(ctx);
-    int rc = somatic_run(ctx, n, t, forced_dev, out_dev);
-    if (rc) return rc;
-    tm.stop(1);
-    return tm.finish();
+    return sx_run_timed(ctx, [&](unsigned* launches) { return sx_k2b_run(ctx, n, t, forced_dev, out_dev, launches); });
 }
 
 extern "C" int sx_site_gl_somatic(sx_ctx* ctx, const sx_pileup_batch* n, const sx_pileup_batch* t, const uint8_t* forced_host, sx_ssnv_result* out_host)
@@ -333,7 +330,8 @@ extern "C" int sx_site_gl_somatic(sx_ctx* ctx, const sx_pileup_batch* n, const s
     if (forced_host && (rc = sx_upload(ctx, sx_host_slot(21), forced_host, n->n_sites, d_forced, 0))) return rc;
     sx_ssnv_result* d_out = nullptr;
     if ((rc = sx_take(ctx, sx_host_slot(22), n->n_sites, d_out, 0))) return rc;
-    if ((rc = somatic_run(ctx, &dn, &dt, d_forced, d_out))) return rc;
+    unsigned launches = 0;
+    if ((rc = sx_k2b_run(ctx, &dn, &dt, d_forced, d_out, &launches))) return rc;
     if ((rc = sx_download(ctx, out_host, d_out, n->n_sites))) return rc;
-    return tm.finish(1);
+    return tm.finish(launches);
 }

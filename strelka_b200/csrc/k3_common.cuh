@@ -151,5 +151,5 @@ __device__ __forceinline__ bt_state backtrace_start(const sx_ga_scores& sc, cons
 
 // k3_group.cu: classifies the batch, runs every matrix with Q <= 128 and R <= 255 in 8-lane groups, and returns the list of the
 // remaining (large) problems for the warp-per-matrix kernel.
-int sx_k3_group_run(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* d, sx_ga_result* res_dev, uint32_t* cigar_dev, const uint32_t** large_order_dev,
-                    uint32_t* n_large, uint32_t* large_slot_need);
+int sx_k3_group_launch(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* d, sx_ga_result* res_dev, uint32_t* cigar_dev, const uint32_t** large_order_dev,
+                       uint32_t* n_large, uint32_t* large_slot_need);

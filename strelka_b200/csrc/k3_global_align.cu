@@ -6,7 +6,7 @@
 // as called from ActiveRegionProcessor::discoverIndelsAndMismatches (starling_common/ActiveRegionProcessor.cpp:591).
 //
 // This file holds the entry points and the kernel for LARGE matrices (Q > 128 or R > 255, and batches whose penalties do not fit
-// the key encoding of k3_group.cu, which takes everything else first -- see sx_k3_group_run).
+// the key encoding of k3_group.cu, which takes everything else first -- see sx_k3_group_launch).
 //
 // One warp per DP matrix.  Lane l owns the strip of T = ceil(Q/32) consecutive query rows and keeps the three state scores
 // of its rows IN REGISTERS (T is a template parameter up to 4, i.e. Q <= 128; longer queries fall back to a shared-memory
@@ -397,12 +397,15 @@ __global__ void __launch_bounds__(K3_WARPS * 32) k3_global_align_kernel(const ch
     }
 }
 
-int k3_run(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* d, sx_ga_result* res_dev, uint32_t* cigar_dev)
+} // namespace
+
+// K3's launcher.  It counts 4 launches whatever ran, the count sx_global_align_dev has always reported.
+int sx_k3_run(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* d, sx_ga_result* res_dev, uint32_t* cigar_dev, unsigned* launches)
 {
     // small matrices (the common case: haplotypes of an active region) run in 8-lane groups; what is left comes back as a list
     const uint32_t* large = nullptr;
     uint32_t n_large = 0, need = 0;
-    int rc = sx_k3_group_run(ctx, sc, d, res_dev, cigar_dev, &large, &n_large, &need);
+    int rc = sx_k3_group_launch(ctx, sc, d, res_dev, cigar_dev, &large, &n_large, &need);
     if (rc) return rc;
     if (n_large)
     {
@@ -418,9 +421,9 @@ int k3_run(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* d, sx_ga_resu
                                                                          large);
         SX_CUDA(ctx, cudaGetLastError());
     }
+    *launches += 4;
     return SX_OK;
 }
-} // namespace
 
 extern "C" int sx_global_align_dev(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* d, sx_ga_result* res_dev, uint32_t* cigar_dev)
 {
@@ -428,12 +431,7 @@ extern "C" int sx_global_align_dev(sx_ctx* ctx, const sx_ga_scores* sc, const sx
     ctx->timing = sx_timing{};
     if (!sc || !d || !res_dev || !cigar_dev) return sx_fail(ctx, SX_ERR_ARG, "sx_global_align_dev: NULL argument");
     if (d->n == 0) return SX_OK;
-    SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    sx_kernel_timer t(ctx);
-    int rc = k3_run(ctx, sc, d, res_dev, cigar_dev);
-    if (rc) return rc;
-    t.stop(4);
-    return t.finish();
+    return sx_run_timed(ctx, [&](unsigned* launches) { return sx_k3_run(ctx, sc, d, res_dev, cigar_dev, launches); });
 }
 
 extern "C" int sx_global_align(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* b, sx_ga_result* res_host, uint32_t* cigar_host)
@@ -460,7 +458,8 @@ extern "C" int sx_global_align(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_
     if ((rc = sx_take(ctx, sx_host_slot(13), b->n, d_res, 0))) return rc;
     if ((rc = sx_take(ctx, sx_host_slot(14), (size_t)b->n * b->max_ops, d_cig, 16))) return rc;
     SX_CUDA(ctx, cudaMemsetAsync(d_cig, 0, (size_t)b->n * b->max_ops * 4, ctx->s_compute)); // unused cigar slots read as 0
-    if ((rc = k3_run(ctx, sc, &d, d_res, d_cig))) return rc;
+    unsigned device_entry_count = 0; // (the launcher counts what sx_global_align_dev reports; this entry has always reported one launch)
+    if ((rc = sx_k3_run(ctx, sc, &d, d_res, d_cig, &device_entry_count))) return rc;
     if ((rc = sx_download(ctx, res_host, d_res, b->n))) return rc;
     if ((rc = sx_download(ctx, cigar_host, d_cig, (size_t)b->n * b->max_ops))) return rc;
     return t.finish(1);

@@ -175,7 +175,7 @@ __global__ void __launch_bounds__(KG_WARPS * 32) kg_align_kernel(const char* __r
         // value, a delete value, an insert value) in that order, so a plain integer max of keys is exactly AlignerBase::max3's "largest
         // value, first argument wins ties", the tag of the winner says which argument won, and the three-way maxima become single
         // VIMNMX3 / VIADDMNMX instructions.  The tag is replicated in three 2-bit fields so the back-pointer byte of a cell is two
-        // bit-selects of the three winners (no shifts).  sx_k3_group_run keeps batches whose penalties could overflow 64*score out of
+        // bit-selects of the three winners (no shifts).  sx_k3_group_launch keeps batches whose penalties could overflow 64*score out of
         // this kernel.
         int rM[T], rD[T], rI[T];
         char qc[T];
@@ -411,8 +411,8 @@ int kg_launch(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* d, sx_ga_r
 }
 } // namespace
 
-int sx_k3_group_run(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* d, sx_ga_result* res_dev, uint32_t* cigar_dev, const uint32_t** large_order_dev,
-                    uint32_t* n_large, uint32_t* large_slot_need)
+int sx_k3_group_launch(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* d, sx_ga_result* res_dev, uint32_t* cigar_dev, const uint32_t** large_order_dev,
+                       uint32_t* n_large, uint32_t* large_slot_need)
 {
     kg_info* d_info = nullptr;
     uint32_t* d_cursor = nullptr;

@@ -501,15 +501,11 @@ extern "C" void sx_default_pileup_opts(sx_pileup_opts* o)
     o->reserved_ = 0;
 }
 
-// all pointers (batch arrays and output columns) are device pointers; enqueues the three passes (one 8-byte round trip between the scans
-// and the fill checks the capacities) and returns without waiting for the fill
+// K4's launcher: enqueues the three passes (one 8-byte round trip between the scans and the fill checks the capacities) and returns without
+// waiting for the fill
 int sx_k4_run(sx_ctx* ctx, const sx_pileup_reads_batch* d, const sx_pileup_columns* out, unsigned* launches_out)
 {
-    if (!d || !out || !out->site_off || !out->t2_off || !out->n_spandel || !out->n_submapped || !out->calls || !out->t2_calls)
-        return sx_fail(ctx, SX_ERR_ARG, "sx_pileup_reads_dev: NULL argument");
-    if (d->report_end < d->report_begin) return sx_fail(ctx, SX_ERR_ARG, "sx_pileup_reads_dev: empty report range");
     const uint32_t n_sites = static_cast<uint32_t>(d->report_end - d->report_begin);
-    SX_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->s_compute;
     if (d->qual_bits != 0 && d->qual_bits != 8 && d->qual_bits != 4) return sx_fail(ctx, SX_ERR_ARG, "sx_pileup_reads: qual_bits must be 0, 8 or 4");
     const uint32_t shift = d->buffer_pos ? d->max_pos_shift : 0u;
@@ -609,12 +605,10 @@ extern "C" int sx_pileup_reads_dev(sx_ctx* ctx, const sx_pileup_reads_batch* d, 
 {
     if (!ctx) return SX_ERR_ARG;
     ctx->timing = sx_timing{};
-    sx_kernel_timer t(ctx);
-    unsigned launches = 0;
-    int rc = sx_k4_run(ctx, d, out, &launches);
-    if (rc) return rc;
-    t.stop(launches);
-    rc = t.finish();
+    if (!d || !out || !out->site_off || !out->t2_off || !out->n_spandel || !out->n_submapped || !out->calls || !out->t2_calls)
+        return sx_fail(ctx, SX_ERR_ARG, "sx_pileup_reads_dev: NULL argument");
+    if (d->report_end < d->report_begin) return sx_fail(ctx, SX_ERR_ARG, "sx_pileup_reads_dev: empty report range");
+    const int rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k4_run(ctx, d, out, launches); });
     if (rc) return rc;
     return sx_check_status(ctx, "sx_pileup_reads");
 }
@@ -645,7 +639,9 @@ extern "C" int sx_pileup_reads(sx_ctx* ctx, const sx_pileup_reads_batch* b, sx_p
     dc.n_submapped = dc.n_spandel + (n_sites + 1);
     if ((rc = sx_take(ctx, sx_host_slot(7), out->calls_capacity, dc.calls, 64))) return rc;
     if ((rc = sx_take(ctx, sx_host_slot(8), out->t2_capacity, dc.t2_calls, 64))) return rc;
-    const int rc_dev = sx_pileup_reads_dev(ctx, &d, &dc);
+    ctx->timing = sx_timing{}; // (it covers the K4 run alone, not the staging above)
+    int rc_dev = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k4_run(ctx, &d, &dc, launches); });
+    if (!rc_dev) rc_dev = sx_check_status(ctx, "sx_pileup_reads");
     if (rc_dev && rc_dev != SX_ERR_NOMEM) return rc_dev;
     // offsets and counts are valid even when a capacity was too small (the caller can size and retry)
     if ((rc = sx_download(ctx, out->site_off, dc.site_off, (size_t)n_sites + 1))) return rc;

@@ -193,15 +193,17 @@ __global__ void __launch_bounds__(K5_WARPS * 32) k5_indel_gl_kernel(const uint32
     }
 }
 
-int k5_run(sx_ctx* ctx, const sx_indel_batch* d, sx_indel_result* out_dev)
+} // namespace
+
+int sx_k5_run(sx_ctx* ctx, const sx_indel_batch* d, sx_indel_result* out_dev, unsigned* launches)
 {
     const int grid = static_cast<int>(std::min<uint32_t>((d->n_loci + K5_WARPS - 1) / K5_WARPS, (uint32_t)ctx->sm_count * 8));
     k5_indel_gl_kernel<<<grid, K5_WARPS * 32, 0, ctx->s_compute>>>(d->read_off, d->lnp_off, d->allele_off, d->ploidy, d->allele_del_len, d->allele_ins_len, d->allele_lnp,
                                                                   d->read_length, d->non_ambig, d->is_fwd, d->n_loci, ctx->d_tables, out_dev, ctx->d_status);
     SX_CUDA(ctx, cudaGetLastError());
+    *launches += 1;
     return SX_OK;
 }
-} // namespace
 
 extern "C" int sx_indel_gl_dev(sx_ctx* ctx, const sx_indel_batch* d, sx_indel_result* out_dev)
 {
@@ -209,12 +211,8 @@ extern "C" int sx_indel_gl_dev(sx_ctx* ctx, const sx_indel_batch* d, sx_indel_re
     ctx->timing = sx_timing{};
     if (!d || !out_dev) return sx_fail(ctx, SX_ERR_ARG, "sx_indel_gl_dev: NULL argument");
     if (d->n_loci == 0) return SX_OK;
-    SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    sx_kernel_timer t(ctx);
-    int rc = k5_run(ctx, d, out_dev);
+    const int rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k5_run(ctx, d, out_dev, launches); });
     if (rc) return rc;
-    t.stop(1);
-    if ((rc = t.finish())) return rc;
     return sx_check_status(ctx, "sx_indel_gl");
 }
 
@@ -241,8 +239,9 @@ extern "C" int sx_indel_gl(sx_ctx* ctx, const sx_indel_batch* b, sx_indel_result
     if ((rc = sx_upload(ctx, sx_host_slot(9), b->is_fwd, n_reads, d.is_fwd, 16))) return rc;
     sx_indel_result* d_out = nullptr;
     if ((rc = sx_take(ctx, sx_host_slot(10), n_loci, d_out, 0))) return rc;
-    if ((rc = k5_run(ctx, &d, d_out))) return rc;
+    unsigned launches = 0;
+    if ((rc = sx_k5_run(ctx, &d, d_out, &launches))) return rc;
     if ((rc = sx_download(ctx, out_host, d_out, n_loci))) return rc;
-    if ((rc = t.finish(1))) return rc;
+    if ((rc = t.finish(launches))) return rc;
     return sx_check_status(ctx, "sx_indel_gl");
 }

@@ -484,8 +484,9 @@ void k5b_err_terms_of(const sx_sindel_opts& o, const double* err_prob, const uin
         out[i] = make_float2(static_cast<float>(logSharedIndelErrorRate), static_cast<float>(logSharedIndelErrorRateComplement));
     }
 }
+} // namespace
 
-int k5b_check(sx_ctx* ctx, const char* what, const sx_sindel_opts* o, const sx_sindel_batch* b, const double* err_prob, const uint32_t n_err, const void* out)
+int sx_k5b_check(sx_ctx* ctx, const char* what, const sx_sindel_opts* o, const sx_sindel_batch* b, const double* err_prob, const uint32_t n_err, const void* out)
 {
     if (!o || !b || !out) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL argument", what);
     if (o->min_read_bp_flank[0] < 0 || o->min_read_bp_flank[1] < 0) return sx_fail(ctx, SX_ERR_ARG, "%s: negative min_read_bp_flank", what);
@@ -494,8 +495,8 @@ int k5b_check(sx_ctx* ctx, const char* what, const sx_sindel_opts* o, const sx_s
     return SX_OK;
 }
 
-// uploads the per-call constants and error terms (host staging slots 0 and 1) and launches
-int k5b_run(sx_ctx* ctx, const sx_sindel_opts* o, const sx_sindel_batch* d, const double* err_prob, const uint32_t n_err, sx_sindel_result* out_dev)
+// K5b's launcher: uploads the per-call constants and error terms (host staging slots 0 and 1) and launches
+int sx_k5b_run(sx_ctx* ctx, const sx_sindel_opts* o, const sx_sindel_batch* d, const double* err_prob, const uint32_t n_err, sx_sindel_result* out_dev, unsigned* launches)
 {
     static_assert(sizeof(k5b_consts) % 4 == 0, "k5b_consts is copied in words");
     k5b_consts C;
@@ -511,9 +512,9 @@ int k5b_run(sx_ctx* ctx, const sx_sindel_opts* o, const sx_sindel_batch* d, cons
     const int grid = static_cast<int>(std::min<uint32_t>((d->n_loci + K5B_WARPS - 1) / K5B_WARPS, (uint32_t)ctx->sm_count * 8));
     k5b_somatic_indel_kernel<<<grid, K5B_WARPS * 32, 0, ctx->s_compute>>>(*d, d_consts, d_et, n_err, out_dev, ctx->d_status);
     SX_CUDA(ctx, cudaGetLastError());
+    *launches += 1;
     return SX_OK;
 }
-} // namespace
 
 extern "C" void sx_default_sindel_opts(sx_sindel_opts* o)
 {
@@ -534,14 +535,10 @@ extern "C" int sx_somatic_indel_dev(sx_ctx* ctx, const sx_sindel_opts* opts, con
 {
     if (!ctx) return SX_ERR_ARG;
     ctx->timing = sx_timing{};
-    int rc = k5b_check(ctx, "sx_somatic_indel_dev", opts, d, err_prob_host, n_err, out_dev);
+    int rc = sx_k5b_check(ctx, "sx_somatic_indel_dev", opts, d, err_prob_host, n_err, out_dev);
     if (rc) return rc;
     if (d->n_loci == 0) return SX_OK;
-    SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    sx_kernel_timer t(ctx);
-    if ((rc = k5b_run(ctx, opts, d, err_prob_host, n_err, out_dev))) return rc;
-    t.stop(1);
-    if ((rc = t.finish())) return rc;
+    if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k5b_run(ctx, opts, d, err_prob_host, n_err, out_dev, launches); }))) return rc;
     return sx_check_status(ctx, "sx_somatic_indel_dev", SX_ST_SINDEL_ARG);
 }
 
@@ -550,7 +547,7 @@ extern "C" int sx_somatic_indel(sx_ctx* ctx, const sx_sindel_opts* opts, const s
 {
     if (!ctx) return SX_ERR_ARG;
     ctx->timing = sx_timing{};
-    int rc = k5b_check(ctx, "sx_somatic_indel", opts, b, err_prob_host, n_err, out_host);
+    int rc = sx_k5b_check(ctx, "sx_somatic_indel", opts, b, err_prob_host, n_err, out_host);
     if (rc) return rc;
     if (b->n_loci == 0) return SX_OK;
     const size_t n_loci = b->n_loci, n_alts = b->alt_off[n_loci], n_reads = b->read_off[2 * n_loci];
@@ -569,8 +566,9 @@ extern "C" int sx_somatic_indel(sx_ctx* ctx, const sx_sindel_opts* opts, const s
     if ((rc = sx_upload(ctx, sx_host_slot(8), b->reads, n_reads, d.reads, 16))) return rc;
     sx_sindel_result* d_out = nullptr;
     if ((rc = sx_take(ctx, sx_host_slot(9), n_loci, d_out, 0))) return rc;
-    if ((rc = k5b_run(ctx, opts, &d, err_prob_host, n_err, d_out))) return rc;
+    unsigned launches = 0;
+    if ((rc = sx_k5b_run(ctx, opts, &d, err_prob_host, n_err, d_out, &launches))) return rc;
     if ((rc = sx_download(ctx, out_host, d_out, n_loci))) return rc;
-    if ((rc = t.finish(1))) return rc;
+    if ((rc = t.finish(launches))) return rc;
     return sx_check_status(ctx, "sx_somatic_indel", SX_ST_SINDEL_ARG);
 }

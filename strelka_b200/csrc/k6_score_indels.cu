@@ -108,8 +108,23 @@ k6_layout k6_plan(const uint32_t maxA, const uint32_t maxE, const size_t T)
     return L;
 }
 
-int k6_run(sx_ctx* ctx, const sx_score_indels_batch* d, const double* lnp_dev, const sx_score_indels_out* out_dev, unsigned* launches)
+int k6_check_args(sx_ctx* ctx, const sx_score_indels_batch* b, const double* lnp, const sx_score_indels_out* out, const char* what)
 {
+    if (!b || !out) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL argument", what);
+    if (b->n_reads == 0) return SX_OK;
+    if (!lnp || !b->region_read_off || !b->region_key_off || !b->aln_off || !b->aln_pos || !b->aln_seg_off || !b->aln_key_off || !b->read_len || !b->non_ambig ||
+        !b->read_flags || !b->rec_off || !out->recs || !out->n_rec || !out->max_aln || !out->eval_aln)
+        return sx_fail(ctx, SX_ERR_ARG, "%s: NULL array", what);
+    if ((b->n_keys && !b->keys) || b->n_regions == 0) return sx_fail(ctx, SX_ERR_ARG, "%s: reads without a region / keys without a table", what);
+    if (b->opts.min_read_bp_flank < 0) return sx_fail(ctx, SX_ERR_ARG, "%s: negative min_read_bp_flank", what);
+    return SX_OK;
+}
+} // namespace
+
+// K6's launcher: one 8-byte round trip sizes the scratch, the kernel itself is only enqueued
+int sx_k6_run(sx_ctx* ctx, const sx_score_indels_batch* d, const double* lnp_dev, const sx_score_indels_out* out_dev, unsigned* launches)
+{
+    if (d->n_reads == 0) return SX_OK;
     cudaStream_t st(ctx->s_compute);
     // sizes of the launch: the deepest read of the batch decides the scratch
     uint32_t* d_max(nullptr);
@@ -183,22 +198,9 @@ int k6_run(sx_ctx* ctx, const sx_score_indels_batch* d, const double* lnp_dev, c
     }
     k6_score_list_kernel<<<(unsigned)(T / threads), threads, 0, st>>>(v, S, list, d_max + 2, ctx->d_status);
     SX_CUDA(ctx, cudaGetLastError());
-    *launches = 2 + extra;
+    *launches += 2 + extra;
     return SX_OK;
 }
-
-int k6_check_args(sx_ctx* ctx, const sx_score_indels_batch* b, const double* lnp, const sx_score_indels_out* out, const char* what)
-{
-    if (!b || !out) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL argument", what);
-    if (b->n_reads == 0) return SX_OK;
-    if (!lnp || !b->region_read_off || !b->region_key_off || !b->aln_off || !b->aln_pos || !b->aln_seg_off || !b->aln_key_off || !b->read_len || !b->non_ambig ||
-        !b->read_flags || !b->rec_off || !out->recs || !out->n_rec || !out->max_aln || !out->eval_aln)
-        return sx_fail(ctx, SX_ERR_ARG, "%s: NULL array", what);
-    if ((b->n_keys && !b->keys) || b->n_regions == 0) return sx_fail(ctx, SX_ERR_ARG, "%s: reads without a region / keys without a table", what);
-    if (b->opts.min_read_bp_flank < 0) return sx_fail(ctx, SX_ERR_ARG, "%s: negative min_read_bp_flank", what);
-    return SX_OK;
-}
-} // namespace
 
 extern "C" void sx_default_score_indels_opts(sx_score_indels_opts* o)
 {
@@ -217,12 +219,7 @@ extern "C" int sx_score_indels_dev(sx_ctx* ctx, const sx_score_indels_batch* d, 
     int rc;
     if ((rc = k6_check_args(ctx, d, lnp_dev, out_dev, "sx_score_indels_dev"))) return rc;
     if (d->n_reads == 0) return SX_OK;
-    SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    sx_kernel_timer t(ctx);
-    unsigned launches(0);
-    if ((rc = k6_run(ctx, d, lnp_dev, out_dev, &launches))) return rc;
-    t.stop(launches);
-    if ((rc = t.finish())) return rc;
+    if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k6_run(ctx, d, lnp_dev, out_dev, launches); }))) return rc;
     return sx_check_status(ctx, "sx_score_indels");
 }
 
@@ -268,21 +265,11 @@ extern "C" int sx_score_indels(sx_ctx* ctx, const sx_score_indels_batch* b, cons
     if ((rc = sx_take(ctx, sx_host_slot(19), n, o.eval_aln, 0))) return rc;
     SX_CUDA(ctx, cudaMemsetAsync(o.recs, 0, (n_slots + 1) * sizeof(sx_read_indel_score), ctx->s_compute)); // unused slots read back as zeros
     unsigned launches(0);
-    if ((rc = k6_run(ctx, &d, d_lnp, &o, &launches))) return rc;
+    if ((rc = sx_k6_run(ctx, &d, d_lnp, &o, &launches))) return rc;
     if ((rc = sx_download(ctx, out_host->recs, o.recs, n_slots))) return rc;
     if ((rc = sx_download(ctx, out_host->n_rec, o.n_rec, n))) return rc;
     if ((rc = sx_download(ctx, out_host->max_aln, o.max_aln, n))) return rc;
     if ((rc = sx_download(ctx, out_host->eval_aln, o.eval_aln, n))) return rc;
     if ((rc = t.finish(launches))) return rc;
     return sx_check_status(ctx, "sx_score_indels");
-}
-
-// launcher for the device-resident pipeline (sx_pipeline.cu): one 8-byte round trip sizes the scratch, the kernel itself is only enqueued
-int sx_k6_run(sx_ctx* ctx, const sx_score_indels_batch* d, const double* lnp_dev, const sx_score_indels_out* out_dev, unsigned* launches)
-{
-    if (d->n_reads == 0) return SX_OK;
-    unsigned l(0);
-    const int rc(k6_run(ctx, d, lnp_dev, out_dev, &l));
-    *launches += l;
-    return rc;
 }

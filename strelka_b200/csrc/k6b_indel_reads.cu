@@ -354,19 +354,21 @@ extern "C" int sx_link_indel_reads_dev(sx_ctx* ctx, const sx_indel_reads_sample*
     const char* what("sx_link_indel_reads_dev");
     int rc;
     if ((rc = k6b_check(ctx, what, normal, tumor, loci)) || (rc = k6b_check_out(ctx, what, out_dev))) return rc;
-    SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    sx_kernel_timer t(ctx);
-    unsigned launches(0);
     sx_indel_reads_out o(*out_dev);
-    rc = sx_k6b_run(ctx, what, normal, tumor, loci, &o, totals_host, false, &launches);
-    t.stop(launches);
-    const int rc2(t.finish());
-    if (rc == SX_ERR_CAPACITY || rc == SX_OK)
+    bool ran(false);
+    int rc_link(SX_OK);
+    rc = sx_run_timed(ctx, [&](unsigned* launches) {
+        ran = true;
+        rc_link = sx_k6b_run(ctx, what, normal, tumor, loci, &o, totals_host, false, launches);
+        return SX_OK; // (the timer finishes whatever the link returns: its totals stand even when a capacity is too small)
+    });
+    if (!ran) return rc; // (the device could not be set)
+    if (rc_link == SX_ERR_CAPACITY || rc_link == SX_OK)
     {
         const int rc3(sx_check_status(ctx, what, SX_ST_K6B_ID)); // (a bad id outranks the capacity it may have inflated)
         if (rc3) return rc3;
     }
-    return rc ? rc : rc2;
+    return rc_link ? rc_link : rc;
 }
 
 extern "C" int sx_link_indel_reads(sx_ctx* ctx, const sx_indel_reads_sample* normal, const sx_indel_reads_sample* tumor, const sx_indel_loci* loci,
@@ -440,15 +442,15 @@ extern "C" int sx_somatic_indel_from_records_dev(sx_ctx* ctx, const sx_sindel_op
     if ((rc = sx_take(ctx, SX_SLOT_K6B_OUT_READ_OFF, 2 * n_loci + 1, o.read_off, 16))) return rc;
     if ((rc = sx_take(ctx, SX_SLOT_K6B_OUT_STATUS, n_loci, o.status, 16))) return rc;
     if ((rc = sx_take(ctx, SX_SLOT_K6B_OUT_TOTALS, 2, o.totals, 16))) return rc;
-    sx_kernel_timer t(ctx);
-    unsigned launches(0);
-    if ((rc = sx_k6b_run(ctx, what, normal, tumor, loci, &o, nullptr, true, &launches))) return rc;
-    t.stop(launches);
-    if ((rc = t.finish())) return rc;
+    if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k6b_run(ctx, what, normal, tumor, loci, &o, nullptr, true, launches); }))) return rc;
     if ((rc = sx_check_status(ctx, what, SX_ST_K6B_ID))) return rc;
+    // K5b on the link's output: its checks and status word are reported as sx_somatic_indel_dev's, its time and launches added to the link's
     const sx_timing link(ctx->timing);
+    ctx->timing = sx_timing{};
     const sx_sindel_batch b = {loci->n_loci, 0, loci->key, loci->is_forced_output, loci->err_idx, o.alt_off, o.alts, o.read_off, o.reads};
-    if ((rc = sx_somatic_indel_dev(ctx, opts, &b, err_prob_host, n_err, out_dev))) return rc;
+    if ((rc = sx_k5b_check(ctx, "sx_somatic_indel_dev", opts, &b, err_prob_host, n_err, out_dev))) return rc;
+    if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k5b_run(ctx, opts, &b, err_prob_host, n_err, out_dev, launches); }))) return rc;
+    if ((rc = sx_check_status(ctx, "sx_somatic_indel_dev", SX_ST_SINDEL_ARG))) return rc;
     k6b_flag_results_kernel<<<std::max(1, std::min<int>((int)((n_loci + 255) / 256), ctx->sm_count * 16)), 256, 0, ctx->s_compute>>>(loci->n_loci, o.status, out_dev);
     SX_CUDA(ctx, cudaGetLastError());
     SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));

@@ -349,7 +349,7 @@ int k7_offsets(sx_ctx* ctx, const uint32_t n, const sx_enum_out* o, const k7_cou
     return sx_scan(ctx, SX_SLOT_K7_SUMS, J, launches);
 }
 
-int k7_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsigned* launches)
+int k7_plan_two_pass(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsigned* launches)
 {
     cudaStream_t st(ctx->s_compute);
     const uint32_t n(d->n_reads);
@@ -375,7 +375,7 @@ int k7_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsigned* 
     v.b = *d;
     k7_count_kernel<<<(unsigned)blocks, K7_THREADS, 0, st>>>(v, arena, per_thread, maxA, maxF, read_region, o->status, c);
     SX_CUDA(ctx, cudaGetLastError());
-    *launches = 2; // (with the frame count)
+    *launches += 2; // (with the frame count)
     if ((rc = k7_offsets(ctx, n, o, c, launches))) return rc;
     k7_write_kernel<<<(unsigned)blocks, K7_THREADS, 0, st>>>(v, arena, per_thread, maxA, maxF, read_region, o->status, c, *o, ctx->d_status);
     SX_CUDA(ctx, cudaGetLastError());
@@ -383,7 +383,7 @@ int k7_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsigned* 
     return SX_OK;
 }
 
-int k7_run_fast(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsigned* launches)
+int k7_plan_fast(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsigned* launches)
 {
     cudaStream_t st(ctx->s_compute);
     const uint32_t n(d->n_reads);
@@ -472,7 +472,7 @@ int k7_run_fast(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsig
         k7_search_arena_kernel<<<(unsigned)blocks, K7_THREADS, 0, st>>>(v, arena, per_thread, maxA, maxF, read_region, o->status, R, 2, 0, c, L);
         SX_CUDA(ctx, cudaGetLastError());
     }
-    *launches = (two_levels ? 4 : 3) + extra; // (with the frame count)
+    *launches += (two_levels ? 4 : 3) + extra; // (with the frame count)
     if ((rc = k7_offsets(ctx, n, o, c, launches))) return rc;
     const int g1(std::max(1, std::min<int>((int)((n + 127) / 128), ctx->sm_count * 16)));
     k7_gather_kernel<<<g1, 128, 0, st>>>(n, c, L, *o, ctx->d_status, nullptr, nullptr); // (every read, in read order: walking the active list instead, in read or class order, was slower)
@@ -499,6 +499,12 @@ int k7_check_args(sx_ctx* ctx, const sx_enum_batch* b, const sx_enum_out* o, con
 }
 
 } // namespace
+
+// K7's launcher: the batch's options pick the launch plan
+int sx_k7_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsigned* launches)
+{
+    return (d->opts.flags & SX_ENUM_F_FAST) ? k7_plan_fast(ctx, d, o, launches) : k7_plan_two_pass(ctx, d, o, launches);
+}
 
 int sx_k7_active_reads(sx_ctx* ctx, const uint32_t n_reads, const uint8_t* gate, uint32_t* list, uint32_t* count)
 {
@@ -535,19 +541,15 @@ extern "C" int sx_enumerate_alignments_dev(sx_ctx* ctx, const sx_enum_batch* d, 
     ctx->timing = sx_timing{};
     int rc;
     if ((rc = k7_check_args(ctx, d, out_dev, "sx_enumerate_alignments_dev"))) return rc;
-    SX_CUDA(ctx, cudaSetDevice(ctx->device));
     if (d->n_reads == 0)
     {
+        SX_CUDA(ctx, cudaSetDevice(ctx->device));
         SX_CUDA(ctx, cudaMemsetAsync(out_dev->totals, 0, 12, ctx->s_compute));
         SX_CUDA(ctx, cudaMemsetAsync(out_dev->aln_off, 0, 4, ctx->s_compute));
         SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
         return SX_OK;
     }
-    sx_kernel_timer t(ctx);
-    unsigned launches(0);
-    if ((rc = (d->opts.flags & SX_ENUM_F_FAST) ? k7_run_fast(ctx, d, out_dev, &launches) : k7_run(ctx, d, out_dev, &launches))) return rc;
-    t.stop(launches);
-    if ((rc = t.finish())) return rc;
+    if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k7_run(ctx, d, out_dev, launches); }))) return rc;
     return sx_check_status(ctx, "sx_enumerate_alignments", SX_ST_K7_CAP);
 }
 
@@ -602,7 +604,7 @@ extern "C" int sx_enumerate_alignments(sx_ctx* ctx, const sx_enum_batch* b, sx_e
     if ((rc = sx_take(ctx, sx_host_slot(24), o.cap_alns, o.aln_lead_key, 16))) return rc;
     if ((rc = sx_take(ctx, sx_host_slot(25), o.cap_alns, o.aln_trail_key, 16))) return rc;
     unsigned launches(0);
-    if ((rc = (d.opts.flags & SX_ENUM_F_FAST) ? k7_run_fast(ctx, &d, &o, &launches) : k7_run(ctx, &d, &o, &launches))) return rc;
+    if ((rc = sx_k7_run(ctx, &d, &o, &launches))) return rc;
     // the totals decide how much comes back
     if ((rc = sx_download(ctx, out_host->totals, o.totals, 3))) return rc;
     if ((rc = sx_download(ctx, out_host->aln_off, o.aln_off, n + 1))) return rc;
@@ -621,13 +623,4 @@ extern "C" int sx_enumerate_alignments(sx_ctx* ctx, const sx_enum_batch* b, sx_e
     }
     if ((rc = t.finish(launches))) return rc;
     return sx_check_status(ctx, "sx_enumerate_alignments", SX_ST_K7_CAP, out_host->totals);
-}
-
-// asynchronous launcher for the device-resident pipeline (sx_pipeline.cu)
-int sx_k7_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsigned* launches)
-{
-    unsigned l(0);
-    const int rc((d->opts.flags & SX_ENUM_F_FAST) ? k7_run_fast(ctx, d, o, &l) : k7_run(ctx, d, o, &l));
-    *launches += l;
-    return rc;
 }

@@ -96,9 +96,19 @@ __global__ void k7g_gates_kernel(const sx_gate_batch b, const sx_gate_out o, uin
     }
     (void)read_region;
 }
+} // namespace
 
-int k7a_run(sx_ctx* ctx, const k7a_view& v, const sx_prep_out* o, unsigned* launches)
+// K7a's launcher
+int sx_k7a_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_region* regions, const uint8_t* seq4, const char* ref, const uint32_t* key_ins_off, const char* key_ins,
+               const sx_prep_out* o, unsigned* launches)
 {
+    k7a_view v;
+    v.b = *d;
+    v.regions = regions;
+    v.seq4 = seq4;
+    v.ref = ref;
+    v.key_ins_off = key_ins_off;
+    v.key_ins = key_ins;
     cudaStream_t st(ctx->s_compute);
     const uint32_t n(v.b.n_reads);
     int rc;
@@ -127,7 +137,7 @@ int k7a_run(sx_ctx* ctx, const k7a_view& v, const sx_prep_out* o, unsigned* laun
     }
     k7a_count_kernel<<<grid(n), 128, 0, st>>>(v, read_byte, read_region, list, n_list, stage, *o);
     SX_CUDA(ctx, cudaGetLastError());
-    *launches = 2 + extra;
+    *launches += 2 + extra;
     const sx_scan_set J = {1, {{o->in_key_off, n, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, o->totals}}};
     if ((rc = sx_scan(ctx, SX_SLOT_K7A_K9_SUMS, J, launches))) return rc;
     k7a_write_kernel<<<grid(n), 128, 0, st>>>(v, read_byte, read_region, list, n_list, stage, *o, ctx->d_status);
@@ -136,6 +146,19 @@ int k7a_run(sx_ctx* ctx, const k7a_view& v, const sx_prep_out* o, unsigned* laun
     return SX_OK;
 }
 
+// K7g's launcher
+int sx_k7g_run(sx_ctx* ctx, const sx_gate_batch* d, const sx_gate_out* o, unsigned* launches)
+{
+    if (d->n_reads == 0) return SX_OK;
+    const unsigned grid((unsigned)std::max(1, std::min<int>((int)((d->n_reads + 127) / 128), ctx->sm_count * 16)));
+    k7g_gates_kernel<<<grid, 128, 0, ctx->s_compute>>>(*d, *o, nullptr);
+    SX_CUDA(ctx, cudaGetLastError());
+    *launches += 1;
+    return SX_OK;
+}
+
+namespace
+{
 int k7a_check_args(sx_ctx* ctx, const sx_enum_batch* b, const sx_region* regions, const uint8_t* seq4, const char* ref, const uint32_t* key_ins_off, const char* key_ins,
                    const sx_prep_out* o, const char* what)
 {
@@ -148,10 +171,7 @@ int k7a_check_args(sx_ctx* ctx, const sx_enum_batch* b, const sx_region* regions
     if (b->n_regions == 0) return sx_fail(ctx, SX_ERR_ARG, "%s: reads without a region", what);
     return SX_OK;
 }
-} // namespace
 
-namespace
-{
 int k7g_check_args(sx_ctx* ctx, const sx_gate_batch* b, const sx_gate_out* o, const char* what)
 {
     if (!b || !o) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL argument", what);
@@ -171,13 +191,7 @@ extern "C" int sx_realign_gates_dev(sx_ctx* ctx, const sx_gate_batch* d, sx_gate
     int rc;
     if ((rc = k7g_check_args(ctx, d, out_dev, "sx_realign_gates_dev"))) return rc;
     if (d->n_reads == 0) return SX_OK;
-    SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    sx_kernel_timer t(ctx);
-    const unsigned grid((unsigned)std::max(1, std::min<int>((int)((d->n_reads + 127) / 128), ctx->sm_count * 16)));
-    k7g_gates_kernel<<<grid, 128, 0, ctx->s_compute>>>(*d, *out_dev, nullptr);
-    SX_CUDA(ctx, cudaGetLastError());
-    t.stop(1);
-    if ((rc = t.finish())) return rc;
+    if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k7g_run(ctx, d, out_dev, launches); }))) return rc;
     return sx_check_status(ctx, "sx_realign_gates");
 }
 
@@ -206,13 +220,12 @@ extern "C" int sx_realign_gates(sx_ctx* ctx, const sx_gate_batch* b, sx_gate_out
     if ((rc = sx_take(ctx, sx_host_slot(10), n, o.gate, 16))) return rc;
     if ((rc = sx_take(ctx, sx_host_slot(11), n, o.in_pos, 16))) return rc;
     if ((rc = sx_take(ctx, sx_host_slot(12), n_segs, o.in_segs, 16))) return rc;
-    const unsigned grid((unsigned)std::max(1, std::min<int>((int)((b->n_reads + 127) / 128), ctx->sm_count * 16)));
-    k7g_gates_kernel<<<grid, 128, 0, ctx->s_compute>>>(d, o, nullptr);
-    SX_CUDA(ctx, cudaGetLastError());
+    unsigned launches(0);
+    if ((rc = sx_k7g_run(ctx, &d, &o, &launches))) return rc;
     if ((rc = sx_download(ctx, out_host->gate, o.gate, n))) return rc;
     if ((rc = sx_download(ctx, out_host->in_pos, o.in_pos, n))) return rc;
     if ((rc = sx_download(ctx, out_host->in_segs, o.in_segs, n_segs))) return rc;
-    if ((rc = t.finish(1))) return rc;
+    if ((rc = t.finish(launches))) return rc;
     return sx_check_status(ctx, "sx_realign_gates");
 }
 
@@ -223,26 +236,15 @@ extern "C" int sx_alignment_indels_dev(sx_ctx* ctx, const sx_enum_batch* d, cons
     ctx->timing = sx_timing{};
     int rc;
     if ((rc = k7a_check_args(ctx, d, regions, seq4, ref, key_ins_off, key_ins, out_dev, "sx_alignment_indels_dev"))) return rc;
-    SX_CUDA(ctx, cudaSetDevice(ctx->device));
     if (d->n_reads == 0)
     {
+        SX_CUDA(ctx, cudaSetDevice(ctx->device));
         SX_CUDA(ctx, cudaMemsetAsync(out_dev->totals, 0, 4, ctx->s_compute));
         SX_CUDA(ctx, cudaMemsetAsync(out_dev->in_key_off, 0, 4, ctx->s_compute));
         SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
         return SX_OK;
     }
-    k7a_view v;
-    v.b = *d;
-    v.regions = regions;
-    v.seq4 = seq4;
-    v.ref = ref;
-    v.key_ins_off = key_ins_off;
-    v.key_ins = key_ins;
-    sx_kernel_timer t(ctx);
-    unsigned launches(0);
-    if ((rc = k7a_run(ctx, v, out_dev, &launches))) return rc;
-    t.stop(launches);
-    if ((rc = t.finish())) return rc;
+    if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k7a_run(ctx, d, regions, seq4, ref, key_ins_off, key_ins, out_dev, launches); }))) return rc;
     return sx_check_status(ctx, "sx_alignment_indels", SX_ST_K7A_CAP);
 }
 
@@ -261,23 +263,26 @@ extern "C" int sx_alignment_indels(sx_ctx* ctx, const sx_enum_batch* b, const sx
     }
     SX_CUDA(ctx, cudaSetDevice(ctx->device));
     sx_call_timer t(ctx);
-    k7a_view v;
-    v.b = *b;
+    sx_enum_batch d(*b);
+    const sx_region* d_regions(nullptr);
+    const uint8_t* d_seq4(nullptr);
+    const char *d_ref(nullptr), *d_key_ins(nullptr);
+    const uint32_t* d_key_ins_off(nullptr);
     const size_t n(b->n_reads), nr(b->n_regions), n_segs(b->in_seg_off[b->n_reads]);
     const sx_region& end(regions[b->n_regions]); // the sentinel carries the pool sizes
-    if ((rc = sx_upload(ctx, sx_host_slot(0), b->region_read_off, nr + 1, v.b.region_read_off, 16))) return rc;
-    if ((rc = sx_upload(ctx, sx_host_slot(1), b->region_key_off, nr + 1, v.b.region_key_off, 16))) return rc;
-    if ((rc = sx_upload(ctx, sx_host_slot(2), b->keys, b->n_keys, v.b.keys, 16))) return rc;
-    if ((rc = sx_upload(ctx, sx_host_slot(3), b->in_pos, n, v.b.in_pos, 16))) return rc;
-    if ((rc = sx_upload(ctx, sx_host_slot(4), b->in_seg_off, n + 1, v.b.in_seg_off, 16))) return rc;
-    if ((rc = sx_upload(ctx, sx_host_slot(5), b->in_segs, n_segs, v.b.in_segs, 16))) return rc;
-    if ((rc = sx_upload(ctx, sx_host_slot(6), b->read_len, n, v.b.read_len, 16))) return rc;
-    if (b->gate && (rc = sx_upload(ctx, sx_host_slot(17), b->gate, n, v.b.gate, 16))) return rc;
-    if ((rc = sx_upload(ctx, sx_host_slot(7), regions, nr + 1, v.regions, 16))) return rc;
-    if ((rc = sx_upload(ctx, sx_host_slot(8), seq4, (size_t)end.seq_off + SX_POOL_SLACK, v.seq4, 16))) return rc;
-    if ((rc = sx_upload(ctx, sx_host_slot(9), ref, (size_t)end.ref_off + SX_POOL_SLACK, v.ref, 16))) return rc;
-    if ((rc = sx_upload(ctx, sx_host_slot(10), key_ins_off, b->n_keys ? (size_t)b->n_keys + 1 : 0, v.key_ins_off, 16))) return rc;
-    if ((rc = sx_upload(ctx, sx_host_slot(11), key_ins, b->n_keys ? key_ins_off[b->n_keys] : 0, v.key_ins, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(0), b->region_read_off, nr + 1, d.region_read_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(1), b->region_key_off, nr + 1, d.region_key_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(2), b->keys, b->n_keys, d.keys, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(3), b->in_pos, n, d.in_pos, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(4), b->in_seg_off, n + 1, d.in_seg_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(5), b->in_segs, n_segs, d.in_segs, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(6), b->read_len, n, d.read_len, 16))) return rc;
+    if (b->gate && (rc = sx_upload(ctx, sx_host_slot(17), b->gate, n, d.gate, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(7), regions, nr + 1, d_regions, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(8), seq4, (size_t)end.seq_off + SX_POOL_SLACK, d_seq4, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(9), ref, (size_t)end.ref_off + SX_POOL_SLACK, d_ref, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(10), key_ins_off, b->n_keys ? (size_t)b->n_keys + 1 : 0, d_key_ins_off, 16))) return rc;
+    if ((rc = sx_upload(ctx, sx_host_slot(11), key_ins, b->n_keys ? key_ins_off[b->n_keys] : 0, d_key_ins, 16))) return rc;
     sx_prep_out o(*out_host);
     if ((rc = sx_take(ctx, sx_host_slot(12), 4, o.totals, 0))) return rc;
     if ((rc = sx_take(ctx, sx_host_slot(13), n + 1, o.in_key_off, 16))) return rc;
@@ -285,7 +290,7 @@ extern "C" int sx_alignment_indels(sx_ctx* ctx, const sx_enum_batch* b, const sx
     if ((rc = sx_take(ctx, sx_host_slot(15), n, o.in_lead_key, 16))) return rc;
     if ((rc = sx_take(ctx, sx_host_slot(16), n, o.in_trail_key, 16))) return rc;
     unsigned launches(0);
-    if ((rc = k7a_run(ctx, v, &o, &launches))) return rc;
+    if ((rc = sx_k7a_run(ctx, &d, d_regions, d_seq4, d_ref, d_key_ins_off, d_key_ins, &o, &launches))) return rc;
     if ((rc = sx_download(ctx, out_host->totals, o.totals, 1))) return rc;
     if ((rc = sx_download(ctx, out_host->in_key_off, o.in_key_off, n + 1))) return rc;
     if ((rc = sx_download(ctx, out_host->in_lead_key, o.in_lead_key, n))) return rc;
@@ -294,31 +299,4 @@ extern "C" int sx_alignment_indels(sx_ctx* ctx, const sx_enum_batch* b, const sx
     if (out_host->totals[0] <= o.cap_keys && (rc = sx_download(ctx, out_host->in_keys, o.in_keys, out_host->totals[0]))) return rc;
     if ((rc = t.finish(launches))) return rc;
     return sx_check_status(ctx, "sx_alignment_indels", SX_ST_K7A_CAP, out_host->totals);
-}
-
-// ---- asynchronous launchers for the device-resident pipeline (sx_pipeline.cu): everything is enqueued on ctx->s_compute, nothing waits
-int sx_k7g_run(sx_ctx* ctx, const sx_gate_batch* d, const sx_gate_out* o, unsigned* launches)
-{
-    if (d->n_reads == 0) return SX_OK;
-    const unsigned grid((unsigned)std::max(1, std::min<int>((int)((d->n_reads + 127) / 128), ctx->sm_count * 16)));
-    k7g_gates_kernel<<<grid, 128, 0, ctx->s_compute>>>(*d, *o, nullptr);
-    SX_CUDA(ctx, cudaGetLastError());
-    *launches += 1;
-    return SX_OK;
-}
-
-int sx_k7a_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_region* regions, const uint8_t* seq4, const char* ref, const uint32_t* key_ins_off, const char* key_ins,
-               const sx_prep_out* o, unsigned* launches)
-{
-    k7a_view v;
-    v.b = *d;
-    v.regions = regions;
-    v.seq4 = seq4;
-    v.ref = ref;
-    v.key_ins_off = key_ins_off;
-    v.key_ins = key_ins;
-    unsigned l(0);
-    const int rc(k7a_run(ctx, v, o, &l));
-    *launches += l;
-    return rc;
 }

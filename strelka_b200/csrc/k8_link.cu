@@ -145,9 +145,11 @@ __global__ void k8_pad_kernel(const k8_view v, const uint32_t n_alns, const uint
     if (fits && blockIdx.x == 0 && threadIdx.x == 0) // K1 loads 16-byte slices: up to 16 no-op segments of slack after the last one, where they fit
         for (uint32_t s = totals[0]; s < o.cap_segs && s < totals[0] + 16u; ++s) o.segs[s] = sx_aln_seg{0, SX_SEG_HARDCLIP, 0};
 }
+} // namespace
 
-int k8_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* e, const uint32_t n_alns, const uint32_t* key_ins_off, const char* key_ins, const sx_link_out* o,
-           unsigned* launches)
+// K7b's launcher
+int sx_k8_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* e, const uint32_t n_alns, const uint32_t* key_ins_off, const char* key_ins, const sx_link_out* o,
+              unsigned* launches)
 {
     cudaStream_t st(ctx->s_compute);
     int rc;
@@ -174,7 +176,7 @@ int k8_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* e, const uint
     SX_CUDA(ctx, cudaGetLastError());
     k8_region_kernel<<<grid((uint32_t)std::min<uint64_t>((uint64_t)nr * 32u, 0xffffff00u)), 128, 0, st>>>(v, seg_n, ins_n, reg_seg, reg_ins);
     SX_CUDA(ctx, cudaGetLastError());
-    *launches = 4;
+    *launches += 4;
     const sx_scan_set J = {2, {{reg_seg, nr, SX_SCAN_EXCLUSIVE, o->totals}, {reg_ins, nr, SX_SCAN_EXCLUSIVE, o->totals + 1}}};
     if ((rc = sx_scan(ctx, SX_SLOT_K8_SUMS, J, launches))) return rc;
     k8_write_kernel<<<grid(n_alns), 128, 0, st>>>(v, n_alns, aln_read, read_region, seg_n, ins_n, reg_seg, reg_ins, *o);
@@ -185,6 +187,8 @@ int k8_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* e, const uint
     return SX_OK;
 }
 
+namespace
+{
 int k8_check_args(sx_ctx* ctx, const sx_enum_batch* b, const sx_enum_out* e, const uint32_t* key_ins_off, const char* key_ins, const sx_link_out* o, const char* what)
 {
     if (!b || !e || !o) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL argument", what);
@@ -204,12 +208,7 @@ extern "C" int sx_link_alignments_dev(sx_ctx* ctx, const sx_enum_batch* d, const
     ctx->timing = sx_timing{};
     int rc;
     if ((rc = k8_check_args(ctx, d, e, key_ins_off, key_ins, out_dev, "sx_link_alignments_dev"))) return rc;
-    SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    sx_kernel_timer t(ctx);
-    unsigned launches(0);
-    if ((rc = k8_run(ctx, d, e, n_alns, key_ins_off, key_ins, out_dev, &launches))) return rc;
-    t.stop(launches);
-    if ((rc = t.finish())) return rc;
+    if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k8_run(ctx, d, e, n_alns, key_ins_off, key_ins, out_dev, launches); }))) return rc;
     return sx_check_status(ctx, "sx_link_alignments", SX_ST_K8_NO_KEY | SX_ST_K8_KIND | SX_ST_K8_CAP);
 }
 
@@ -249,7 +248,7 @@ extern "C" int sx_link_alignments(sx_ctx* ctx, const sx_enum_batch* b, const sx_
     if ((rc = sx_take(ctx, sx_host_slot(17), o.cap_ins, o.ins, SX_POOL_SLACK + 16))) return rc;
     if (out_host->k6_segs && (rc = sx_take(ctx, sx_host_slot(18), n_segs, o.k6_segs, 16))) return rc;
     unsigned launches(0);
-    if ((rc = k8_run(ctx, &d, &de, n_alns, d_key_ins_off, d_key_ins, &o, &launches))) return rc;
+    if ((rc = sx_k8_run(ctx, &d, &de, n_alns, d_key_ins_off, d_key_ins, &o, &launches))) return rc;
     if ((rc = sx_download(ctx, out_host->totals, o.totals, 2))) return rc;
     if ((rc = sx_download(ctx, out_host->regions, o.regions, nr + 1))) return rc;
     SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
@@ -263,14 +262,4 @@ extern "C" int sx_link_alignments(sx_ctx* ctx, const sx_enum_batch* b, const sx_
     }
     if ((rc = t.finish(launches))) return rc;
     return sx_check_status(ctx, "sx_link_alignments", SX_ST_K8_NO_KEY | SX_ST_K8_KIND | SX_ST_K8_CAP, out_host->totals);
-}
-
-// asynchronous launcher for the device-resident pipeline (sx_pipeline.cu)
-int sx_k8_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* e, uint32_t n_alns, const uint32_t* key_ins_off, const char* key_ins, const sx_link_out* o,
-              unsigned* launches)
-{
-    unsigned l(0);
-    const int rc(k8_run(ctx, d, e, n_alns, key_ins_off, key_ins, o, &l));
-    *launches += l;
-    return rc;
 }

@@ -49,9 +49,12 @@ __global__ void __launch_bounds__(128) k9_choose_kernel(const k9_view v, const u
         o.best_aln[r] = best;
     }
 }
+} // namespace
 
-int k9_run(sx_ctx* ctx, const sx_realign_batch* d, const double* lnp, const sx_realign_out* o, unsigned* launches)
+// K9's launcher
+int sx_k9_run(sx_ctx* ctx, const sx_realign_batch* d, const double* lnp, const sx_realign_out* o, unsigned* launches)
 {
+    if (d->n_reads == 0) return SX_OK;
     cudaStream_t st(ctx->s_compute);
     const uint32_t n(d->n_reads);
     int rc;
@@ -61,7 +64,7 @@ int k9_run(sx_ctx* ctx, const sx_realign_batch* d, const double* lnp, const sx_r
     const auto grid = [cap](const uint32_t m) { return (unsigned)std::max(1, std::min<int>((int)((m + 127) / 128), cap)); };
     k9_slots_kernel<<<grid(std::max(n, d->n_regions)), 128, 0, st>>>(*d, o->seg_off, read_region);
     SX_CUDA(ctx, cudaGetLastError());
-    *launches = 1;
+    *launches += 1;
     const sx_scan_set J = {1, {{o->seg_off, n, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, o->totals}}};
     if ((rc = sx_scan(ctx, SX_SLOT_K7A_K9_SUMS, J, launches))) return rc;
     k9_view v;
@@ -73,6 +76,8 @@ int k9_run(sx_ctx* ctx, const sx_realign_batch* d, const double* lnp, const sx_r
     return SX_OK;
 }
 
+namespace
+{
 int k9_check_args(sx_ctx* ctx, const sx_realign_batch* b, const double* lnp, const sx_realign_out* o, const char* what)
 {
     if (!b || !o) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL argument", what);
@@ -92,19 +97,15 @@ extern "C" int sx_choose_realignment_dev(sx_ctx* ctx, const sx_realign_batch* d,
     ctx->timing = sx_timing{};
     int rc;
     if ((rc = k9_check_args(ctx, d, lnp_dev, out_dev, "sx_choose_realignment_dev"))) return rc;
-    SX_CUDA(ctx, cudaSetDevice(ctx->device));
     if (d->n_reads == 0)
     {
+        SX_CUDA(ctx, cudaSetDevice(ctx->device));
         SX_CUDA(ctx, cudaMemsetAsync(out_dev->totals, 0, 4, ctx->s_compute));
         SX_CUDA(ctx, cudaMemsetAsync(out_dev->seg_off, 0, 4, ctx->s_compute));
         SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
         return SX_OK;
     }
-    sx_kernel_timer t(ctx);
-    unsigned launches(0);
-    if ((rc = k9_run(ctx, d, lnp_dev, out_dev, &launches))) return rc;
-    t.stop(launches);
-    if ((rc = t.finish())) return rc;
+    if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k9_run(ctx, d, lnp_dev, out_dev, launches); }))) return rc;
     return sx_check_status(ctx, "sx_choose_realignment", SX_ST_K9_CAP);
 }
 
@@ -147,7 +148,7 @@ extern "C" int sx_choose_realignment(sx_ctx* ctx, const sx_realign_batch* b, con
     if ((rc = sx_take(ctx, sx_host_slot(17), n, o.best_aln, 16))) return rc;
     if ((rc = sx_take(ctx, sx_host_slot(18), o.cap_segs, o.segs, 16))) return rc;
     unsigned launches(0);
-    if ((rc = k9_run(ctx, &d, d_lnp, &o, &launches))) return rc;
+    if ((rc = sx_k9_run(ctx, &d, d_lnp, &o, &launches))) return rc;
     if ((rc = sx_download(ctx, out_host->totals, o.totals, 1))) return rc;
     if ((rc = sx_download(ctx, out_host->seg_off, o.seg_off, n + 1))) return rc;
     SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
@@ -161,14 +162,4 @@ extern "C" int sx_choose_realignment(sx_ctx* ctx, const sx_realign_batch* b, con
     }
     if ((rc = t.finish(launches))) return rc;
     return sx_check_status(ctx, "sx_choose_realignment", SX_ST_K9_CAP, out_host->totals);
-}
-
-// asynchronous launcher for the device-resident pipeline (sx_pipeline.cu)
-int sx_k9_run(sx_ctx* ctx, const sx_realign_batch* d, const double* lnp, const sx_realign_out* o, unsigned* launches)
-{
-    if (d->n_reads == 0) return SX_OK;
-    unsigned l(0);
-    const int rc(k9_run(ctx, d, lnp, o, &l));
-    *launches += l;
-    return rc;
 }

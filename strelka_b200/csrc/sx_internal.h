@@ -279,29 +279,26 @@ int sx_scan(sx_ctx* ctx, sx_slot sums_slot, const sx_scan_set& job, unsigned* la
 // own) are tested before the others.  `totals`, when the caller has them, are the stage's totals the capacity messages quote.
 int sx_check_status(sx_ctx* ctx, const char* what, int first = 0, const uint32_t* totals = nullptr);
 
-// timing helpers: record kernel time on the compute stream
-struct sx_kernel_timer
+// The body of a *_dev entry point: on the context's device, `run(unsigned* launches)` enqueues a stage through its launcher, between two
+// events on the compute stream.  Once the stream has passed the second, the time between them and the launches are added to ctx->timing and
+// ctx->total_launches.  An error from `run` is returned at once, with nothing added.
+template <typename F> int sx_run_timed(sx_ctx* ctx, F&& run)
 {
-    sx_ctx* ctx;
-    explicit sx_kernel_timer(sx_ctx* c) : ctx(c) { cudaEventRecord(c->ev_a, c->s_compute); }
-    void stop(unsigned launches)
-    {
-        cudaEventRecord(ctx->ev_b, ctx->s_compute);
-        pending = launches;
-    }
-    int finish()
-    {
-        cudaError_t e = cudaEventSynchronize(ctx->ev_b);
-        if (e != cudaSuccess) return sx_fail(ctx, SX_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
-        float ms = 0;
-        cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b);
-        ctx->timing.kernel_ms += ms;
-        ctx->timing.launches += pending;
-        ctx->total_launches += pending;
-        return SX_OK;
-    }
-    unsigned pending = 0;
-};
+    SX_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaEventRecord(ctx->ev_a, ctx->s_compute);
+    unsigned launches = 0;
+    const int rc = run(&launches);
+    if (rc) return rc;
+    cudaEventRecord(ctx->ev_b, ctx->s_compute);
+    const cudaError_t e = cudaEventSynchronize(ctx->ev_b);
+    if (e != cudaSuccess) return sx_fail(ctx, SX_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
+    float ms = 0;
+    cudaEventElapsedTime(&ms, ctx->ev_a, ctx->ev_b);
+    ctx->timing.kernel_ms += ms;
+    ctx->timing.launches += launches;
+    ctx->total_launches += launches;
+    return SX_OK;
+}
 
 // the host-array counterpart: the whole call on the compute stream, ev_a before the uploads and ev_b after the downloads
 struct sx_call_timer
@@ -328,7 +325,23 @@ int sx_k1_launch(sx_ctx* ctx, const sx_align_batch* dev, uint32_t region_begin, 
                  cudaStream_t st);
 size_t sx_k1_region_smem(const sx_region* r0, const sx_region* r1, const sx_aln* alns);
 
-// asynchronous stage launchers of the device-resident pipeline (sx_pipeline.cu); each lives beside its kernels
+// The stage launchers, each beside its kernels and the only code that launches them.  A launcher enqueues its stage on ctx->s_compute
+// (device pointers in and out) and adds the stage's launches to *launches; it does no timing, reads no status word and leaves the device
+// as the caller set it.  The *_dev entries run them under sx_run_timed, the host-array entries after their uploads (K1's and K2a's
+// through sx_k1_launch and germline_run, as their batches are measured on the host), and sx_process_window_dev one after another.
+int sx_k1_run(sx_ctx* ctx, const sx_align_batch* d, double* lnp_dev, unsigned* launches);
+int sx_k1_read_max_run(sx_ctx* ctx, const sx_align_batch* d, const double* lnp_dev, double* max_lnp_dev, uint32_t* max_aln_dev, unsigned* launches);
+int sx_k2a_run(sx_ctx* ctx, const sx_pileup_batch* d, int is_always_test, sx_digt_result* out_dev, unsigned* launches);
+int sx_k2b_run(sx_ctx* ctx, const sx_pileup_batch* n, const sx_pileup_batch* t, const uint8_t* forced_dev, sx_ssnv_result* out_dev, unsigned* launches);
+int sx_k3_run(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* d, sx_ga_result* res_dev, uint32_t* cigar_dev, unsigned* launches);
+int sx_k4_run(sx_ctx* ctx, const sx_pileup_reads_batch* d, const sx_pileup_columns* out, unsigned* launches);
+int sx_k5_run(sx_ctx* ctx, const sx_indel_batch* d, sx_indel_result* out_dev, unsigned* launches);
+int sx_k5b_run(sx_ctx* ctx, const sx_sindel_opts* o, const sx_sindel_batch* d, const double* err_prob, uint32_t n_err, sx_sindel_result* out_dev, unsigned* launches);
+// K5b's argument checks, reported under `what` (the K5b entries, and sx_somatic_indel_from_records_dev before its K5b run)
+int sx_k5b_check(sx_ctx* ctx, const char* what, const sx_sindel_opts* o, const sx_sindel_batch* b, const double* err_prob, uint32_t n_err, const void* out);
+int sx_k6_run(sx_ctx* ctx, const sx_score_indels_batch* d, const double* lnp_dev, const sx_score_indels_out* out_dev, unsigned* launches);
+int sx_k6b_run(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* normal, const sx_indel_reads_sample* tumor, const sx_indel_loci* loci, sx_indel_reads_out* out_dev,
+               uint32_t* totals_host, bool own_out, unsigned* launches);
 int sx_k7g_run(sx_ctx* ctx, const sx_gate_batch* d, const sx_gate_out* o, unsigned* launches);
 int sx_k7a_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_region* regions, const uint8_t* seq4, const char* ref, const uint32_t* key_ins_off, const char* key_ins,
                const sx_prep_out* o, unsigned* launches);
@@ -337,10 +350,4 @@ int sx_k7_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsigne
 int sx_k7_active_reads(sx_ctx* ctx, uint32_t n_reads, const uint8_t* gate, uint32_t* list, uint32_t* count);
 int sx_k8_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* e, uint32_t n_alns, const uint32_t* key_ins_off, const char* key_ins, const sx_link_out* o,
               unsigned* launches);
-int sx_k1_run_dev(sx_ctx* ctx, const sx_align_batch* d, double* lnp_dev, unsigned* launches);
-int sx_k6_run(sx_ctx* ctx, const sx_score_indels_batch* d, const double* lnp_dev, const sx_score_indels_out* out_dev, unsigned* launches);
-int sx_k6b_run(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* normal, const sx_indel_reads_sample* tumor, const sx_indel_loci* loci, sx_indel_reads_out* out_dev,
-               uint32_t* totals_host, bool own_out, unsigned* launches);
 int sx_k9_run(sx_ctx* ctx, const sx_realign_batch* d, const double* lnp, const sx_realign_out* o, unsigned* launches);
-int sx_k4_run(sx_ctx* ctx, const sx_pileup_reads_batch* d, const sx_pileup_columns* out, unsigned* launches);
-int sx_k2a_run(sx_ctx* ctx, const sx_pileup_batch* d, int is_always_test, sx_digt_result* out_dev, unsigned* launches);

@@ -220,7 +220,10 @@ extern "C" int sx_last_window_timing(const sx_ctx* ctx, float* ms)
     return SX_OK;
 }
 
-extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint32_t* totals_host)
+namespace
+{
+// the window pass of sx_process_window_dev, which sx_process_window runs on the window it has uploaded
+int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint32_t* totals_host)
 {
     if (!ctx) return SX_ERR_ARG;
     ctx->timing = sx_timing{};
@@ -442,7 +445,7 @@ extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_w
         ab.ins_bytes = link_totals[1];
         ab.qual_bits = b->qual_bits == 4 ? 4u : 8u;
         memcpy(ab.qual_dict, b->qual_dict, 16);
-        if ((rc = sx_k1_run_dev(ctx, &ab, lnp, &launches))) return rc;
+        if ((rc = sx_k1_run(ctx, &ab, lnp, &launches))) return rc;
     }
     // ---------------------------------------------------------------------------------------------------------------- K6 score_indels
     SX_CUDA(ctx, mark(SX_WIN_ST_SCORE_INDELS));
@@ -645,6 +648,12 @@ extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_w
         return sx_fail(ctx, SX_ERR_CAPACITY, "sx_process_window_dev: %u variant sites, cap_variant_sites is %u", totals[8], out->cap_variant_sites);
     return sx_check_status(ctx, "sx_process_window");
 }
+} // namespace
+
+extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint32_t* totals_host)
+{
+    return window_pass(ctx, b, out, totals_host);
+}
 
 // ---------------------------------------------------------------------------------------------------------------------------------------
 // host arrays in, host arrays out
@@ -720,7 +729,7 @@ extern "C" int sx_process_window(sx_ctx* ctx, const sx_window_batch* b, sx_windo
     o.cap_variant_sites = out->cap_variant_sites;
     uint32_t totals[SX_WIN_TOTALS];
     memset(totals, 0, sizeof(totals));
-    rc = sx_process_window_dev(ctx, &d, &o, totals);
+    rc = window_pass(ctx, &d, &o, totals);
     if (totals_host) memcpy(totals_host, totals, sizeof(totals));
     if (rc) return rc;
     const float kernel_ms(ctx->timing.kernel_ms);

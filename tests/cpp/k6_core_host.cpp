@@ -7,7 +7,7 @@
 #include <vector>
 
 // list_walk == 0: the plain body, region by region, read by read.
-// list_walk != 0: what k6_run and k6_score_list_kernel do -- the host memsets of n_rec / max_aln / eval_aln for every read, then
+// list_walk != 0: what sx_k6_run and k6_score_list_kernel do -- the host memsets of n_rec / max_aln / eval_aln for every read, then
 // the body on the dense list of reads that have alignments, walked backwards (the kernel's regrouping makes the order arbitrary), each
 // read with its region from k6_region_of and the scratch k6_score_read_tiered picks.  counts[0] = reads skipped (no alignment),
 // counts[1 + tier] = listed reads per k6_scratch_tier.
@@ -55,7 +55,7 @@ extern "C" int k6core_run(const sx_score_indels_batch* b, const double* lnp, sx_
     }
     else
     {
-        std::fill(n_rec, n_rec + b->n_reads, 0u); // k6_run's memsets
+        std::fill(n_rec, n_rec + b->n_reads, 0u); // sx_k6_run's memsets
         std::fill(max_aln, max_aln + b->n_reads, 0xFFFFFFFFu);
         std::fill(eval_aln, eval_aln + b->n_reads, 0xFFFFFFFFu);
         std::vector<uint32_t> list; // k6_max_kernel's list

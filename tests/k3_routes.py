@@ -6,7 +6,7 @@ Each DP problem of a batch goes down one of these paths, picked from its shape a
                    shared-memory strip dp_shared_strip, T >= 5                        Q > 128
   status 2         no result: k3_slot_bytes(Q, R) exceeds the opt-in shared memory per block, or Q == 0 or R == 0 (device entry)
 and the warp kernel's launch runs 4, 2 or 1 warps per CTA, whichever is the most that fit the batch's largest slot.
-(k3_group.cu: kg_bucket, sx_k3_group_run; k3_global_align.cu: k3_run, k3_global_align_kernel; k3_common.cuh: k3_slot_bytes.)
+(k3_group.cu: kg_bucket, sx_k3_group_launch; k3_global_align.cu: sx_k3_run, k3_global_align_kernel; k3_common.cuh: k3_slot_bytes.)
 test_k3_routes.py checks the constants below against those sources, so a routing change cannot leave this mirror behind.
 """
 from __future__ import annotations

@@ -180,7 +180,7 @@ def test_k6_device_body_and_list_walk_on_the_host(tmp_path):
     for case in range(60):
         for extra, (sb, lnp) in enumerate((specgen.score_indels_case(case), _k6_list_case(case))):
             want = reflib.ox_score_indels(sb, lnp)
-            # 0: the plain per-read body; 1: what the list kernel does (k6_run's memsets, then the listed reads in reverse order, each
+            # 0: the plain per-read body; 1: what the list kernel does (sx_k6_run's memsets, then the listed reads in reverse order, each
             # with its region from k6_region_of and the scratch tier the kernel picks)
             for list_walk in (0, 1):
                 out = B.ScoreIndelsOut(sb)
