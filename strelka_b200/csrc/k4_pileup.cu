@@ -21,7 +21,9 @@
 //      reads can touch.  A column holds, in this order, the calls of window c-1's reads (forward spill), of window c's own reads and of
 //      window c+1's reads (back spill): all reads of an earlier window precede all reads of a later one.  So the cursors start at
 //      site_off[s] + spill[s] for the window's own sites, at site_off[s] for the next window's sites and at site_off[s+1] - back[s]
-//      for the previous window's.
+//      for the previous window's.  A read waits on one global round trip: the records (32 per load) and the next read's path are
+//      loaded a read ahead, the path's offsets are warp scans, the bases, qualities and reference are staged by one batch of loads,
+//      and the candidate-SNV look-ups search the window's slice of cand_snv, staged in shared memory (pass 1 sizes it).
 // Everything is integer/byte work; the only table is qphred_cache::mappedq, built on the host (sx_context.cu).
 #include "sx_internal.h"
 
@@ -34,6 +36,8 @@ constexpr int K4_WARPS = 4;
 constexpr uint32_t K4_MAX_W = 2048;    // window size limit (shared memory: 16 bytes per window site and warp)
 constexpr uint32_t K4_MAX_READ = 1024; // read length limit (delta + mismatch arrays)
 constexpr uint32_t K4_MAX_SEGS = 64;   // path segments per read
+constexpr uint32_t K4_STAGE = 6;       // elements of each staged array a lane loads per pass (one pass for reads of up to 192 bases)
+constexpr uint32_t K4_MAX_CAND = 512;  // cand_snv keys a warp holds in shared memory (a window with more searches them in place)
 constexpr unsigned FULL = 0xffffffffu;
 
 struct k4_args
@@ -52,6 +56,7 @@ struct k4_args
     int32_t origin; // position of window 0's first site (= report_begin - W)
     uint32_t W, n_windows, n_sites;
     uint32_t Lcap; // read-length capacity of the per-warp arrays (the batch's longest read, rounded up)
+    uint32_t Ccap; // capacity of the per-warp cand_snv slice (fill pass only)
     sx_pileup_opts opt;
 };
 
@@ -121,17 +126,51 @@ template <typename CodeFn> __device__ __forceinline__ bool read_preamble(const k
     return true;
 }
 
+// the cand_snv keys ((site << 2) | base id) of the sites a window's reads can reach: sites [(c-2) W, (c+1) W), cut to [0, 2^30 - 1)
+// (a key outside the range is searched in the whole array)
+__device__ __forceinline__ void cand_key_range(const k4_args& A, uint32_t c, uint32_t& key_lo, uint32_t& key_hi)
+{
+    const int64_t s0 = (static_cast<int64_t>(c) - 2) * A.W, s1 = s0 + 3 * static_cast<int64_t>(A.W), top = (1 << 30) - 1;
+    key_lo = static_cast<uint32_t>(i64min(i64max(s0, 0), top)) << 2;
+    key_hi = static_cast<uint32_t>(i64min(i64max(s1, 0), top)) << 2;
+}
+
+__device__ __forceinline__ uint32_t lower_bound_key(const uint32_t* keys, uint32_t n, uint32_t key)
+{
+    uint32_t lo = 0, hi = n;
+    while (lo < hi)
+    {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (keys[mid] < key) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
-// pass 1: column sizes as difference arrays
+// pass 1: column sizes as difference arrays, and the largest cand_snv slice of any window (max_cand), by which the fill sizes its
+// shared-memory copy of the slices
 // ---------------------------------------------------------------------------------------------------------------------
 __global__ void k4_count_kernel(k4_args A, int* __restrict__ d1, int* __restrict__ d2, int* __restrict__ s1, int* __restrict__ s2, int* __restrict__ b1,
-                                int* __restrict__ b2, int* __restrict__ dsd, int* __restrict__ dsm, int* __restrict__ status)
+                                int* __restrict__ b2, int* __restrict__ dsd, int* __restrict__ dsm, uint32_t* __restrict__ max_cand, int* __restrict__ status)
 {
     const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= A.n_reads) return;
     const sx_pileup_read rd = A.reads[r];
     const int32_t bp = bpos_of(A, r);
-    if (r > 0 && bpos_of(A, r - 1) > bp) atomicOr(status, SX_ST_READ_ORDER);
+    const int32_t bp_prev = r > 0 ? bpos_of(A, r - 1) : INT32_MIN;
+    if (bp_prev > bp) atomicOr(status, SX_ST_READ_ORDER);
+    if (A.n_cand_snv && bp >= A.origin) // the first read of a window measures the window's slice
+    {
+        const uint32_t c = static_cast<uint32_t>((static_cast<int64_t>(bp) - A.origin) / A.W);
+        if (c < A.n_windows && bp_prev < static_cast<int64_t>(A.origin) + static_cast<int64_t>(c) * A.W)
+        {
+            uint32_t key_lo, key_hi;
+            cand_key_range(A, c, key_lo, key_hi);
+            const uint32_t n = lower_bound_key(A.cand_snv, A.n_cand_snv, key_hi) - lower_bound_key(A.cand_snv, A.n_cand_snv, key_lo);
+            if (n) atomicMax(max_cand, n);
+        }
+    }
     if (rd.flags & SX_PRF_SKIP) return;
     const sx_aln_seg* path = A.segs + rd.seg_off;
     const uint32_t as = A.reads[r + 1].seg_off - rd.seg_off;
@@ -210,23 +249,12 @@ __global__ void k4_count_kernel(k4_args A, int* __restrict__ d1, int* __restrict
 // ---------------------------------------------------------------------------------------------------------------------
 // pass 3: one warp per window, reads in order
 // ---------------------------------------------------------------------------------------------------------------------
-__host__ __device__ inline uint32_t k4_warp_smem(uint32_t W, uint32_t Lcap)
+__host__ __device__ inline uint32_t k4_warp_smem(uint32_t W, uint32_t Lcap, uint32_t Ccap)
 {
     // run1[3W], run2[3W] (uint32), delta[Lcap + 4] (int), mism[Lcap] (uint8), segment table 3 x K4_MAX_SEGS uint32, and the staged
-    // read: packed bases [Lcap/2 + 16], qualities [Lcap], reference bases under the alignment [W + 16], mappedq row [80]; Lcap % 16 == 0
-    return 2u * 3u * W * 4u + (Lcap + 4u) * 4u + Lcap + 3u * K4_MAX_SEGS * 4u + (Lcap / 2u + 16u) + Lcap + (W + 16u) + 80u;
-}
-
-__device__ __forceinline__ uint32_t lower_bound_pos(const k4_args& A, int64_t pos)
-{
-    uint32_t lo = 0, hi = A.n_reads;
-    while (lo < hi)
-    {
-        const uint32_t mid = (lo + hi) >> 1;
-        if (bpos_of(A, mid) < pos) lo = mid + 1;
-        else hi = mid;
-    }
-    return lo;
+    // read: packed bases [Lcap/2 + 16], qualities [Lcap], reference bases under the alignment [W + 16], mappedq row [80]; Lcap % 16 == 0;
+    // then the window's cand_snv slice [Ccap] (uint32, 4-aligned: W % 32 == 0)
+    return 2u * 3u * W * 4u + (Lcap + 4u) * 4u + Lcap + 3u * K4_MAX_SEGS * 4u + (Lcap / 2u + 16u) + Lcap + (W + 16u) + 80u + Ccap * 4u;
 }
 
 __global__ void __launch_bounds__(K4_WARPS * 32) k4_fill_kernel(k4_args A, const uint32_t* __restrict__ site_off, const uint32_t* __restrict__ t2_off,
@@ -238,7 +266,7 @@ __global__ void __launch_bounds__(K4_WARPS * 32) k4_fill_kernel(k4_args A, const
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t c = blockIdx.x * K4_WARPS + warp;
     if (c >= A.n_windows) return;
-    unsigned char* wsm = smem + (size_t)warp * k4_warp_smem(A.W, A.Lcap);
+    unsigned char* wsm = smem + (size_t)warp * k4_warp_smem(A.W, A.Lcap, A.Ccap);
     uint32_t* run1 = reinterpret_cast<uint32_t*>(wsm);
     uint32_t* run2 = run1 + 3 * A.W;
     int* delta = reinterpret_cast<int*>(run2 + 3 * A.W);
@@ -250,19 +278,35 @@ __global__ void __launch_bounds__(K4_WARPS * 32) k4_fill_kernel(k4_args A, const
     uint8_t* ql = seq + (A.Lcap / 2u + 16u);
     char* refb = reinterpret_cast<char*>(ql + A.Lcap);                  // refb[i] = reference base at rd.pos + i ('N' outside the segment)
     uint8_t* mqrow = reinterpret_cast<uint8_t*>(refb + (A.W + 16u));    // mappedq[adjustedMapq][*]
+    uint32_t* cand_sm = reinterpret_cast<uint32_t*>(mqrow + 80u);       // the window's cand_snv slice
     uint32_t mqrow_of = 0xffffffffu;
 
     const int64_t win_pos0 = static_cast<int64_t>(A.origin) + static_cast<int64_t>(c) * A.W;
     const int64_t site0 = win_pos0 - A.W - A.report_begin; // site index of local index 0: the first site of window c-1 (may be negative)
-    uint32_t lo = 0, hi = 0;
-    if (lane == 0)
+    // four binary searches side by side, one per lane: the window's reads [lo, hi) and its cand_snv slice [cand_lo, cand_hi)
+    uint32_t lo = 0, hi = 0, cand_lo = 0, cand_hi = 0;
     {
-        lo = lower_bound_pos(A, win_pos0);
-        hi = lower_bound_pos(A, win_pos0 + A.W);
+        uint32_t key_lo, key_hi;
+        cand_key_range(A, c, key_lo, key_hi);
+        uint32_t l = 0, h = lane < 2 ? A.n_reads : (lane < 4 ? A.n_cand_snv : 0u);
+        const int64_t key = lane == 0 ? win_pos0 : lane == 1 ? win_pos0 + A.W : lane == 2 ? key_lo : key_hi;
+        while (l < h)
+        {
+            const uint32_t mid = (l + h) >> 1;
+            const int64_t v = lane < 2 ? static_cast<int64_t>(bpos_of(A, mid)) : static_cast<int64_t>(A.cand_snv[mid]);
+            if (v < key) l = mid + 1;
+            else h = mid;
+        }
+        lo = __shfl_sync(FULL, l, 0);
+        hi = __shfl_sync(FULL, l, 1);
+        cand_lo = __shfl_sync(FULL, l, 2);
+        cand_hi = __shfl_sync(FULL, l, 3);
     }
-    lo = __shfl_sync(FULL, lo, 0);
-    hi = __shfl_sync(FULL, hi, 0);
     if (lo == hi) return;
+    // the slice is searched in shared memory where it fits the capacity the largest slice of the batch set, in place otherwise
+    const uint32_t n_cand = cand_hi - cand_lo;
+    if (n_cand <= A.Ccap)
+        for (uint32_t i = lane; i < n_cand; i += 32) cand_sm[i] = A.cand_snv[cand_lo + i];
     // write cursor of every site this window's reads can reach: the start of its column + (own sites only) the calls of window c-1's
     // reads, which all precede this window's reads
     for (uint32_t li = lane; li < 3 * A.W; li += 32)
@@ -293,63 +337,150 @@ __global__ void __launch_bounds__(K4_WARPS * 32) k4_fill_kernel(k4_args A, const
     }
     __syncwarp();
     const bool isDensity = A.opt.mismatchDensityFilterFlankSize > 0;
+    // the quality of read base p: ql holds the qualities as stored; dictionary-coded ones are two 4-bit codes a byte
+    unsigned long long qd_lo, qd_hi;
+    memcpy(&qd_lo, A.qual_dict, 8);
+    memcpy(&qd_hi, A.qual_dict + 8, 8);
+    const auto qual_at = [&](uint32_t p) -> uint32_t {
+        if (A.qual_bits != 4) return ql[p];
+        const uint32_t code = (ql[p >> 1] >> ((~p & 1u) << 2)) & 15u;
+        return static_cast<uint32_t>((code < 8u ? qd_lo : qd_hi) >> (8u * (code & 7u))) & 0xffu;
+    };
     const uint32_t fs = A.opt.mismatchDensityFilterFlankSize, fs2 = fs * 2;
+
+    // The read records, one per lane, 32 reads at a time (rec: the five words of reads[base + lane], rec_end: the next read's seg_off),
+    // and the path of the next read, one segment word per lane: both are loaded one read ahead, so their latency overlaps the current
+    // read's base passes and a read waits on one round trip, the staging of its bases.
+    constexpr uint32_t REC_WORDS = sizeof(sx_pileup_read) / 4;
+    static_assert(sizeof(sx_pileup_read) == 20 && sizeof(sx_aln_seg) == 4, "record layouts");
+    const uint32_t* segw = reinterpret_cast<const uint32_t*>(A.segs); // len | kind << 16 | flags << 24
+    uint32_t base = lo, rec[REC_WORDS], rec_end = 0;
+    auto load_records = [&](uint32_t b) {
+        base = b;
+        if (b + lane < hi)
+        {
+            const uint32_t* g = reinterpret_cast<const uint32_t*>(A.reads + b + lane);
+#pragma unroll
+            for (uint32_t k = 0; k < REC_WORDS; ++k) rec[k] = g[k];
+            rec_end = A.reads[b + lane + 1].seg_off;
+        }
+    };
+    uint32_t nseg0 = 0, nseg1 = 0; // segments lane and lane + 32 of the next read's path
+    auto load_path = [&](uint32_t r) {
+        const uint32_t so = __shfl_sync(FULL, rec[2], r - base), as = __shfl_sync(FULL, rec_end, r - base) - so;
+        nseg0 = lane < as && as <= K4_MAX_SEGS ? segw[so + lane] : 0u;
+        nseg1 = lane + 32 < as && as <= K4_MAX_SEGS ? segw[so + lane + 32] : 0u;
+    };
+    load_records(lo);
+    load_path(lo);
 
     for (uint32_t r = lo; r < hi; ++r)
     {
-        const sx_pileup_read rd = A.reads[r];
-        if (!(rd.flags & SX_PRF_TIER1OR2) || (rd.flags & SX_PRF_SKIP)) continue; // sub-mapped reads only count (pass 1)
-        const uint32_t as = A.reads[r + 1].seg_off - rd.seg_off;
-        if (rd.len > A.Lcap || as > K4_MAX_SEGS) continue; // flagged by pass 1
-        const sx_aln_seg* path = A.segs + rd.seg_off;
-        const uint32_t read_size = rd.len;
-        // segment table (lane 0; paths are a handful of segments)
-        uint32_t ref_span = 0, first = as, last = as;
-        if (lane == 0)
+        sx_pileup_read rd;
         {
-            uint32_t rh = 0, fh = 0;
-            for (uint32_t i = 0; i < as; ++i)
-            {
-                const uint32_t k = path[i].kind, len = path[i].len;
-                seg_kl[i] = (k << 16) | len;
-                seg_rd[i] = rh;
-                seg_rf[i] = fh;
-                if (k == SX_SEG_MATCH)
-                {
-                    if (first == as) first = i;
-                    last = i;
-                }
-                if (kind_read(k)) rh += len;
-                if (kind_ref(k)) fh += len;
-            }
-            ref_span = fh;
+            const uint32_t j = r - base, w4 = __shfl_sync(FULL, rec[4], j);
+            rd.seq_off = __shfl_sync(FULL, rec[0], j);
+            rd.qual_off = __shfl_sync(FULL, rec[1], j);
+            rd.seg_off = __shfl_sync(FULL, rec[2], j);
+            rd.pos = static_cast<int32_t>(__shfl_sync(FULL, rec[3], j));
+            rd.len = static_cast<uint16_t>(w4);
+            rd.mapq = static_cast<uint8_t>(w4 >> 16);
+            rd.flags = static_cast<uint8_t>(w4 >> 24);
         }
-        ref_span = __shfl_sync(FULL, ref_span, 0);
-        first = __shfl_sync(FULL, first, 0);
-        last = __shfl_sync(FULL, last, 0);
+        const uint32_t as = __shfl_sync(FULL, rec_end, r - base) - rd.seg_off;
+        const uint32_t seg0 = nseg0, seg1 = nseg1;
+        if (r + 1 < hi)
+        {
+            if (r + 1 - base == 32) load_records(r + 1);
+            load_path(r + 1);
+        }
+        if (!(rd.flags & SX_PRF_TIER1OR2) || (rd.flags & SX_PRF_SKIP)) continue; // sub-mapped reads only count (pass 1)
+        if (rd.len > A.Lcap || as > K4_MAX_SEGS) continue; // flagged by pass 1
+        const uint32_t read_size = rd.len;
+        // segment table: lane i holds segments i and i + 32; their read and reference offsets are warp scans of the lengths
+        uint32_t ref_span, first, last;
+        {
+            const uint32_t k0 = (seg0 >> 16) & 0xffu, len0 = seg0 & 0xffffu, k1 = (seg1 >> 16) & 0xffu, len1 = seg1 & 0xffffu;
+            const bool v0 = lane < as, v1 = lane + 32 < as;
+            uint32_t rd0 = v0 && kind_read(k0) ? len0 : 0u, rf0 = v0 && kind_ref(k0) ? len0 : 0u;
+            uint32_t rd1 = v1 && kind_read(k1) ? len1 : 0u, rf1 = v1 && kind_ref(k1) ? len1 : 0u;
+            const uint32_t own_rd0 = rd0, own_rf0 = rf0, own_rd1 = rd1, own_rf1 = rf1;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1)
+            {
+                const uint32_t a = __shfl_up_sync(FULL, rd0, d), b = __shfl_up_sync(FULL, rf0, d);
+                const uint32_t e = __shfl_up_sync(FULL, rd1, d), f = __shfl_up_sync(FULL, rf1, d);
+                if (lane >= (uint32_t)d)
+                {
+                    rd0 += a;
+                    rf0 += b;
+                    rd1 += e;
+                    rf1 += f;
+                }
+            }
+            const uint32_t rd_half = __shfl_sync(FULL, rd0, 31), rf_half = __shfl_sync(FULL, rf0, 31);
+            if (v0)
+            {
+                seg_kl[lane] = (k0 << 16) | len0;
+                seg_rd[lane] = rd0 - own_rd0;
+                seg_rf[lane] = rf0 - own_rf0;
+            }
+            if (v1)
+            {
+                seg_kl[lane + 32] = (k1 << 16) | len1;
+                seg_rd[lane + 32] = rd_half + rd1 - own_rd1;
+                seg_rf[lane + 32] = rf_half + rf1 - own_rf1;
+            }
+            ref_span = rf_half + __shfl_sync(FULL, rf1, 31);
+            const uint32_t m0 = __ballot_sync(FULL, v0 && k0 == SX_SEG_MATCH), m1 = __ballot_sync(FULL, v1 && k1 == SX_SEG_MATCH);
+            first = m0 ? __ffs(m0) - 1 : m1 ? 32 + __ffs(m1) - 1 : as;
+            last = m1 ? 63 - __clz(m1) : m0 ? 31 - __clz(m0) : as;
+        }
         __syncwarp();
         if (ref_span > A.W) continue; // flagged by pass 1
         if (rd.pos >= A.report_end || static_cast<int64_t>(rd.pos) + ref_span <= A.report_begin) continue; // (the preamble's range test, before staging)
         const uint32_t adjustedMapq = max(5u, (uint32_t)rd.mapq);
         {
-            // stage the read: every later access is shared memory
+            // stage the read: every later access is shared memory.  Each pass issues all of a lane's loads -- K4_STAGE elements of the
+            // packed bases, the qualities as stored (packed ones are decoded where they are read) and the reference, and the mappedq row
+            // when the mapping quality changes -- before its first store: one round trip for a read and span of up to 32 K4_STAGE.
             const uint8_t* gs = A.seq4 + rd.seq_off;
             const uint8_t* gq = A.qual + rd.qual_off;
-            for (uint32_t i = lane; i < (read_size + 1) / 2; i += 32) seq[i] = gs[i];
-            if (A.qual_bits == 4)
-                for (uint32_t i = lane; i < read_size; i += 32) ql[i] = A.qual_dict[(gq[i >> 1] >> ((~i & 1u) << 2)) & 15u];
-            else
-                for (uint32_t i = lane; i < read_size; i += 32) ql[i] = gq[i];
-            for (uint32_t i = lane; i < ref_span; i += 32)
+            const uint32_t n_seq = (read_size + 1) / 2, n_ql = A.qual_bits == 4 ? n_seq : read_size, n_all = max(max(n_seq, n_ql), ref_span);
+            // the span's offsets that fall inside the reference: [ref_lo, ref_hi); 'N' elsewhere
+            const int64_t ref0 = static_cast<int64_t>(rd.pos) - A.ref_begin;
+            const uint32_t ref_lo = static_cast<uint32_t>(i64min(i64max(-ref0, 0), ref_span));
+            const uint32_t ref_hi = static_cast<uint32_t>(i64min(i64max(static_cast<int64_t>(A.ref_len) - ref0, 0), ref_span));
+            const char* gr = A.ref + ref0;
+            const bool new_mq = mqrow_of != adjustedMapq;
+            const uint8_t* gmq = tables->mappedq[min(adjustedMapq, 90u)];
+            for (uint32_t b = 0; b < n_all; b += 32 * K4_STAGE)
             {
-                const int64_t ri = static_cast<int64_t>(rd.pos) + i - A.ref_begin;
-                refb[i] = (ri >= 0 && ri < static_cast<int64_t>(A.ref_len)) ? A.ref[ri] : 'N';
+                uint32_t vs[K4_STAGE], vq[K4_STAGE], vr[K4_STAGE], vm[3];
+#pragma unroll
+                for (uint32_t k = 0; k < K4_STAGE; ++k)
+                {
+                    const uint32_t i = b + lane + 32 * k;
+                    vs[k] = i < n_seq ? gs[i] : 0u;
+                    vq[k] = i < n_ql ? gq[i] : 0u;
+                    vr[k] = i >= ref_lo && i < ref_hi ? static_cast<uint8_t>(gr[i]) : static_cast<uint32_t>('N');
+                }
+#pragma unroll
+                for (uint32_t k = 0; k < 3; ++k) vm[k] = b == 0 && new_mq && lane + 32 * k <= SX_MAX_QSCORE ? gmq[lane + 32 * k] : 0u;
+                __syncwarp(); // (keeps every load of the pass ahead of the first store that waits on one)
+#pragma unroll
+                for (uint32_t k = 0; k < K4_STAGE; ++k)
+                {
+                    const uint32_t i = b + lane + 32 * k;
+                    if (i < n_seq) seq[i] = static_cast<uint8_t>(vs[k]);
+                    if (i < n_ql) ql[i] = static_cast<uint8_t>(vq[k]);
+                    if (i < ref_span) refb[i] = static_cast<char>(vr[k]);
+                }
+#pragma unroll
+                for (uint32_t k = 0; k < 3; ++k)
+                    if (b == 0 && new_mq && lane + 32 * k <= SX_MAX_QSCORE) mqrow[lane + 32 * k] = static_cast<uint8_t>(vm[k]);
             }
-            if (mqrow_of != adjustedMapq)
-            {
-                for (uint32_t i = lane; i <= SX_MAX_QSCORE; i += 32) mqrow[i] = tables->mappedq[min(adjustedMapq, 90u)][i];
-                mqrow_of = adjustedMapq;
-            }
+            mqrow_of = adjustedMapq;
         }
         __syncwarp();
         read_window w;
@@ -399,14 +530,13 @@ __global__ void __launch_bounds__(K4_WARPS * 32) k4_fill_kernel(k4_args A, const
                 if (id < 4 && rel >= 0 && rel < (1 << 30))
                 {
                     const uint32_t key = (static_cast<uint32_t>(rel) << 2) | static_cast<uint32_t>(id);
-                    uint32_t l2 = 0, h2 = A.n_cand_snv;
-                    while (l2 < h2)
-                    {
-                        const uint32_t mid = (l2 + h2) >> 1;
-                        if (A.cand_snv[mid] < key) l2 = mid + 1;
-                        else h2 = mid;
-                    }
-                    cand = l2 < A.n_cand_snv && A.cand_snv[l2] == key;
+                    uint32_t key_lo, key_hi; // (recomputed here, off the common path, rather than held in registers through the read loop)
+                    cand_key_range(A, c, key_lo, key_hi);
+                    const bool in_slice = key >= key_lo && key < key_hi;
+                    const uint32_t* keys = !in_slice ? A.cand_snv : n_cand <= A.Ccap ? cand_sm : A.cand_snv + cand_lo;
+                    const uint32_t n = in_slice ? n_cand : A.n_cand_snv;
+                    const uint32_t l2 = lower_bound_key(keys, n, key);
+                    cand = l2 < n && keys[l2] == key;
                 }
                 if (!cand)
                 {
@@ -452,7 +582,7 @@ __global__ void __launch_bounds__(K4_WARPS * 32) k4_fill_kernel(k4_args A, const
                 atomicOr(status, SX_ST_BASE);
                 continue;
             }
-            uint32_t qscore = ql[p];
+            uint32_t qscore = qual_at(p);
             if (is_mapq_adjust)
             {
                 if (qscore > SX_MAX_QSCORE)
@@ -501,8 +631,8 @@ extern "C" void sx_default_pileup_opts(sx_pileup_opts* o)
     o->reserved_ = 0;
 }
 
-// K4's launcher: enqueues the three passes (one 8-byte round trip between the scans and the fill checks the capacities) and returns without
-// waiting for the fill
+// K4's launcher: enqueues the three passes (one 12-byte round trip between the scans and the fill checks the capacities and sizes the
+// fill's cand_snv slices) and returns without waiting for the fill
 int sx_k4_run(sx_ctx* ctx, const sx_pileup_reads_batch* d, const sx_pileup_columns* out, unsigned* launches_out)
 {
     const uint32_t n_sites = static_cast<uint32_t>(d->report_end - d->report_begin);
@@ -533,6 +663,7 @@ int sx_k4_run(sx_ctx* ctx, const sx_pileup_reads_batch* d, const sx_pileup_colum
     A.origin = d->report_begin - static_cast<int32_t>(W);
     A.W = W;
     A.Lcap = Lcap;
+    A.Ccap = 0;
     // the windows cover every buffer position a read reaching the report range can have: its best alignment starts before report_end,
     // its buffer position is at most `shift` later
     A.n_windows = static_cast<uint32_t>((static_cast<int64_t>(d->report_end) + shift - A.origin + W - 1) / W);
@@ -556,10 +687,13 @@ int sx_k4_run(sx_ctx* ctx, const sx_pileup_reads_batch* d, const sx_pileup_colum
     SX_CUDA(ctx, cudaMemsetAsync(dsm, 0, (size_t)n_sites * 4, st));
     SX_CUDA(ctx, cudaMemsetAsync(s1, 0, (size_t)(n_sites + 1) * 8, st));
     SX_CUDA(ctx, cudaMemsetAsync(b1, 0, (size_t)(n_sites + 1) * 8, st));
+    uint32_t* max_cand_d = nullptr;
+    if ((rc = sx_take(ctx, SX_SLOT_K4_MAX_CAND, 1, max_cand_d, 64))) return rc;
+    SX_CUDA(ctx, cudaMemsetAsync(max_cand_d, 0, 4, st));
     unsigned launches = 0;
     if (d->n_reads)
     {
-        k4_count_kernel<<<(d->n_reads + 127) / 128, 128, 0, st>>>(A, d1, d2, s1, s2, b1, b2, dsd, dsm, ctx->d_status);
+        k4_count_kernel<<<(d->n_reads + 127) / 128, 128, 0, st>>>(A, d1, d2, s1, s2, b1, b2, dsd, dsm, max_cand_d, ctx->d_status);
         SX_CUDA(ctx, cudaGetLastError());
         ++launches;
     }
@@ -580,9 +714,10 @@ int sx_k4_run(sx_ctx* ctx, const sx_pileup_reads_batch* d, const sx_pileup_colum
         const sx_scan_set offsets = {2, {{u(d1), n + 1, SX_SCAN_EXCLUSIVE, nullptr}, {u(d2), n + 1, SX_SCAN_EXCLUSIVE, nullptr}}};
         if ((rc = sx_scan(ctx, SX_SLOT_K4_TILE_SUMS, offsets, &launches))) return rc;
     }
-    uint32_t totals[2] = {0, 0};
+    uint32_t totals[2] = {0, 0}, max_cand = 0;
     SX_CUDA(ctx, cudaMemcpyAsync(&totals[0], out->site_off + n_sites, 4, cudaMemcpyDeviceToHost, st));
     SX_CUDA(ctx, cudaMemcpyAsync(&totals[1], out->t2_off + n_sites, 4, cudaMemcpyDeviceToHost, st));
+    SX_CUDA(ctx, cudaMemcpyAsync(&max_cand, max_cand_d, 4, cudaMemcpyDeviceToHost, st));
     SX_CUDA(ctx, cudaStreamSynchronize(st));
     if (totals[0] > out->calls_capacity || totals[1] > out->t2_capacity)
         return sx_fail(ctx, SX_ERR_NOMEM, "sx_pileup_reads: the columns hold %u + %u calls, capacities are %llu + %llu", totals[0], totals[1],
@@ -590,7 +725,8 @@ int sx_k4_run(sx_ctx* ctx, const sx_pileup_reads_batch* d, const sx_pileup_colum
     // pass 3: one warp per window walks the window's reads in read-buffer order
     if (d->n_reads)
     {
-        const size_t smem = (size_t)k4_warp_smem(W, Lcap) * K4_WARPS;
+        A.Ccap = std::min(max_cand, K4_MAX_CAND);
+        const size_t smem = (size_t)k4_warp_smem(W, Lcap, A.Ccap) * K4_WARPS;
         if (smem > 48 * 1024) SX_CUDA(ctx, cudaFuncSetAttribute(k4_fill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(ctx->smem_optin)));
         k4_fill_kernel<<<(A.n_windows + K4_WARPS - 1) / K4_WARPS, K4_WARPS * 32, smem, st>>>(A, out->site_off, out->t2_off, s1, s2, b1, b2, out->calls, out->t2_calls, ctx->d_tables,
                                                                                          ctx->d_status);

@@ -94,7 +94,7 @@ enum sx_slot : int
     SX_SLOT_K1_SMEM_NEED = SX_SLOT_HOST_END,
     SX_SLOT_K2A_SCRATCH, SX_SLOT_K2A_MAX_SITE,
     SX_SLOT_K3_INFO, SX_SLOT_K3_CURSOR, SX_SLOT_K3_ORDER, SX_SLOT_K3_SCRATCH,
-    SX_SLOT_K4_SCAN_S, SX_SLOT_K4_SCAN_B, SX_SLOT_K4_TILE_SUMS,
+    SX_SLOT_K4_SCAN_S, SX_SLOT_K4_SCAN_B, SX_SLOT_K4_TILE_SUMS, SX_SLOT_K4_MAX_CAND,
     SX_SLOT_K6_MAX, SX_SLOT_K6_LIST, SX_SLOT_K6_ARENA, SX_SLOT_K6_CLASS, SX_SLOT_K6_HIST, SX_SLOT_K6_LIST_BY_CLASS,
     SX_SLOT_K6B_LOCUS_OF, SX_SLOT_K6B_PAIR_OFF, SX_SLOT_K6B_CURSOR, SX_SLOT_K6B_SUMS, SX_SLOT_K6B_ALT_IDS,
     SX_SLOT_K6B_PAIR_ID, SX_SLOT_K6B_PAIR_REC, SX_SLOT_K6B_PAIR_READ, SX_SLOT_K6B_PAIR_ORDER,
