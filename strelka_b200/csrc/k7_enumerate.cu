@@ -298,18 +298,100 @@ __global__ void __launch_bounds__(K7_THREADS) k7_search_arena_kernel(const k7_vi
     }
 }
 
-__global__ void k7_gather_kernel(const uint32_t n_reads, const k7_counts c, const k7_log L, const sx_enum_out o, int* __restrict__ d_status,
-                                 const uint32_t* __restrict__ list, const uint32_t* __restrict__ n_list)
+// One warp per read with alignments.  The blob is loaded into shared memory in one coalesced pass, lane 0 walks its record headers there, and
+// the lanes write every output array of the read (per alignment, then segments, then keys) at consecutive addresses: one thread walking its
+// own blob wrote every field to a different sector.  A read whose blob or alignment count exceeds the warp's share is written by lane 0 alone.
+constexpr int K7_GATHER_WARPS = 4;
+constexpr uint32_t K7_GATHER_WORDS = 1024; // blob words per warp
+constexpr uint32_t K7_GATHER_ALNS = 128;   // alignments per warp
+
+__global__ void __launch_bounds__(K7_GATHER_WARPS * 32) k7_gather_kernel(const uint32_t n_reads, const k7_counts c, const k7_log L, const sx_enum_out o,
+                                                                          int* __restrict__ d_status)
 {
+    __shared__ uint32_t s_blob[K7_GATHER_WARPS][K7_GATHER_WORDS];
+    __shared__ uint16_t s_at[K7_GATHER_WARPS][K7_GATHER_ALNS + 1], s_sp[K7_GATHER_WARPS][K7_GATHER_ALNS + 1], s_kp[K7_GATHER_WARPS][K7_GATHER_ALNS + 1];
     if (!k7_fits(o, d_status)) return;
-    // with a list (in read order: the CSR output is written in read order): only the searched reads have a blob
-    const uint32_t n_work(list ? *n_list : n_reads);
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_work; i += gridDim.x * blockDim.x)
+    const uint32_t lane(threadIdx.x & 31u), wi(threadIdx.x >> 5);
+    uint32_t* blob(s_blob[wi]);
+    uint16_t *at(s_at[wi]), *sp(s_sp[wi]), *kp(s_kp[wi]);
+    const uint32_t warps(gridDim.x * K7_GATHER_WARPS);
+    for (uint32_t base = (blockIdx.x * K7_GATHER_WARPS + wi) * 32u; base < n_reads; base += warps * 32u)
     {
-        const uint32_t r(list ? list[i] : i);
-        const uint32_t na(c.aln[r + 1] - c.aln[r]);
-        if (na == 0 || L.blob_off[r] == UINT32_MAX) continue;
-        k7_blob_gather(L.words + L.blob_off[r], na, o, c.aln[r], c.seg[r], c.key[r]);
+        // the warp's 32 reads: which of them have a blob
+        const uint32_t rl(base + lane);
+        const bool has(rl < n_reads && c.aln[rl + 1] != c.aln[rl] && L.blob_off[rl] != UINT32_MAX);
+        unsigned m(__ballot_sync(0xffffffffu, has));
+        while (m)
+        {
+            const uint32_t r(base + (uint32_t)__ffs(m) - 1u);
+            m &= m - 1u;
+            // (the segment and key offsets have n_reads entries: the last read ends at the totals)
+            const uint32_t a0(c.aln[r]), na(c.aln[r + 1] - a0), s0(c.seg[r]), k0(c.key[r]);
+            const uint32_t ns((r + 1 < n_reads ? c.seg[r + 1] : o.totals[1]) - s0), nk((r + 1 < n_reads ? c.key[r + 1] : o.totals[2]) - k0);
+            const uint32_t off(L.blob_off[r]);
+            const uint32_t* src(L.words + off);
+            const uint32_t bound(min(3u * na + ns + nk, L.cap - off)); // the blob's words: at most one per key
+            if (na > K7_GATHER_ALNS || bound > K7_GATHER_WORDS)
+            {
+                if (lane == 0) k7_blob_gather(src, na, o, a0, s0, k0);
+                continue;
+            }
+            for (uint32_t i = lane; i < bound; i += 32) blob[i] = src[i];
+            __syncwarp();
+            if (lane == 0)
+            {
+                uint32_t w(0), ps(0), pk(0);
+                for (uint32_t i = 0; i < na; ++i)
+                {
+                    at[i] = (uint16_t)w;
+                    sp[i] = (uint16_t)ps;
+                    kp[i] = (uint16_t)pk;
+                    const uint32_t h(blob[w + 2]);
+                    ps += h & 0xFFu;
+                    pk += h >> 8;
+                    w += 3u + (h & 0xFFu) + ((h >> 8) + 1u) / 2u;
+                }
+                sp[na] = (uint16_t)ps;
+                kp[na] = (uint16_t)pk;
+            }
+            __syncwarp();
+            for (uint32_t i = lane; i < na; i += 32)
+            {
+                const uint32_t* rec(blob + at[i]);
+                o.aln_pos[a0 + i] = (int32_t)rec[0];
+                o.aln_lead_key[a0 + i] = (uint16_t)(rec[1] & 0xFFFFu);
+                o.aln_trail_key[a0 + i] = (uint16_t)(rec[1] >> 16);
+                o.aln_seg_off[a0 + i] = s0 + sp[i];
+                o.aln_key_off[a0 + i] = k0 + kp[i];
+            }
+            // segment j / key j of the read belongs to the last alignment whose prefix is <= j
+            for (uint32_t j = lane; j < ns; j += 32)
+            {
+                uint32_t lo(0), hi(na - 1);
+                while (lo < hi)
+                {
+                    const uint32_t mid((lo + hi + 1) / 2);
+                    if (sp[mid] <= j) lo = mid;
+                    else hi = mid - 1;
+                }
+                const uint32_t w(blob[at[lo] + 3u + (j - sp[lo])]);
+                o.segs[s0 + j] = sx_aln_seg{(uint16_t)(w & 0xFFFFu), (uint8_t)((w >> 16) & 0xFFu), (uint8_t)(w >> 24)};
+            }
+            for (uint32_t j = lane; j < nk; j += 32)
+            {
+                uint32_t lo(0), hi(na - 1);
+                while (lo < hi)
+                {
+                    const uint32_t mid((lo + hi + 1) / 2);
+                    if (kp[mid] <= j) lo = mid;
+                    else hi = mid - 1;
+                }
+                const uint32_t q(j - kp[lo]);
+                const uint32_t w(blob[at[lo] + 3u + (blob[at[lo] + 2u] & 0xFFu) + q / 2u]);
+                o.aln_keys[k0 + j] = (uint16_t)((q & 1u) ? (w >> 16) : (w & 0xFFFFu));
+            }
+            __syncwarp();
+        }
     }
 }
 
@@ -474,8 +556,8 @@ int k7_plan_fast(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsi
     }
     *launches += (two_levels ? 4 : 3) + extra; // (with the frame count)
     if ((rc = k7_offsets(ctx, n, o, c, launches))) return rc;
-    const int g1(std::max(1, std::min<int>((int)((n + 127) / 128), ctx->sm_count * 16)));
-    k7_gather_kernel<<<g1, 128, 0, st>>>(n, c, L, *o, ctx->d_status, nullptr, nullptr); // (every read, in read order: walking the active list instead, in read or class order, was slower)
+    const int g1(std::max(1, std::min<int>((int)((n + K7_GATHER_WARPS * 32 - 1) / (K7_GATHER_WARPS * 32)), ctx->sm_count * 16)));
+    k7_gather_kernel<<<g1, K7_GATHER_WARPS * 32, 0, st>>>(n, c, L, *o, ctx->d_status); // (every read, in read order: walking the active list instead, in read or class order, was slower)
     SX_CUDA(ctx, cudaGetLastError());
     *launches += 1;
     return SX_OK;
