@@ -4,6 +4,7 @@
 from __future__ import annotations
 
 import ctypes as C
+from types import SimpleNamespace
 from typing import Optional, Tuple
 
 import numpy as np
@@ -51,47 +52,45 @@ class DeviceArray:
             pass
 
 
+def _device_twin(ctx: "Context", host: C.Structure, owner, slack: int, adopt: Optional[dict] = None):
+    """The device twin of ABI struct `host`: a copy whose every non-NULL pointer field points at `adopt[field]` where given, else at an
+    upload of the owner's array of the field's name into a buffer `slack` bytes longer.  NULL fields stay NULL.  Returns (struct,
+    {field: DeviceArray})."""
+    c = type(host).from_buffer_copy(host)
+    bufs = {}
+    for name, typ in type(host)._fields_:
+        if typ is not C.c_void_p or not getattr(host, name):
+            continue
+        if adopt and name in adopt:
+            setattr(c, name, adopt[name])
+            continue
+        arr = getattr(owner, name, None)
+        if arr is None:
+            raise ValueError(f"{type(host).__name__}.{name} is set on the host, but {type(owner).__name__} has no array of that name to upload")
+        bufs[name] = DeviceArray(ctx, arr.nbytes + slack).upload(arr)
+        setattr(c, name, bufs[name].ptr)
+    return c, bufs
+
+
 class DevAlignBatch:
     """sx_align_batch whose pools live in HBM (inputs resident before the timed region)."""
 
     def __init__(self, ctx: "Context", hb: B.AlignBatch):
         self.host = hb
-        self.bufs = {}
-        for name in ("regions", "read_len", "seq4", "qual", "ref", "alns", "segs", "ins", "exc_off", "exc"):
-            arr = getattr(hb, name)
-            if arr is None:  # exception arrays exist only in the SX_FMT_BASEQ format
-                continue
-            self.bufs[name] = DeviceArray(ctx, arr.nbytes + 64).upload(arr)
-        self.c = A.SxAlignBatch(
-            hb.n_regions, hb.n_reads, hb.n_alns, hb.n_segs,
-            self.bufs["regions"].ptr, self.bufs["read_len"].ptr, self.bufs["seq4"].ptr, self.bufs["qual"].ptr, self.bufs["ref"].ptr,
-            self.bufs["alns"].ptr, self.bufs["segs"].ptr, self.bufs["ins"].ptr,
-            hb.used["seq4"], hb.used["qual"], hb.used["ref"], hb.used["ins"], hb.qual_bits, hb.qual_dict, hb.fmt,
-            self.bufs["exc_off"].ptr if "exc_off" in self.bufs else None, self.bufs["exc"].ptr if "exc" in self.bufs else None,
-        )
+        self.c, self.bufs = _device_twin(ctx, hb.c, hb, 64)
         self.out = DeviceArray(ctx, hb.n_alns * 8)
 
 
 class DevPileupBatch:
     def __init__(self, ctx: "Context", hb: B.PileupBatch):
         self.host = hb
-        self.bufs = {}
-        ptrs = {}
-        for name in ("site_off", "calls", "t2_off", "t2_calls", "ref_base", "ploidy"):
-            arr = getattr(hb, name)
-            if arr is None:
-                ptrs[name] = None
-            else:
-                self.bufs[name] = DeviceArray(ctx, arr.nbytes + 64).upload(arr)
-                ptrs[name] = self.bufs[name].ptr
-        self.c = A.SxPileupBatch(hb.n_sites, ptrs["site_off"], ptrs["calls"], ptrs["t2_off"], ptrs["t2_calls"], ptrs["ref_base"], ptrs["ploidy"])
+        self.c, self.bufs = _device_twin(ctx, hb.c, hb, 64)
 
 
 class DevGaBatch:
     def __init__(self, ctx: "Context", hb: B.GaBatch):
         self.host = hb
-        self.bufs = {n: DeviceArray(ctx, getattr(hb, n).nbytes + 64).upload(getattr(hb, n)) for n in ("query", "ref", "query_off", "ref_off")}
-        self.c = A.SxGaBatch(hb.n, self.bufs["query"].ptr, self.bufs["ref"].ptr, self.bufs["query_off"].ptr, self.bufs["ref_off"].ptr, hb.max_ops)
+        self.c, self.bufs = _device_twin(ctx, hb.c, hb, 64)
         self.res = DeviceArray(ctx, hb.n * A.GA_RESULT_DT.itemsize)
         self.cigar = DeviceArray(ctx, hb.n * hb.max_ops * 4 + 16)
 
@@ -203,78 +202,158 @@ class Context:
     def site_gl_somatic_dev(self, dn: DevPileupBatch, dt: DevPileupBatch, forced: Optional[DeviceArray], out: DeviceArray) -> None:
         self._chk(self.lib.sx_site_gl_somatic_dev(self.h, C.byref(dn.c), C.byref(dt.c), forced.ptr if forced else None, out.ptr))
 
+    # ---- K5
+    def indel_gl(self, ib: "B.IndelBatch", out=None) -> np.ndarray:
+        if out is None:
+            out = np.zeros(ib.n_loci, A.INDEL_RESULT_DT)
+        self._chk(self.lib.sx_indel_gl(self.h, C.byref(ib.c), out.ctypes.data))
+        return out
 
-def _indel_gl(self, ib: "B.IndelBatch", out=None) -> np.ndarray:
-    if out is None:
-        out = np.zeros(ib.n_loci, A.INDEL_RESULT_DT)
-    self._chk(self.lib.sx_indel_gl(self.h, C.byref(ib.c), out.ctypes.data))
-    return out
+    # ---- K5b
+    def somatic_indel(self, sb: "B.SomaticIndelBatch", opts: Optional[A.SxSindelOpts] = None, out=None) -> np.ndarray:
+        """K5b: get_somatic_indel of every locus (host arrays in, sx_sindel_result records out)."""
+        if out is None:
+            out = np.zeros(sb.n_loci, A.SINDEL_RESULT_DT)
+        o = opts or A.default_sindel_opts()
+        self._chk(self.lib.sx_somatic_indel(self.h, C.byref(o), C.byref(sb.c), A.ptr(sb.err_prob), sb.err_prob.size, out.ctypes.data))
+        return out
+
+    def somatic_indel_dev(self, db: DevSomaticIndelBatch, opts: Optional[A.SxSindelOpts] = None) -> None:
+        o = opts or A.default_sindel_opts()
+        hb = db.host
+        self._chk(self.lib.sx_somatic_indel_dev(self.h, C.byref(o), C.byref(db.c), A.ptr(hb.err_prob), hb.err_prob.size, db.out.ptr))
+
+    # ---- K4
+    def pileup_reads(self, pb: B.PileupReadsBatch):
+        """K4: per-position base_call columns of a read batch (host buffers in, host columns out)."""
+        out = B.PileupColumns(pb)
+        self._chk(self.lib.sx_pileup_reads(self.h, C.byref(pb.c), C.byref(out.c)))
+        return out.trimmed()
+
+    # ---- K6
+    def score_indels(self, sb: B.ScoreIndelsBatch, lnp: np.ndarray):
+        """K6: the arg-max epilogue of scoreCandidateAlignments + score_indels (host buffers in, host records out).
+        Returns (records in key order per read, n_rec[n_reads], max_aln[n_reads], eval_aln[n_reads])."""
+        lnp = np.ascontiguousarray(lnp, dtype=np.float64)
+        assert lnp.size >= sb.n_alns
+        out = B.ScoreIndelsOut(sb)
+        self._chk(self.lib.sx_score_indels(self.h, C.byref(sb.c), lnp.ctypes.data, C.byref(out.c)))
+        return out.compact()
+
+    def score_indels_dev(self, db: DevScoreIndelsBatch, lnp_dev: DeviceArray) -> None:
+        self._chk(self.lib.sx_score_indels_dev(self.h, C.byref(db.c), lnp_dev.ptr, C.byref(db.out)))
+
+    # ---- K6b
+    def link_indel_reads(self, normal: B.IndelReadsSample, tumor: B.IndelReadsSample, loci: B.IndelLoci, cap_reads=None, cap_alts=None) -> B.IndelReadsOut:
+        """K6b: two samples' K6 records -> K5b's per-locus read lists (host arrays in and out).  SX_ERR_CAPACITY leaves the needed sizes in
+        the SxError's `totals`."""
+        cr, ca = self._link_caps(normal, tumor, loci.n_loci)
+        out = B.IndelReadsOut(loci.n_loci, cr if cap_reads is None else cap_reads, ca if cap_alts is None else cap_alts)
+        totals = np.zeros(2, np.uint32)
+        rc = self.lib.sx_link_indel_reads(self.h, C.byref(normal.c), C.byref(tumor.c), C.byref(loci.c), C.byref(out.c), totals.ctypes.data)
+        self._chk_totals(rc, totals)
+        return out
+
+    @staticmethod
+    def _link_caps(normal, tumor, n_loci: int) -> Tuple[int, int]:
+        """Capacities no batch exceeds: an entry per record, two alternates per entry and SX_SINDEL_MAX_ALTS per locus."""
+        cap_reads = sum(int(np.asarray(s.n_rec[: s.n_reads], np.int64).sum()) for s in (normal, tumor))
+        return cap_reads, min(2 * cap_reads, A.SX_SINDEL_MAX_ALTS * n_loci)
+
+    def link_indel_reads_dev(self, normal: DevIndelReadsSample, tumor: DevIndelReadsSample, loci: DevIndelLoci, cap_reads: int, cap_alts: int) -> B.IndelReadsOut:
+        """K6b on device-resident inputs, into device arrays of the given capacities; returns their host copies."""
+        n = loci.host.n_loci
+        out = B.IndelReadsOut(n, cap_reads, cap_alts)
+        d = {k: DeviceArray(self, getattr(out, k).nbytes + 64) for k in ("alt_off", "alts", "read_off", "reads", "status", "totals")}
+        c = A.SxIndelReadsOut(cap_alts=cap_alts, cap_reads=cap_reads, **{k: x.ptr for k, x in d.items()})
+        totals = np.zeros(2, np.uint32)
+        rc = self.lib.sx_link_indel_reads_dev(self.h, C.byref(normal.c), C.byref(tumor.c), C.byref(loci.c), C.byref(c), totals.ctypes.data)
+        self._chk_totals(rc, totals)
+        for k in ("alt_off", "read_off", "totals"):
+            getattr(out, k)[:] = d[k].download(np.uint32, getattr(out, k).size)
+        out.status[:n] = d["status"].download(np.uint32, n)
+        out.reads[: int(out.totals[0])] = d["reads"].download(A.SINDEL_READ_DT, int(out.totals[0]))
+        out.alts[: int(out.totals[1])] = d["alts"].download(A.INDEL_KEY_DT, int(out.totals[1]))
+        for x in d.values():
+            x.free()
+        return out
+
+    def _chk_totals(self, rc: int, totals: np.ndarray) -> None:
+        try:
+            self._chk(rc)
+        except SxError as e:
+            e.totals = totals.copy()
+            raise
+
+    # ---- K7
+    def enumerate_alignments(self, eb: B.EnumBatch, cap_alns=None, cap_segs=None, cap_keys=None) -> B.EnumOut:
+        """K7: the candidate alignments of every read (getCandidateAlignments), host buffers in, host CSR out."""
+        out = B.EnumOut(eb, cap_alns, cap_segs, cap_keys)
+        self._chk(self.lib.sx_enumerate_alignments(self.h, C.byref(eb.c), C.byref(out.c)))
+        return out
+
+    def enumerate_alignments_dev(self, db: DevEnumBatch) -> None:
+        self._chk(self.lib.sx_enumerate_alignments_dev(self.h, C.byref(db.c), C.byref(db.out)))
+
+    # ---- K7b
+    def link_alignments(self, eb: B.EnumBatch, out: B.EnumOut, regions: np.ndarray, cap_segs=None, cap_ins=None) -> B.LinkOut:
+        """K7b: K7's alignments as the alignment part of a K1 batch (host buffers).  `regions`: the K1 batch's region records."""
+        n_alns = int(out.totals[0])
+        lo = B.LinkOut(regions, n_alns, cap_segs if cap_segs is not None else 2 * int(out.totals[1]) + 8 * eb.n_regions + 64,
+                       cap_ins if cap_ins is not None else 64 * n_alns + 16 * eb.n_regions + 64, n_enum_segs=int(out.totals[1]))
+        self._chk(self.lib.sx_link_alignments(self.h, C.byref(eb.c), C.byref(out.c), n_alns, A.ptr(eb.ins_off), A.ptr(eb.ins_pool), C.byref(lo.c)))
+        return lo
+
+    # ---- K7a
+    def alignment_indels(self, eb: B.EnumBatch, pools: B.AlignBatch, cap_keys=None) -> B.PrepOut:
+        """K7a: the window entries every read's input alignment already contains (host buffers).  `pools`: the K1 batch holding the reads
+        and reference windows (B.read_pools_of)."""
+        po = B.PrepOut(eb, cap_keys)
+        self._chk(self.lib.sx_alignment_indels(self.h, C.byref(eb.c), A.ptr(pools.regions), A.ptr(pools.seq4), A.ptr(pools.ref), A.ptr(eb.ins_off), A.ptr(eb.ins_pool),
+                                               C.byref(po.c)))
+        return po
+
+    # ---- K9
+    def choose_realignment(self, rb: B.RealignBatch, lnp: np.ndarray, cap_segs=None) -> B.RealignOut:
+        """K9: rseg.realignment of every read from its candidate alignments and their scores (host buffers)."""
+        lnp = np.ascontiguousarray(lnp, dtype=np.float64)
+        ro = B.RealignOut(rb, cap_segs)
+        self._chk(self.lib.sx_choose_realignment(self.h, C.byref(rb.c), lnp.ctypes.data, C.byref(ro.c)))
+        return ro
+
+    # ---- K7g
+    def realign_gates(self, gb: B.GateBatch) -> B.GateOut:
+        """K7g: which reads go into the alignment search and with which (normalized) input alignment (host buffers)."""
+        go = B.GateOut(gb)
+        self._chk(self.lib.sx_realign_gates(self.h, C.byref(gb.c), C.byref(go.c)))
+        return go
 
 
-Context.indel_gl = _indel_gl  # K5
-
-
-def _somatic_indel(self, sb: "B.SomaticIndelBatch", opts: Optional[A.SxSindelOpts] = None, out=None) -> np.ndarray:
-    """K5b: get_somatic_indel of every locus (host arrays in, sx_sindel_result records out)."""
-    if out is None:
-        out = np.zeros(sb.n_loci, A.SINDEL_RESULT_DT)
-    o = opts or A.default_sindel_opts()
-    self._chk(self.lib.sx_somatic_indel(self.h, C.byref(o), C.byref(sb.c), A.ptr(sb.err_prob), sb.err_prob.size, out.ctypes.data))
-    return out
+# the name under which the test suite's host-memory context (tests/mockctx.py) takes K7's device entry
+_enumerate_alignments_dev = Context.enumerate_alignments_dev
 
 
 class DevSomaticIndelBatch:
     """sx_sindel_batch whose arrays live in HBM, with a device output buffer; the error-rate table stays on the host."""
 
-    _ARRAYS = ("key", "is_forced_output", "err_idx", "alt_off", "alts", "read_off", "reads")
-
     def __init__(self, ctx: "Context", hb: "B.SomaticIndelBatch"):
         self.host = hb
-        self.bufs = {n: DeviceArray(ctx, getattr(hb, n).nbytes + 64).upload(getattr(hb, n)) for n in self._ARRAYS}
-        self.c = A.SxSindelBatch(hb.n_loci, 0, *(self.bufs[n].ptr for n in self._ARRAYS))
+        self.c, self.bufs = _device_twin(ctx, hb.c, hb, 64)
         self.out = DeviceArray(ctx, max(1, hb.n_loci) * A.SINDEL_RESULT_DT.itemsize)
 
     def download(self) -> np.ndarray:
         return self.out.download(A.SINDEL_RESULT_DT, self.host.n_loci)
 
 
-def _somatic_indel_dev(self, db: DevSomaticIndelBatch, opts: Optional[A.SxSindelOpts] = None) -> None:
-    o = opts or A.default_sindel_opts()
-    hb = db.host
-    self._chk(self.lib.sx_somatic_indel_dev(self.h, C.byref(o), C.byref(db.c), A.ptr(hb.err_prob), hb.err_prob.size, db.out.ptr))
-
-
-Context.somatic_indel = _somatic_indel  # K5b
-Context.somatic_indel_dev = _somatic_indel_dev
-
-
-def _pileup_reads(self, pb: B.PileupReadsBatch):
-    """K4: per-position base_call columns of a read batch (host buffers in, host columns out)."""
-    out = B.PileupColumns(pb)
-    self._chk(self.lib.sx_pileup_reads(self.h, C.byref(pb.c), C.byref(out.c)))
-    return out.trimmed()
-
-
-Context.pileup_reads = _pileup_reads
-
-
 class DevScoreIndelsBatch:
     """sx_score_indels_batch whose arrays live in HBM, with device output buffers; `lnp` is usually DevAlignBatch.out."""
 
-    _ARRAYS = ("region_read_off", "region_key_off", "keys", "aln_off", "aln_pos", "aln_seg_off", "segs", "aln_key_off", "aln_keys", "read_len", "non_ambig",
-               "read_flags", "rec_off")
-
     def __init__(self, ctx: "Context", hb: B.ScoreIndelsBatch):
         self.host = hb
-        self.bufs = {n: DeviceArray(ctx, getattr(hb, n).nbytes + 64).upload(getattr(hb, n)) for n in self._ARRAYS}
-        p = {n: self.bufs[n].ptr for n in self._ARRAYS}
-        self.c = A.SxScoreIndelsBatch(
-            hb.n_regions, hb.n_reads, hb.n_alns, hb.n_keys, p["region_read_off"], p["region_key_off"], p["keys"], p["aln_off"], p["aln_pos"], p["aln_seg_off"],
-            p["segs"], p["aln_key_off"], p["aln_keys"], p["read_len"], p["non_ambig"], None, None, p["read_flags"], p["rec_off"], hb.opts,
-        )
+        self.c, self.bufs = _device_twin(ctx, hb.c, hb, 64)
         self.recs = DeviceArray(ctx, (hb.n_rec_slots + 1) * A.READ_INDEL_SCORE_DT.itemsize)
         self.n_rec, self.max_aln, self.eval_aln = (DeviceArray(ctx, (hb.n_reads + 1) * 4) for _ in range(3))
-        self.out = A.SxScoreIndelsOut(self.recs.ptr, self.n_rec.ptr, self.max_aln.ptr, self.eval_aln.ptr)
+        self.out = A.SxScoreIndelsOut(recs=self.recs.ptr, n_rec=self.n_rec.ptr, max_aln=self.max_aln.ptr, eval_aln=self.eval_aln.ptr)
 
     def download(self):
         hb = self.host
@@ -286,65 +365,14 @@ class DevScoreIndelsBatch:
         return out.compact()
 
 
-def _score_indels(self, sb: B.ScoreIndelsBatch, lnp: np.ndarray):
-    """K6: the arg-max epilogue of scoreCandidateAlignments + score_indels (host buffers in, host records out).
-    Returns (records in key order per read, n_rec[n_reads], max_aln[n_reads], eval_aln[n_reads])."""
-    lnp = np.ascontiguousarray(lnp, dtype=np.float64)
-    assert lnp.size >= sb.n_alns
-    out = B.ScoreIndelsOut(sb)
-    self._chk(self.lib.sx_score_indels(self.h, C.byref(sb.c), lnp.ctypes.data, C.byref(out.c)))
-    return out.compact()
-
-
-def _score_indels_dev(self, db: DevScoreIndelsBatch, lnp_dev: DeviceArray) -> None:
-    self._chk(self.lib.sx_score_indels_dev(self.h, C.byref(db.c), lnp_dev.ptr, C.byref(db.out)))
-
-
-Context.score_indels = _score_indels  # K6
-Context.score_indels_dev = _score_indels_dev
-
-
-def _link_caps(normal, tumor, n_loci: int) -> Tuple[int, int]:
-    """Capacities no batch exceeds: an entry per record, two alternates per entry and SX_SINDEL_MAX_ALTS per locus."""
-    cap_reads = sum(int(np.asarray(s.n_rec[: s.n_reads], np.int64).sum()) for s in (normal, tumor))
-    return cap_reads, min(2 * cap_reads, A.SX_SINDEL_MAX_ALTS * n_loci)
-
-
-def _link_indel_reads(self, normal: B.IndelReadsSample, tumor: B.IndelReadsSample, loci: B.IndelLoci, cap_reads=None, cap_alts=None) -> B.IndelReadsOut:
-    """K6b: two samples' K6 records -> K5b's per-locus read lists (host arrays in and out).  SX_ERR_CAPACITY leaves the needed sizes in
-    the SxError's `totals`."""
-    cr, ca = _link_caps(normal, tumor, loci.n_loci)
-    out = B.IndelReadsOut(loci.n_loci, cr if cap_reads is None else cap_reads, ca if cap_alts is None else cap_alts)
-    totals = np.zeros(2, np.uint32)
-    rc = self.lib.sx_link_indel_reads(self.h, C.byref(normal.c), C.byref(tumor.c), C.byref(loci.c), C.byref(out.c), totals.ctypes.data)
-    _chk_totals(self, rc, totals)
-    return out
-
-
-def _chk_totals(self, rc: int, totals: np.ndarray) -> None:
-    try:
-        self._chk(rc)
-    except SxError as e:
-        e.totals = totals.copy()
-        raise
-
-
 class DevIndelReadsSample:
     """sx_indel_reads_sample in HBM.  `from_score_indels` adopts a DevScoreIndelsBatch: its read arrays and the recs / n_rec arrays K6
     wrote, which that object owns -- so two samples scored on ONE context stay apart.  A constructor from two DevWindow passes is not
     built (DESIGN section 8)."""
 
     def __init__(self, ctx: "Context", hs: B.IndelReadsSample, adopt: Optional[dict] = None):
-        self.host, self.bufs = hs, {}
-        p = dict(adopt or {})
-        for n in B.IndelReadsSample.ARRAYS:
-            a = getattr(hs, n)
-            if n not in p:
-                p[n] = None
-                if a is not None:
-                    self.bufs[n] = DeviceArray(ctx, a.nbytes + 64).upload(a)
-                    p[n] = self.bufs[n].ptr
-        self.c = A.SxIndelReadsSample(hs.n_regions, hs.n_reads, hs.n_keys, 0, *(p[n] for n in B.IndelReadsSample.ARRAYS))
+        self.host = hs
+        self.c, self.bufs = _device_twin(ctx, hs.c, hs, 64, adopt)
 
     @staticmethod
     def from_score_indels(ctx: "Context", db: DevScoreIndelsBatch, key_gid, read_id=None) -> "DevIndelReadsSample":
@@ -360,31 +388,7 @@ class DevIndelReadsSample:
 class DevIndelLoci:
     def __init__(self, ctx: "Context", hl: B.IndelLoci):
         self.host = hl
-        self.bufs = {n: DeviceArray(ctx, getattr(hl, n).nbytes + 64).upload(getattr(hl, n)) for n in B.IndelLoci.ARRAYS}
-        self.c = A.SxIndelLoci(hl.n_loci, hl.n_gid, *(self.bufs[n].ptr for n in B.IndelLoci.ARRAYS))
-
-
-def _link_indel_reads_dev(self, normal: DevIndelReadsSample, tumor: DevIndelReadsSample, loci: DevIndelLoci, cap_reads: int, cap_alts: int) -> B.IndelReadsOut:
-    """K6b on device-resident inputs, into device arrays of the given capacities; returns their host copies."""
-    n = loci.host.n_loci
-    out = B.IndelReadsOut(n, cap_reads, cap_alts)
-    d = {k: DeviceArray(self, getattr(out, k).nbytes + 64) for k in ("alt_off", "alts", "read_off", "reads", "status", "totals")}
-    c = A.SxIndelReadsOut(d["alt_off"].ptr, d["alts"].ptr, d["read_off"].ptr, d["reads"].ptr, d["status"].ptr, d["totals"].ptr, cap_alts, cap_reads)
-    totals = np.zeros(2, np.uint32)
-    rc = self.lib.sx_link_indel_reads_dev(self.h, C.byref(normal.c), C.byref(tumor.c), C.byref(loci.c), C.byref(c), totals.ctypes.data)
-    _chk_totals(self, rc, totals)
-    for k in ("alt_off", "read_off", "totals"):
-        getattr(out, k)[:] = d[k].download(np.uint32, getattr(out, k).size)
-    out.status[:n] = d["status"].download(np.uint32, n)
-    out.reads[: int(out.totals[0])] = d["reads"].download(A.SINDEL_READ_DT, int(out.totals[0]))
-    out.alts[: int(out.totals[1])] = d["alts"].download(A.INDEL_KEY_DT, int(out.totals[1]))
-    for x in d.values():
-        x.free()
-    return out
-
-
-Context.link_indel_reads = _link_indel_reads  # K6b
-Context.link_indel_reads_dev = _link_indel_reads_dev
+        self.c, self.bufs = _device_twin(ctx, hl.c, hl, 64)
 
 
 class DevSomaticIndelChain:
@@ -408,23 +412,14 @@ class DevSomaticIndelChain:
 class DevEnumBatch:
     """An sx_enum_batch and its sx_enum_out resident in device memory (for sx_enumerate_alignments_dev)."""
 
-    _ARRAYS = ("region_read_off", "region_key_off", "keys", "key_hap", "realign_begin", "realign_end", "in_pos", "in_seg_off", "in_segs", "in_key_off", "in_keys",
-               "use_key_off", "use_keys", "in_lead_key", "in_trail_key", "read_len")
-
     def __init__(self, ctx: "Context", hb: B.EnumBatch, cap_alns=None, cap_segs=None, cap_keys=None):
         self.host = hb
-        self.bufs = {n: DeviceArray(ctx, getattr(hb, n).nbytes + 64).upload(getattr(hb, n)) for n in self._ARRAYS}
-        p = {n: self.bufs[n].ptr for n in self._ARRAYS}
-        self.c = A.SxEnumBatch(hb.n_regions, hb.n_reads, hb.n_keys, p["region_read_off"], p["region_key_off"], p["keys"], p["key_hap"] if hb.has_hap else None,
-                               p["realign_begin"], p["realign_end"], p["in_pos"], p["in_seg_off"], p["in_segs"], p["in_key_off"], p["in_keys"], p["use_key_off"],
-                               p["use_keys"], p["in_lead_key"], p["in_trail_key"], p["read_len"], None, hb.opts)
+        self.c, self.bufs = _device_twin(ctx, hb.c, hb, 64)
         self.shape = B.EnumOut(hb, cap_alns, cap_segs, cap_keys)  # host twin: sizes and the download target
         s = self.shape
         self.obufs = {n: DeviceArray(ctx, getattr(s, n).nbytes + 64) for n in ("totals", "aln_off", "status", "aln_pos", "aln_seg_off", "segs", "aln_key_off",
                                                                                "aln_keys", "aln_lead_key", "aln_trail_key")}
-        o = {n: b.ptr for n, b in self.obufs.items()}
-        self.out = A.SxEnumOut(s.cap_alns, s.cap_segs, s.cap_keys, o["totals"], o["aln_off"], o["status"], o["aln_pos"], o["aln_seg_off"], o["segs"], o["aln_key_off"],
-                               o["aln_keys"], o["aln_lead_key"], o["aln_trail_key"])
+        self.out = A.SxEnumOut(cap_alns=s.cap_alns, cap_segs=s.cap_segs, cap_keys=s.cap_keys, **{n: b.ptr for n, b in self.obufs.items()})
 
     def download(self) -> B.EnumOut:
         s = self.shape
@@ -432,45 +427,6 @@ class DevEnumBatch:
             a = getattr(s, n)
             a[...] = buf.download(a.dtype, a.size)
         return s
-
-
-def _enumerate_alignments(self, eb: B.EnumBatch, cap_alns=None, cap_segs=None, cap_keys=None) -> B.EnumOut:
-    """K7: the candidate alignments of every read (getCandidateAlignments), host buffers in, host CSR out."""
-    out = B.EnumOut(eb, cap_alns, cap_segs, cap_keys)
-    self._chk(self.lib.sx_enumerate_alignments(self.h, C.byref(eb.c), C.byref(out.c)))
-    return out
-
-
-def _enumerate_alignments_dev(self, db: DevEnumBatch) -> None:
-    self._chk(self.lib.sx_enumerate_alignments_dev(self.h, C.byref(db.c), C.byref(db.out)))
-
-
-Context.enumerate_alignments = _enumerate_alignments  # K7
-Context.enumerate_alignments_dev = _enumerate_alignments_dev
-
-
-def _link_alignments(self, eb: B.EnumBatch, out: B.EnumOut, regions: np.ndarray, cap_segs=None, cap_ins=None) -> B.LinkOut:
-    """K7b: K7's alignments as the alignment part of a K1 batch (host buffers).  `regions`: the K1 batch's region records."""
-    n_alns = int(out.totals[0])
-    lo = B.LinkOut(regions, n_alns, cap_segs if cap_segs is not None else 2 * int(out.totals[1]) + 8 * eb.n_regions + 64,
-                   cap_ins if cap_ins is not None else 64 * n_alns + 16 * eb.n_regions + 64, n_enum_segs=int(out.totals[1]))
-    self._chk(self.lib.sx_link_alignments(self.h, C.byref(eb.c), C.byref(out.c), n_alns, A.ptr(eb.ins_off), A.ptr(eb.ins_pool), C.byref(lo.c)))
-    return lo
-
-
-Context.link_alignments = _link_alignments  # K7b
-
-
-def _alignment_indels(self, eb: B.EnumBatch, pools: B.AlignBatch, cap_keys=None) -> B.PrepOut:
-    """K7a: the window entries every read's input alignment already contains (host buffers).  `pools`: the K1 batch holding the reads
-    and reference windows (B.read_pools_of)."""
-    po = B.PrepOut(eb, cap_keys)
-    self._chk(self.lib.sx_alignment_indels(self.h, C.byref(eb.c), A.ptr(pools.regions), A.ptr(pools.seq4), A.ptr(pools.ref), A.ptr(eb.ins_off), A.ptr(eb.ins_pool),
-                                           C.byref(po.c)))
-    return po
-
-
-Context.alignment_indels = _alignment_indels  # K7a
 
 
 class DevRealignChain:
@@ -493,7 +449,7 @@ class DevRealignChain:
         self.prep = {"totals": DeviceArray(ctx, 16), "in_key_off": DeviceArray(ctx, (n + 1) * 4 + 16), "in_keys": DeviceArray(ctx, self.cap_in_keys * 2 + 16),
                      "in_lead_key": DeviceArray(ctx, n * 2 + 16), "in_trail_key": DeviceArray(ctx, n * 2 + 16)}
         p = self.prep
-        self.prep_out = A.SxPrepOut(self.cap_in_keys, p["totals"].ptr, p["in_key_off"].ptr, p["in_keys"].ptr, p["in_lead_key"].ptr, p["in_trail_key"].ptr)
+        self.prep_out = A.SxPrepOut(cap_keys=self.cap_in_keys, **{k: x.ptr for k, x in p.items()})
         # K7 reads what K7a writes
         c = self.enum.c
         c.in_key_off, c.in_keys, c.in_lead_key, c.in_trail_key = p["in_key_off"].ptr, p["in_keys"].ptr, p["in_lead_key"].ptr, p["in_trail_key"].ptr
@@ -521,9 +477,10 @@ class DevRealignChain:
                  "raw_segs": DeviceArray(ctx, raw.raw_segs.nbytes + 16).upload(raw.raw_segs), "gate": DeviceArray(ctx, n + 16), "in_pos": DeviceArray(ctx, n * 4 + 16),
                  "in_segs": DeviceArray(ctx, raw.raw_segs.nbytes + 16)}
             b0 = self.enum.bufs
-            self.gate_batch = A.SxGateBatch(eb.n_regions, n, b0["region_read_off"].ptr, b0["region_key_off"].ptr, b0["keys"].ptr, b0["realign_begin"].ptr,
-                                            b0["realign_end"].ptr, g["raw_pos"].ptr, g["seg_off"].ptr, g["raw_segs"].ptr, b0["read_len"].ptr, None, eb.opts.max_indel_size)
-            self.gate_out = A.SxGateOut(g["gate"].ptr, g["in_pos"].ptr, g["in_segs"].ptr)
+            self.gate_batch = A.SxGateBatch(n_regions=eb.n_regions, n_reads=n, max_indel_size=eb.opts.max_indel_size,
+                                            **{k: b0[k].ptr for k in ("region_read_off", "region_key_off", "keys", "realign_begin", "realign_end", "read_len")},
+                                            **{k: g[k].ptr for k in ("raw_pos", "seg_off", "raw_segs")})
+            self.gate_out = A.SxGateOut(gate=g["gate"].ptr, in_pos=g["in_pos"].ptr, in_segs=g["in_segs"].ptr)
             c.in_pos, c.in_seg_off, c.in_segs, c.gate = g["in_pos"].ptr, g["seg_off"].ptr, g["in_segs"].ptr, g["gate"].ptr
             self.gates = g
 
@@ -547,21 +504,25 @@ class DevRealignChain:
                          "ins": DeviceArray(ctx, cap_ins + A.SX_POOL_SLACK + 16), "k6_segs": DeviceArray(ctx, (nS + 16) * 4 + 16)}
             self.lnp = DeviceArray(ctx, (nA + 1) * 8 + 16)
         L = self.link
-        lo = A.SxLinkOut(L["cap_segs"], L["cap_ins"], L["totals"].ptr, pc.regions, L["alns"].ptr, L["segs"].ptr, L["ins"].ptr, L["k6_segs"].ptr)
+        lo = A.SxLinkOut(cap_segs=L["cap_segs"], cap_ins=L["cap_ins"], regions=pc.regions, **{k: L[k].ptr for k in ("totals", "alns", "segs", "ins", "k6_segs")})
         ctx._chk(ctx.lib.sx_link_alignments_dev(ctx.h, C.byref(e.c), C.byref(e.out), nA, self.key_ins_off.ptr, self.key_ins.ptr, C.byref(lo)))
         self.ms["k7b_link"] = ctx.timing().kernel_ms
         n_k1_segs, ins_bytes = (int(x) for x in L["totals"].download(np.uint32, 2))
         self.k1_totals = (n_k1_segs, ins_bytes)
-        k1 = A.SxAlignBatch(eb.n_regions, eb.n_reads, nA, n_k1_segs, pc.regions, pc.read_len, pc.seq4, pc.qual, pc.ref, L["alns"].ptr, L["segs"].ptr, L["ins"].ptr,
-                            pc.seq4_bytes, pc.qual_bytes, pc.ref_bytes, ins_bytes, pc.qual_bits, pc.qual_dict, 0, None, None)
+        k1 = A.SxAlignBatch(n_regions=eb.n_regions, n_reads=eb.n_reads, n_alns=nA, n_segs=n_k1_segs, regions=pc.regions, read_len=pc.read_len, seq4=pc.seq4, qual=pc.qual,
+                            ref=pc.ref, alns=L["alns"].ptr, segs=L["segs"].ptr, ins=L["ins"].ptr, seq4_bytes=pc.seq4_bytes, qual_bytes=pc.qual_bytes, ref_bytes=pc.ref_bytes,
+                            ins_bytes=ins_bytes, qual_bits=pc.qual_bits, qual_dict=pc.qual_dict)
         ctx._chk(ctx.lib.sx_score_alignments_dev(ctx.h, C.byref(k1), self.lnp.ptr))
         self.ms["k1_score_alignments"] = ctx.timing().kernel_ms
         o = e.obufs
         b = e.bufs
-        k6 = A.SxScoreIndelsBatch(eb.n_regions, eb.n_reads, nA, eb.n_keys, b["region_read_off"].ptr, b["region_key_off"].ptr, b["keys"].ptr, o["aln_off"].ptr,
-                                  o["aln_pos"].ptr, o["aln_seg_off"].ptr, L["k6_segs"].ptr, o["aln_key_off"].ptr, o["aln_keys"].ptr, b["read_len"].ptr, b["read_len"].ptr,
-                                  None, None, self.read_flags.ptr, self.rec_off.ptr, A.default_score_indels_opts())
-        out = A.SxScoreIndelsOut(self.recs.ptr, self.n_rec.ptr, self.max_aln.ptr, self.eval_aln.ptr)
+        k6 = A.SxScoreIndelsBatch(n_regions=eb.n_regions, n_reads=eb.n_reads, n_alns=nA, n_keys=eb.n_keys, region_read_off=b["region_read_off"].ptr,
+                                  region_key_off=b["region_key_off"].ptr, keys=b["keys"].ptr, aln_off=o["aln_off"].ptr, aln_pos=o["aln_pos"].ptr,
+                                  aln_seg_off=o["aln_seg_off"].ptr, segs=L["k6_segs"].ptr, aln_key_off=o["aln_key_off"].ptr, aln_keys=o["aln_keys"].ptr,
+                                  read_len=b["read_len"].ptr,
+                                  non_ambig=b["read_len"].ptr,  # the enum batch has no per-read count of non-N bases: every base counts
+                                  read_flags=self.read_flags.ptr, rec_off=self.rec_off.ptr, opts=A.default_score_indels_opts())
+        out = A.SxScoreIndelsOut(recs=self.recs.ptr, n_rec=self.n_rec.ptr, max_aln=self.max_aln.ptr, eval_aln=self.eval_aln.ptr)
         ctx._chk(ctx.lib.sx_score_indels_dev(ctx.h, C.byref(k6), self.lnp.ptr, C.byref(out)))
         self.ms["k6_score_indels"] = ctx.timing().kernel_ms
         # K9: rseg.realignment of every read, in K4's segment kinds
@@ -573,11 +534,13 @@ class DevRealignChain:
                             "n_seg": DeviceArray(ctx, n * 2 + 16), "status": DeviceArray(ctx, n + 16), "best_aln": DeviceArray(ctx, n * 4 + 16),
                             "segs": DeviceArray(ctx, cap * 4 + 16)}
         R = self.realign
-        rb = A.SxRealignBatch(eb.n_regions, n, nA, b["region_read_off"].ptr, b["region_key_off"].ptr, b["keys"].ptr, o["aln_off"].ptr, o["aln_pos"].ptr,
-                              o["aln_seg_off"].ptr, o["segs"].ptr, o["aln_key_off"].ptr, o["aln_keys"].ptr, b["read_len"].ptr, None, 1, 1, 2.302585092994046)
+        rb = A.SxRealignBatch(n_regions=eb.n_regions, n_reads=n, n_alns=nA, region_read_off=b["region_read_off"].ptr, region_key_off=b["region_key_off"].ptr,
+                              keys=b["keys"].ptr, aln_off=o["aln_off"].ptr, aln_pos=o["aln_pos"].ptr, aln_seg_off=o["aln_seg_off"].ptr, segs=o["segs"].ptr,
+                              aln_key_off=o["aln_key_off"].ptr, aln_keys=o["aln_keys"].ptr, read_len=b["read_len"].ptr, is_smoothed_alignments=1, k4_kinds=1,
+                              smoothed_lnp_range=2.302585092994046)
         if self.gates is not None:  # the mapper's alignments are at hand: K9's output is then getBestAlignment() of every read (K4's input)
             rb.raw_pos, rb.raw_seg_off, rb.raw_segs = self.gates["raw_pos"].ptr, self.gates["seg_off"].ptr, self.gates["raw_segs"].ptr
-        ro = A.SxRealignOut(R["cap"], R["totals"].ptr, R["seg_off"].ptr, R["pos"].ptr, R["n_seg"].ptr, R["status"].ptr, R["best_aln"].ptr, R["segs"].ptr)
+        ro = A.SxRealignOut(cap_segs=R["cap"], **{k: R[k].ptr for k in ("totals", "seg_off", "pos", "n_seg", "status", "best_aln", "segs")})
         ctx._chk(ctx.lib.sx_choose_realignment_dev(ctx.h, C.byref(rb), self.lnp.ptr, C.byref(ro)))
         self.ms["k9_choose_realignment"] = ctx.timing().kernel_ms
         return dict(self.ms)
@@ -608,50 +571,18 @@ class DevRealignChain:
             d.free()
 
 
-def _choose_realignment(self, rb: B.RealignBatch, lnp: np.ndarray, cap_segs=None) -> B.RealignOut:
-    """K9: rseg.realignment of every read from its candidate alignments and their scores (host buffers)."""
-    lnp = np.ascontiguousarray(lnp, dtype=np.float64)
-    ro = B.RealignOut(rb, cap_segs)
-    self._chk(self.lib.sx_choose_realignment(self.h, C.byref(rb.c), lnp.ctypes.data, C.byref(ro.c)))
-    return ro
-
-
-Context.choose_realignment = _choose_realignment  # K9
-
-
-def _realign_gates(self, gb: B.GateBatch) -> B.GateOut:
-    """K7g: which reads go into the alignment search and with which (normalized) input alignment (host buffers)."""
-    go = B.GateOut(gb)
-    self._chk(self.lib.sx_realign_gates(self.h, C.byref(gb.c), C.byref(go.c)))
-    return go
-
-
-Context.realign_gates = _realign_gates  # K7g
-
-
 class DevWindow:
     """sx_process_window_dev on a B.WindowBatch: every input array resident in HBM, every output array the caller may want to read
     back allocated here (tests download them; bench.py leaves them where they are)."""
 
     def __init__(self, ctx: "Context", w: "B.WindowBatch", keep_outputs: bool = True, cap_best_segs=None):
         self.ctx, self.w = ctx, w
-        self.bufs = {}
-        p = {}
-        for name in B.WindowBatch.ARRAYS:
-            arr = w.a.get(name)
-            if arr is None:
-                p[name] = None
-                continue
-            arr = np.ascontiguousarray(arr)
-            self.bufs[name] = DeviceArray(ctx, arr.nbytes + 80).upload(arr)
-            p[name] = self.bufs[name].ptr
         c = A.SxWindowBatch()
         ctx.lib.sx_default_window_opts(C.byref(c))
         c.n_regions, c.n_reads, c.n_keys = w.n_regions, w.n_reads, w.n_keys
-        for name in B.WindowBatch.ARRAYS:
-            if name != "cand_snv":
-                setattr(c, name, p[name])
-        c.cand_snv, c.n_cand_snv = p["cand_snv"], (int(w.a["cand_snv"].size) if w.a.get("cand_snv") is not None else 0)
+        for name in B.WindowBatch.ARRAYS:  # host pointers: the twin below puts each array in device memory
+            setattr(c, name, A.ptr(w.a.get(name)))
+        c.n_cand_snv = int(w.a["cand_snv"].size) if w.a.get("cand_snv") is not None else 0
         c.seq4_bytes, c.qual_bytes, c.ref_bytes = w.used["seq4"], w.used["qual"], w.used["ref"]
         c.qual_bits = w.qual_bits
         c.qual_dict = (C.c_uint8 * 16)(*(w.qual_dict + [0] * (16 - len(w.qual_dict))))
@@ -661,7 +592,7 @@ class DevWindow:
             keep = c.enum_opts.max_alns_per_read
             c.enum_opts = w.enum_opts
             c.enum_opts.max_alns_per_read = max(keep, w.enum_opts.max_alns_per_read)
-        self.c = c
+        self.c, self.bufs = _device_twin(ctx, c, SimpleNamespace(**w.a), 80)
         self.out = A.SxWindowOut()
         self.obufs = {}
         n, ns = w.n_reads, w.n_sites
@@ -681,7 +612,8 @@ class DevWindow:
             o.cap_best_segs = self.cap_best
             if w.do_site_gl:
                 o.variant_sites, o.cap_variant_sites = b["variant_sites"].ptr, ns // 8 + 1024
-            o.cols = A.SxPileupColumns(b["site_off"].ptr, b["calls"].ptr, b["t2_off"].ptr, b["t2_calls"].ptr, b["n_spandel"].ptr, b["n_submapped"].ptr, bases, bases)
+            o.cols = A.SxPileupColumns(calls_capacity=bases, t2_capacity=bases,
+                                       **{k: b[k].ptr for k in ("site_off", "calls", "t2_off", "t2_calls", "n_spandel", "n_submapped")})
             self.n_slots = n_slots
         else:  # only the call records come out; everything else stays in the context's own buffers
             cap_v = ns // 8 + 1024

@@ -181,10 +181,10 @@ class AlignBatch:
         self.n_segs = int(alns["seg_off"][-1]) if n_segs is None else int(n_segs)
         self.used = used
         self.c = A.SxAlignBatch(
-            self.n_regions, self.n_reads, self.n_alns, self.n_segs,
-            A.ptr(regions), A.ptr(read_len), A.ptr(seq4), A.ptr(qual), A.ptr(ref), A.ptr(alns), A.ptr(segs), A.ptr(ins),
-            used["seq4"], used["qual"], used["ref"], used["ins"], qual_bits, self.qual_dict, fmt,
-            A.ptr(exc_off) if exc_off is not None else None, A.ptr(exc) if exc is not None else None,
+            n_regions=self.n_regions, n_reads=self.n_reads, n_alns=self.n_alns, n_segs=self.n_segs,
+            regions=A.ptr(regions), read_len=A.ptr(read_len), seq4=A.ptr(seq4), qual=A.ptr(qual), ref=A.ptr(ref), alns=A.ptr(alns), segs=A.ptr(segs), ins=A.ptr(ins),
+            seq4_bytes=used["seq4"], qual_bytes=used["qual"], ref_bytes=used["ref"], ins_bytes=used["ins"], qual_bits=qual_bits, qual_dict=self.qual_dict, format=fmt,
+            exc_off=A.ptr(exc_off), exc=A.ptr(exc),
         )
 
     def cells(self) -> int:
@@ -392,9 +392,8 @@ class PileupBatch:
             self.t2_calls = np.zeros(1, np.uint16)
         self.n_sites = len(self.site_off) - 1
         assert len(self.ref_base) == self.n_sites
-        self.c = A.SxPileupBatch(
-            self.n_sites, A.ptr(self.site_off), A.ptr(self.calls), A.ptr(self.t2_off), A.ptr(self.t2_calls), A.ptr(self.ref_base), A.ptr(self.ploidy)
-        )
+        self.c = A.SxPileupBatch(n_sites=self.n_sites, site_off=A.ptr(self.site_off), calls=A.ptr(self.calls), t2_off=A.ptr(self.t2_off), t2_calls=A.ptr(self.t2_calls),
+                                 ref_base=A.ptr(self.ref_base), ploidy=A.ptr(self.ploidy))
 
     @property
     def n_calls(self) -> int:
@@ -424,7 +423,7 @@ class GaBatch:
         self.ref_off = np.zeros(self.n + 1, np.uint32)
         self.ref_off[1:] = np.cumsum([len(r) for r in refs])
         self.max_ops = max_ops
-        self.c = A.SxGaBatch(self.n, A.ptr(self.query), A.ptr(self.ref), A.ptr(self.query_off), A.ptr(self.ref_off), max_ops)
+        self.c = A.SxGaBatch(n=self.n, query=A.ptr(self.query), ref=A.ptr(self.ref), query_off=A.ptr(self.query_off), ref_off=A.ptr(self.ref_off), max_ops=max_ops)
 
     def cells(self) -> int:
         q = np.diff(self.query_off).astype(np.int64)
@@ -468,8 +467,9 @@ class IndelBatch:
         self.allele_lnp, self.read_length, self.non_ambig, self.is_fwd = pad(lnp, np.float32), pad(rl, np.uint16), pad(na, np.uint16), pad(fw, np.uint8)
         if self.ploidy.size == 0:
             self.ploidy = np.zeros(1, np.uint8)
-        self.c = A.SxIndelBatch(n, A.ptr(self.read_off), A.ptr(self.lnp_off), A.ptr(self.allele_off), A.ptr(self.ploidy), A.ptr(self.allele_del_len),
-                                A.ptr(self.allele_ins_len), A.ptr(self.allele_lnp), A.ptr(self.read_length), A.ptr(self.non_ambig), A.ptr(self.is_fwd))
+        self.c = A.SxIndelBatch(n_loci=n, read_off=A.ptr(self.read_off), lnp_off=A.ptr(self.lnp_off), allele_off=A.ptr(self.allele_off), ploidy=A.ptr(self.ploidy),
+                                allele_del_len=A.ptr(self.allele_del_len), allele_ins_len=A.ptr(self.allele_ins_len), allele_lnp=A.ptr(self.allele_lnp),
+                                read_length=A.ptr(self.read_length), non_ambig=A.ptr(self.non_ambig), is_fwd=A.ptr(self.is_fwd))
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -493,7 +493,8 @@ class SomaticIndelBatch:
         assert self.alt_off[-1] == self.alts.size and self.read_off[-1] == self.reads.size
         self._keep = [a if a.size else np.zeros(1, a.dtype) for a in (self.key, self.is_forced_output, self.err_idx, self.alts, self.reads)]
         k, f, e, al, rd = self._keep
-        self.c = A.SxSindelBatch(n, 0, A.ptr(k), A.ptr(f), A.ptr(e), A.ptr(self.alt_off), A.ptr(al), A.ptr(self.read_off), A.ptr(rd))
+        self.c = A.SxSindelBatch(n_loci=n, key=A.ptr(k), is_forced_output=A.ptr(f), err_idx=A.ptr(e), alt_off=A.ptr(self.alt_off), alts=A.ptr(al), read_off=A.ptr(self.read_off),
+                                 reads=A.ptr(rd))
 
     @staticmethod
     def from_loci(loci) -> "SomaticIndelBatch":
@@ -550,10 +551,9 @@ class IndelReadsSample:
         assert self.read_id is None or self.read_id.size >= n
         self._keep = [a if a.size else np.zeros(1, a.dtype) for a in (self.recs, self.n_rec, self.key_gid)]
         rc, nr, kg = self._keep
-        self.c = A.SxIndelReadsSample(self.n_regions, n, self.n_keys, 0, A.ptr(self.region_read_off), A.ptr(self.region_key_off), A.ptr(kg), A.ptr(self.rec_off),
-                                      A.ptr(rc), A.ptr(nr), A.ptr(self.read_len), A.ptr(self.non_ambig), A.ptr(self.read_flags), A.ptr(self.read_id))
-
-    ARRAYS = ("region_read_off", "region_key_off", "key_gid", "rec_off", "recs", "n_rec", "read_len", "non_ambig", "read_flags", "read_id")
+        self.c = A.SxIndelReadsSample(n_regions=self.n_regions, n_reads=n, n_keys=self.n_keys, region_read_off=A.ptr(self.region_read_off),
+                                      region_key_off=A.ptr(self.region_key_off), key_gid=A.ptr(kg), rec_off=A.ptr(self.rec_off), recs=A.ptr(rc), n_rec=A.ptr(nr),
+                                      read_len=A.ptr(self.read_len), non_ambig=A.ptr(self.non_ambig), read_flags=A.ptr(self.read_flags), read_id=A.ptr(self.read_id))
 
 
 class IndelLoci:
@@ -570,9 +570,8 @@ class IndelLoci:
         self.err_prob = np.ascontiguousarray(err_prob, np.float64)
         assert self.key.size == n and self.is_forced_output.size == n and self.err_idx.size == n
         self._keep = [a if a.size else np.zeros(1, a.dtype) for a in (self.gid, self.key, self.is_forced_output, self.err_idx, self.gid_key)]
-        self.c = A.SxIndelLoci(n, self.n_gid, *(A.ptr(a) for a in self._keep))
-
-    ARRAYS = ("gid", "key", "is_forced_output", "err_idx", "gid_key")
+        g, k, f, e, gk = self._keep
+        self.c = A.SxIndelLoci(n_loci=n, n_gid=self.n_gid, gid=A.ptr(g), key=A.ptr(k), is_forced_output=A.ptr(f), err_idx=A.ptr(e), gid_key=A.ptr(gk))
 
 
 class IndelReadsOut:
@@ -586,8 +585,8 @@ class IndelReadsOut:
         self.reads = np.zeros(max(1, cap_reads), A.SINDEL_READ_DT)
         self.status = np.zeros(max(1, n_loci), np.uint32)
         self.totals = np.zeros(2, np.uint32)
-        self.c = A.SxIndelReadsOut(A.ptr(self.alt_off), A.ptr(self.alts), A.ptr(self.read_off), A.ptr(self.reads), A.ptr(self.status), A.ptr(self.totals),
-                                   cap_alts, cap_reads)
+        self.c = A.SxIndelReadsOut(alt_off=A.ptr(self.alt_off), alts=A.ptr(self.alts), read_off=A.ptr(self.read_off), reads=A.ptr(self.reads), status=A.ptr(self.status),
+                                   totals=A.ptr(self.totals), cap_alts=cap_alts, cap_reads=cap_reads)
 
     def trimmed(self):
         """(alt_off, alts, read_off, reads, status, totals) without the unused capacity."""
@@ -703,8 +702,9 @@ class PileupReadsBatch:
         self.n_sites = report_end - report_begin
         self.opts = opts or A.default_pileup_opts()
         self.c = A.SxPileupReadsBatch(
-            len(reads), len(segs), A.ptr(self.reads), A.ptr(self.seq4), A.ptr(self.qual), A.ptr(self.segs), A.ptr(self.ref), ref_begin, len(ref),
-            report_begin, report_end, A.ptr(self.cand_snv), len(keys), span, int(hdr["len"].max(initial=1)), 0, self.opts,
+            n_reads=len(reads), n_segs=len(segs), reads=A.ptr(self.reads), seq4=A.ptr(self.seq4), qual=A.ptr(self.qual), segs=A.ptr(self.segs), ref=A.ptr(self.ref),
+            ref_begin=ref_begin, ref_len=len(ref), report_begin=report_begin, report_end=report_end, cand_snv=A.ptr(self.cand_snv), n_cand_snv=len(keys), max_ref_span=span,
+            max_read_len=int(hdr["len"].max(initial=1)), opts=self.opts,
         )
         self.buffer_pos = None
         if buffer_pos is not None:
@@ -724,7 +724,8 @@ class PileupColumns:
         self.site_off, self.t2_off = np.zeros(n + 1, np.uint32), np.zeros(n + 1, np.uint32)
         self.calls, self.t2_calls = np.zeros(cap, np.uint16), np.zeros(cap, np.uint16)
         self.n_spandel, self.n_submapped = np.zeros(n, np.uint32), np.zeros(n, np.uint32)
-        self.c = A.SxPileupColumns(A.ptr(self.site_off), A.ptr(self.calls), A.ptr(self.t2_off), A.ptr(self.t2_calls), A.ptr(self.n_spandel), A.ptr(self.n_submapped), cap, cap)
+        self.c = A.SxPileupColumns(site_off=A.ptr(self.site_off), calls=A.ptr(self.calls), t2_off=A.ptr(self.t2_off), t2_calls=A.ptr(self.t2_calls),
+                                   n_spandel=A.ptr(self.n_spandel), n_submapped=A.ptr(self.n_submapped), calls_capacity=cap, t2_capacity=cap)
 
     def trimmed(self):
         return (self.site_off, self.calls[: int(self.site_off[-1])], self.t2_off, self.t2_calls[: int(self.t2_off[-1])], self.n_spandel, self.n_submapped)
@@ -806,10 +807,14 @@ class ScoreIndelsBatch:
         self.ins_pool = np.frombuffer(bytes(ins_pool) + b"\0", dtype=np.uint8).copy()
         self.ins_off = u32(ins_off)
         self.opts = opts or A.default_score_indels_opts()
-        self.c = A.SxScoreIndelsBatch(
-            self.n_regions, self.n_reads, self.n_alns, self.n_keys, A.ptr(self.region_read_off), A.ptr(self.region_key_off), A.ptr(self.keys),
-            A.ptr(self.aln_off), A.ptr(self.aln_pos), A.ptr(self.aln_seg_off), A.ptr(self.segs), A.ptr(self.aln_key_off), A.ptr(self.aln_keys),
-            A.ptr(self.read_len), A.ptr(self.non_ambig), None, None, A.ptr(self.read_flags), A.ptr(self.rec_off), self.opts,
+        self.c = self._struct()
+
+    def _struct(self) -> A.SxScoreIndelsBatch:
+        return A.SxScoreIndelsBatch(
+            n_regions=self.n_regions, n_reads=self.n_reads, n_alns=self.n_alns, n_keys=self.n_keys, region_read_off=A.ptr(self.region_read_off),
+            region_key_off=A.ptr(self.region_key_off), keys=A.ptr(self.keys), aln_off=A.ptr(self.aln_off), aln_pos=A.ptr(self.aln_pos), aln_seg_off=A.ptr(self.aln_seg_off),
+            segs=A.ptr(self.segs), aln_key_off=A.ptr(self.aln_key_off), aln_keys=A.ptr(self.aln_keys), read_len=A.ptr(self.read_len), non_ambig=A.ptr(self.non_ambig),
+            read_flags=A.ptr(self.read_flags), rec_off=A.ptr(self.rec_off), opts=self.opts,
         )
 
     @classmethod
@@ -823,11 +828,7 @@ class ScoreIndelsBatch:
         self.n_segs, self.n_aln_keys, self.n_rec_slots = int(self.aln_seg_off[self.n_alns]), int(self.aln_key_off[self.n_alns]), int(self.rec_off[-1])
         self.ins_pool = self.ins_off = None
         self.opts = opts or A.default_score_indels_opts()
-        self.c = A.SxScoreIndelsBatch(
-            self.n_regions, self.n_reads, self.n_alns, self.n_keys, A.ptr(self.region_read_off), A.ptr(self.region_key_off), A.ptr(self.keys),
-            A.ptr(self.aln_off), A.ptr(self.aln_pos), A.ptr(self.aln_seg_off), A.ptr(self.segs), A.ptr(self.aln_key_off), A.ptr(self.aln_keys),
-            A.ptr(self.read_len), A.ptr(self.non_ambig), None, None, A.ptr(self.read_flags), A.ptr(self.rec_off), self.opts,
-        )
+        self.c = self._struct()
         return self
 
     def algorithmic_bytes(self) -> int:
@@ -843,7 +844,7 @@ class ScoreIndelsOut:
         self.n_rec = np.zeros(sb.n_reads + 1, np.uint32)
         self.max_aln = np.zeros(sb.n_reads + 1, np.uint32)
         self.eval_aln = np.zeros(sb.n_reads + 1, np.uint32)
-        self.c = A.SxScoreIndelsOut(A.ptr(self.recs), A.ptr(self.n_rec), A.ptr(self.max_aln), A.ptr(self.eval_aln))
+        self.c = A.SxScoreIndelsOut(recs=A.ptr(self.recs), n_rec=A.ptr(self.n_rec), max_aln=A.ptr(self.max_aln), eval_aln=A.ptr(self.eval_aln))
         self._sb = sb
 
     def compact(self):
@@ -1054,10 +1055,11 @@ class EnumBatch:
         self.read_pool = np.frombuffer(bytes(read_pool) + b"\0", dtype=np.uint8).copy()
         self.read_off = u32(read_off)
         self.c = A.SxEnumBatch(
-            self.n_regions, self.n_reads, self.n_keys, A.ptr(self.region_read_off), A.ptr(self.region_key_off), A.ptr(self.keys),
-            A.ptr(self.key_hap) if any_hap else None, A.ptr(self.realign_begin), A.ptr(self.realign_end), A.ptr(self.in_pos), A.ptr(self.in_seg_off),
-            A.ptr(self.in_segs), A.ptr(self.in_key_off), A.ptr(self.in_keys), A.ptr(self.use_key_off), A.ptr(self.use_keys), A.ptr(self.in_lead_key),
-            A.ptr(self.in_trail_key), A.ptr(self.read_len), None, self.opts,
+            n_regions=self.n_regions, n_reads=self.n_reads, n_keys=self.n_keys, region_read_off=A.ptr(self.region_read_off), region_key_off=A.ptr(self.region_key_off),
+            keys=A.ptr(self.keys), key_hap=A.ptr(self.key_hap) if any_hap else None, realign_begin=A.ptr(self.realign_begin), realign_end=A.ptr(self.realign_end),
+            in_pos=A.ptr(self.in_pos), in_seg_off=A.ptr(self.in_seg_off), in_segs=A.ptr(self.in_segs), in_key_off=A.ptr(self.in_key_off), in_keys=A.ptr(self.in_keys),
+            use_key_off=A.ptr(self.use_key_off), use_keys=A.ptr(self.use_keys), in_lead_key=A.ptr(self.in_lead_key), in_trail_key=A.ptr(self.in_trail_key),
+            read_len=A.ptr(self.read_len), opts=self.opts,
         )
 
     def set_gate(self, gate: Optional[np.ndarray]):
@@ -1090,9 +1092,9 @@ class EnumOut:
         self.aln_keys = np.zeros(self.cap_keys + 1, np.uint16)
         self.aln_lead_key = np.zeros(self.cap_alns + 1, np.uint16)
         self.aln_trail_key = np.zeros(self.cap_alns + 1, np.uint16)
-        self.c = A.SxEnumOut(self.cap_alns, self.cap_segs, self.cap_keys, A.ptr(self.totals), A.ptr(self.aln_off), A.ptr(self.status), A.ptr(self.aln_pos),
-                             A.ptr(self.aln_seg_off), A.ptr(self.segs), A.ptr(self.aln_key_off), A.ptr(self.aln_keys), A.ptr(self.aln_lead_key),
-                             A.ptr(self.aln_trail_key))
+        self.c = A.SxEnumOut(cap_alns=self.cap_alns, cap_segs=self.cap_segs, cap_keys=self.cap_keys, totals=A.ptr(self.totals), aln_off=A.ptr(self.aln_off),
+                             status=A.ptr(self.status), aln_pos=A.ptr(self.aln_pos), aln_seg_off=A.ptr(self.aln_seg_off), segs=A.ptr(self.segs),
+                             aln_key_off=A.ptr(self.aln_key_off), aln_keys=A.ptr(self.aln_keys), aln_lead_key=A.ptr(self.aln_lead_key), aln_trail_key=A.ptr(self.aln_trail_key))
         self._n_reads = eb.n_reads
 
     def trimmed(self):
@@ -1127,8 +1129,8 @@ class LinkOut:
         self.segs["kind"][:] = A.SX_SEG_HARDCLIP
         self.ins = np.zeros(self.cap_ins + A.SX_POOL_SLACK + 16, np.uint8)
         self.k6_segs = np.zeros(n_enum_segs + 16, dtype=A.ALN_SEG_DT) if n_enum_segs else None  # K7's segments with K6's kinds
-        self.c = A.SxLinkOut(self.cap_segs, self.cap_ins, A.ptr(self.totals), A.ptr(self.regions), A.ptr(self.alns), A.ptr(self.segs), A.ptr(self.ins),
-                             A.ptr(self.k6_segs) if n_enum_segs else None)
+        self.c = A.SxLinkOut(cap_segs=self.cap_segs, cap_ins=self.cap_ins, totals=A.ptr(self.totals), regions=A.ptr(self.regions), alns=A.ptr(self.alns),
+                             segs=A.ptr(self.segs), ins=A.ptr(self.ins), k6_segs=A.ptr(self.k6_segs))
 
     def align_batch(self, reads_of: "AlignBatch") -> "AlignBatch":
         """the K1 batch made of `reads_of`'s read / quality / reference pools and the linked alignments."""
@@ -1178,7 +1180,8 @@ class PrepOut:
         self.in_keys = np.zeros(self.cap_keys + 1, np.uint16)
         self.in_lead_key = np.zeros(eb.n_reads + 1, np.uint16)
         self.in_trail_key = np.zeros(eb.n_reads + 1, np.uint16)
-        self.c = A.SxPrepOut(self.cap_keys, A.ptr(self.totals), A.ptr(self.in_key_off), A.ptr(self.in_keys), A.ptr(self.in_lead_key), A.ptr(self.in_trail_key))
+        self.c = A.SxPrepOut(cap_keys=self.cap_keys, totals=A.ptr(self.totals), in_key_off=A.ptr(self.in_key_off), in_keys=A.ptr(self.in_keys),
+                             in_lead_key=A.ptr(self.in_lead_key), in_trail_key=A.ptr(self.in_trail_key))
         self._n = eb.n_reads
 
     def trimmed(self):
@@ -1209,9 +1212,11 @@ class RealignBatch:
         self.n_alns = int(out.totals[0])
         self.pin_flags = pin_flags
         self.raw = raw  # the mapper's alignments: with them the output is getBestAlignment() of every read
-        self.c = A.SxRealignBatch(eb.n_regions, eb.n_reads, self.n_alns, A.ptr(eb.region_read_off), A.ptr(eb.region_key_off), A.ptr(eb.keys), A.ptr(out.aln_off),
-                                  A.ptr(out.aln_pos), A.ptr(out.aln_seg_off), A.ptr(out.segs), A.ptr(out.aln_key_off), A.ptr(out.aln_keys), A.ptr(eb.read_len),
-                                  A.ptr(pin_flags) if pin_flags is not None else None, 1 if is_smoothed else 0, 1 if k4_kinds else 0, smoothed_lnp_range)
+        self.c = A.SxRealignBatch(n_regions=eb.n_regions, n_reads=eb.n_reads, n_alns=self.n_alns, region_read_off=A.ptr(eb.region_read_off),
+                                  region_key_off=A.ptr(eb.region_key_off), keys=A.ptr(eb.keys), aln_off=A.ptr(out.aln_off), aln_pos=A.ptr(out.aln_pos),
+                                  aln_seg_off=A.ptr(out.aln_seg_off), segs=A.ptr(out.segs), aln_key_off=A.ptr(out.aln_key_off), aln_keys=A.ptr(out.aln_keys),
+                                  read_len=A.ptr(eb.read_len), pin_flags=A.ptr(pin_flags), is_smoothed_alignments=1 if is_smoothed else 0, k4_kinds=1 if k4_kinds else 0,
+                                  smoothed_lnp_range=smoothed_lnp_range)
         if raw is not None:
             self.c.raw_pos, self.c.raw_seg_off, self.c.raw_segs = A.ptr(raw.raw_pos), A.ptr(raw.seg_off), A.ptr(raw.raw_segs)
 
@@ -1230,8 +1235,8 @@ class RealignOut:
         self.status = np.zeros(n + 1, np.uint8)
         self.best_aln = np.zeros(n + 1, np.uint32)
         self.segs = np.zeros(self.cap_segs + 1, dtype=A.ALN_SEG_DT)
-        self.c = A.SxRealignOut(self.cap_segs, A.ptr(self.totals), A.ptr(self.seg_off), A.ptr(self.pos), A.ptr(self.n_seg), A.ptr(self.status), A.ptr(self.best_aln),
-                                A.ptr(self.segs))
+        self.c = A.SxRealignOut(cap_segs=self.cap_segs, totals=A.ptr(self.totals), seg_off=A.ptr(self.seg_off), pos=A.ptr(self.pos), n_seg=A.ptr(self.n_seg),
+                                status=A.ptr(self.status), best_aln=A.ptr(self.best_aln), segs=A.ptr(self.segs))
         self._n = n
 
     def realignment_of(self, r: int):
@@ -1264,9 +1269,9 @@ class GateBatch:
             self.raw_segs[: len(segs)] = np.array(segs, dtype=A.ALN_SEG_DT)
         self.n_segs = len(segs)
         self.pin_flags = pin_flags
-        self.c = A.SxGateBatch(eb.n_regions, eb.n_reads, A.ptr(eb.region_read_off), A.ptr(eb.region_key_off), A.ptr(eb.keys), A.ptr(eb.realign_begin),
-                               A.ptr(eb.realign_end), A.ptr(self.raw_pos), A.ptr(self.seg_off), A.ptr(self.raw_segs), A.ptr(eb.read_len),
-                               A.ptr(pin_flags) if pin_flags is not None else None, max_indel_size)
+        self.c = A.SxGateBatch(n_regions=eb.n_regions, n_reads=eb.n_reads, region_read_off=A.ptr(eb.region_read_off), region_key_off=A.ptr(eb.region_key_off),
+                               keys=A.ptr(eb.keys), realign_begin=A.ptr(eb.realign_begin), realign_end=A.ptr(eb.realign_end), raw_pos=A.ptr(self.raw_pos),
+                               seg_off=A.ptr(self.seg_off), raw_segs=A.ptr(self.raw_segs), read_len=A.ptr(eb.read_len), pin_flags=A.ptr(pin_flags), max_indel_size=max_indel_size)
 
 
 class GateOut:
@@ -1275,7 +1280,7 @@ class GateOut:
         self.gate = np.zeros(n + 1, np.uint8)
         self.in_pos = np.zeros(n + 1, np.int32)
         self.in_segs = np.zeros(gb.n_segs + 4, dtype=A.ALN_SEG_DT)
-        self.c = A.SxGateOut(A.ptr(self.gate), A.ptr(self.in_pos), A.ptr(self.in_segs))
+        self.c = A.SxGateOut(gate=A.ptr(self.gate), in_pos=A.ptr(self.in_pos), in_segs=A.ptr(self.in_segs))
         self._gb = gb
 
     def alignment_of(self, r: int):

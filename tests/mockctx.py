@@ -42,6 +42,10 @@ class _MockLib:
         C.memmove(dst, src, n)
         return 0
 
+    # ---- host-only entries
+    def sx_default_window_opts(self, batch):
+        A.load().sx_default_window_opts(batch)
+
     # ---- kernels
     def sx_alignment_indels_dev(self, h, batch, regions, seq4, ref, kio, ki, out):
         return reflib._k7acore.k7acore_run(batch, regions, seq4, ref, kio, ki, out)
