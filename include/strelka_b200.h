@@ -1145,6 +1145,82 @@ int sx_process_window(sx_ctx* ctx, const sx_window_batch* batch_host, sx_window_
 int sx_last_window_timing(const sx_ctx* ctx, float* ms);
 
 /* ==========================================================================================
+ * process_somatic_window   (strelka2's per-position path for a window of positions: the normal and the tumor sample through process_window's
+ *   chain, then the somatic SNV and indel models, every intermediate in device memory)
+ *   replaces  align_pos + pileup_pos_reads of each sample   as sx_process_window_dev, per sample
+ *             position_somatic_snv_call per position        applications/strelka/strelka_pos_processor.cpp:181-219
+ *             process_pos_indel_somatic's calls              :305-348 (get_somatic_indel on the two samples' read_path_lnp)
+ *   as  normal chain -> tumor chain -> K2b -> SNV records -> K6b link -> K5b -> indel records, on the compute stream.
+ *
+ * Each sample is a complete window description (its own regions, reads, window entries and pools) and goes through exactly the chain of
+ *   sx_process_window_dev, with the same per-read reporting (gates, SX_ENUM_ST_*, SX_REALIGN_ST_*) into sample[s] of the output.  Both batches
+ *   must have do_site_gl = 0 (strelka2 runs no germline site model), the same ref_begin, report_begin and report_end, and the same
+ *   pileup_opts.useTier2Evidence, equal to sindel_opts.useTier2Evidence; out.sample[s].site_gl / variant_sites must be NULL.  Anything else
+ *   is SX_ERR_ARG.
+ * K2b runs at every position of [report_begin, report_end) on the two samples' tier1 columns, and on their tier2 columns when
+ *   useTier2Evidence is set (strelka_pos_processor.cpp:181-219), with ref_base from the normal sample's reference segment and
+ *   snv_forced_output (is_forced_output_pos) when given.
+ * The SNV records are the positions where somatic_snv_genotype_grid::is_output() (somatic_result_set.hh:62-71): QSS != 0, or forced output at a
+ *   position whose reference base is not 'N' (position_somatic_snv_strand_grid.cpp:242-246 clears the flag there), in ascending position.
+ * The link (K6b) and K5b run on the two samples' K6 records, read lengths, SX_PRF_TIER1 flags and 'N'-free base counts where the passes left
+ *   them, with key_gid / read_id as sx_indel_reads_sample's.  indel[l] is sx_somatic_indel_from_records_dev's result of locus l.
+ * An indel record is written, in ascending locus index, for every locus that
+ *   - has a link status (SX_SINDEL_ST_CAP / SX_INDEL_READS_ST_DUP_READ): the caller's CPU path calls these; or
+ *   - is forced output, or has QSI != 0 (somatic_indel_call::is_output(), somatic_result_set.hh:86-96) and a non-empty read_path_lnp in at least
+ *     one sample: process_pos_indel_somatic skips an unforced candidate whose two lists are empty (strelka_pos_processor.cpp:324-327).
+ * The choice of loci and the other candidate filters stay with the caller (breakpoints, mismatches, isCandidateIndel, vcf_indel_seq ==
+ *   vcf_ref_seq, the window-edge contract: INTEGRATION section 4h).
+ * A record array shorter than its records gives SX_ERR_CAPACITY after the whole pass, with as many records as fit written and totals saying
+ *   how many there are.  An array of out.sample[s] that is too small gives SX_ERR_CAPACITY from that sample's pass, with the pass's
+ *   totals in out.sample[s].totals (when given), as sx_process_window_dev's totals_host.  Either record array may be NULL (no records are made); site_snv / indel may be NULL (the context keeps them).
+ * ======================================================================================== */
+typedef struct sx_somatic_window_batch {   /* the struct is host memory; its arrays are device memory except err_prob */
+    sx_window_batch sample[2];             /* [0] normal, [1] tumor */
+    const uint32_t* key_gid[2];            /* [sample[s].n_keys] batch-wide id of each window entry (sx_indel_reads_sample.key_gid) */
+    const uint32_t* read_id[2];            /* [sample[s].n_reads] rseg.getReadIndex(), or NULL: the read's index in its batch */
+    const uint8_t* snv_forced_output;      /* [report_end - report_begin] is_forced_output_pos, or NULL (none) */
+    sx_indel_loci loci;                    /* the candidates to call, as for sx_somatic_indel_from_records_dev */
+    sx_sindel_opts sindel_opts;
+    const double* err_prob;                /* HOST memory: [n_err] the distinct indelToRefErrorProb values, as sx_somatic_indel_dev */
+    uint32_t n_err;
+    uint32_t pad;
+} sx_somatic_window_batch;
+
+typedef struct sx_somatic_site_call {      /* one SNV record */
+    int32_t pos;
+    uint32_t n_calls[2];                   /* depth of the position's tier1 column: normal, tumor */
+    uint32_t pad;
+    sx_ssnv_result r;
+} sx_somatic_site_call;
+
+typedef struct sx_somatic_indel_call {     /* one indel record */
+    uint32_t locus;                        /* index into loci */
+    uint32_t pad;
+    sx_sindel_result r;
+} sx_somatic_indel_call;
+
+#define SX_SWIN_TOTALS 4 /* SNV records, indel records, linked read entries, linked alternates */
+
+typedef struct sx_somatic_window_out {     /* device pointers, each may be NULL (capacities count only for non-NULL arrays) */
+    sx_window_out sample[2];               /* per-sample outputs as sx_process_window_dev writes them (site_gl and variant_sites NULL) */
+    sx_ssnv_result* site_snv;              /* [report_end - report_begin] */
+    sx_somatic_site_call* snv_calls;       /* [cap_snv_calls] */
+    sx_sindel_result* indel;               /* [loci.n_loci] */
+    sx_somatic_indel_call* indel_calls;    /* [cap_indel_calls] */
+    uint32_t* totals;                      /* [SX_SWIN_TOTALS] */
+    uint32_t cap_snv_calls, cap_indel_calls;
+} sx_somatic_window_out;
+
+enum { SX_SWIN_ST_NORMAL = 0, SX_SWIN_ST_TUMOR, SX_SWIN_ST_SITE_SNV, SX_SWIN_ST_SNV_CALLS, SX_SWIN_ST_LINK, SX_SWIN_ST_INDEL, SX_SWIN_ST_INDEL_CALLS,
+       SX_SWIN_N_STAGES };
+
+int sx_process_somatic_window_dev(sx_ctx* ctx, const sx_somatic_window_batch* batch_dev, sx_somatic_window_out* out_dev,
+                                  uint32_t* totals_host /* [SX_SWIN_TOTALS] or NULL */);
+/* device time of each stage of the most recent sx_process_somatic_window_dev on ctx (CUDA events on the compute stream), ms[SX_SWIN_N_STAGES];
+ * sx_last_window_timing then reports the tumor sample's pass */
+int sx_last_somatic_window_timing(const sx_ctx* ctx, float* ms);
+
+/* ==========================================================================================
  * Multi-GPU: regions shard across ranks with no data-path collective; one gather of fixed-size
  * call records at the end (the in-memory analogue of concatIndexVcf,
  * src/python/lib/strelkaSharedWorkflow.py:126-136).  The NCCL communicator is created from an

@@ -346,6 +346,25 @@ SX_WIN_TOTALS, SX_WIN_N_STAGES = 10, 10
 SX_WIN_STAGE_NAMES = ("prep", "k7g_gates", "k7a_keys", "k7_enumerate", "k7b_link", "k1_score", "k6_score_indels", "k9_choose", "k4_pileup", "k2a_site_gl")
 
 
+# somatic window pass
+SOMATIC_SITE_CALL_DT = np.dtype([("pos", "<i4"), ("n_calls", "<u4", (2,)), ("pad", "<u4"), ("r", SSNV_RESULT_DT)])  # sx_somatic_site_call, 304 bytes
+SOMATIC_INDEL_CALL_DT = np.dtype([("locus", "<u4"), ("pad", "<u4"), ("r", SINDEL_RESULT_DT)])  # sx_somatic_indel_call, 408 bytes
+
+
+class SxSomaticWindowBatch(C.Structure):
+    _fields_ = [("sample", SxWindowBatch * 2), ("key_gid", C.c_void_p * 2), ("read_id", C.c_void_p * 2), ("snv_forced_output", C.c_void_p), ("loci", SxIndelLoci),
+                ("sindel_opts", SxSindelOpts), ("err_prob", C.c_void_p), ("n_err", C.c_uint32), ("pad", C.c_uint32)]
+
+
+class SxSomaticWindowOut(C.Structure):
+    _fields_ = [("sample", SxWindowOut * 2)] + [(n, C.c_void_p) for n in ("site_snv", "snv_calls", "indel", "indel_calls", "totals")] + [
+        ("cap_snv_calls", C.c_uint32), ("cap_indel_calls", C.c_uint32)]
+
+
+SX_SWIN_TOTALS, SX_SWIN_N_STAGES = 4, 7
+SX_SWIN_STAGE_NAMES = ("normal", "tumor", "k2b_site_snv", "snv_calls", "k6b_link", "k5b_indel", "indel_calls")
+
+
 class SxGateOut(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("gate", "in_pos", "in_segs")]
 
@@ -450,6 +469,8 @@ SYMBOLS = [
     ("sx_process_window_dev", C.c_int, [_P, C.POINTER(SxWindowBatch), C.POINTER(SxWindowOut), _P]),
     ("sx_process_window", C.c_int, [_P, C.POINTER(SxWindowBatch), C.POINTER(SxWindowOut), _P]),
     ("sx_last_window_timing", C.c_int, [_P, _P]),
+    ("sx_process_somatic_window_dev", C.c_int, [_P, C.POINTER(SxSomaticWindowBatch), C.POINTER(SxSomaticWindowOut), _P]),
+    ("sx_last_somatic_window_timing", C.c_int, [_P, _P]),
     ("sx_comm_get_unique_id", C.c_int, [_P]),
     ("sx_comm_init", C.c_int, [_P, _P, C.c_int, C.c_int]),
     ("sx_gather_records", C.c_int, [_P, _P, C.c_size_t, _P, C.c_int]),

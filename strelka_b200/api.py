@@ -367,8 +367,8 @@ class DevScoreIndelsBatch:
 
 class DevIndelReadsSample:
     """sx_indel_reads_sample in HBM.  `from_score_indels` adopts a DevScoreIndelsBatch: its read arrays and the recs / n_rec arrays K6
-    wrote, which that object owns -- so two samples scored on ONE context stay apart.  A constructor from two DevWindow passes is not
-    built (DESIGN section 8)."""
+    wrote, which that object owns -- so two samples scored on ONE context stay apart.  `from_window` does the same with a DevWindow's
+    pass."""
 
     def __init__(self, ctx: "Context", hs: B.IndelReadsSample, adopt: Optional[dict] = None):
         self.host = hs
@@ -382,6 +382,22 @@ class DevIndelReadsSample:
         adopt.update(recs=db.recs.ptr, n_rec=db.n_rec.ptr)
         self = DevIndelReadsSample(ctx, hs, adopt)
         self.score = db  # (keeps the adopted buffers alive)
+        return self
+
+    @staticmethod
+    def from_window(ctx: "Context", dw: "DevWindow", key_gid, read_id, non_ambig) -> "DevIndelReadsSample":
+        """The sample of a DevWindow pass (keep_outputs): the window's read arrays and the recs / n_rec its pass wrote, adopted; key_gid,
+        read_id and `non_ambig` (each read's count of bases that are not 'N', uint16) uploaded."""
+        w = dw.w
+        n = w.n_reads
+        assert len(non_ambig) >= n
+        sb = SimpleNamespace(n_regions=w.n_regions, n_reads=n, n_keys=w.n_keys, non_ambig=np.ascontiguousarray(non_ambig, np.uint16),
+                             **{k: w.a[k] for k in ("region_read_off", "region_key_off", "rec_off", "read_len", "read_flags")})
+        hs = B.IndelReadsSample(sb, np.zeros(dw.n_slots + 1, A.READ_INDEL_SCORE_DT), np.zeros(n + 1, np.uint32), key_gid, read_id)
+        adopt = {k: dw.bufs[k].ptr for k in ("region_read_off", "region_key_off", "rec_off", "read_len", "read_flags")}
+        adopt.update(recs=dw.obufs["recs"].ptr, n_rec=dw.obufs["n_rec"].ptr)
+        self = DevIndelReadsSample(ctx, hs, adopt)
+        self.window = dw  # (keeps the adopted buffers alive)
         return self
 
 
@@ -648,4 +664,78 @@ class DevWindow:
 
     def free(self):
         for x in list(self.bufs.values()) + list(self.obufs.values()):
+            x.free()
+
+
+class DevSomaticWindow:
+    """sx_process_somatic_window_dev on two B.WindowBatch samples (normal, tumor) of one window of positions and the candidate loci: every
+    input resident in HBM, every output allocated here.  The samples' per-read and column outputs are DevWindow's (`normal` / `tumor`).
+    useTier2Evidence of the pile-up and of K5b is `use_tier2`.  records_only: only the two record lists and the totals come out; every other
+    output (the samples', site_snv, indel) is left NULL, so the pass keeps it in the context's own buffers."""
+
+    def __init__(self, ctx: "Context", normal: "B.WindowBatch", tumor: "B.WindowBatch", loci: "B.IndelLoci", key_gid, read_id=None, snv_forced=None,
+                 use_tier2: bool = False, opts: Optional[A.SxSindelOpts] = None, cap_snv_calls=None, cap_indel_calls=None, records_only: bool = False):
+        assert not normal.do_site_gl and not tumor.do_site_gl, "strelka2 runs no germline site model: build the samples with do_site_gl=False"
+        self.ctx, self.loci = ctx, loci
+        self.records_only = records_only
+        self.windows = [DevWindow(ctx, w, keep_outputs=not records_only) for w in (normal, tumor)]
+        self.normal, self.tumor = self.windows
+        self.n_sites, n_loci = normal.n_sites, loci.n_loci
+        self.opts = A.SxSindelOpts.from_buffer_copy(opts) if opts is not None else A.default_sindel_opts()
+        self.opts.useTier2Evidence = int(use_tier2)
+        for dw in self.windows:
+            dw.c.pileup_opts.useTier2Evidence = int(use_tier2)
+            dw.out.site_gl = dw.out.variant_sites = None
+            dw.out.cap_variant_sites = 0
+        self.dloci = DevIndelLoci(ctx, loci)
+        up = lambda a, dt: None if a is None else DeviceArray(ctx, np.ascontiguousarray(a, dt).nbytes + 64).upload(np.ascontiguousarray(a, dt))
+        self.inbufs = {"key_gid": [up(k, np.uint32) for k in key_gid], "read_id": [up(r, np.uint32) for r in (read_id or (None, None))],
+                       "snv_forced": up(snv_forced, np.uint8)}
+        self.err_prob = np.ascontiguousarray(loci.err_prob, np.float64)
+        ib = self.inbufs
+        self.c = A.SxSomaticWindowBatch(sample=(A.SxWindowBatch * 2)(*(dw.c for dw in self.windows)),
+                                        key_gid=(C.c_void_p * 2)(*(x.ptr if x else None for x in ib["key_gid"])),
+                                        read_id=(C.c_void_p * 2)(*(x.ptr if x else None for x in ib["read_id"])),
+                                        snv_forced_output=ib["snv_forced"].ptr if ib["snv_forced"] else None, loci=self.dloci.c, sindel_opts=self.opts,
+                                        err_prob=A.ptr(self.err_prob), n_err=self.err_prob.size)
+        self.cap_snv = max(1, self.n_sites) if cap_snv_calls is None else cap_snv_calls
+        self.cap_indel = max(1, n_loci) if cap_indel_calls is None else cap_indel_calls
+        self.obufs = {"site_snv": DeviceArray(ctx, (self.n_sites + 1) * A.SSNV_RESULT_DT.itemsize),
+                      "snv_calls": DeviceArray(ctx, (self.cap_snv + 1) * A.SOMATIC_SITE_CALL_DT.itemsize),
+                      "indel": DeviceArray(ctx, (n_loci + 1) * A.SINDEL_RESULT_DT.itemsize),
+                      "indel_calls": DeviceArray(ctx, (self.cap_indel + 1) * A.SOMATIC_INDEL_CALL_DT.itemsize), "totals": DeviceArray(ctx, 64)}
+        if records_only:
+            for k in ("site_snv", "indel"):
+                self.obufs.pop(k).free()
+        samples = (A.SxWindowOut * 2)() if records_only else (A.SxWindowOut * 2)(*(dw.out for dw in self.windows))
+        self.out = A.SxSomaticWindowOut(sample=samples, cap_snv_calls=self.cap_snv, cap_indel_calls=self.cap_indel, **{k: b.ptr for k, b in self.obufs.items()})
+        self.totals = np.zeros(A.SX_SWIN_TOTALS, np.uint32)
+
+    def run(self):
+        """one pass; returns the per-stage device times (ms).  SX_ERR_CAPACITY leaves the totals in the SxError's `totals`."""
+        ctx = self.ctx
+        rc = ctx.lib.sx_process_somatic_window_dev(ctx.h, C.byref(self.c), C.byref(self.out), self.totals.ctypes.data)
+        ctx._chk_totals(rc, self.totals)
+        ms = np.zeros(A.SX_SWIN_N_STAGES, np.float32)
+        ctx.lib.sx_last_somatic_window_timing(ctx.h, ms.ctypes.data)
+        return dict(zip(A.SX_SWIN_STAGE_NAMES, (float(x) for x in ms)))
+
+    def download(self):
+        """dict: each sample's DevWindow.download(), the per-position and per-locus results, the two record lists and the totals (records_only:
+        the record lists and the totals)"""
+        b, t = self.obufs, self.totals
+        records = {"snv_calls": b["snv_calls"].download(A.SOMATIC_SITE_CALL_DT, min(int(t[0]), self.cap_snv)),
+                   "indel_calls": b["indel_calls"].download(A.SOMATIC_INDEL_CALL_DT, min(int(t[1]), self.cap_indel)), "totals": t.copy()}
+        if self.records_only:
+            return records
+        for dw in self.windows:  # (each sample's totals are where the pass wrote them)
+            dw.totals[:] = dw.obufs["totals"].download(np.uint32, A.SX_WIN_TOTALS)
+        return {"normal": self.normal.download(), "tumor": self.tumor.download(), "site_snv": b["site_snv"].download(A.SSNV_RESULT_DT, self.n_sites),
+                "indel": b["indel"].download(A.SINDEL_RESULT_DT, self.loci.n_loci), **records}
+
+    def free(self):
+        for dw in self.windows:
+            dw.free()
+        bufs = list(self.obufs.values()) + list(self.dloci.bufs.values()) + [x for x in self.inbufs["key_gid"] + self.inbufs["read_id"] + [self.inbufs["snv_forced"]] if x]
+        for x in bufs:
             x.free()

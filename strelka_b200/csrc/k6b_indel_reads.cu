@@ -214,11 +214,7 @@ int k6b_check(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* normal
 {
     int rc;
     if ((rc = k6b_check_sample(ctx, what, normal)) || (rc = k6b_check_sample(ctx, what, tumor))) return rc;
-    if (!loci) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL argument", what);
-    if (loci->n_loci && (!loci->gid || !loci->key || !loci->is_forced_output || !loci->err_idx || !loci->gid_key || loci->n_gid == 0))
-        return sx_fail(ctx, SX_ERR_ARG, "%s: NULL loci array", what);
-    if (loci->n_loci > 0x7fffffffu) return sx_fail(ctx, SX_ERR_RANGE, "%s: more than 2^31 - 1 loci", what);
-    return SX_OK;
+    return sx_k6b_check_loci(ctx, what, loci);
 }
 
 int k6b_check_out(sx_ctx* ctx, const char* what, const sx_indel_reads_out* o)
@@ -228,6 +224,15 @@ int k6b_check_out(sx_ctx* ctx, const char* what, const sx_indel_reads_out* o)
 }
 
 } // namespace
+
+int sx_k6b_check_loci(sx_ctx* ctx, const char* what, const sx_indel_loci* loci)
+{
+    if (!loci) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL argument", what);
+    if (loci->n_loci && (!loci->gid || !loci->key || !loci->is_forced_output || !loci->err_idx || !loci->gid_key || loci->n_gid == 0))
+        return sx_fail(ctx, SX_ERR_ARG, "%s: NULL loci array", what);
+    if (loci->n_loci > 0x7fffffffu) return sx_fail(ctx, SX_ERR_RANGE, "%s: more than 2^31 - 1 loci", what);
+    return SX_OK;
+}
 
 // The stage's launcher, beside its kernels like sx_k6_run: everything is enqueued on the compute stream, with two small round trips (the
 // pair total, then the output totals).  own_out: the entry and table arrays are taken from the context's SX_SLOT_K6B_OUT_* buffers once
@@ -425,6 +430,34 @@ extern "C" int sx_link_indel_reads(sx_ctx* ctx, const sx_indel_reads_sample* nor
     return rc_run;
 }
 
+int sx_k6b_own_out(sx_ctx* ctx, const uint32_t n_loci, sx_indel_reads_out* o)
+{
+    *o = sx_indel_reads_out{};
+    int rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K6B_OUT_ALT_OFF, (size_t)n_loci + 1, o->alt_off, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K6B_OUT_READ_OFF, 2 * (size_t)n_loci + 1, o->read_off, 16))) return rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K6B_OUT_STATUS, n_loci, o->status, 16))) return rc;
+    return sx_take(ctx, SX_SLOT_K6B_OUT_TOTALS, 2, o->totals, 16);
+}
+
+sx_sindel_batch sx_sindel_batch_of(const sx_indel_loci* loci, const sx_indel_reads_out* o)
+{
+    return sx_sindel_batch{loci->n_loci, 0, loci->key, loci->is_forced_output, loci->err_idx, o->alt_off, o->alts, o->read_off, o->reads};
+}
+
+int sx_sindel_from_links_run(sx_ctx* ctx, const sx_sindel_opts* opts, const sx_indel_loci* loci, const sx_indel_reads_out* o, const double* err_prob, const uint32_t n_err,
+                             sx_sindel_result* out_dev, unsigned* launches)
+{
+    int rc;
+    const sx_sindel_batch b(sx_sindel_batch_of(loci, o));
+    if ((rc = sx_k5b_run(ctx, opts, &b, err_prob, n_err, out_dev, launches))) return rc;
+    const uint32_t n_loci(loci->n_loci);
+    k6b_flag_results_kernel<<<std::max(1, std::min<int>((int)((n_loci + 255) / 256), ctx->sm_count * 16)), 256, 0, ctx->s_compute>>>(n_loci, o->status, out_dev);
+    SX_CUDA(ctx, cudaGetLastError());
+    *launches += 1;
+    return SX_OK;
+}
+
 extern "C" int sx_somatic_indel_from_records_dev(sx_ctx* ctx, const sx_sindel_opts* opts, const sx_indel_reads_sample* normal, const sx_indel_reads_sample* tumor,
                                                  const sx_indel_loci* loci, const double* err_prob_host, uint32_t n_err, sx_sindel_result* out_dev)
 {
@@ -436,26 +469,18 @@ extern "C" int sx_somatic_indel_from_records_dev(sx_ctx* ctx, const sx_sindel_op
     if (!opts || !out_dev) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL argument", what);
     if (loci->n_loci == 0) return SX_OK;
     SX_CUDA(ctx, cudaSetDevice(ctx->device));
-    const size_t n_loci(loci->n_loci);
-    sx_indel_reads_out o{};
-    if ((rc = sx_take(ctx, SX_SLOT_K6B_OUT_ALT_OFF, n_loci + 1, o.alt_off, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K6B_OUT_READ_OFF, 2 * n_loci + 1, o.read_off, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K6B_OUT_STATUS, n_loci, o.status, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K6B_OUT_TOTALS, 2, o.totals, 16))) return rc;
+    sx_indel_reads_out o;
+    if ((rc = sx_k6b_own_out(ctx, loci->n_loci, &o))) return rc;
     if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k6b_run(ctx, what, normal, tumor, loci, &o, nullptr, true, launches); }))) return rc;
     if ((rc = sx_check_status(ctx, what, SX_ST_K6B_ID))) return rc;
-    // K5b on the link's output: its checks and status word are reported as sx_somatic_indel_dev's, its time and launches added to the link's
+    // K5b and the flags on the link's output: its checks and status word are reported as sx_somatic_indel_dev's, its time and launches added to the link's
     const sx_timing link(ctx->timing);
     ctx->timing = sx_timing{};
-    const sx_sindel_batch b = {loci->n_loci, 0, loci->key, loci->is_forced_output, loci->err_idx, o.alt_off, o.alts, o.read_off, o.reads};
+    const sx_sindel_batch b(sx_sindel_batch_of(loci, &o));
     if ((rc = sx_k5b_check(ctx, "sx_somatic_indel_dev", opts, &b, err_prob_host, n_err, out_dev))) return rc;
-    if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k5b_run(ctx, opts, &b, err_prob_host, n_err, out_dev, launches); }))) return rc;
+    if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_sindel_from_links_run(ctx, opts, loci, &o, err_prob_host, n_err, out_dev, launches); }))) return rc;
     if ((rc = sx_check_status(ctx, "sx_somatic_indel_dev", SX_ST_SINDEL_ARG))) return rc;
-    k6b_flag_results_kernel<<<std::max(1, std::min<int>((int)((n_loci + 255) / 256), ctx->sm_count * 16)), 256, 0, ctx->s_compute>>>(loci->n_loci, o.status, out_dev);
-    SX_CUDA(ctx, cudaGetLastError());
-    SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
     ctx->timing.kernel_ms += link.kernel_ms;
-    ctx->timing.launches += link.launches + 1;
-    ctx->total_launches += 1;
+    ctx->timing.launches += link.launches;
     return SX_OK;
 }

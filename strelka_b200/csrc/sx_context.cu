@@ -468,6 +468,8 @@ extern "C" void sx_destroy(sx_ctx* ctx)
     for (auto ev : ctx->ev_pool) cudaEventDestroy(ev);
     for (auto& ev : ctx->ev_win)
         if (ev) cudaEventDestroy(ev);
+    for (auto& ev : ctx->ev_swin)
+        if (ev) cudaEventDestroy(ev);
     for (auto& ev : ctx->ev_user)
         if (ev) cudaEventDestroy(ev);
     if (ctx->ev_a) cudaEventDestroy(ctx->ev_a);

@@ -122,6 +122,10 @@ enum sx_slot : int
     SX_SLOT_WIN_BEST_SEGS, SX_SLOT_WIN_PILEUP_READS,
     SX_SLOT_WIN_SITE_OFF, SX_SLOT_WIN_T2_OFF, SX_SLOT_WIN_N_SPANDEL, SX_SLOT_WIN_N_SUBMAPPED, SX_SLOT_WIN_CALLS, SX_SLOT_WIN_T2_CALLS,
     SX_SLOT_WIN_SITE_GL, SX_SLOT_WIN_VARIANT_CHUNKS, SX_SLOT_WIN_VARIANT_SUMS,
+    // somatic window pass (sx_process_somatic_window_dev): the normal sample's results that the later stages read, kept apart from the
+    // tumor sample's pass (which uses the SX_SLOT_WIN_* buffers), and the somatic stages' own outputs and scratch
+    SX_SLOT_SWIN_NON_AMBIG, SX_SLOT_SWIN_RECS, SX_SLOT_SWIN_N_REC, SX_SLOT_SWIN_SITE_OFF, SX_SLOT_SWIN_T2_OFF, SX_SLOT_SWIN_CALLS, SX_SLOT_SWIN_T2_CALLS,
+    SX_SLOT_SWIN_SITE_SNV, SX_SLOT_SWIN_INDEL, SX_SLOT_SWIN_SNV_CHUNKS, SX_SLOT_SWIN_SNV_SUMS, SX_SLOT_SWIN_INDEL_CHUNKS, SX_SLOT_SWIN_INDEL_SUMS,
     // window pass: what sx_process_window uploads (the window batch's arrays) and the outputs it downloads
     SX_SLOT_WUP_REGION_READ_OFF, SX_SLOT_WUP_REGION_KEY_OFF, SX_SLOT_WUP_KEYS, SX_SLOT_WUP_KEY_HAP, SX_SLOT_WUP_KEY_INS_OFF, SX_SLOT_WUP_KEY_INS,
     SX_SLOT_WUP_REALIGN_BEGIN, SX_SLOT_WUP_REALIGN_END, SX_SLOT_WUP_RAW_POS, SX_SLOT_WUP_RAW_SEG_OFF, SX_SLOT_WUP_RAW_SEGS, SX_SLOT_WUP_READ_LEN,
@@ -199,6 +203,8 @@ struct sx_ctx
     cudaEvent_t ev_user[2] = {};     // sx_timer_mark
     cudaEvent_t ev_win[16] = {};     // stage boundaries of sx_process_window_dev (created on first use)
     float win_ms[16] = {};
+    cudaEvent_t ev_swin[16] = {};    // stage boundaries of sx_process_somatic_window_dev (created on first use)
+    float swin_ms[16] = {};
     cudaStream_t s_comm = nullptr;   // the gather's own stream (created by sx_comm_init)
     cudaEvent_t ev_comm = nullptr;   // compute -> comm ordering
     std::vector<unsigned long long> comm_counts; // per-rank byte counts of the last gather (root: receive offsets)
@@ -342,6 +348,17 @@ int sx_k5b_check(sx_ctx* ctx, const char* what, const sx_sindel_opts* o, const s
 int sx_k6_run(sx_ctx* ctx, const sx_score_indels_batch* d, const double* lnp_dev, const sx_score_indels_out* out_dev, unsigned* launches);
 int sx_k6b_run(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* normal, const sx_indel_reads_sample* tumor, const sx_indel_loci* loci, sx_indel_reads_out* out_dev,
                uint32_t* totals_host, bool own_out, unsigned* launches);
+// K6b's argument checks of the loci, reported under `what`
+int sx_k6b_check_loci(sx_ctx* ctx, const char* what, const sx_indel_loci* loci);
+// The link's offset, status and totals arrays in the context's SX_SLOT_K6B_OUT_* buffers (its entries and alternates are taken by sx_k6b_run
+// with own_out once their totals are known), and the sx_sindel_batch they form with the loci
+int sx_k6b_own_out(sx_ctx* ctx, uint32_t n_loci, sx_indel_reads_out* o);
+sx_sindel_batch sx_sindel_batch_of(const sx_indel_loci* loci, const sx_indel_reads_out* o);
+// K5b -> the link's flags into the results, enqueued on the compute stream behind the link (sx_k6b_run with own_out into `o`, from
+// sx_k6b_own_out): the second half of sx_somatic_indel_from_records_dev and of the somatic window pass.  The arguments are checked by the
+// caller (sx_k5b_check); the status word is the caller's to read.
+int sx_sindel_from_links_run(sx_ctx* ctx, const sx_sindel_opts* opts, const sx_indel_loci* loci, const sx_indel_reads_out* o, const double* err_prob, uint32_t n_err,
+                             sx_sindel_result* out_dev, unsigned* launches);
 int sx_k7g_run(sx_ctx* ctx, const sx_gate_batch* d, const sx_gate_out* o, unsigned* launches);
 int sx_k7a_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_region* regions, const uint8_t* seq4, const char* ref, const uint32_t* key_ins_off, const char* key_ins,
                const sx_prep_out* o, unsigned* launches);

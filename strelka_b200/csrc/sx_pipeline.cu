@@ -122,25 +122,25 @@ __global__ void sxp_pileup_reads_kernel(const sx_window_batch b, const prep_out 
     if (max_span) atomicMax(&p.maxima[2], max_span);
 }
 
-// ---- variant-site compaction, order-preserving: per 1024-site chunk a count, an exclusive scan over the chunks (sx_scan), ranked writes
+// ---- order-preserving compaction of the items a selector keeps: per 1024-item chunk a count, an exclusive scan over the chunks (sx_scan), ranked
+// writes.  A selector S has `bool keep(i)` and `S::record make(i)` (the record of a kept item); one instance per record kind.
 constexpr uint32_t VC_CHUNK = 1024, VC_THREADS = 256;
-__device__ __forceinline__ bool is_variant_site(const sx_digt_result& g) { return g.is_computed && g.genome.max_gt != g.ref_gt; }
 
-__global__ void __launch_bounds__(VC_THREADS) sxp_variant_count_kernel(const sx_digt_result* __restrict__ gl, const uint32_t n_sites, uint32_t* __restrict__ chunk_cnt)
+template <class S> __global__ void __launch_bounds__(VC_THREADS) sxp_compact_count_kernel(const S sel, const uint32_t n, uint32_t* __restrict__ chunk_cnt)
 {
     const uint32_t base(blockIdx.x * VC_CHUNK);
     int total(0);
     for (uint32_t i = 0; i < VC_CHUNK / VC_THREADS; ++i)
     {
         const uint32_t s(base + i * VC_THREADS + threadIdx.x);
-        total += __syncthreads_count(s < n_sites && is_variant_site(gl[s]));
+        total += __syncthreads_count(s < n && sel.keep(s));
     }
     if (threadIdx.x == 0) chunk_cnt[blockIdx.x] = (uint32_t)total;
 }
 
-__global__ void __launch_bounds__(VC_THREADS) sxp_variant_write_kernel(const sx_digt_result* __restrict__ gl, const uint32_t* __restrict__ site_off, const uint32_t n_sites,
-                                                                      const int32_t report_begin, const uint32_t* __restrict__ chunk_off, sx_site_call* __restrict__ out,
-                                                                      const uint32_t cap)
+template <class S>
+__global__ void __launch_bounds__(VC_THREADS) sxp_compact_write_kernel(const S sel, const uint32_t n, const uint32_t* __restrict__ chunk_off, typename S::record* __restrict__ out,
+                                                                       const uint32_t cap)
 {
     __shared__ uint32_t warp_cnt[VC_THREADS / 32];
     __shared__ uint32_t run;
@@ -150,7 +150,7 @@ __global__ void __launch_bounds__(VC_THREADS) sxp_variant_write_kernel(const sx_
     for (uint32_t i = 0; i < VC_CHUNK / VC_THREADS; ++i)
     {
         const uint32_t s(base + i * VC_THREADS + threadIdx.x);
-        const bool v(s < n_sites && is_variant_site(gl[s]));
+        const bool v(s < n && sel.keep(s));
         const unsigned m(__ballot_sync(0xffffffffu, v));
         if (lane == 0) warp_cnt[wid] = __popc(m);
         __syncthreads();
@@ -159,14 +159,7 @@ __global__ void __launch_bounds__(VC_THREADS) sxp_variant_write_kernel(const sx_
         if (v)
         {
             const uint32_t at(before + __popc(m & ((1u << lane) - 1u)));
-            if (at < cap)
-            {
-                sx_site_call c;
-                c.pos = report_begin + (int32_t)s;
-                c.n_calls = site_off[s + 1] - site_off[s];
-                c.gl = gl[s];
-                out[at] = c;
-            }
+            if (at < cap) out[at] = sel.make(s);
         }
         __syncthreads();
         if (threadIdx.x == 0)
@@ -178,6 +171,73 @@ __global__ void __launch_bounds__(VC_THREADS) sxp_variant_write_kernel(const sx_
         __syncthreads();
     }
 }
+
+// germline: the computed sites whose most likely genotype is not the reference's
+struct variant_site_sel
+{
+    using record = sx_site_call;
+    const sx_digt_result* gl;
+    const uint32_t* site_off;
+    int32_t report_begin;
+    __device__ bool keep(const uint32_t s) const { return gl[s].is_computed && gl[s].genome.max_gt != gl[s].ref_gt; }
+    __device__ record make(const uint32_t s) const
+    {
+        sx_site_call c;
+        c.pos = report_begin + (int32_t)s;
+        c.n_calls = site_off[s + 1] - site_off[s];
+        c.gl = gl[s];
+        return c;
+    }
+};
+
+// somatic SNV: somatic_snv_genotype_grid::is_output() (somatic_result_set.hh:62-71).  qphred is defined where the model ran; a forced position
+// whose reference base is 'N' loses the flag (position_somatic_snv_strand_grid.cpp:242-246).
+struct somatic_site_sel
+{
+    using record = sx_somatic_site_call;
+    const sx_ssnv_result* r;
+    const uint8_t* forced; // or NULL
+    const char* ref_base;
+    const uint32_t* n_off;
+    const uint32_t* t_off;
+    int32_t report_begin;
+    __device__ bool keep(const uint32_t s) const { return (r[s].is_computed && r[s].qphred != 0) || (forced && forced[s] && ref_base[s] != 'N'); }
+    __device__ record make(const uint32_t s) const
+    {
+        sx_somatic_site_call c;
+        c.pos = report_begin + (int32_t)s;
+        c.n_calls[0] = n_off[s + 1] - n_off[s];
+        c.n_calls[1] = t_off[s + 1] - t_off[s];
+        c.pad = 0;
+        c.r = r[s];
+        return c;
+    }
+};
+
+// somatic indel: a locus the link flagged (the caller's CPU path calls it), else somatic_indel_call::is_output() (somatic_result_set.hh:86-96)
+// of a locus that process_pos_indel_somatic calls at all -- an unforced candidate with both read_path_lnp empty is skipped
+// (strelka_pos_processor.cpp:324-327).  The link's read_off holds the offsets of the two lists of locus l at 2l, 2l+1, 2l+2.
+struct somatic_indel_sel
+{
+    using record = sx_somatic_indel_call;
+    const sx_sindel_result* r;
+    const uint8_t* forced;
+    const uint32_t* status;
+    const uint32_t* read_off;
+    __device__ bool keep(const uint32_t l) const
+    {
+        if (status[l] || forced[l]) return true;
+        return r[l].qphred != 0 && read_off[2 * l + 2] != read_off[2 * l];
+    }
+    __device__ record make(const uint32_t l) const
+    {
+        sx_somatic_indel_call c;
+        c.locus = l;
+        c.pad = 0;
+        c.r = r[l];
+        return c;
+    }
+};
 
 // the window pass's buffers: `count` elements and 64 bytes of slack
 template <typename T> int take(sx_ctx* ctx, sx_slot slot, size_t count, T*& p) { return sx_take(ctx, slot, count, p, 64); }
@@ -198,6 +258,52 @@ int read_status(sx_ctx* ctx, int* st)
     SX_CUDA(ctx, cudaMemcpyAsync(st, ctx->d_status, sizeof(int), cudaMemcpyDeviceToHost, ctx->s_compute));
     return SX_OK;
 }
+
+// The compaction of `n` items (n > 0) into out[cap]: two launches and the scan's, on the compute stream; *total (host memory) receives the
+// number of kept items once the stream has passed the copy.
+template <class S> int compact(sx_ctx* ctx, const S& sel, const uint32_t n, sx_slot chunk_slot, sx_slot sums_slot, typename S::record* out, const uint32_t cap,
+                               uint32_t* total, unsigned* launches)
+{
+    cudaStream_t st(ctx->s_compute);
+    const uint32_t n_chunks((n + VC_CHUNK - 1) / VC_CHUNK);
+    uint32_t* chunk_cnt(nullptr);
+    int rc;
+    if ((rc = take(ctx, chunk_slot, (size_t)n_chunks + 4, chunk_cnt))) return rc;
+    sxp_compact_count_kernel<<<n_chunks, VC_THREADS, 0, st>>>(sel, n, chunk_cnt);
+    SX_CUDA(ctx, cudaGetLastError());
+    const sx_scan_set J = {1, {{chunk_cnt, n_chunks, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, nullptr}}};
+    if ((rc = sx_scan(ctx, sums_slot, J, launches))) return rc;
+    sxp_compact_write_kernel<<<n_chunks, VC_THREADS, 0, st>>>(sel, n, chunk_cnt, out, cap);
+    SX_CUDA(ctx, cudaGetLastError());
+    *launches += 2;
+    SX_CUDA(ctx, cudaMemcpyAsync(total, chunk_cnt + n_chunks, 4, cudaMemcpyDeviceToHost, st));
+    return SX_OK;
+}
+
+// The slots of the window pass's results that a later stage reads, where the caller's output array does not take their place: the pass's own
+// (WIN_SLOTS), or a bank that survives a second pass on the same context (the somatic pass's normal sample)
+// t2_all_bases: the tier2 columns' own buffer is sized like the tier1 columns' (no more calls than the reads have bases) also without tier2
+// evidence -- the pile-up puts the tier2 reads' calls there either way, and the somatic pass reads the columns of both samples from these
+// buffers.  (The germline pass keeps its 64-call buffer.)
+struct win_slots
+{
+    sx_slot non_ambig, recs, n_rec, site_off, t2_off, calls, t2_calls;
+    bool t2_all_bases;
+};
+constexpr win_slots WIN_SLOTS = {SX_SLOT_WIN_NON_AMBIG, SX_SLOT_WIN_RECS, SX_SLOT_WIN_N_REC, SX_SLOT_WIN_SITE_OFF, SX_SLOT_WIN_T2_OFF, SX_SLOT_WIN_CALLS, SX_SLOT_WIN_T2_CALLS, false};
+constexpr win_slots SWIN_TUMOR_SLOTS = {SX_SLOT_WIN_NON_AMBIG, SX_SLOT_WIN_RECS, SX_SLOT_WIN_N_REC, SX_SLOT_WIN_SITE_OFF, SX_SLOT_WIN_T2_OFF, SX_SLOT_WIN_CALLS,
+                                        SX_SLOT_WIN_T2_CALLS, true};
+constexpr win_slots SWIN_NORMAL_SLOTS = {SX_SLOT_SWIN_NON_AMBIG, SX_SLOT_SWIN_RECS, SX_SLOT_SWIN_N_REC, SX_SLOT_SWIN_SITE_OFF, SX_SLOT_SWIN_T2_OFF, SX_SLOT_SWIN_CALLS,
+                                         SX_SLOT_SWIN_T2_CALLS, true};
+
+// ... and where those results are once the pass has run
+struct win_kept
+{
+    const uint16_t* non_ambig;
+    const sx_read_indel_score* recs;
+    const uint32_t* n_rec;
+    sx_pileup_columns cols;
+};
 } // namespace
 
 extern "C" void sx_default_window_opts(sx_window_batch* b)
@@ -223,7 +329,7 @@ extern "C" int sx_last_window_timing(const sx_ctx* ctx, float* ms)
 namespace
 {
 // the window pass of sx_process_window_dev, which sx_process_window runs on the window it has uploaded
-int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint32_t* totals_host)
+int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint32_t* totals_host, const win_slots& S = WIN_SLOTS, win_kept* kept = nullptr)
 {
     if (!ctx) return SX_ERR_ARG;
     ctx->timing = sx_timing{};
@@ -255,7 +361,7 @@ int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint3
     if ((rc = take(ctx, SX_SLOT_WIN_SEQ_OFF, (size_t)n + 1, P.seq_off))) return rc;
     if ((rc = take(ctx, SX_SLOT_WIN_QUAL_OFF, (size_t)n + 1, P.qual_off))) return rc;
     if ((rc = take(ctx, SX_SLOT_WIN_BPOS, (size_t)n + 1, P.bpos))) return rc;
-    if ((rc = take(ctx, SX_SLOT_WIN_NON_AMBIG, (size_t)n + 1, P.non_ambig))) return rc;
+    if ((rc = take(ctx, S.non_ambig, (size_t)n + 1, P.non_ambig))) return rc;
     if ((rc = take(ctx, SX_SLOT_WIN_PIN, (size_t)n + 1, P.pin))) return rc;
     if ((rc = take(ctx, SX_SLOT_WIN_MAXIMA, 4, P.maxima))) return rc;
     SX_CUDA(ctx, cudaMemsetAsync(P.maxima, 0, 16, st));
@@ -456,8 +562,8 @@ int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint3
     if (n)
     {
         SX_CUDA(ctx, cudaStreamSynchronize(st));
-        if ((rc = pick(ctx, SX_SLOT_WIN_RECS, (size_t)n_rec_slots + 1, out->recs, so.recs))) return rc;
-        if ((rc = pick(ctx, SX_SLOT_WIN_N_REC, (size_t)n + 1, out->n_rec, so.n_rec))) return rc;
+        if ((rc = pick(ctx, S.recs, (size_t)n_rec_slots + 1, out->recs, so.recs))) return rc;
+        if ((rc = pick(ctx, S.n_rec, (size_t)n + 1, out->n_rec, so.n_rec))) return rc;
         if ((rc = take(ctx, SX_SLOT_WIN_MAX_ALN, (size_t)n + 1, so.max_aln))) return rc;
         if ((rc = take(ctx, SX_SLOT_WIN_EVAL_ALN, (size_t)n + 1, so.eval_aln))) return rc;
         sx_score_indels_batch sb;
@@ -554,13 +660,13 @@ int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint3
     {
         // the columns never hold more calls than the reads have bases
         total_bases = (uint64_t)b->seq4_bytes * 2u + 16u;
-        const uint64_t cap_calls(cols.calls ? cols.calls_capacity : total_bases), cap_t2(cols.t2_calls ? cols.t2_capacity : (b->pileup_opts.useTier2Evidence ? total_bases : 64u));
-        if ((rc = pick(ctx, SX_SLOT_WIN_SITE_OFF, (size_t)n_sites + 2, out->cols.site_off, cols.site_off))) return rc;
-        if ((rc = pick(ctx, SX_SLOT_WIN_T2_OFF, (size_t)n_sites + 2, out->cols.t2_off, cols.t2_off))) return rc;
+        const uint64_t cap_calls(cols.calls ? cols.calls_capacity : total_bases), cap_t2(cols.t2_calls ? cols.t2_capacity : (b->pileup_opts.useTier2Evidence || S.t2_all_bases ? total_bases : 64u));
+        if ((rc = pick(ctx, S.site_off, (size_t)n_sites + 2, out->cols.site_off, cols.site_off))) return rc;
+        if ((rc = pick(ctx, S.t2_off, (size_t)n_sites + 2, out->cols.t2_off, cols.t2_off))) return rc;
         if ((rc = pick(ctx, SX_SLOT_WIN_N_SPANDEL, (size_t)n_sites + 2, out->cols.n_spandel, cols.n_spandel))) return rc;
         if ((rc = pick(ctx, SX_SLOT_WIN_N_SUBMAPPED, (size_t)n_sites + 2, out->cols.n_submapped, cols.n_submapped))) return rc;
-        if ((rc = pick(ctx, SX_SLOT_WIN_CALLS, (size_t)cap_calls + 16, out->cols.calls, cols.calls))) return rc;
-        if ((rc = pick(ctx, SX_SLOT_WIN_T2_CALLS, (size_t)cap_t2 + 16, out->cols.t2_calls, cols.t2_calls))) return rc;
+        if ((rc = pick(ctx, S.calls, (size_t)cap_calls + 16, out->cols.calls, cols.calls))) return rc;
+        if ((rc = pick(ctx, S.t2_calls, (size_t)cap_t2 + 16, out->cols.t2_calls, cols.t2_calls))) return rc;
         cols.calls_capacity = cap_calls;
         cols.t2_capacity = cap_t2;
         sx_pileup_reads_batch pb;
@@ -608,17 +714,9 @@ int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint3
         if ((rc = sx_k2a_run(ctx, &k2, b->is_always_test, gl, &launches))) return rc;
         if (out->variant_sites)
         {
-            const uint32_t n_chunks((n_sites + VC_CHUNK - 1) / VC_CHUNK);
-            uint32_t* chunk_cnt(nullptr);
-            if ((rc = take(ctx, SX_SLOT_WIN_VARIANT_CHUNKS, (size_t)n_chunks + 4, chunk_cnt))) return rc;
-            sxp_variant_count_kernel<<<n_chunks, VC_THREADS, 0, st>>>(gl, n_sites, chunk_cnt);
-            SX_CUDA(ctx, cudaGetLastError());
-            const sx_scan_set J = {1, {{chunk_cnt, n_chunks, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, nullptr}}};
-            if ((rc = sx_scan(ctx, SX_SLOT_WIN_VARIANT_SUMS, J, &launches))) return rc;
-            sxp_variant_write_kernel<<<n_chunks, VC_THREADS, 0, st>>>(gl, cols.site_off, n_sites, b->report_begin, chunk_cnt, out->variant_sites, out->cap_variant_sites);
-            SX_CUDA(ctx, cudaGetLastError());
-            launches += 2;
-            SX_CUDA(ctx, cudaMemcpyAsync(&totals[8], chunk_cnt + n_chunks, 4, cudaMemcpyDeviceToHost, st));
+            const variant_site_sel sel = {gl, cols.site_off, b->report_begin};
+            if ((rc = compact(ctx, sel, n_sites, SX_SLOT_WIN_VARIANT_CHUNKS, SX_SLOT_WIN_VARIANT_SUMS, out->variant_sites, out->cap_variant_sites, &totals[8], &launches)))
+                return rc;
         }
     }
     else if (out->variant_sites)
@@ -646,6 +744,7 @@ int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint3
     ctx->total_launches += launches;
     if (out->variant_sites && totals[8] > out->cap_variant_sites)
         return sx_fail(ctx, SX_ERR_CAPACITY, "sx_process_window_dev: %u variant sites, cap_variant_sites is %u", totals[8], out->cap_variant_sites);
+    if (kept) *kept = win_kept{P.non_ambig, so.recs, so.n_rec, cols};
     return sx_check_status(ctx, "sx_process_window");
 }
 } // namespace
@@ -653,6 +752,165 @@ int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint3
 extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint32_t* totals_host)
 {
     return window_pass(ctx, b, out, totals_host);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------------------
+// the somatic window pass: both samples through window_pass, then K2b, the SNV records, the link, K5b and the indel records
+// ---------------------------------------------------------------------------------------------------------------------------------------
+extern "C" int sx_last_somatic_window_timing(const sx_ctx* ctx, float* ms)
+{
+    if (!ctx || !ms) return SX_ERR_ARG;
+    for (int i = 0; i < SX_SWIN_N_STAGES; ++i) ms[i] = ctx->swin_ms[i];
+    return SX_OK;
+}
+
+namespace
+{
+// one sample's side of the link: the window batch's read arrays and the K6 records / 'N'-free counts its pass left
+sx_indel_reads_sample indel_reads_sample_of(const sx_window_batch& b, const win_kept& k, const uint32_t* key_gid, const uint32_t* read_id)
+{
+    sx_indel_reads_sample s;
+    memset(&s, 0, sizeof(s));
+    s.n_regions = b.n_regions;
+    s.n_reads = b.n_reads;
+    s.n_keys = b.n_keys;
+    s.region_read_off = b.region_read_off;
+    s.region_key_off = b.region_key_off;
+    s.key_gid = key_gid;
+    s.rec_off = b.rec_off;
+    s.recs = k.recs;
+    s.n_rec = k.n_rec;
+    s.read_len = b.read_len;
+    s.non_ambig = k.non_ambig;
+    s.read_flags = b.read_flags; // SX_SIF_TIER1 is SX_PRF_TIER1
+    s.read_id = read_id;
+    return s;
+}
+
+// a sample's tier1 (and with tier2 evidence its tier2) columns as K2b's batch
+sx_pileup_batch somatic_pileup_of(const sx_pileup_columns& c, const uint32_t n_sites, const char* ref_base, const bool tier2)
+{
+    sx_pileup_batch p;
+    memset(&p, 0, sizeof(p));
+    p.n_sites = n_sites;
+    p.site_off = c.site_off;
+    p.calls = c.calls;
+    p.t2_off = tier2 ? c.t2_off : nullptr;
+    p.t2_calls = tier2 ? c.t2_calls : nullptr;
+    p.ref_base = ref_base;
+    return p;
+}
+} // namespace
+
+extern "C" int sx_process_somatic_window_dev(sx_ctx* ctx, const sx_somatic_window_batch* sb, sx_somatic_window_out* so, uint32_t* totals_host)
+{
+    if (!ctx) return SX_ERR_ARG;
+    ctx->timing = sx_timing{};
+    const char* what("sx_process_somatic_window_dev");
+    if (!sb || !so) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL argument", what);
+    const sx_window_batch &bn(sb->sample[0]), &bt(sb->sample[1]);
+    for (int s = 0; s < 2; ++s)
+    {
+        const sx_window_batch& b(sb->sample[s]);
+        if (b.do_site_gl) return sx_fail(ctx, SX_ERR_ARG, "%s: sample %d: do_site_gl must be 0 (strelka2 runs no germline site model)", what, s);
+        if (so->sample[s].site_gl || so->sample[s].variant_sites) return sx_fail(ctx, SX_ERR_ARG, "%s: sample %d: site_gl / variant_sites must be NULL", what, s);
+        if (b.n_keys && !sb->key_gid[s]) return sx_fail(ctx, SX_ERR_ARG, "%s: sample %d: NULL key_gid", what, s);
+        if (b.report_end >= b.report_begin &&
+            ((int64_t)b.report_begin < (int64_t)b.ref_begin || (uint64_t)((int64_t)b.report_end - (int64_t)b.ref_begin) > b.ref_bytes || !b.ref))
+            return sx_fail(ctx, SX_ERR_ARG, "%s: sample %d: the report range leaves the reference segment", what, s);
+    }
+    if (bn.ref_begin != bt.ref_begin || bn.report_begin != bt.report_begin || bn.report_end != bt.report_end)
+        return sx_fail(ctx, SX_ERR_ARG, "%s: the samples differ in ref_begin / report_begin / report_end", what);
+    if (bn.pileup_opts.useTier2Evidence != bt.pileup_opts.useTier2Evidence || bn.pileup_opts.useTier2Evidence != sb->sindel_opts.useTier2Evidence)
+        return sx_fail(ctx, SX_ERR_ARG, "%s: pileup_opts.useTier2Evidence of both samples must equal sindel_opts.useTier2Evidence", what);
+    const sx_indel_loci& loci(sb->loci);
+    int rc;
+    if ((rc = sx_k6b_check_loci(ctx, what, &loci))) return rc;
+    SX_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st(ctx->s_compute);
+    const uint32_t n_sites(bn.report_end >= bn.report_begin ? (uint32_t)(bn.report_end - bn.report_begin) : 0u), n_loci(loci.n_loci);
+    const bool tier2(sb->sindel_opts.useTier2Evidence != 0);
+    sx_ssnv_result* site_snv(so->site_snv);
+    sx_sindel_result* indel(so->indel);
+    if (!site_snv && (rc = take(ctx, SX_SLOT_SWIN_SITE_SNV, (size_t)n_sites + 1, site_snv))) return rc;
+    if (!indel && (rc = take(ctx, SX_SLOT_SWIN_INDEL, (size_t)n_loci + 1, indel))) return rc;
+    sx_indel_reads_out lo;
+    if ((rc = sx_k6b_own_out(ctx, n_loci, &lo))) return rc;
+    {
+        const sx_sindel_batch kb(sx_sindel_batch_of(&loci, &lo));
+        if ((rc = sx_k5b_check(ctx, what, &sb->sindel_opts, &kb, sb->err_prob, sb->n_err, indel))) return rc;
+    }
+    for (int i = 0; i <= SX_SWIN_N_STAGES; ++i)
+        if (!ctx->ev_swin[i]) SX_CUDA(ctx, cudaEventCreate(&ctx->ev_swin[i]));
+    auto mark = [&](int i) { return cudaEventRecord(ctx->ev_swin[i], st); };
+    unsigned launches(0), pass_launches(0); // (the passes add theirs to ctx->total_launches themselves)
+    uint32_t totals[SX_SWIN_TOTALS] = {0, 0, 0, 0};
+
+    // ---------------------------------------------------------------------------------------------------------------- the two chains
+    // The normal sample's results that the stages below read go to the SX_SLOT_SWIN_* bank, so the tumor sample's pass leaves them be.
+    win_kept kept[2];
+    // A sample's SX_ERR_CAPACITY (an output array of out.sample[s] too small) leaves that pass's totals in out.sample[s].totals, as
+    // sx_process_window_dev's totals_host would.
+    const auto sample_pass = [&](const int s, const win_slots& slots) -> int {
+        uint32_t wt[SX_WIN_TOTALS] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+        const int r(window_pass(ctx, &sb->sample[s], &so->sample[s], wt, slots, &kept[s]));
+        if (r == SX_ERR_CAPACITY && so->sample[s].totals) cudaMemcpy(so->sample[s].totals, wt, sizeof(wt), cudaMemcpyHostToDevice);
+        pass_launches += ctx->timing.launches;
+        return r;
+    };
+    SX_CUDA(ctx, mark(SX_SWIN_ST_NORMAL));
+    if ((rc = sample_pass(0, SWIN_NORMAL_SLOTS))) return rc;
+    SX_CUDA(ctx, mark(SX_SWIN_ST_TUMOR));
+    if ((rc = sample_pass(1, SWIN_TUMOR_SLOTS))) return rc;
+    // ---------------------------------------------------------------------------------------------------------------- K2b and the SNV records
+    SX_CUDA(ctx, mark(SX_SWIN_ST_SITE_SNV));
+    const char* ref_base(bn.ref + ((int64_t)bn.report_begin - (int64_t)bn.ref_begin));
+    const sx_pileup_batch pn(somatic_pileup_of(kept[0].cols, n_sites, ref_base, tier2)), pt(somatic_pileup_of(kept[1].cols, n_sites, ref_base, tier2));
+    if (n_sites && (rc = sx_k2b_run(ctx, &pn, &pt, sb->snv_forced_output, site_snv, &launches))) return rc;
+    SX_CUDA(ctx, mark(SX_SWIN_ST_SNV_CALLS));
+    if (n_sites && so->snv_calls)
+    {
+        const somatic_site_sel sel = {site_snv, sb->snv_forced_output, ref_base, pn.site_off, pt.site_off, bn.report_begin};
+        if ((rc = compact(ctx, sel, n_sites, SX_SLOT_SWIN_SNV_CHUNKS, SX_SLOT_SWIN_SNV_SUMS, so->snv_calls, so->cap_snv_calls, &totals[0], &launches))) return rc;
+    }
+    // ---------------------------------------------------------------------------------------------------------------- link, K5b, the indel records
+    SX_CUDA(ctx, mark(SX_SWIN_ST_LINK));
+    if (n_loci)
+    {
+        const sx_indel_reads_sample rn(indel_reads_sample_of(bn, kept[0], sb->key_gid[0], sb->read_id[0])), rt(indel_reads_sample_of(bt, kept[1], sb->key_gid[1], sb->read_id[1]));
+        if ((rc = sx_k6b_run(ctx, what, &rn, &rt, &loci, &lo, &totals[2], true, &launches))) return rc;
+        SX_CUDA(ctx, mark(SX_SWIN_ST_INDEL));
+        if ((rc = sx_sindel_from_links_run(ctx, &sb->sindel_opts, &loci, &lo, sb->err_prob, sb->n_err, indel, &launches))) return rc;
+    }
+    else SX_CUDA(ctx, mark(SX_SWIN_ST_INDEL));
+    SX_CUDA(ctx, mark(SX_SWIN_ST_INDEL_CALLS));
+    if (n_loci && so->indel_calls)
+    {
+        const somatic_indel_sel sel = {indel, loci.is_forced_output, lo.status, lo.read_off};
+        if ((rc = compact(ctx, sel, n_loci, SX_SLOT_SWIN_INDEL_CHUNKS, SX_SLOT_SWIN_INDEL_SUMS, so->indel_calls, so->cap_indel_calls, &totals[1], &launches))) return rc;
+    }
+    SX_CUDA(ctx, mark(SX_SWIN_N_STAGES));
+    // ---------------------------------------------------------------------------------------------------------------- the end: one wait, the totals, the status
+    SX_CUDA(ctx, cudaStreamSynchronize(st));
+    if (so->totals) SX_CUDA(ctx, cudaMemcpyAsync(so->totals, totals, sizeof(totals), cudaMemcpyHostToDevice, st));
+    if (totals_host) memcpy(totals_host, totals, sizeof(totals));
+    float sum(0);
+    for (int i = 0; i < SX_SWIN_N_STAGES; ++i)
+    {
+        float ms(0);
+        cudaEventElapsedTime(&ms, ctx->ev_swin[i], ctx->ev_swin[i + 1]);
+        ctx->swin_ms[i] = ms;
+        sum += ms;
+    }
+    ctx->timing.kernel_ms = sum;
+    ctx->timing.launches = pass_launches + launches;
+    ctx->total_launches += launches;
+    if ((rc = sx_check_status(ctx, what, SX_ST_K6B_ID))) return rc;
+    if (so->snv_calls && totals[0] > so->cap_snv_calls)
+        return sx_fail(ctx, SX_ERR_CAPACITY, "%s: %u somatic SNV records, cap_snv_calls is %u", what, totals[0], so->cap_snv_calls);
+    if (so->indel_calls && totals[1] > so->cap_indel_calls)
+        return sx_fail(ctx, SX_ERR_CAPACITY, "%s: %u somatic indel records, cap_indel_calls is %u", what, totals[1], so->cap_indel_calls);
+    return SX_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------------------
