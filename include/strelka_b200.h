@@ -755,6 +755,72 @@ int sx_somatic_indel_from_records_dev(sx_ctx* ctx, const sx_sindel_opts* opts, c
                                       const sx_indel_loci* loci_dev, const double* err_prob_host, uint32_t n_err, sx_sindel_result* out_dev /*[n_loci]*/);
 
 /* ==========================================================================================
+ * K6g  allele_groups   (K6's records of one sample -> K5's per-group read lists, in device memory)
+ *   replaces what getVariantAlleleGroupGenotypeLhoodsForSample reads of the IndelBuffer before K5's loop
+ *   (starling_common/AlleleGroupGenotype.cpp:185-258, called by updateIndelLocusWithSampleInfo,
+ *   applications/starling/starling_pos_processor.cpp:1337-1400):
+ *     getAlleleGroupSupportingReadIds / getAlleleGroupIntersectionReadIds
+ *                                      starling_common/OrthogonalVariantAlleleCandidateGroupUtil.cpp:64-128
+ *     getAlleleLogLhoodFromRead        :132-196, with the contrast-group fold of AlleleGroupGenotype.cpp:216-242
+ *     getExemplarReadScore             AlleleGroupGenotype.cpp:160-180
+ *
+ * One call is one sample.  A group is A non-reference alleles (1 <= A <= SX_INDEL_MAX_ALLELES, in the caller's order) plus a
+ * contrast group of C alleles (C >= 0), both as batch-wide ids (sx_indel_reads_sample.key_gid), and callerPloidy 1 or 2.  One id
+ * may appear in any number of groups, as an allele or as a contrast.  Per group:
+ *   - Only SX_RIS_SCORED records are read_path_lnp entries (SX_RIS_SUBOVERLAP records are not, :617-627).
+ *   - The supporting reads are the tier-1 reads (SX_SIF_TIER1) with an entry in EVERY allele of the group (contrast alleles do not
+ *     count; minDistanceFromReadEdge is 0 on this path), in ascending read id: the order K5 sums its doubles in.
+ *   - A supporting read's allele log-likelihoods: L[0] = the std::max of `ref` over the group's and the contrast's alleles where the
+ *     read has an entry (in that order); L[1+a] = `indel` of allele a; then, in contrast order, a contrast allele's value (its
+ *     `indel`, or L[0] as the first step left it where the read has no entry) replaces L[0] when greater; L keeps A+1 entries.  Every
+ *     value is a ReadPathScores float, so allele_lnp holds it without loss.
+ *   - read_length, non_ambig and is_fwd (SX_SIF_FWD) are the read's (the exemplar entry is always found).
+ *   - A read id twice in the list of an id the group names sets SX_INDEL_READS_ST_DUP_READ in the group's status; the group keeps
+ *     its alleles and ploidy and gets no reads (the map would overwrite; a DNA window never does this).  Nothing is truncated.
+ *   - A group with A outside 1..SX_INDEL_MAX_ALLELES, a ploidy outside {1,2} or an id at or past n_gid is refused: SX_ERR_ARG.
+ *   - totals = {reads, allele_lnp floats} of the unflagged groups.  A capacity below them returns SX_ERR_CAPACITY with totals,
+ *     status and the three offset arrays written, and no per-read value.
+ *   - Every output byte is written, and the output does not depend on thread scheduling: two runs are byte-identical.
+ * With its offset, allele and per-read arrays the output IS an sx_indel_batch of n_groups loci.
+ * ======================================================================================== */
+typedef struct sx_allele_groups {
+    uint32_t n_groups, n_gid;
+    const uint32_t* allele_off;        /* [n_groups + 1] group g's alleles are allele_gid[allele_off[g] .. allele_off[g+1]) */
+    const uint32_t* allele_gid;
+    const uint32_t* contrast_off;      /* [n_groups + 1] its contrast alleles contrast_gid[contrast_off[g] .. contrast_off[g+1]) */
+    const uint32_t* contrast_gid;      /* not NULL when n_groups > 0, even if every contrast group is empty */
+    const uint8_t* ploidy;             /* [n_groups] callerPloidy, 1 or 2 */
+    const sx_indel_key* gid_key;       /* [n_gid] the entry of every id: del_len / ins_len become K5's allele_del_len / allele_ins_len */
+} sx_allele_groups;
+
+typedef struct sx_allele_group_reads_out { /* caller-allocated; the first ten arrays are an sx_indel_batch's */
+    uint32_t* read_off;                /* [n_groups + 1] */
+    uint32_t* lnp_off;                 /* [n_groups + 1] */
+    uint32_t* allele_off;              /* [n_groups + 1] as the groups' */
+    uint8_t* ploidy;                   /* [n_groups] */
+    uint16_t* allele_del_len;          /* [groups.allele_off[n_groups]] */
+    uint16_t* allele_ins_len;          /* [groups.allele_off[n_groups]] */
+    float* allele_lnp;                 /* [cap_lnp] per supporting read, A+1 floats */
+    uint16_t* read_length;             /* [cap_reads] */
+    uint16_t* non_ambig;               /* [cap_reads] */
+    uint8_t* is_fwd;                   /* [cap_reads] */
+    uint32_t* status;                  /* [n_groups] 0, or SX_INDEL_READS_ST_DUP_READ */
+    uint32_t* totals;                  /* [2] supporting reads, allele_lnp floats */
+    uint32_t cap_reads, cap_lnp;
+} sx_allele_group_reads_out;
+
+/* Host arrays in and out.  totals_host ([2], may be NULL) receives the totals also when the call returns SX_ERR_CAPACITY. */
+int sx_link_allele_groups(sx_ctx* ctx, const sx_indel_reads_sample* sample, const sx_allele_groups* groups, sx_allele_group_reads_out* out_host,
+                          uint32_t* totals_host);
+/* Device pointers inside every struct (out_dev->totals too); totals_host is host memory. */
+int sx_link_allele_groups_dev(sx_ctx* ctx, const sx_indel_reads_sample* sample_dev, const sx_allele_groups* groups_dev, sx_allele_group_reads_out* out_dev,
+                              uint32_t* totals_host);
+/* The link followed by K5 on the compute stream, the sx_indel_batch between them in buffers the context owns.  A group the link
+ * flagged gets an all-zero sx_indel_result; status_dev ([n_groups], device memory, may be NULL) receives every group's status. */
+int sx_indel_gl_from_records_dev(sx_ctx* ctx, const sx_indel_reads_sample* sample_dev, const sx_allele_groups* groups_dev, sx_indel_result* out_dev /*[n_groups]*/,
+                                 uint32_t* status_dev);
+
+/* ==========================================================================================
  * K7  enumerate_alignments   (SURVEY 8a row a3 / 8f3: the producer of K1's and K6's input)
  *   replaces  getCandidateAlignments           starling_common/starling_read_align.cpp:1816-1994
  *   with      candidate_alignment_search       :857-1277  (the recursive toggle search)

@@ -3,7 +3,8 @@
 units under oracle/_ref/build/patched/ (git-ignored scratch; the reference tree is read-only and stays untouched, nothing of it enters this
 repository), each edit a call-site substitution, compiles them with the oracle build's flags and links
 
-    oracle/_ref/bin/starling2_sx   germline caller: computeSampleDiploidSiteGenotype -> sx_site_gl_germline (K2a), haplotype alignment -> sx_global_align (K3)
+    oracle/_ref/bin/starling2_sx   germline caller: computeSampleDiploidSiteGenotype -> sx_site_gl_germline (K2a), haplotype alignment -> sx_global_align (K3),
+                                   getVariantAlleleGroupGenotypeLhoodsForSample -> sx_indel_gl (K5)
     oracle/_ref/bin/strelka2_sx    somatic caller:  position_somatic_snv_call -> sx_site_gl_somatic (K2b), get_somatic_indel -> sx_somatic_indel (K5b)
     oracle/_ref/bin/starling2, strelka2   the unmodified reference binaries (oracle/build_ref.sh --bins)
 
@@ -27,7 +28,13 @@ EDITS = [
     ("applications/starling/starling_pos_processor.cpp",
      [(r"dopt\.pdcaller\(\)\.position_snp_call_pprob_digt\(\s*opt,\s*good_epi,\s*dgt,\s*opt\.is_all_sites\(\)\);",
        "if (sx_shim::enabled()) sx_shim::site_gl_germline(opt, sif.cleanedPileup.rawPileup(), opt.is_all_sites(), dgt);\n"
-       "    else dopt.pdcaller().position_snp_call_pprob_digt(opt, good_epi, dgt, opt.is_all_sites());")], ""),
+       "    else dopt.pdcaller().position_snp_call_pprob_digt(opt, good_epi, dgt, opt.is_all_sites());"),
+      (r"getVariantAlleleGroupGenotypeLhoodsForSample\(\s*opt,\s*dopt,\s*sample_opt,\s*callerPloidy,\s*sampleIndex,\s*alleleGroup,\s*contrastGroup,\s*"
+       r"genotypeLogLhood,\s*sampleInfo\.supportCounts\);",
+       "if (sx_shim::enabled()) sx_shim::germline_indel(opt, dopt, sample_opt, callerPloidy, sampleIndex, alleleGroup, contrastGroup, genotypeLogLhood,\n"
+       "                                                sampleInfo.supportCounts);\n"
+       "    else getVariantAlleleGroupGenotypeLhoodsForSample(opt, dopt, sample_opt, callerPloidy, sampleIndex, alleleGroup, contrastGroup,\n"
+       "                                                      genotypeLogLhood, sampleInfo.supportCounts);")], "#define SX_SHIM_GERMLINE\n"),
     ("starling_common/ActiveRegionProcessor.cpp",
      [(r"_aligner\.align\(haplotypeSeq\.cbegin\(\),\s*haplotypeSeq\.cend\(\),\s*_refSegment\.cbegin\(\),\s*_refSegment\.cend\(\),\s*result\);",
        "if (sx_shim::enabled()) sx_shim::global_align(_aligner.getScores(), haplotypeSeq, _refSegment, result);\n"

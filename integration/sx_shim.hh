@@ -34,12 +34,15 @@ inline bool enabled()
 
 struct Counters
 {
-    unsigned long long site_gl_germline = 0, site_gl_somatic = 0, global_align = 0, somatic_indel = 0;
+    unsigned long long site_gl_germline = 0, site_gl_somatic = 0, global_align = 0, somatic_indel = 0, germline_indel = 0;
+    bool germline_indel_route = false; // set by the translation unit that routes germline indel genotyping (SX_SHIM_GERMLINE)
     ~Counters()
     {
+        // (fields are read by position: a new counter goes at the end, and only binaries with its route print it)
         if (std::getenv("SX_SHIM_REPORT"))
-            std::fprintf(stderr, "sx_shim: %llu germline site calls, %llu somatic site calls, %llu haplotype alignments through libstrelka_b200.so, %llu somatic indel calls\n",
-                         site_gl_germline, site_gl_somatic, global_align, somatic_indel);
+            std::fprintf(stderr, "sx_shim: %llu germline site calls, %llu somatic site calls, %llu haplotype alignments through libstrelka_b200.so, %llu somatic indel calls%s",
+                         site_gl_germline, site_gl_somatic, global_align, somatic_indel, germline_indel_route ? ", " : "\n");
+        if (std::getenv("SX_SHIM_REPORT") && germline_indel_route) std::fprintf(stderr, "%llu germline indel calls\n", germline_indel);
     }
 };
 inline Counters& counters()
@@ -300,6 +303,109 @@ inline void somatic_indel(const strelka_options& opt, const strelka_deriv_option
     sindel.rs.qphred = r.qphred;
     sindel.rs.from_ntype_qphred = r.from_ntype_qphred;
     sindel.rs.is_overlap = r.is_overlap != 0;
+}
+#endif
+
+#ifdef SX_SHIM_GERMLINE
+inline bool register_germline_indel_route()
+{
+    counters().germline_indel_route = true;
+    return true;
+}
+static const bool germline_indel_route_registered = register_germline_indel_route();
+
+/// getVariantAlleleGroupGenotypeLhoodsForSample(opt, dopt, sample_opt, callerPloidy, sampleIndex, alleleGroup, contrastGroup, genotypeLogLhood,
+/// supportCounts) of updateIndelLocusWithSampleInfo (applications/starling/starling_pos_processor.cpp:1384) as a one-group sx_indel_gl batch.
+/// The batch is filled with the reference's own getAlleleGroupSupportingReadIds / getAlleleLogLhoodFromRead and the contrast fold of
+/// AlleleGroupGenotype.cpp:225-238.  K5's context is made for the run's randomBaseMatchProb, readConfidentSupportThreshold and the sample's
+/// min_read_bp_flank; a group outside K5's domain (no or more than SX_INDEL_MAX_ALLELES alleles, a ploidy other than 1 or 2), or a call with
+/// other values of those options than the context was made for, keeps the reference function.
+inline void germline_indel(const starling_base_options& opt, const starling_base_deriv_options& dopt, const starling_sample_options& sample_opt,
+                           const unsigned callerPloidy, const unsigned sampleIndex, const OrthogonalVariantAlleleCandidateGroup& alleleGroup,
+                           const OrthogonalVariantAlleleCandidateGroup& contrastGroup, std::vector<double>& genotypeLogLhood, LocusSupportingReadStats& stats)
+{
+    sx_params p(params_of(opt));
+    p.randomBaseMatchProb = opt.randomBaseMatchProb;
+    p.readConfidentSupportThreshold = opt.readConfidentSupportThreshold.numval();
+    p.min_read_bp_flank = sample_opt.min_read_bp_flank;
+    struct Holder // K5's context: its tables are made from these options at sx_create
+    {
+        sx_ctx* ctx = nullptr;
+        sx_params p;
+        explicit Holder(const sx_params& q) : p(q)
+        {
+            const char* dev(std::getenv("SX_SHIM_DEVICE"));
+            if (sx_create(dev ? std::atoi(dev) : 0, &q, &ctx) != SX_OK) throw blt_exception(sx_last_error(nullptr));
+        }
+        ~Holder() { sx_destroy(ctx); }
+    };
+    static Holder h(p);
+    const unsigned A(alleleGroup.size());
+    if (A < 1 || A > SX_INDEL_MAX_ALLELES || (callerPloidy != 1 && callerPloidy != 2) || h.p.randomBaseMatchProb != p.randomBaseMatchProb ||
+        h.p.readConfidentSupportThreshold != p.readConfidentSupportThreshold || h.p.min_read_bp_flank != p.min_read_bp_flank)
+    {
+        getVariantAlleleGroupGenotypeLhoodsForSample(opt, dopt, sample_opt, callerPloidy, sampleIndex, alleleGroup, contrastGroup, genotypeLogLhood, stats);
+        return;
+    }
+    std::set<unsigned> readIds;
+    getAlleleGroupSupportingReadIds(sampleIndex, alleleGroup, readIds, true);
+    OrthogonalVariantAlleleCandidateGroup extended(alleleGroup);
+    for (const auto& it : contrastGroup.alleles) extended.alleles.push_back(it);
+    std::vector<float> lnp;
+    std::vector<uint16_t> read_length, non_ambig, del_len, ins_len;
+    std::vector<uint8_t> is_fwd;
+    for (const unsigned readId : readIds)
+    {
+        std::vector<double> v(extended.size() + 1);
+        getAlleleLogLhoodFromRead(sampleIndex, extended, readId, v);
+        for (unsigned i = A + 1; i < v.size(); ++i)
+            if (v[i] > v[0]) v[0] = v[i];
+        for (unsigned i = 0; i <= A; ++i) lnp.push_back(static_cast<float>(v[i])); // (ReadPathScores floats: exact)
+        const ReadPathScores* ex(nullptr); // getExemplarReadScore
+        for (unsigned a = 0; a < A && !ex; ++a)
+        {
+            const auto& m(alleleGroup.data(a).getSampleData(sampleIndex).read_path_lnp);
+            const auto f(m.find(readId));
+            if (f != m.end()) ex = &f->second;
+        }
+        read_length.push_back(ex->read_length);
+        non_ambig.push_back(ex->nonAmbiguousBasesInRead);
+        is_fwd.push_back(ex->is_fwd_strand ? 1 : 0);
+    }
+    for (unsigned a = 0; a < A; ++a)
+    {
+        del_len.push_back(static_cast<uint16_t>(alleleGroup.key(a).delete_length()));
+        ins_len.push_back(static_cast<uint16_t>(alleleGroup.key(a).insert_length()));
+    }
+    const uint32_t n(readIds.size()), read_off[2] = {0, n}, lnp_off[2] = {0, n * (A + 1)}, allele_off[2] = {0, A};
+    const uint8_t ploidy(static_cast<uint8_t>(callerPloidy));
+    const float f0(0.f);
+    const uint16_t u0(0);
+    const uint8_t b0(0);
+    sx_indel_batch b;
+    b.n_loci = 1;
+    b.read_off = read_off;
+    b.lnp_off = lnp_off;
+    b.allele_off = allele_off;
+    b.ploidy = &ploidy;
+    b.allele_del_len = del_len.data();
+    b.allele_ins_len = ins_len.data();
+    b.allele_lnp = n ? lnp.data() : &f0;
+    b.read_length = n ? read_length.data() : &u0;
+    b.non_ambig = n ? non_ambig.data() : &u0;
+    b.is_fwd = n ? is_fwd.data() : &b0;
+    sx_indel_result r;
+    check(h.ctx, sx_indel_gl(h.ctx, &b, &r));
+    ++counters().germline_indel;
+    genotypeLogLhood.assign(r.gt_lhood, r.gt_lhood + r.n_gt);
+    stats.setAltCount(A);
+    for (int s = 0; s < 2; ++s)
+    {
+        SupportingReadCountGroup& c(stats.getCounts(s == 1));
+        for (unsigned a = 0; a <= A; ++a)
+            if (r.support[s][a]) c.incrementAlleleCount(a, r.support[s][a]);
+        c.nonConfidentCount += r.support[s][SX_INDEL_MAX_ALLELES + 1];
+    }
 }
 #endif
 } // namespace sx_shim

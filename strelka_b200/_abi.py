@@ -138,6 +138,20 @@ class SxIndelReadsOut(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("alt_off", "alts", "read_off", "reads", "status", "totals")] + [("cap_alts", C.c_uint32), ("cap_reads", C.c_uint32)]
 
 
+# K6g allele_groups
+SX_INDEL_MAX_ALLELES = 4
+
+
+class SxAlleleGroups(C.Structure):
+    _fields_ = [("n_groups", C.c_uint32), ("n_gid", C.c_uint32)] + [(n, C.c_void_p) for n in (
+        "allele_off", "allele_gid", "contrast_off", "contrast_gid", "ploidy", "gid_key")]
+
+
+class SxAlleleGroupReadsOut(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("read_off", "lnp_off", "allele_off", "ploidy", "allele_del_len", "allele_ins_len", "allele_lnp", "read_length", "non_ambig",
+                                          "is_fwd", "status", "totals")] + [("cap_reads", C.c_uint32), ("cap_lnp", C.c_uint32)]
+
+
 def default_sindel_opts() -> SxSindelOpts:
     o = SxSindelOpts()
     load().sx_default_sindel_opts(C.byref(o))
@@ -462,6 +476,9 @@ SYMBOLS = [
     ("sx_link_indel_reads_dev", C.c_int, [_P, C.POINTER(SxIndelReadsSample), C.POINTER(SxIndelReadsSample), C.POINTER(SxIndelLoci), C.POINTER(SxIndelReadsOut), _P]),
     ("sx_somatic_indel_from_records_dev", C.c_int, [_P, C.POINTER(SxSindelOpts), C.POINTER(SxIndelReadsSample), C.POINTER(SxIndelReadsSample), C.POINTER(SxIndelLoci),
                                                     _P, C.c_uint32, _P]),
+    ("sx_link_allele_groups", C.c_int, [_P, C.POINTER(SxIndelReadsSample), C.POINTER(SxAlleleGroups), C.POINTER(SxAlleleGroupReadsOut), _P]),
+    ("sx_link_allele_groups_dev", C.c_int, [_P, C.POINTER(SxIndelReadsSample), C.POINTER(SxAlleleGroups), C.POINTER(SxAlleleGroupReadsOut), _P]),
+    ("sx_indel_gl_from_records_dev", C.c_int, [_P, C.POINTER(SxIndelReadsSample), C.POINTER(SxAlleleGroups), _P, _P]),
     ("sx_default_pileup_opts", None, [C.POINTER(SxPileupOpts)]),
     ("sx_pileup_reads", C.c_int, [_P, C.POINTER(SxPileupReadsBatch), C.POINTER(SxPileupColumns)]),
     ("sx_pileup_reads_dev", C.c_int, [_P, C.POINTER(SxPileupReadsBatch), C.POINTER(SxPileupColumns)]),

@@ -278,6 +278,35 @@ class Context:
             x.free()
         return out
 
+    # ---- K6g
+    def link_allele_groups(self, sample: B.IndelReadsSample, groups: B.AlleleGroups, cap_reads=None, cap_lnp=None) -> B.AlleleGroupReadsOut:
+        """K6g: one sample's K6 records -> K5's per-group read lists (host arrays in and out).  SX_ERR_CAPACITY leaves the needed sizes in
+        the SxError's `totals`."""
+        cr, cl = B.allele_group_caps(sample, groups)
+        out = B.AlleleGroupReadsOut(groups.n_groups, int(groups.allele_off[-1]), cr if cap_reads is None else cap_reads, cl if cap_lnp is None else cap_lnp)
+        totals = np.zeros(2, np.uint32)
+        rc = self.lib.sx_link_allele_groups(self.h, C.byref(sample.c), C.byref(groups.c), C.byref(out.c), totals.ctypes.data)
+        self._chk_totals(rc, totals)
+        return out
+
+    def link_allele_groups_dev(self, sample: DevIndelReadsSample, groups: DevAlleleGroups, cap_reads: int, cap_lnp: int) -> B.AlleleGroupReadsOut:
+        """K6g on device-resident inputs, into device arrays of the given capacities; returns their host copies."""
+        hg = groups.host
+        out = B.AlleleGroupReadsOut(hg.n_groups, int(hg.allele_off[-1]), cap_reads, cap_lnp)
+        d = {k: DeviceArray(self, getattr(out, k).nbytes + 64) for k in out.ARRAYS}
+        c = A.SxAlleleGroupReadsOut(cap_reads=cap_reads, cap_lnp=cap_lnp, **{k: x.ptr for k, x in d.items()})
+        totals = np.zeros(2, np.uint32)
+        rc = self.lib.sx_link_allele_groups_dev(self.h, C.byref(sample.c), C.byref(groups.c), C.byref(c), totals.ctypes.data)
+        self._chk_totals(rc, totals)
+        n, r, f, a = hg.n_groups, int(totals[0]), int(totals[1]), int(hg.allele_off[-1])
+        for k, cnt in (("read_off", n + 1), ("lnp_off", n + 1), ("allele_off", n + 1), ("totals", 2), ("status", n), ("ploidy", n), ("allele_del_len", a),
+                       ("allele_ins_len", a), ("allele_lnp", f), ("read_length", r), ("non_ambig", r), ("is_fwd", r)):
+            arr = getattr(out, k)
+            arr[:cnt] = d[k].download(arr.dtype, cnt)
+        for x in d.values():
+            x.free()
+        return out
+
     def _chk_totals(self, rc: int, totals: np.ndarray) -> None:
         try:
             self._chk(rc)
@@ -405,6 +434,33 @@ class DevIndelLoci:
     def __init__(self, ctx: "Context", hl: B.IndelLoci):
         self.host = hl
         self.c, self.bufs = _device_twin(ctx, hl.c, hl, 64)
+
+
+class DevAlleleGroups:
+    def __init__(self, ctx: "Context", hg: B.AlleleGroups):
+        self.host = hg
+        self.c, self.bufs = _device_twin(ctx, hg.c, hg, 64)
+
+
+class DevGermlineIndelChain:
+    """K6's records of one sample -> germline indel genotype likelihoods without a host step (sx_indel_gl_from_records_dev): the K6g link,
+    then K5 on the sx_indel_batch the link left in the context's buffers.  The sample's recs / n_rec arrays are caller-owned
+    (DevIndelReadsSample, from_score_indels or from_window).  `download()` returns (results, status): a group the link flagged has its
+    status and an all-zero result."""
+
+    def __init__(self, ctx: "Context", sample: DevIndelReadsSample, groups: B.AlleleGroups):
+        self.ctx, self.sample, self.groups = ctx, sample, DevAlleleGroups(ctx, groups)
+        n = max(1, groups.n_groups)
+        self.out = DeviceArray(ctx, n * A.INDEL_RESULT_DT.itemsize)
+        self.status = DeviceArray(ctx, n * 4)
+
+    def run(self) -> None:
+        ctx = self.ctx
+        ctx._chk(ctx.lib.sx_indel_gl_from_records_dev(ctx.h, C.byref(self.sample.c), C.byref(self.groups.c), self.out.ptr, self.status.ptr))
+
+    def download(self) -> Tuple[np.ndarray, np.ndarray]:
+        n = self.groups.host.n_groups
+        return self.out.download(A.INDEL_RESULT_DT, n), self.status.download(np.uint32, n)
 
 
 class DevSomaticIndelChain:

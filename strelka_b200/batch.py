@@ -471,6 +471,20 @@ class IndelBatch:
                                 allele_del_len=A.ptr(self.allele_del_len), allele_ins_len=A.ptr(self.allele_ins_len), allele_lnp=A.ptr(self.allele_lnp),
                                 read_length=A.ptr(self.read_length), non_ambig=A.ptr(self.non_ambig), is_fwd=A.ptr(self.is_fwd))
 
+    @staticmethod
+    def from_arrays(read_off, lnp_off, allele_off, ploidy, allele_del_len, allele_ins_len, allele_lnp, read_length, non_ambig, is_fwd) -> "IndelBatch":
+        """An IndelBatch over flat arrays (the K6g link's output)."""
+        ib = IndelBatch.__new__(IndelBatch)
+        ib.n_loci = int(np.asarray(read_off).size - 1)
+        for k, v, dt in (("read_off", read_off, np.uint32), ("lnp_off", lnp_off, np.uint32), ("allele_off", allele_off, np.uint32), ("ploidy", ploidy, np.uint8),
+                         ("allele_del_len", allele_del_len, np.uint16), ("allele_ins_len", allele_ins_len, np.uint16), ("allele_lnp", allele_lnp, np.float32),
+                         ("read_length", read_length, np.uint16), ("non_ambig", non_ambig, np.uint16), ("is_fwd", is_fwd, np.uint8)):
+            a = np.ascontiguousarray(v, dt)
+            setattr(ib, k, a if a.size else np.zeros(1, dt))
+        ib.c = A.SxIndelBatch(n_loci=ib.n_loci, **{k: A.ptr(getattr(ib, k)) for k in ("read_off", "lnp_off", "allele_off", "ploidy", "allele_del_len", "allele_ins_len",
+                                                                                       "allele_lnp", "read_length", "non_ambig", "is_fwd")})
+        return ib
+
 
 # ------------------------------------------------------------------------------------------------------------------
 # K5b somatic_indel
@@ -644,6 +658,158 @@ def link_indel_reads(normal: IndelReadsSample, tumor: IndelReadsSample, loci: In
             out.alts[aa : aa + len(alts_of[l])] = loci.gid_key[alts_of[l]]
             aa += len(alts_of[l])
     out.alt_off[loci.n_loci], out.read_off[2 * loci.n_loci] = aa, at
+    return out
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# K6g allele_groups
+# ------------------------------------------------------------------------------------------------------------------
+class AlleleGroups:
+    """sx_allele_groups: per group its non-reference alleles and contrast alleles as batch-wide ids, and its ploidy; gid_key is the entry of
+    every id.  `from_lists` takes one list of ids per group."""
+
+    def __init__(self, allele_off, allele_gid, contrast_off, contrast_gid, ploidy, gid_key):
+        self.allele_off = np.ascontiguousarray(allele_off, np.uint32)
+        self.allele_gid = np.ascontiguousarray(allele_gid, np.uint32)
+        self.contrast_off = np.ascontiguousarray(contrast_off, np.uint32)
+        self.contrast_gid = np.ascontiguousarray(contrast_gid, np.uint32)
+        self.ploidy = np.ascontiguousarray(ploidy, np.uint8)
+        self.gid_key = np.ascontiguousarray(gid_key, A.INDEL_KEY_DT)
+        self.n_groups = n = self.ploidy.size
+        self.n_gid = self.gid_key.size
+        assert self.allele_off.size == n + 1 and self.contrast_off.size == n + 1
+        self._keep = [a if a.size else np.zeros(1, a.dtype) for a in (self.allele_gid, self.contrast_gid, self.ploidy, self.gid_key)]
+        ag, cg, pl, gk = self._keep
+        self.c = A.SxAlleleGroups(n_groups=n, n_gid=self.n_gid, allele_off=A.ptr(self.allele_off), allele_gid=A.ptr(ag), contrast_off=A.ptr(self.contrast_off),
+                                  contrast_gid=A.ptr(cg), ploidy=A.ptr(pl), gid_key=A.ptr(gk))
+
+    @staticmethod
+    def from_lists(alleles, contrasts, ploidy, gid_key) -> "AlleleGroups":
+        off = lambda ls: np.concatenate([[0], np.cumsum([len(x) for x in ls], dtype=np.int64)]).astype(np.uint32)
+        flat = lambda ls: np.array([g for x in ls for g in x], np.uint32)
+        return AlleleGroups(off(alleles), flat(alleles), off(contrasts), flat(contrasts), ploidy, gid_key)
+
+    def group(self, g: int):
+        """(alleles, contrasts, ploidy) of group g"""
+        a = self.allele_gid[self.allele_off[g] : self.allele_off[g + 1]]
+        c = self.contrast_gid[self.contrast_off[g] : self.contrast_off[g + 1]]
+        return [int(x) for x in a], [int(x) for x in c], int(self.ploidy[g])
+
+
+class AlleleGroupReadsOut:
+    """sx_allele_group_reads_out with capacities; `batch()` is the sx_indel_batch (IndelBatch) its arrays form."""
+
+    ARRAYS = ("read_off", "lnp_off", "allele_off", "ploidy", "allele_del_len", "allele_ins_len", "allele_lnp", "read_length", "non_ambig", "is_fwd", "status", "totals")
+
+    def __init__(self, n_groups: int, n_alleles: int, cap_reads: int, cap_lnp: int):
+        self.n_groups, self.n_alleles = n_groups, n_alleles
+        self.read_off, self.lnp_off, self.allele_off = (np.zeros(n_groups + 1, np.uint32) for _ in range(3))
+        self.ploidy = np.zeros(max(1, n_groups), np.uint8)
+        self.allele_del_len, self.allele_ins_len = (np.zeros(max(1, n_alleles), np.uint16) for _ in range(2))
+        self.allele_lnp = np.zeros(max(1, cap_lnp), np.float32)
+        self.read_length, self.non_ambig = (np.zeros(max(1, cap_reads), np.uint16) for _ in range(2))
+        self.is_fwd = np.zeros(max(1, cap_reads), np.uint8)
+        self.status = np.zeros(max(1, n_groups), np.uint32)
+        self.totals = np.zeros(2, np.uint32)
+        self.c = A.SxAlleleGroupReadsOut(cap_reads=cap_reads, cap_lnp=cap_lnp, **{k: A.ptr(getattr(self, k)) for k in self.ARRAYS})
+
+    def trimmed(self):
+        """Every output array without the unused capacity, in ARRAYS order."""
+        n, r, f, a = self.n_groups, int(self.totals[0]), int(self.totals[1]), self.n_alleles
+        return (self.read_off, self.lnp_off, self.allele_off, self.ploidy[:n], self.allele_del_len[:a], self.allele_ins_len[:a], self.allele_lnp[:f], self.read_length[:r],
+                self.non_ambig[:r], self.is_fwd[:r], self.status[:n], self.totals)
+
+    def batch(self) -> IndelBatch:
+        return IndelBatch.from_arrays(*self.trimmed()[:10])
+
+
+def allele_group_caps(sample: IndelReadsSample, groups: AlleleGroups):
+    """Capacities no call exceeds: every scored entry of each group's first allele supports it."""
+    n = sample.n_rec[: sample.n_reads].astype(np.int64)
+    read_of = np.repeat(np.arange(sample.n_reads), n)
+    at = sample.rec_off[read_of].astype(np.int64) + np.arange(read_of.size) - np.repeat(np.cumsum(n) - n, n)
+    region = np.repeat(np.arange(sample.n_regions), np.diff(sample.region_read_off[: sample.n_regions + 1]).astype(np.int64))
+    scored = (sample.recs["flags"][at] & A.SX_RIS_SCORED) != 0
+    key = sample.region_key_off[region[read_of[scored]]].astype(np.int64) + sample.recs["key"][at[scored]]
+    cnt = np.bincount(sample.key_gid[np.minimum(key, max(0, sample.key_gid.size - 1))], minlength=groups.n_gid) if key.size else np.zeros(groups.n_gid, np.int64)
+    first = groups.allele_gid[groups.allele_off[:-1]] if groups.n_groups else np.zeros(0, np.uint32)
+    per = cnt[np.minimum(first, max(0, cnt.size - 1))] if cnt.size else np.zeros(first.size, np.int64)
+    return int(per.sum()), int((per * np.diff(groups.allele_off.astype(np.int64)) + per).sum())
+
+
+def link_allele_groups(sample: IndelReadsSample, groups: AlleleGroups) -> AlleleGroupReadsOut:
+    """Host restatement of sx_link_allele_groups with dicts: read_path_lnp[read id] = entry per id, then per group the supporting reads in
+    ascending id and their allele log-likelihoods with the contrast fold.  A third check beside the oracle and the kernel body; not a fast
+    path.  Raises ValueError where the library refuses the call."""
+    named = set(groups.allele_gid.tolist()) | set(groups.contrast_gid.tolist())
+    for g in range(groups.n_groups):
+        al, co, pl = groups.group(g)
+        if not 1 <= len(al) <= A.SX_INDEL_MAX_ALLELES or pl not in (1, 2) or any(x >= groups.n_gid for x in al + co):
+            raise ValueError(f"group {g} is outside the link's domain")
+    maps = {x: {} for x in named}
+    dup = set()
+    region = np.repeat(np.arange(sample.n_regions), np.diff(sample.region_read_off[: sample.n_regions + 1]).astype(np.int64))
+    for r in range(sample.n_reads):
+        k0 = int(sample.region_key_off[region[r]]) if sample.n_rec[r] else 0
+        rid = r if sample.read_id is None else int(sample.read_id[r])
+        for rec in sample.recs[int(sample.rec_off[r]) : int(sample.rec_off[r]) + int(sample.n_rec[r])]:
+            if not rec["flags"] & A.SX_RIS_SCORED:
+                continue
+            if int(rec["key"]) >= int(sample.region_key_off[region[r] + 1]) - k0 or int(sample.key_gid[k0 + int(rec["key"])]) >= groups.n_gid:
+                raise ValueError(f"read {r}: a window index outside its region's window, or an id at or past n_gid")
+            m = maps.get(int(sample.key_gid[k0 + int(rec["key"])]))
+            if m is None:
+                continue
+            if rid in m:
+                dup.add(int(sample.key_gid[k0 + int(rec["key"])]))
+            m[rid] = (float(rec["ref_lnp"]), float(rec["indel_lnp"]), r)
+    n_al = int(groups.allele_off[-1])
+    rows = []
+    status = np.zeros(groups.n_groups, np.uint32)
+    for g in range(groups.n_groups):
+        al, co, _ = groups.group(g)
+        if any(x in dup for x in al + co):
+            status[g] = A.SX_INDEL_READS_ST_DUP_READ
+            rows.append([])
+            continue
+        tier1 = lambda rid: sample.read_flags[maps[al[0]][rid][2]] & A.SX_SIF_TIER1
+        sup = sorted(rid for rid in maps[al[0]] if tier1(rid) and all(rid in maps[x] for x in al[1:]))
+        rows.append([])
+        for rid in sup:
+            lnp = np.zeros(len(al) + 1, np.float32)
+            l0 = None
+            for a, x in enumerate(al):
+                ref, indel, _ = maps[x][rid]
+                l0 = np.float32(ref) if l0 is None else max(l0, np.float32(ref))
+                lnp[1 + a] = indel
+            for x in co:
+                if rid in maps[x]:
+                    l0 = max(l0, np.float32(maps[x][rid][0]))
+            uncovered = l0
+            for x in co:
+                v = np.float32(maps[x][rid][1]) if rid in maps[x] else uncovered
+                if v > l0:
+                    l0 = v
+            lnp[0] = l0
+            rows[g].append((lnp, maps[al[0]][rid][2]))
+    n_reads = sum(len(x) for x in rows)
+    n_lnp = sum(len(x) * (len(groups.group(g)[0]) + 1) for g, x in enumerate(rows))
+    out = AlleleGroupReadsOut(groups.n_groups, n_al, n_reads, n_lnp)
+    out.totals[:] = (n_reads, n_lnp)
+    out.status[: groups.n_groups] = status
+    out.ploidy[: groups.n_groups] = groups.ploidy
+    out.allele_off[:] = groups.allele_off
+    out.allele_del_len[:n_al] = groups.gid_key["del_len"][groups.allele_gid]
+    out.allele_ins_len[:n_al] = groups.gid_key["ins_len"][groups.allele_gid]
+    at = f = 0
+    for g, x in enumerate(rows):
+        out.read_off[g], out.lnp_off[g] = at, f
+        for lnp, r in x:
+            out.allele_lnp[f : f + lnp.size] = lnp
+            out.read_length[at], out.non_ambig[at] = sample.read_len[r], sample.non_ambig[r]
+            out.is_fwd[at] = 1 if sample.read_flags[r] & A.SX_SIF_FWD else 0
+            at, f = at + 1, f + lnp.size
+    out.read_off[groups.n_groups], out.lnp_off[groups.n_groups] = at, f
     return out
 
 

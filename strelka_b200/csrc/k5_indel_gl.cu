@@ -8,8 +8,9 @@
 //
 // One warp per locus.  32 reads at a time: each lane evaluates its read's term for every genotype (double log-sum-exp with the
 // reference's log1p switch) into shared memory; lanes 0..G-1 then add the 32 terms of "their" genotype in read order, so the double
-// sums keep the reference's order.  Supporting-read counts come from ballots.  Values agree with the reference to the accuracy of
-// CUDA's double exp/log/log1p (<= 1 ulp each; tested at 1e-10 relative), the integer counts exactly.
+// sums keep the reference's order.  Supporting-read counts come from ballots.  exp / log / log1p are the libm mirrors of
+// sx_libm_mirror_d.h, so the double likelihoods are the reference's bits (tests/test_gpu_parity.py::test_k5_indel_gl compares them bit for
+// bit), and the integer counts are exact.
 #include "sx_device_util.cuh"
 #include "sx_internal.h"
 #include "sx_log_sum.cuh"

@@ -200,20 +200,10 @@ __global__ void k6b_flag_results_kernel(const uint32_t n_loci, const uint32_t* _
     }
 }
 
-int k6b_check_sample(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* s)
-{
-    if (!s) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL argument", what);
-    if (s->n_reads == 0) return SX_OK;
-    if (!s->region_read_off || !s->region_key_off || !s->rec_off || !s->recs || !s->n_rec || !s->read_len || !s->non_ambig || !s->read_flags || (s->n_keys && !s->key_gid))
-        return sx_fail(ctx, SX_ERR_ARG, "%s: NULL sample array", what);
-    if (s->n_regions == 0) return sx_fail(ctx, SX_ERR_ARG, "%s: reads without a region", what);
-    return SX_OK;
-}
-
 int k6b_check(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* normal, const sx_indel_reads_sample* tumor, const sx_indel_loci* loci)
 {
     int rc;
-    if ((rc = k6b_check_sample(ctx, what, normal)) || (rc = k6b_check_sample(ctx, what, tumor))) return rc;
+    if ((rc = sx_k6b_check_sample(ctx, what, normal)) || (rc = sx_k6b_check_sample(ctx, what, tumor))) return rc;
     return sx_k6b_check_loci(ctx, what, loci);
 }
 
@@ -224,6 +214,16 @@ int k6b_check_out(sx_ctx* ctx, const char* what, const sx_indel_reads_out* o)
 }
 
 } // namespace
+
+int sx_k6b_check_sample(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* s)
+{
+    if (!s) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL argument", what);
+    if (s->n_reads == 0) return SX_OK;
+    if (!s->region_read_off || !s->region_key_off || !s->rec_off || !s->recs || !s->n_rec || !s->read_len || !s->non_ambig || !s->read_flags || (s->n_keys && !s->key_gid))
+        return sx_fail(ctx, SX_ERR_ARG, "%s: NULL sample array", what);
+    if (s->n_regions == 0) return sx_fail(ctx, SX_ERR_ARG, "%s: reads without a region", what);
+    return SX_OK;
+}
 
 int sx_k6b_check_loci(sx_ctx* ctx, const char* what, const sx_indel_loci* loci)
 {
@@ -323,9 +323,10 @@ int sx_k6b_run(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* norma
 namespace
 {
 template <typename T> bool k6b_ends_at(const T* off, const uint32_t n, const uint32_t end) { return n == 0 || (off[0] == 0 && off[n] == end); }
+} // namespace
 
 // host staging of one sample: slots base .. base + 9
-int k6b_upload_sample(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* h, const int base, const uint32_t n_gid, sx_indel_reads_sample* d)
+int sx_k6b_upload_sample(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* h, const int base, const uint32_t n_gid, sx_indel_reads_sample* d)
 {
     *d = *h;
     if (h->n_reads == 0) return SX_OK;
@@ -349,7 +350,6 @@ int k6b_upload_sample(sx_ctx* ctx, const char* what, const sx_indel_reads_sample
     if (h->read_id && (rc = sx_upload(ctx, sx_host_slot(base + 9), h->read_id, n, d->read_id, 16))) return rc;
     return SX_OK;
 }
-} // namespace
 
 extern "C" int sx_link_indel_reads_dev(sx_ctx* ctx, const sx_indel_reads_sample* normal, const sx_indel_reads_sample* tumor, const sx_indel_loci* loci,
                                        sx_indel_reads_out* out_dev, uint32_t* totals_host)
@@ -394,7 +394,7 @@ extern "C" int sx_link_indel_reads(sx_ctx* ctx, const sx_indel_reads_sample* nor
     sx_call_timer t(ctx);
     sx_indel_reads_sample dn, dt;
     sx_indel_loci dl(*loci);
-    if ((rc = k6b_upload_sample(ctx, what, normal, 0, loci->n_gid, &dn)) || (rc = k6b_upload_sample(ctx, what, tumor, 10, loci->n_gid, &dt))) return rc;
+    if ((rc = sx_k6b_upload_sample(ctx, what, normal, 0, loci->n_gid, &dn)) || (rc = sx_k6b_upload_sample(ctx, what, tumor, 10, loci->n_gid, &dt))) return rc;
     if ((rc = sx_upload(ctx, sx_host_slot(20), loci->gid, n_loci, dl.gid, 16))) return rc;
     if ((rc = sx_upload(ctx, sx_host_slot(21), loci->gid_key, n_loci ? loci->n_gid : 0, dl.gid_key, 16))) return rc;
     // (key, is_forced_output and err_idx pass through to K5b; the link does not read them)

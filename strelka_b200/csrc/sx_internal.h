@@ -101,6 +101,11 @@ enum sx_slot : int
     // K6b's output where the library owns it: the sx_sindel_batch between the link and K5b (sx_somatic_indel_from_records_dev), and the
     // device side of sx_link_indel_reads
     SX_SLOT_K6B_OUT_ALT_OFF, SX_SLOT_K6B_OUT_ALTS, SX_SLOT_K6B_OUT_READ_OFF, SX_SLOT_K6B_OUT_READS, SX_SLOT_K6B_OUT_STATUS, SX_SLOT_K6B_OUT_TOTALS,
+    SX_SLOT_K6G_LIST_OF, SX_SLOT_K6G_LIST_OFF, SX_SLOT_K6G_CURSOR, SX_SLOT_K6G_DUP, SX_SLOT_K6G_SUMS, SX_SLOT_K6G_TOTAL64,
+    SX_SLOT_K6G_PAIR_ID, SX_SLOT_K6G_PAIR_REC, SX_SLOT_K6G_PAIR_READ, SX_SLOT_K6G_PAIR_ORDER,
+    // K6g's output where the library owns it: the sx_indel_batch between the link and K5 (sx_indel_gl_from_records_dev)
+    SX_SLOT_K6G_OUT_READ_OFF, SX_SLOT_K6G_OUT_LNP_OFF, SX_SLOT_K6G_OUT_ALLELE_OFF, SX_SLOT_K6G_OUT_PLOIDY, SX_SLOT_K6G_OUT_DEL_LEN, SX_SLOT_K6G_OUT_INS_LEN,
+    SX_SLOT_K6G_OUT_LNP, SX_SLOT_K6G_OUT_READ_LENGTH, SX_SLOT_K6G_OUT_NON_AMBIG, SX_SLOT_K6G_OUT_IS_FWD, SX_SLOT_K6G_OUT_STATUS, SX_SLOT_K6G_OUT_TOTALS,
     SX_SLOT_K7_READ_REGION, SX_SLOT_K7_ARENA, SX_SLOT_K7_ARENA_DEEP, SX_SLOT_K7_CNT_SEG, SX_SLOT_K7_CNT_KEY, SX_SLOT_K7_SUMS,
     SX_SLOT_K7_LOG, SX_SLOT_K7_LOG_OFF, SX_SLOT_K7_LOG_CURSOR, SX_SLOT_K7_RETRY1, SX_SLOT_K7_RETRY2, SX_SLOT_K7_RETRY_N, SX_SLOT_K7_ACTIVE,
     SX_SLOT_K7_CLASS, SX_SLOT_K7_HIST, SX_SLOT_K7_ACTIVE_BY_CLASS,
@@ -172,6 +177,8 @@ enum sx_status_bit : int
     SX_ST_INDEL_READS_DUP = 1 << 22, // K6b: one read id twice in a locus's list.  Like SX_ST_SINDEL_CAP a per-locus status (SX_INDEL_READS_ST_DUP_READ),
                                      // never in the device word
     SX_ST_K6B_ID = 1 << 23,      // K6b: a window index past its region's window, or an id at or past n_gid
+    SX_ST_K6G_GROUP = 1 << 24,   // K6g: a group with an allele count outside 1..SX_INDEL_MAX_ALLELES, a ploidy outside {1,2}, an id at or past n_gid,
+                                 // or offsets that do not start at 0 and ascend
 };
 static_assert(SX_ST_SINDEL_CAP == SX_SINDEL_ST_CAP, "the per-locus capacity status of K5b is its status bit");
 
@@ -350,6 +357,9 @@ int sx_k6b_run(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* norma
                uint32_t* totals_host, bool own_out, unsigned* launches);
 // K6b's argument checks of the loci, reported under `what`
 int sx_k6b_check_loci(sx_ctx* ctx, const char* what, const sx_indel_loci* loci);
+// ... of one sample (K6b and K6g), and the host staging of one sample's arrays into host slots base .. base + 9 (ids checked against n_gid)
+int sx_k6b_check_sample(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* s);
+int sx_k6b_upload_sample(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* h, int base, uint32_t n_gid, sx_indel_reads_sample* d);
 // The link's offset, status and totals arrays in the context's SX_SLOT_K6B_OUT_* buffers (its entries and alternates are taken by sx_k6b_run
 // with own_out once their totals are known), and the sx_sindel_batch they form with the loci
 int sx_k6b_own_out(sx_ctx* ctx, uint32_t n_loci, sx_indel_reads_out* o);
@@ -359,6 +369,11 @@ sx_sindel_batch sx_sindel_batch_of(const sx_indel_loci* loci, const sx_indel_rea
 // caller (sx_k5b_check); the status word is the caller's to read.
 int sx_sindel_from_links_run(sx_ctx* ctx, const sx_sindel_opts* opts, const sx_indel_loci* loci, const sx_indel_reads_out* o, const double* err_prob, uint32_t n_err,
                              sx_sindel_result* out_dev, unsigned* launches);
+// K6g: one sample's K6 records -> K5's per-group read lists.  totals_host receives {reads, allele_lnp floats} (also on SX_ERR_CAPACITY).
+// own_out: the allele and per-read arrays are taken from the context's SX_SLOT_K6G_OUT_* buffers once the totals are known, instead of checked
+// against the caller's capacities.  The status word (SX_ST_K6G_GROUP, SX_ST_K6B_ID) is the caller's to read.
+int sx_k6g_run(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* sample, const sx_allele_groups* groups, sx_allele_group_reads_out* out_dev,
+               uint32_t* totals_host, bool own_out, unsigned* launches);
 int sx_k7g_run(sx_ctx* ctx, const sx_gate_batch* d, const sx_gate_out* o, unsigned* launches);
 int sx_k7a_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_region* regions, const uint8_t* seq4, const char* ref, const uint32_t* key_ins_off, const char* key_ins,
                const sx_prep_out* o, unsigned* launches);
