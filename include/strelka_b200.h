@@ -335,10 +335,15 @@ typedef struct sx_ssnv_result { /* somatic_snv_genotype_grid + snv_result_set */
     float tumor_lhood[30];
     float strandBias;
     uint32_t ref_gt;
-    uint32_t is_computed;        /* 0: early return; nothing below is meaningful */
+    uint32_t is_computed;        /* 0: an 'N' reference, an all-reference tier1 view, or QSS 0 unforced; every other field is then 0,
+                                    except ref_gt, which is set unless the reference base is 'N' */
     uint32_t snv_tier;
     uint32_t snv_from_ntype_tier;
-    uint32_t ntype;              /* NTYPE: REF 0, HOM 1, HET 2, CONFLICT 3 */
+    uint32_t ntype;              /* NTYPE: REF 0, HOM 1, HET 2, CONFLICT 3.  A tier whose six posteriors are all NaN (a quality-0 call can
+                                    make a whole term list -inf; a non-strand shared-site error rate below 0 after its float rounding makes
+                                    ln of it NaN) has QSS 3070 and QSS_NT 0, as the reference's, and NTYPE REF here; the reference leaves
+                                    that tier's ntype unassigned (its snv_result_set is default-initialised and qscore_calculator.cpp:201
+                                    never holds), so its value there is unspecified */
     uint32_t max_gt;
     int32_t qphred;              /* QSS */
     int32_t from_ntype_qphred;   /* QSS_NT */

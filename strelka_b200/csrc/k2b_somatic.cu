@@ -117,6 +117,9 @@ __device__ __forceinline__ sample_acc accumulate_sample(const som_tables& T, con
         const float e = sx_expf(f_sub(x2, x1));
         const float l = (fabsf(e) < 0.01f) ? static_cast<float>(sx_log1p(static_cast<double>(e))) : sx_logf(f_add(1.0f, e));
         lh = f_add(f_add(x1, l), ln_one_half);
+        // A quality-0 reference call on each strand makes both sums -inf and x2 - x1 NaN.  The reference's x86-64 float arithmetic makes that
+        // the default NaN 0xffc00000, which expf, logf and the additions pass on; the device's arithmetic returns 0x7fffffff instead.
+        if (isnan(lh)) lh = __uint_as_float(0xffc00000u);
     }
     // get_most_frequent_alt_id  (blt_common/snp_pos_info.hh:175-198): first strict maximum over base ids != ref
     uint32_t alt_id = ref_gt, max_count = 0;
@@ -200,6 +203,9 @@ __global__ void __launch_bounds__(K2B_WARPS * 32) k2b_somatic_kernel(const uint3
             uint32_t* w = reinterpret_cast<uint32_t*>(res);
             for (uint32_t i = lane; i < sizeof(sx_ssnv_result) / 4; i += 32) w[i] = 0u;
         }
+        // Every lane of the warp reaches this barrier once per site (site, and each branch below, is warp-uniform), and it comes before the
+        // site's first write to s_nl / s_tl / s_scr: it orders the previous site's cross-lane reads of them (:251-253, result_set_grid)
+        // before those writes, including when that site left through one of the `continue`s below without reaching the barrier at its end.
         __syncwarp();
         const char rb = ref_base[site];
         const uint32_t ref_gt = rb == 'A' ? 0u : rb == 'C' ? 1u : rb == 'G' ? 2u : rb == 'T' ? 3u : 4u;

@@ -840,3 +840,179 @@ def raw_alignments_for(eb, case: int):
 
 
 GATES_GOLDEN_CASES = 12
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# K2b / K5 edge batches, run at every parameter point of tests/site_params.py
+# ------------------------------------------------------------------------------------------------------------------------------
+SOMATIC_EDGE_KINDS = ("plain", "normal_empty", "tumor_empty", "both_empty", "q_extreme", "t1_tier_filtered", "t1_all_filtered", "n_ref", "alt_tie", "deep",
+                      "t1_weak")
+# the kinds that are computed only when forced: both samples empty, or no tier1 call left in either (an all-reference tier1 view ends the
+# site before the model, position_somatic_snv_strand_grid.cpp:253).  An 'N' reference is never computed.  A tier1 result of qphred 0
+# ("t1_weak") makes the tier2 result a copy of it (:272-277), which is reported only when forced (:311-312).
+SOMATIC_FORCED_ONLY_KINDS = ("both_empty", "t1_all_filtered")
+_ORD_Q = np.array([11, 17, 25, 30, 37, 40, 41, 60], np.uint8)
+_ORD_Q_P = np.array([0.04, 0.04, 0.1, 0.1, 0.5, 0.1, 0.08, 0.04])
+
+
+def _edge_calls(rng, n, ref_id, mix, q=None, filt=0.0, tfilt=0.0):
+    """n calls: base ids drawn from mix {base_id: weight} (the rest of the weight goes to ref_id), ordinary qualities unless `q` is
+    given, both strands, a few neighbour mismatches, a fraction `filt` filtered of which a fraction `tfilt` tier-specifically."""
+    ids = [ref_id] + list(mix)
+    w = np.array([max(0.0, 1.0 - sum(mix.values()))] + list(mix.values()))
+    base = rng.choice(np.array(ids), size=n, p=w / w.sum()) if n else np.zeros(0, np.int64)
+    if q is None:
+        q = rng.choice(_ORD_Q, size=n, p=_ORD_Q_P)
+    f = rng.random(n) < filt
+    tf = f & (rng.random(n) < tfilt)
+    return list(B.pack_call(q, base, rng.random(n) < 0.5, rng.random(n) < 0.1, f, tf))
+
+
+def somatic_edge_sites(rng: np.random.Generator, reps: int = 120):
+    """-> (normal PileupBatch, tumor PileupBatch, forced[n], kind[n]): `reps` sites of each SOMATIC_EDGE_KINDS kind in random order,
+    about 40% of them forced, tier2 calls on both samples (somatic_tier2_view drops them).  Kinds: ordinary sites; an empty normal,
+    tumor or both; qualities 0, 1 and 63 among ordinary ones; tier1 calls mostly filtered, tier-specifically, so that they survive into
+    the tier2 view; every tier1 call filtered; an 'N' reference; two or three alt bases of equal count; several hundred calls per
+    sample; a tier1 view too weak for a call with a strong tier2 one."""
+    kinds = rng.permutation(np.repeat(np.arange(len(SOMATIC_EDGE_KINDS)), reps))
+    sn, st, sn2, st2, refs = [], [], [], [], []
+    for k in kinds.tolist():
+        kind = SOMATIC_EDGE_KINDS[k]
+        ref_id = int(rng.integers(0, 4))
+        alt = (ref_id + int(rng.integers(1, 4))) % 4
+        noise = {alt: float(rng.choice([0.0, 0.0, 0.01, 0.02]))}
+        taf = {alt: float(rng.choice([0.05, 0.15, 0.3, 0.5]))}
+        n_n, n_t = int(rng.poisson(30)), int(rng.poisson(50))
+        m_n, m_t = int(rng.poisson(4)), int(rng.poisson(8))
+        nmix, tmix, t2mix = noise, taf, taf
+        nkw, tkw = {}, {}
+        ref = BASES[ref_id]
+        if kind == "normal_empty":
+            n_n = m_n = 0
+        elif kind == "tumor_empty":
+            n_t = m_t = 0
+            nmix = {alt: float(rng.choice([0.0, 0.3, 0.5]))}
+        elif kind == "both_empty":
+            n_n = m_n = n_t = m_t = 0
+        elif kind == "q_extreme":
+            for kw, nn in ((nkw, n_n), (tkw, n_t)):
+                q = rng.choice(_ORD_Q, size=nn, p=_ORD_Q_P)
+                x = rng.random(nn) < float(rng.choice([0.1, 0.3, 0.6]))
+                q[x] = rng.choice(np.array([0, 1, 63], np.uint8), size=int(x.sum()))
+                kw["q"] = q
+        elif kind == "t1_tier_filtered":
+            nkw = dict(filt=0.3, tfilt=0.8)
+            tkw = dict(filt=float(rng.choice([0.5, 0.7, 0.9])), tfilt=0.85)
+        elif kind == "t1_all_filtered":
+            nkw = tkw = dict(filt=1.0, tfilt=0.5)
+        elif kind == "n_ref":
+            ref = "N"
+        elif kind == "alt_tie":
+            others = [b for b in range(4) if b != ref_id]
+            rng.shuffle(others)
+            c = int(rng.integers(1, 12))
+            ties = others[: int(rng.choice([2, 2, 3]))]
+            nr = int(rng.poisson(30))
+            sample = [ref_id] * nr + [b for b in ties for _ in range(c)]
+            sample = [sample[i] for i in rng.permutation(len(sample))]
+            n_t, tmix = len(sample), None
+            tkw = dict(base=np.array(sample))
+            if rng.random() < 0.5:  # a tie in the normal as well
+                nsample = [ref_id] * int(rng.poisson(30)) + ties[:2] * int(rng.integers(1, 3))
+                n_n, nmix, nkw = len(nsample), None, dict(base=np.array(nsample))
+        elif kind == "deep":
+            n_n, n_t = int(rng.integers(300, 800)), int(rng.integers(300, 800))
+            tmix = {alt: float(rng.choice([0.02, 0.05, 0.1, 0.3]))}
+        elif kind == "t1_weak":
+            n_t, tmix = int(rng.integers(40, 80)), {alt: 1.0 / 80}
+            m_t, t2mix = int(rng.integers(15, 40)), {alt: 0.5}
+
+        def calls(n, mix, kw):
+            if "base" in kw:  # the exact base sequence given
+                b = kw["base"]
+                return list(B.pack_call(rng.choice(_ORD_Q, size=len(b), p=_ORD_Q_P), b, rng.random(len(b)) < 0.5, 0, 0, 0))
+            return _edge_calls(rng, n, ref_id, mix, **kw)
+
+        sn.append(calls(n_n, nmix, nkw))
+        st.append(calls(n_t, tmix, tkw))
+        # tier2 calls: a third of them filtered (a filtered tier2 call never survives)
+        sn2.append(_edge_calls(rng, m_n, ref_id, nmix or noise, filt=0.3))
+        st2.append(_edge_calls(rng, m_t, ref_id, t2mix or taf, filt=0.3))
+        refs.append(ref)
+    refs = "".join(refs)
+    forced = (rng.random(len(kinds)) < 0.4).astype(np.uint8)
+    return B.PileupBatch.from_sites(sn, refs, None, sn2), B.PileupBatch.from_sites(st, refs, None, st2), forced, kinds.astype(np.uint8)
+
+
+SOMATIC_TIER2_MODES = ("both", "neither", "normal_only", "tumor_only")
+
+
+def somatic_tier2_view(npb, tpb, mode: str):
+    """the pair with tier2 calls on both samples, on neither, or on one only (the ABI then evaluates tier1 only, like the reference's
+    is_tier2 = both samples have them)"""
+    keep_n, keep_t = {"both": (True, True), "neither": (False, False), "normal_only": (True, False), "tumor_only": (False, True)}[mode]
+
+    def view(pb, keep):
+        return pb if keep else B.PileupBatch(pb.site_off, pb.calls, pb.ref_base, pb.ploidy)
+
+    return view(npb, keep_n), view(tpb, keep_t)
+
+
+def pileup_take(pb, idx) -> "B.PileupBatch":
+    """the sites idx[0], idx[1], ... of pb as a new batch (calls, tier2 calls, reference bases)"""
+    idx = np.asarray(idx, np.int64)
+
+    def gather(off, calls):
+        off = off.astype(np.int64)
+        depth = off[idx + 1] - off[idx]
+        new_off = np.concatenate([[0], np.cumsum(depth)])
+        src = np.repeat(off[idx] - new_off[:-1], depth) + np.arange(int(new_off[-1]))
+        return new_off.astype(np.uint32), calls[src]
+
+    off, calls = gather(pb.site_off, pb.calls)
+    t2_off = t2_calls = None
+    if pb.t2_off is not None:
+        t2_off, t2_calls = gather(pb.t2_off, pb.t2_calls)
+    return B.PileupBatch(off, calls, pb.ref_base[idx], None if pb.ploidy is None else pb.ploidy[idx], t2_off, t2_calls)
+
+
+INDEL_EDGE_READ_COUNTS = (0, 1, 31, 32, 33, 63, 64, 65)  # K5 evaluates 32 reads per step
+
+
+def indel_edge_loci(rng: np.random.Generator, reps: int = 2):
+    """K5 loci: every read count of INDEL_EDGE_READ_COUNTS with A = 1..4 alleles at ploidy 1 and 2 (ploidy 2 with four alleles has
+    SX_INDEL_MAX_GT = 15 genotypes), `reps` times.  Allele lengths from 0 to past the read length; read lengths and non-ambiguous base
+    counts from 0 up, many below twice the largest flank; per read one strongly supported allele, an exact tie of two or more
+    alleles, all alleles equal, or scores close together (posteriors near the support thresholds)."""
+    lens = np.array([0, 0, 1, 2, 5, 20, 39, 40, 41, 79, 80, 81, 200], np.int64)
+    loci = []
+    for _ in range(reps):
+        for n in INDEL_EDGE_READ_COUNTS:
+            for A_ in range(1, 5):
+                for ploidy in (1, 2):
+                    alleles = []
+                    for _a in range(A_):
+                        d, i = int(rng.choice(lens)), int(rng.choice(lens))
+                        u = rng.random()
+                        alleles.append((max(d, 1), 0) if u < 0.4 else (0, max(i, 1)) if u < 0.8 else (d, i))
+                    reads = []
+                    for _r in range(n):
+                        rl = int(rng.choice([1, 8, 20, 50, 78, 79, 80, 81, 100, 150, 151, 300]))
+                        na = int(rng.choice([rl, rl, max(0, rl - 3), int(rng.integers(0, rl + 1))]))
+                        u = rng.random()
+                        v = rng.normal(-60.0, 15.0, A_ + 1)
+                        if u < 0.4:
+                            v[int(rng.integers(0, A_ + 1))] = rng.normal(-8.0, 4.0)
+                        elif u < 0.65:
+                            tie = rng.choice(A_ + 1, size=int(rng.integers(2, A_ + 2)), replace=False)
+                            v[tie] = rng.normal(-8.0, 4.0)
+                        elif u < 0.75:
+                            v[:] = v[0]
+                        else:
+                            v = rng.normal(-10.0, 1.0, A_ + 1)
+                        v = np.minimum(v, -0.01)
+                        if rng.random() < 0.05:
+                            v[int(rng.integers(0, A_ + 1))] = -1000.0
+                        reads.append(([float(np.float32(x)) for x in v], rl, na, int(rng.random() < 0.5)))
+                    loci.append({"ploidy": ploidy, "alleles": alleles, "reads": reads})
+    return loci
