@@ -1292,6 +1292,105 @@ int sx_process_somatic_window_dev(sx_ctx* ctx, const sx_somatic_window_batch* ba
 int sx_last_somatic_window_timing(const sx_ctx* ctx, float* ms);
 
 /* ==========================================================================================
+ * K2c  site_continuous
+ *   replaces the germline caller's continuous-frequency site model (--call-continuous-vf):
+ *   starling_pos_processor::process_pos_snp's skip test (applications/starling/starling_pos_processor.cpp:154-172), CleanPileupFilter
+ *   (tier1), process_pos_snp_continuous (:926-996), updateContinuousSnvLocusWithSampleInfo (:751-881), updateContinuousSnvLocusInfo
+ *   (:885-921) and starling_continuous_variant_caller's getAlleleSequencingErrorQscore / strandBias.
+ *
+ * A batch is S samples (1..SX_CONT_MAX_SAMPLES) over the same n_sites consecutive positions pos_begin, pos_begin + 1, ...  Sample s is an
+ * sx_pileup_batch whose tier1 calls are used; its t2 arrays and ploidy are not read, and only sample 0's ref_base is read.  Calls with a
+ * base id of 4 or more count as ANY ('N').
+ *
+ * Per site:
+ *   - No records when the site is not forced and every sample's raw column (filtered calls included) is empty.
+ *   - The candidate loci are the bases 0..3 other than the reference base, in that order (four of them under an 'N' reference).  An alt
+ *     locus is reported when the site is forced or some sample's AF > min_het_vf.  If none is reported, the reference locus
+ *     (alt = SX_CONT_REF_LOCUS) is reported once.  Records come in that order, sites ascending.
+ *   - Per (locus, sample), over the sample's cleaned calls (is_call_filter == 0):
+ *       AD: ANY calls skipped; reference- and alt-base calls per strand, every other base to non_confident per strand.  Under an 'N'
+ *           reference the reference counts are 0.  The reference locus has no alt: its alt counts are 0.
+ *       total_depth = every non-ANY cleaned call; allele_depth = the alt's count (the reference's for the reference locus);
+ *       af = allele_depth / total_depth (0 when total_depth is 0);
+ *       gt: SX_CONT_GT_HOMREF for the reference locus, else HOM if af >= 1 - min_het_vf, HOMREF if af < min_het_vf, else HET;
+ *       gq = getAlleleSequencingErrorQscore(allele_depth, total_depth, expected_qscore, max_qscore) (it is also GQX);
+ *       strand_bias: strandBias(fwdAlt, revAlt, fwdOther, revOther) over all cleaned calls (ANY and the reference count as other),
+ *           clamped to +-max_abs_sample_strand_bias as std::min(M, std::max(-M, sb)) (a NaN becomes -M); 0 for the reference locus.
+ *       used / unused: the cleaned calls and the filtered ones.  The reference's spanningDeletionReadCount here is the cleaned pileup's,
+ *           which CleanPileupFilter resets to 0 and never sets, so it adds nothing to total_depth and is not an output.
+ *   - Per locus: qual = the largest sample gq (0 for the reference locus); strand_bias = strandBias of the four strand counts summed over
+ *     the samples, unclamped (0 with zero counts for the reference locus).
+ *
+ * Numerics.  Every integer and af are exact.  gq comes from a double evaluation of x = -10 log10(gamma_p(a, n * 10^(-q/10))) whose error
+ * bound is stated in k2c_core.cuh; when x + 0.5 lies within that bound of an integer in 1..max_qscore the sample entry's status gets
+ * SX_CONT_ST_QSCORE_TIE (its gq is then the device's rounding, which may differ from the reference's).  The strand biases are doubles
+ * within a measured bound of the reference's x87 evaluation (DESIGN.md section 3); a NaN is stored as the x86-64 default NaN.
+ * ======================================================================================== */
+#define SX_CONT_MAX_SAMPLES 8
+#define SX_CONT_REF_LOCUS 4          /* sx_cont_locus.alt of the reference locus */
+#define SX_CONT_GT_HOMREF 0          /* 0/0 */
+#define SX_CONT_GT_HET 1             /* 0/1 */
+#define SX_CONT_GT_HOM 2             /* 1/1 */
+#define SX_CONT_ST_QSCORE_TIE 0x2000000 /* per-entry status: the qscore's rounding is within the error bound of a boundary */
+
+typedef struct sx_cont_opts { /* starling_base_options / starling_options fields of the model */
+    double min_het_vf;                 /* 0.01; must lie in (0, 0.5), as the reference asserts */
+    double max_abs_sample_strand_bias; /* maxAbsSampleVariantStrandBias, 99; >= 0 */
+    int32_t expected_qscore;           /* continuousFrequencyCallerExpectedObservationQuality, 17; 0..70 */
+    int32_t max_qscore;                /* continuousFrequencyCallerMaxQscore, 40; 0..1000 */
+} sx_cont_opts;
+void sx_default_cont_opts(sx_cont_opts* o);
+
+typedef struct sx_cont_batch {
+    uint32_t n_sites;
+    uint32_t n_samples;                         /* 1..SX_CONT_MAX_SAMPLES */
+    int32_t pos_begin;                          /* position of site 0 (written to the records) */
+    uint32_t pad;
+    const uint8_t* forced_output;               /* [n_sites] nonzero: forced output position; NULL: none */
+    sx_pileup_batch sample[SX_CONT_MAX_SAMPLES]; /* each with n_sites sites */
+} sx_cont_batch;
+
+typedef struct sx_cont_locus { /* one record (GermlineContinuousSiteLocusInfo), 40 bytes */
+    double strand_bias;  /* the allele's strandBias over the samples' summed counts */
+    int32_t pos;
+    int32_t qual;        /* anyVariantAlleleQuality */
+    uint32_t sb_fwd_alt, sb_rev_alt, sb_fwd_other, sb_rev_other;
+    uint8_t alt;         /* 0..3, or SX_CONT_REF_LOCUS */
+    uint8_t ref;         /* base_to_id of the reference base: 0..3, 4 for 'N' */
+    uint8_t forced;      /* the position is forced output */
+    uint8_t pad[5];
+} sx_cont_locus;
+
+typedef struct sx_cont_sample { /* one (record, sample) entry, 72 bytes */
+    double af;
+    double strand_bias;  /* clamped */
+    uint32_t ref_fwd, ref_rev, alt_fwd, alt_rev, non_confident_fwd, non_confident_rev;
+    uint32_t total_depth, allele_depth, used, unused;
+    int32_t gq;
+    uint32_t status;     /* SX_CONT_ST_* */
+    uint8_t gt;          /* SX_CONT_GT_* */
+    uint8_t pad[7];
+} sx_cont_sample;
+
+typedef struct sx_cont_out { /* caller-allocated */
+    sx_cont_locus* loci;     /* [cap_loci] */
+    sx_cont_sample* samples; /* [cap_loci * n_samples]: record r's sample s at r * n_samples + s */
+    uint32_t* site_rec_off;  /* [n_sites + 1] or NULL: site i's records are site_rec_off[i] .. site_rec_off[i + 1] */
+    uint32_t cap_loci;
+    uint32_t pad;
+} sx_cont_out;
+
+/* totals_host ([1], may be NULL) receives the record count.  A capacity below it returns SX_ERR_CAPACITY with totals and site_rec_off
+ * written and no record.  Bad options, a sample count outside 1..SX_CONT_MAX_SAMPLES, a sample with another n_sites or a NULL array:
+ * SX_ERR_ARG.  The _dev form takes the batch's arrays and the outputs in device memory (the structs themselves are host memory). */
+int sx_site_continuous(sx_ctx* ctx, const sx_cont_opts* opts, const sx_cont_batch* batch_host, const sx_cont_out* out_host, uint32_t* totals_host);
+int sx_site_continuous_dev(sx_ctx* ctx, const sx_cont_opts* opts, const sx_cont_batch* batch_dev, const sx_cont_out* out_dev, uint32_t* totals_host);
+/* getAlleleSequencingErrorQscore(a[i], n[i], expected_qscore, max_qscore) for n_pairs pairs -> gq[i], status[i] (SX_CONT_ST_QSCORE_TIE);
+ * the _dev form on device arrays */
+int sx_cont_qscore(sx_ctx* ctx, const sx_cont_opts* opts, uint32_t n_pairs, const uint32_t* a, const uint32_t* n, int32_t* gq, uint32_t* status);
+int sx_cont_qscore_dev(sx_ctx* ctx, const sx_cont_opts* opts, uint32_t n_pairs, const uint32_t* a, const uint32_t* n, int32_t* gq, uint32_t* status);
+
+/* ==========================================================================================
  * Multi-GPU: regions shard across ranks with no data-path collective; one gather of fixed-size
  * call records at the end (the in-memory analogue of concatIndexVcf,
  * src/python/lib/strelkaSharedWorkflow.py:126-136).  The NCCL communicator is created from an

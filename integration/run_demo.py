@@ -2,7 +2,8 @@
 """integration/run_demo.py -- runs the reference's bundled demo (SURVEY.md Appendix B: the command lines the python2 workflows would issue) with a
 binary from oracle/_ref/bin/ on the inputs staged under oracle/_ref/demo/ and returns the VCF bodies.
     python integration/run_demo.py somatic strelka2_sx /tmp/out      ->  /tmp/out/snvs.vcf, indels.vcf
-    python integration/run_demo.py germline starling2_sx /tmp/out    ->  /tmp/out/seg.variants.vcf, seg.genome.S1.vcf, seg.genome.S2.vcf"""
+    python integration/run_demo.py germline starling2_sx /tmp/out    ->  /tmp/out/seg.variants.vcf, seg.genome.S1.vcf, seg.genome.S2.vcf
+    python integration/run_demo.py mito starling2_sx /tmp/out        ->  /tmp/out/seg.variants.vcf, seg.genome.S1.vcf (chrM, --call-continuous-vf)"""
 import gzip
 import os
 import subprocess
@@ -32,6 +33,15 @@ def run(mode, binary, out, env=None, timeout=1200):
                f"{Cf}/somaticIndelScoringModels.json", "--normal-align-file", f"{D}/NA12892_demo20.bam", "--tumor-align-file", f"{D}/NA12891_demo20.bam",
                "--somatic-snv-file", f"{out}/snvs.vcf", "--somatic-indel-file", f"{out}/indels.vcf", "--stats-file", f"{out}/stats.xml"]
         files = ["snvs.vcf", "indels.vcf"]
+    elif mode == "mito":
+        # strelkaGermlineWorkflow.py:81-148 for the one chrM segment of runMitoWorkflowDemo.bash (--exome --callContinuousVf chrM): no EVS model
+        # files, the default indel error model, the VF header and --call-continuous-vf
+        M = os.path.join(DEMO, "dataMito")
+        cmd = [exe, "--region", "chrM:1-16571", "--ref", f"{M}/chrM_hg19.fa", "--max-indel-size", "49", "--min-mapping-quality", "20", "--gvcf-output-prefix",
+               f"{out}/seg.", "--gvcf-min-gqx", "15", "--gvcf-min-homref-gqx", "15", "--gvcf-max-snv-strand-bias", "10", "--enable-read-backed-phasing",
+               "--stats-file", f"{out}/stats.xml", "--align-file", f"{M}/NA12878_chrM_200-200.bam", "--gvcf-include-header", "VF", "--call-continuous-vf",
+               "--indel-error-models-file", f"{Cf}/indelErrorModel.json", "--theta-file", f"{Cf}/theta.json"]
+        files = ["seg.variants.vcf", "seg.genome.S1.vcf"]
     else:
         cmd = [exe, "--region", "demo20:1-5000", "--ref", f"{D}/demo20.fa", "--max-indel-size", "49", "--min-mapping-quality", "20", "--gvcf-output-prefix", f"{out}/seg.",
                "--gvcf-min-gqx", "15", "--gvcf-min-homref-gqx", "15", "--gvcf-max-snv-strand-bias", "10", "--enable-read-backed-phasing", "--stats-file", f"{out}/stats.xml",

@@ -16,6 +16,7 @@
 #include "blt_common/snp_pos_info.hh"
 #include "blt_util/blt_exception.hh"
 
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <memory>
@@ -34,15 +35,19 @@ inline bool enabled()
 
 struct Counters
 {
-    unsigned long long site_gl_germline = 0, site_gl_somatic = 0, global_align = 0, somatic_indel = 0, germline_indel = 0;
+    unsigned long long site_gl_germline = 0, site_gl_somatic = 0, global_align = 0, somatic_indel = 0, germline_indel = 0, continuous_site = 0;
     bool germline_indel_route = false; // set by the translation unit that routes germline indel genotyping (SX_SHIM_GERMLINE)
+    bool continuous_route = false;     // ... and continuous-frequency sites (SX_SHIM_CONTINUOUS)
     ~Counters()
     {
         // (fields are read by position: a new counter goes at the end, and only binaries with its route print it)
         if (std::getenv("SX_SHIM_REPORT"))
             std::fprintf(stderr, "sx_shim: %llu germline site calls, %llu somatic site calls, %llu haplotype alignments through libstrelka_b200.so, %llu somatic indel calls%s",
                          site_gl_germline, site_gl_somatic, global_align, somatic_indel, germline_indel_route ? ", " : "\n");
-        if (std::getenv("SX_SHIM_REPORT") && germline_indel_route) std::fprintf(stderr, "%llu germline indel calls\n", germline_indel);
+        // the continuous-site counter is appended only when that route ran, so the line of a diploid run is the one it has always been
+        const bool cont(continuous_route && continuous_site > 0);
+        if (std::getenv("SX_SHIM_REPORT") && germline_indel_route) std::fprintf(stderr, "%llu germline indel calls%s", germline_indel, cont ? ", " : "\n");
+        if (std::getenv("SX_SHIM_REPORT") && cont) std::fprintf(stderr, "%llu continuous site calls\n", continuous_site);
     }
 };
 inline Counters& counters()
@@ -406,6 +411,112 @@ inline void germline_indel(const starling_base_options& opt, const starling_base
             if (r.support[s][a]) c.incrementAlleleCount(a, r.support[s][a]);
         c.nonConfidentCount += r.support[s][SX_INDEL_MAX_ALLELES + 1];
     }
+}
+#endif
+
+#ifdef SX_SHIM_CONTINUOUS
+inline bool register_continuous_route()
+{
+    counters().continuous_route = true;
+    return true;
+}
+static const bool continuous_route_registered = register_continuous_route();
+
+inline sx_cont_opts cont_opts_of(const starling_options& opt)
+{
+    sx_cont_opts o;
+    sx_default_cont_opts(&o);
+    o.min_het_vf = opt.min_het_vf;
+    o.max_abs_sample_strand_bias = opt.maxAbsSampleVariantStrandBias;
+    o.expected_qscore = opt.continuousFrequencyCallerExpectedObservationQuality;
+    o.max_qscore = opt.continuousFrequencyCallerMaxQscore;
+    return o;
+}
+
+/// K2c's records of one position (process_pos_snp_continuous, applications/starling/starling_pos_processor.cpp:926-996) from every sample's RAW
+/// column; the caller builds the loci from them with the reference's own updateSiteSampleInfo / updateContinuousSiteSampleInfo / add_site.
+struct ContinuousSite
+{
+    std::vector<sx_cont_locus> loci;
+    std::vector<sx_cont_sample> samples; // record r's sample s at r * n_samples + s
+};
+
+inline void continuous_site(const starling_options& opt, const std::vector<const snp_pos_info*>& raw, const char ref_base, const bool forced, const pos_t pos,
+                            ContinuousSite& out)
+{
+    sx_ctx* ctx(context(params_of(opt)));
+    const sx_cont_opts o(cont_opts_of(opt));
+    const uint32_t S(static_cast<uint32_t>(raw.size()));
+    const uint16_t none(0);
+    const uint8_t f(forced ? 1 : 0);
+    uint32_t off[SX_CONT_MAX_SAMPLES][2];
+    sx_cont_batch b;
+    std::memset(&b, 0, sizeof(b));
+    b.n_sites = 1;
+    b.n_samples = S;
+    b.pos_begin = static_cast<int32_t>(pos);
+    b.forced_output = &f;
+    for (uint32_t s = 0; s < S; ++s)
+    {
+        off[s][0] = 0;
+        off[s][1] = static_cast<uint32_t>(raw[s]->calls.size());
+        b.sample[s].n_sites = 1;
+        b.sample[s].site_off = off[s];
+        b.sample[s].calls = raw[s]->calls.empty() ? &none : words(raw[s]->calls);
+        b.sample[s].ref_base = &ref_base;
+    }
+    out.loci.resize(4);
+    out.samples.resize(4 * S);
+    uint32_t rec_off[2], total(0);
+    sx_cont_out co;
+    std::memset(&co, 0, sizeof(co));
+    co.loci = out.loci.data();
+    co.samples = out.samples.data();
+    co.site_rec_off = rec_off;
+    co.cap_loci = 4;
+    check(ctx, sx_site_continuous(ctx, &o, &b, &co, &total));
+    out.loci.resize(total);
+    out.samples.resize((size_t)total * S);
+    ++counters().continuous_site;
+}
+
+/// The K2c strand bias is within 1e-9 of the reference's (DESIGN.md section 3).  Within that of a multiple of 0.05 -- a boundary of the
+/// one-decimal SB / SNVSB print or of the HighSNVSB threshold -- the reference's own strandBias decides.
+inline bool near_strand_bias_boundary(const double sb)
+{
+    if (!std::isfinite(sb)) return false;
+    const double k(std::floor(sb / 0.05 + 0.5));
+    return std::fabs(sb - k * 0.05) < 1e-9;
+}
+
+/// the sample strand bias of updateContinuousSnvLocusWithSampleInfo (:789-824) from the cleaned calls, by the reference's function
+inline double reference_sample_strand_bias(const snp_pos_info& cleaned, const unsigned alt)
+{
+    unsigned fa(0), ra(0), fo(0), ro(0);
+    for (const base_call& bc : cleaned.calls)
+    {
+        if (bc.is_fwd_strand) (bc.base_id == alt ? fa : fo)++;
+        else (bc.base_id == alt ? ra : ro)++;
+    }
+    return starling_continuous_variant_caller::strandBias(fa, ra, fo, ro);
+}
+
+/// getAlleleSequencingErrorQscore(a, n, ...) of the continuous indel genotype (starling_pos_processor.cpp:2026-2030) through sx_cont_qscore; a
+/// tie-flagged answer is the reference function's
+inline int cont_qscore(const starling_base_options& opt, const unsigned a, const unsigned n)
+{
+    sx_ctx* ctx(context(params_of(opt)));
+    sx_cont_opts o;
+    sx_default_cont_opts(&o);
+    o.expected_qscore = opt.continuousFrequencyCallerExpectedObservationQuality;
+    o.max_qscore = opt.continuousFrequencyCallerMaxQscore;
+    int32_t gq(0);
+    uint32_t st(0);
+    check(ctx, sx_cont_qscore(ctx, &o, 1, &a, &n, &gq, &st));
+    if (st & SX_CONT_ST_QSCORE_TIE)
+        return starling_continuous_variant_caller::getAlleleSequencingErrorQscore(a, n, opt.continuousFrequencyCallerExpectedObservationQuality,
+                                                                                  opt.continuousFrequencyCallerMaxQscore);
+    return gq;
 }
 #endif
 } // namespace sx_shim

@@ -417,6 +417,31 @@ class SxPileupBatch(C.Structure):
     ]
 
 
+# K2c site_continuous
+SX_CONT_MAX_SAMPLES = 8
+SX_CONT_REF_LOCUS = 4
+SX_CONT_GT_HOMREF, SX_CONT_GT_HET, SX_CONT_GT_HOM = 0, 1, 2
+SX_CONT_ST_QSCORE_TIE = 0x2000000
+CONT_LOCUS_DT = np.dtype([("strand_bias", "<f8"), ("pos", "<i4"), ("qual", "<i4"), ("sb_fwd_alt", "<u4"), ("sb_rev_alt", "<u4"), ("sb_fwd_other", "<u4"),
+                          ("sb_rev_other", "<u4"), ("alt", "u1"), ("ref", "u1"), ("forced", "u1"), ("pad", "u1", (5,))])
+CONT_SAMPLE_DT = np.dtype([("af", "<f8"), ("strand_bias", "<f8")] + [(n, "<u4") for n in (
+    "ref_fwd", "ref_rev", "alt_fwd", "alt_rev", "non_confident_fwd", "non_confident_rev", "total_depth", "allele_depth", "used", "unused")] + [
+    ("gq", "<i4"), ("status", "<u4"), ("gt", "u1"), ("pad", "u1", (7,))])
+
+
+class SxContOpts(C.Structure):
+    _fields_ = [("min_het_vf", C.c_double), ("max_abs_sample_strand_bias", C.c_double), ("expected_qscore", C.c_int32), ("max_qscore", C.c_int32)]
+
+
+class SxContBatch(C.Structure):
+    _fields_ = [("n_sites", C.c_uint32), ("n_samples", C.c_uint32), ("pos_begin", C.c_int32), ("pad", C.c_uint32), ("forced_output", C.c_void_p),
+                ("sample", SxPileupBatch * SX_CONT_MAX_SAMPLES)]
+
+
+class SxContOut(C.Structure):
+    _fields_ = [("loci", C.c_void_p), ("samples", C.c_void_p), ("site_rec_off", C.c_void_p), ("cap_loci", C.c_uint32), ("pad", C.c_uint32)]
+
+
 class SxTiming(C.Structure):
     _fields_ = [("kernel_ms", C.c_float), ("h2d_ms", C.c_float), ("d2h_ms", C.c_float), ("launches", C.c_uint32), ("pad", C.c_uint32)]
 
@@ -488,6 +513,11 @@ SYMBOLS = [
     ("sx_last_window_timing", C.c_int, [_P, _P]),
     ("sx_process_somatic_window_dev", C.c_int, [_P, C.POINTER(SxSomaticWindowBatch), C.POINTER(SxSomaticWindowOut), _P]),
     ("sx_last_somatic_window_timing", C.c_int, [_P, _P]),
+    ("sx_default_cont_opts", None, [C.POINTER(SxContOpts)]),
+    ("sx_site_continuous", C.c_int, [_P, C.POINTER(SxContOpts), C.POINTER(SxContBatch), C.POINTER(SxContOut), _P]),
+    ("sx_site_continuous_dev", C.c_int, [_P, C.POINTER(SxContOpts), C.POINTER(SxContBatch), C.POINTER(SxContOut), _P]),
+    ("sx_cont_qscore", C.c_int, [_P, C.POINTER(SxContOpts), C.c_uint32, _P, _P, _P, _P]),
+    ("sx_cont_qscore_dev", C.c_int, [_P, C.POINTER(SxContOpts), C.c_uint32, _P, _P, _P, _P]),
     ("sx_comm_get_unique_id", C.c_int, [_P]),
     ("sx_comm_init", C.c_int, [_P, _P, C.c_int, C.c_int]),
     ("sx_gather_records", C.c_int, [_P, _P, C.c_size_t, _P, C.c_int]),

@@ -307,6 +307,49 @@ class Context:
             x.free()
         return out
 
+    # ---- K2c
+    def site_continuous(self, b: B.ContBatch, opts: Optional[A.SxContOpts] = None, cap_loci=None) -> B.ContOut:
+        """K2c: the continuous-frequency site model (host arrays in and out).  SX_ERR_CAPACITY leaves the record count in the SxError's
+        `totals`."""
+        out = B.ContOut(b.n_sites, b.n_samples, B.cont_cap(b) if cap_loci is None else cap_loci)
+        rc = self.lib.sx_site_continuous(self.h, C.byref(opts or cont_opts()), C.byref(b.c), C.byref(out.c), out.totals.ctypes.data)
+        self._chk_totals(rc, out.totals)
+        return out
+
+    def site_continuous_dev(self, db: "DevContBatch", opts: Optional[A.SxContOpts] = None, cap_loci=None) -> B.ContOut:
+        """K2c on a DevContBatch, into device arrays; returns their host copies."""
+        n_samples = db.n_samples
+        cap = 4 * db.n_sites if cap_loci is None else cap_loci
+        out = B.ContOut(db.n_sites, n_samples, cap)
+        d = {k: DeviceArray(self, getattr(out, k).nbytes + 64) for k in ("loci", "samples", "site_rec_off")}
+        c = A.SxContOut(cap_loci=cap, **{k: x.ptr for k, x in d.items()})
+        rc = self.lib.sx_site_continuous_dev(self.h, C.byref(opts or cont_opts()), C.byref(db.c), C.byref(c), out.totals.ctypes.data)
+        self._chk_totals(rc, out.totals)
+        n = int(out.totals[0])
+        out.site_rec_off[:] = d["site_rec_off"].download(np.uint32, db.n_sites + 1)
+        out.loci[:n] = d["loci"].download(A.CONT_LOCUS_DT, n)
+        out.samples[: n * n_samples] = d["samples"].download(A.CONT_SAMPLE_DT, n * n_samples)
+        for x in d.values():
+            x.free()
+        return out
+
+    def cont_qscore(self, a: np.ndarray, n: np.ndarray, opts: Optional[A.SxContOpts] = None) -> Tuple[np.ndarray, np.ndarray]:
+        """getAlleleSequencingErrorQscore of (a[i], n[i]) -> (gq, status)"""
+        a, n = np.ascontiguousarray(a, np.uint32), np.ascontiguousarray(n, np.uint32)
+        gq, st = np.zeros(a.size, np.int32), np.zeros(a.size, np.uint32)
+        self._chk(self.lib.sx_cont_qscore(self.h, C.byref(opts or cont_opts()), a.size, a.ctypes.data, n.ctypes.data, gq.ctypes.data, st.ctypes.data))
+        return gq, st
+
+    def cont_qscore_dev(self, a: np.ndarray, n: np.ndarray, opts: Optional[A.SxContOpts] = None) -> Tuple[np.ndarray, np.ndarray]:
+        """cont_qscore through device arrays (sx_cont_qscore_dev)"""
+        a, n = np.ascontiguousarray(a, np.uint32), np.ascontiguousarray(n, np.uint32)
+        d = [DeviceArray(self, a.nbytes + 64).upload(a), DeviceArray(self, n.nbytes + 64).upload(n), DeviceArray(self, a.nbytes + 64), DeviceArray(self, a.nbytes + 64)]
+        self._chk(self.lib.sx_cont_qscore_dev(self.h, C.byref(opts or cont_opts()), a.size, d[0].ptr, d[1].ptr, d[2].ptr, d[3].ptr))
+        gq, st = d[2].download(np.int32, a.size), d[3].download(np.uint32, a.size)
+        for x in d:
+            x.free()
+        return gq, st
+
     def _chk_totals(self, rc: int, totals: np.ndarray) -> None:
         try:
             self._chk(rc)
@@ -641,6 +684,40 @@ class DevRealignChain:
             bufs += list(self.gates.values())
         for d in bufs:
             d.free()
+
+
+def cont_opts() -> A.SxContOpts:
+    """sx_default_cont_opts: the reference's continuous-frequency model options"""
+    o = A.SxContOpts()
+    A.load().sx_default_cont_opts(C.byref(o))
+    return o
+
+
+class DevContBatch:
+    """K2c's batch with every array in HBM.  The object owns (or holds) the device arrays its struct `c` points at: pass the object, not
+    `c`, to Context.site_continuous_dev."""
+
+    def __init__(self, ctx: "Context", hb: B.ContBatch):
+        self.host, self.n_sites, self.n_samples = hb, hb.n_sites, hb.n_samples
+        self.samples = [DevPileupBatch(ctx, p) for p in hb.samples]
+        self.forced = None if hb.forced_output is None else DeviceArray(ctx, hb.forced_output.nbytes + 64).upload(hb.forced_output)
+        self.c = A.SxContBatch(n_sites=hb.n_sites, n_samples=hb.n_samples, pos_begin=hb.pos_begin, forced_output=self.forced.ptr if self.forced else None)
+        for k, p in enumerate(self.samples):
+            self.c.sample[k] = p.c
+
+    @classmethod
+    def from_windows(cls, windows, forced_output: Optional[DeviceArray] = None) -> "DevContBatch":
+        """The tier1 columns that DevWindow passes (keep_outputs) over the same positions left in HBM, one sample per window: no host round
+        trip between the window pass and K2c.  The reference bases are the first window's, from its own reference array."""
+        self = cls.__new__(cls)
+        w0 = windows[0].w
+        self.host, self.n_sites, self.n_samples, self.samples, self.forced = None, w0.n_sites, len(windows), list(windows), forced_output
+        self.c = A.SxContBatch(n_sites=w0.n_sites, n_samples=len(windows), pos_begin=w0.report_begin, forced_output=forced_output.ptr if forced_output else None)
+        for k, dw in enumerate(windows):
+            assert dw.w.n_sites == w0.n_sites and dw.w.report_begin == w0.report_begin, "the windows cover the same positions"
+            self.c.sample[k] = A.SxPileupBatch(n_sites=w0.n_sites, site_off=dw.obufs["site_off"].ptr, calls=dw.obufs["calls"].ptr,
+                                               ref_base=windows[0].bufs["ref"].ptr + (w0.report_begin - w0.ref_begin))
+        return self
 
 
 class DevWindow:

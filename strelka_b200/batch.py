@@ -412,6 +412,46 @@ class PileupBatch:
         return PileupBatch(off, calls, np.frombuffer(ref_bases.encode(), dtype=np.uint8), ploidy, t2_off, t2_calls)
 
 
+class ContBatch:
+    """K2c's input: S PileupBatch samples over the same n_sites consecutive positions from pos_begin, and the forced-output flags (or None).
+    Only sample 0's ref_base is read."""
+
+    def __init__(self, samples: Sequence[PileupBatch], pos_begin: int = 0, forced_output=None):
+        assert 1 <= len(samples) <= A.SX_CONT_MAX_SAMPLES
+        self.samples = list(samples)
+        self.n_sites = self.samples[0].n_sites
+        assert all(p.n_sites == self.n_sites for p in self.samples)
+        self.n_samples = len(self.samples)
+        self.pos_begin = int(pos_begin)
+        self.forced_output = None if forced_output is None else np.ascontiguousarray(forced_output, dtype=np.uint8)
+        assert self.forced_output is None or self.forced_output.size == self.n_sites
+        self.c = A.SxContBatch(n_sites=self.n_sites, n_samples=self.n_samples, pos_begin=self.pos_begin, forced_output=A.ptr(self.forced_output))
+        for k, p in enumerate(self.samples):
+            self.c.sample[k] = p.c
+
+
+class ContOut:
+    """K2c's output arrays (host): records, their (record, sample) entries, per-site record offsets and the total."""
+
+    def __init__(self, n_sites: int, n_samples: int, cap_loci: int):
+        self.n_samples, self.cap_loci = n_samples, int(cap_loci)
+        self.loci = np.zeros(max(1, self.cap_loci), A.CONT_LOCUS_DT)
+        self.samples = np.zeros(max(1, self.cap_loci * n_samples), A.CONT_SAMPLE_DT)
+        self.site_rec_off = np.zeros(n_sites + 1, np.uint32)
+        self.totals = np.zeros(1, np.uint32)
+        self.c = A.SxContOut(loci=A.ptr(self.loci), samples=A.ptr(self.samples), site_rec_off=A.ptr(self.site_rec_off), cap_loci=self.cap_loci)
+
+    def trimmed(self):
+        """(records, entries [records, n_samples], site_rec_off)"""
+        n = int(self.totals[0])
+        return self.loci[:n], self.samples[: n * self.n_samples].reshape(n, self.n_samples), self.site_rec_off
+
+
+def cont_cap(b: ContBatch) -> int:
+    """an upper bound of K2c's record count: four per site (an 'N' reference's forced site)"""
+    return 4 * b.n_sites
+
+
 class GaBatch:
     def __init__(self, queries: Sequence[str], refs: Sequence[str], max_ops: int = 64):
         assert len(queries) == len(refs)

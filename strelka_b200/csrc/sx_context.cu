@@ -542,6 +542,7 @@ constexpr sx_status_entry k_status[] = {
     {SX_ST_K6B_ID, SX_ERR_ARG, "%s: a record's window index outside its region's window, or an indel id at or past n_gid", nullptr, 0},
     {SX_ST_K6G_GROUP, SX_ERR_ARG, "%s: an allele group with an allele count outside 1.." SX_STR(SX_INDEL_MAX_ALLELES)
                                   ", a ploidy outside {1,2}, an id at or past n_gid, or offsets that do not start at 0 and ascend", nullptr, 0},
+    {SX_ST_CONT_TIE, SX_ERR_RANGE, "%s: a qscore within its error bound of a rounding boundary", nullptr, 0}, // (per-entry status only; listed for the disjointness check)
 };
 
 constexpr bool status_bits_disjoint()

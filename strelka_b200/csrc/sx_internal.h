@@ -93,6 +93,7 @@ enum sx_slot : int
     // stage scratch, owned by the stage's launcher while its launches run
     SX_SLOT_K1_SMEM_NEED = SX_SLOT_HOST_END,
     SX_SLOT_K2A_SCRATCH, SX_SLOT_K2A_MAX_SITE,
+    SX_SLOT_K2C_COUNTS, SX_SLOT_K2C_REC_OFF, SX_SLOT_K2C_TOTAL, SX_SLOT_K2C_SUMS,
     SX_SLOT_K3_INFO, SX_SLOT_K3_CURSOR, SX_SLOT_K3_ORDER, SX_SLOT_K3_SCRATCH,
     SX_SLOT_K4_SCAN_S, SX_SLOT_K4_SCAN_B, SX_SLOT_K4_TILE_SUMS, SX_SLOT_K4_MAX_CAND,
     SX_SLOT_K6_MAX, SX_SLOT_K6_LIST, SX_SLOT_K6_ARENA, SX_SLOT_K6_CLASS, SX_SLOT_K6_HIST, SX_SLOT_K6_LIST_BY_CLASS,
@@ -179,8 +180,11 @@ enum sx_status_bit : int
     SX_ST_K6B_ID = 1 << 23,      // K6b: a window index past its region's window, or an id at or past n_gid
     SX_ST_K6G_GROUP = 1 << 24,   // K6g: a group with an allele count outside 1..SX_INDEL_MAX_ALLELES, a ploidy outside {1,2}, an id at or past n_gid,
                                  // or offsets that do not start at 0 and ascend
+    SX_ST_CONT_TIE = 1 << 25,    // K2c: a qscore within its error bound of a rounding boundary.  A per-entry status (SX_CONT_ST_QSCORE_TIE), never in
+                                 // the device word
 };
 static_assert(SX_ST_SINDEL_CAP == SX_SINDEL_ST_CAP, "the per-locus capacity status of K5b is its status bit");
+static_assert(SX_ST_CONT_TIE == SX_CONT_ST_QSCORE_TIE, "the per-entry tie status of K2c is its status bit");
 
 struct sx_buf
 {
@@ -374,6 +378,9 @@ int sx_sindel_from_links_run(sx_ctx* ctx, const sx_sindel_opts* opts, const sx_i
 // against the caller's capacities.  The status word (SX_ST_K6G_GROUP, SX_ST_K6B_ID) is the caller's to read.
 int sx_k6g_run(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* sample, const sx_allele_groups* groups, sx_allele_group_reads_out* out_dev,
                uint32_t* totals_host, bool own_out, unsigned* launches);
+// K2c on device arrays: count, scan, write.  totals_host[0] receives the record count (also on SX_ERR_CAPACITY, which leaves site_rec_off
+// written and no record).  One host synchronisation (the count).
+int sx_k2c_run(sx_ctx* ctx, const sx_cont_opts* o, const sx_cont_batch* d, const sx_cont_out* out, uint32_t* totals_host, unsigned* launches);
 int sx_k7g_run(sx_ctx* ctx, const sx_gate_batch* d, const sx_gate_out* o, unsigned* launches);
 int sx_k7a_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_region* regions, const uint8_t* seq4, const char* ref, const uint32_t* key_ins_off, const char* key_ins,
                const sx_prep_out* o, unsigned* launches);
