@@ -336,7 +336,8 @@ typedef struct sx_ssnv_result { /* somatic_snv_genotype_grid + snv_result_set */
     float strandBias;
     uint32_t ref_gt;
     uint32_t is_computed;        /* 0: an 'N' reference, an all-reference tier1 view, or QSS 0 unforced; every other field is then 0,
-                                    except ref_gt, which is set unless the reference base is 'N' */
+                                    except ref_gt, which is set unless the reference base is 'N'.  In callable mode (below) neither early exit
+                                    applies: every position whose reference base is not 'N' is computed, as a forced one */
     uint32_t snv_tier;
     uint32_t snv_from_ntype_tier;
     uint32_t ntype;              /* NTYPE: REF 0, HOM 1, HET 2, CONFLICT 3.  A tier whose six posteriors are all NaN (a quality-0 call can
@@ -349,7 +350,8 @@ typedef struct sx_ssnv_result { /* somatic_snv_genotype_grid + snv_result_set */
     int32_t from_ntype_qphred;   /* QSS_NT */
     uint32_t normal_alt_id;
     uint32_t tumor_alt_id;
-    uint32_t pad;
+    int32_t nonsomatic_qphred;   /* NQSS, callable mode only (0 otherwise): calculate_result_set_grid's nonsomatic_qphred
+                                    (position_somatic_snv_strand_grid.cpp:186-215) of the tier1 view, whatever snv_tier says (:362) */
 } sx_ssnv_result;
 
 /* normal and tumor must have the same n_sites and ref_base; is_forced_output may be NULL (all 0);
@@ -358,6 +360,26 @@ int sx_site_gl_somatic(sx_ctx* ctx, const sx_pileup_batch* normal_host, const sx
                        const uint8_t* is_forced_output_host, sx_ssnv_result* out_host /*[n_sites]*/);
 int sx_site_gl_somatic_dev(sx_ctx* ctx, const sx_pileup_batch* normal_dev, const sx_pileup_batch* tumor_dev,
                            const uint8_t* is_forced_output_dev, sx_ssnv_result* out_dev);
+/* callable mode: position_somatic_snv_call(..., isComputeNonSomatic = true, sgtg), what strelka2 runs when it writes the somatic callable
+ * regions (--somatic-callable-regions-file, strelka_pos_processor.cpp:211-224).  The all-reference exit and the QSS 0 exit are off, so every
+ * position whose reference base is not 'N' runs both tiers (the tier2 copy of a QSS 0 tier1 still applies) and has its strandBias, and each
+ * such record carries nonsomatic_qphred.  Arguments as sx_site_gl_somatic[_dev]. */
+int sx_site_gl_somatic_callable(sx_ctx* ctx, const sx_pileup_batch* normal_host, const sx_pileup_batch* tumor_host,
+                                const uint8_t* is_forced_output_host, sx_ssnv_result* out_host /*[n_sites]*/);
+int sx_site_gl_somatic_callable_dev(sx_ctx* ctx, const sx_pileup_batch* normal_dev, const sx_pileup_batch* tumor_dev,
+                                    const uint8_t* is_forced_output_dev, sx_ssnv_result* out_dev);
+
+/* The somatic callable regions (SomaticCallableProcessor, applications/strelka/SomaticCallableProcessor.hh:41-54, and RegionProcessor): a
+ * position is callable unless both qphred < 15 and nonsomatic_qphred < 15; consecutive callable positions form one half-open interval
+ * [region_begin[k], region_end[k]), in the coordinates of site_snv[0] = pos_begin (sx_somatic_site_call.pos; the BED line of an interval
+ * is  chrom  region_begin  region_end).  site_snv (device memory, [n_pos]) is the site_snv of a callable-mode somatic window pass, or the
+ * output of sx_site_gl_somatic_callable_dev.  region_begin / region_end are device memory [cap_regions]; *n_regions_host (host memory)
+ * receives the number of intervals.  More intervals than cap_regions gives SX_ERR_CAPACITY, with *n_regions_host set and the first
+ * cap_regions intervals written.
+ * Window edges: an interval that touches pos_begin or pos_begin + n_pos may continue into the neighbouring window; the caller joins an
+ * interval ending at a window's last position + 1 with one beginning there in the next window, as RegionProcessor joins adjacent positions. */
+int sx_somatic_callable_regions_dev(sx_ctx* ctx, const sx_ssnv_result* site_snv_dev, uint32_t n_pos, int32_t pos_begin,
+                                    int32_t* region_begin_dev, int32_t* region_end_dev, uint32_t cap_regions, uint32_t* n_regions_host);
 
 /* ==========================================================================================
  * K5  indel_gl
@@ -1230,7 +1252,8 @@ int sx_last_window_timing(const sx_ctx* ctx, float* ms);
  *   is SX_ERR_ARG.
  * K2b runs at every position of [report_begin, report_end) on the two samples' tier1 columns, and on their tier2 columns when
  *   useTier2Evidence is set (strelka_pos_processor.cpp:181-219), with ref_base from the normal sample's reference segment and
- *   snv_forced_output (is_forced_output_pos) when given.
+ *   snv_forced_output (is_forced_output_pos) when given; in callable mode when is_compute_nonsomatic is set.  The SNV records below are
+ *   the same in both modes except for r.nonsomatic_qphred.
  * The SNV records are the positions where somatic_snv_genotype_grid::is_output() (somatic_result_set.hh:62-71): QSS != 0, or forced output at a
  *   position whose reference base is not 'N' (position_somatic_snv_strand_grid.cpp:242-246 clears the flag there), in ascending position.
  * The link (K6b) and K5b run on the two samples' K6 records, read lengths, SX_PRF_TIER1 flags and 'N'-free base counts where the passes left
@@ -1254,7 +1277,8 @@ typedef struct sx_somatic_window_batch {   /* the struct is host memory; its arr
     sx_sindel_opts sindel_opts;
     const double* err_prob;                /* HOST memory: [n_err] the distinct indelToRefErrorProb values, as sx_somatic_indel_dev */
     uint32_t n_err;
-    uint32_t pad;
+    uint32_t is_compute_nonsomatic;        /* nonzero: K2b runs in callable mode (sx_site_gl_somatic_callable_dev), as strelka2 does when it
+                                              writes the callable regions; site_snv then feeds sx_somatic_callable_regions_dev */
 } sx_somatic_window_batch;
 
 typedef struct sx_somatic_site_call {      /* one SNV record */

@@ -118,7 +118,7 @@ EDITS = [
     ("applications/strelka/strelka_pos_processor.cpp",
      [(r"_dopt\.sscaller_strand_grid\(\)\.position_somatic_snv_call\(\s*normal_cpi_ptr\[0\]->getExtendedPosInfo\(\),\s*tumor_cpi_ptr\[0\]->getExtendedPosInfo\(\),\s*"
        r"normal_epi_t2_ptr,\s*tumor_epi_t2_ptr,\s*isComputeNonSomatic,\s*sgtg\);",
-       "if (sx_shim::enabled() && !isComputeNonSomatic) sx_shim::site_gl_somatic(_opt, normal_cpi_ptr[0]->rawPileup(), tumor_cpi_ptr[0]->rawPileup(), sgtg);\n"
+       "if (sx_shim::enabled()) sx_shim::site_gl_somatic(_opt, normal_cpi_ptr[0]->rawPileup(), tumor_cpi_ptr[0]->rawPileup(), isComputeNonSomatic, sgtg);\n"
        "        else _dopt.sscaller_strand_grid().position_somatic_snv_call(normal_cpi_ptr[0]->getExtendedPosInfo(), tumor_cpi_ptr[0]->getExtendedPosInfo(),\n"
        "                                                                    normal_epi_t2_ptr, tumor_epi_t2_ptr, isComputeNonSomatic, sgtg);"),
       (r"_dopt\.sicaller_grid\(\)\.get_somatic_indel\(\s*_opt,\s*_dopt,\s*normal_sif\.sampleOptions,\s*tumor_sif\.sampleOptions,\s*indelKey,\s*indelData,\s*NORMAL,\s*TUMOR,\s*"

@@ -2,6 +2,7 @@
 """integration/run_demo.py -- runs the reference's bundled demo (SURVEY.md Appendix B: the command lines the python2 workflows would issue) with a
 binary from oracle/_ref/bin/ on the inputs staged under oracle/_ref/demo/ and returns the VCF bodies.
     python integration/run_demo.py somatic strelka2_sx /tmp/out      ->  /tmp/out/snvs.vcf, indels.vcf
+    python integration/run_demo.py somatic-callable strelka2_sx /tmp/out  ->  the same and /tmp/out/callable.bed (--outputCallableRegions)
     python integration/run_demo.py germline starling2_sx /tmp/out    ->  /tmp/out/seg.variants.vcf, seg.genome.S1.vcf, seg.genome.S2.vcf
     python integration/run_demo.py mito starling2_sx /tmp/out        ->  /tmp/out/seg.variants.vcf, seg.genome.S1.vcf (chrM, --call-continuous-vf)"""
 import gzip
@@ -24,7 +25,7 @@ def run(mode, binary, out, env=None, timeout=1200):
     os.makedirs(out, exist_ok=True)
     D, Cf = os.path.join(DEMO, "data"), os.path.join(DEMO, "config")
     exe = os.path.join(BIN, binary)
-    if mode == "somatic":
+    if mode in ("somatic", "somatic-callable"):
         cmd = [exe, "--region", "demo20:1-5000", "--ref", f"{D}/demo20.fa", "--max-indel-size", "49", "--min-mapping-quality", "20", "--somatic-snv-rate", "0.0001",
                "--shared-site-error-rate", "0.0000000005", "--shared-site-error-strand-bias-fraction", "0.0", "--somatic-indel-rate", "0.000001", "--shared-indel-error-factor", "2.2",
                "--tier2-min-mapping-quality", "0", "--strelka-snv-max-filtered-basecall-frac", "0.4", "--strelka-snv-max-spanning-deletion-frac", "0.75",
@@ -33,6 +34,9 @@ def run(mode, binary, out, env=None, timeout=1200):
                f"{Cf}/somaticIndelScoringModels.json", "--normal-align-file", f"{D}/NA12892_demo20.bam", "--tumor-align-file", f"{D}/NA12891_demo20.bam",
                "--somatic-snv-file", f"{out}/snvs.vcf", "--somatic-indel-file", f"{out}/indels.vcf", "--stats-file", f"{out}/stats.xml"]
         files = ["snvs.vcf", "indels.vcf"]
+        if mode == "somatic-callable":  # strelkaSomaticWorkflow.py:125-128 with isOutputCallableRegions
+            cmd += ["--somatic-callable-regions-file", f"{out}/callable.bed"]
+            files.append("callable.bed")
     elif mode == "mito":
         # strelkaGermlineWorkflow.py:81-148 for the one chrM segment of runMitoWorkflowDemo.bash (--exome --callContinuousVf chrM): no EVS model
         # files, the default indel error model, the VF header and --call-continuous-vf

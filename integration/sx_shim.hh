@@ -157,8 +157,10 @@ inline void global_align(const AlignmentScores<int>& sc, const std::string& quer
 }
 
 #ifdef SX_SHIM_SOMATIC
-/// sscaller_strand_grid().position_somatic_snv_call(nepi, tepi, nepi_t2, tepi_t2, isComputeNonSomatic = false, sgtg)
-/// (applications/strelka/strelka_pos_processor.cpp:213-219), from the RAW tumor / normal columns (tier1 + tier2 calls)
+/// sscaller_strand_grid().position_somatic_snv_call(nepi, tepi, nepi_t2, tepi_t2, isComputeNonSomatic, sgtg)
+/// (applications/strelka/strelka_pos_processor.cpp:213-219), from the RAW tumor / normal columns (tier1 + tier2 calls).  With
+/// isComputeNonSomatic (--somatic-callable-regions-file) the call is K2b's callable mode, which also gives sgtg.rs.nonsomatic_qphred for the
+/// reference's own SomaticCallableProcessor; those calls count as somatic site calls.
 inline sx_params somatic_params_of(const strelka_options& opt)
 {
     sx_params p(params_of(opt));
@@ -169,7 +171,8 @@ inline sx_params somatic_params_of(const strelka_options& opt)
     return p;
 }
 
-inline void site_gl_somatic(const strelka_options& opt, const snp_pos_info& normal, const snp_pos_info& tumor, somatic_snv_genotype_grid& sgtg)
+inline void site_gl_somatic(const strelka_options& opt, const snp_pos_info& normal, const snp_pos_info& tumor, const bool isComputeNonSomatic,
+                            somatic_snv_genotype_grid& sgtg)
 {
     sx_ctx* ctx(context(somatic_params_of(opt)));
     const uint16_t none(0);
@@ -195,7 +198,7 @@ inline void site_gl_somatic(const strelka_options& opt, const snp_pos_info& norm
     }
     const uint8_t forced(sgtg.is_forced_output ? 1 : 0);
     sx_ssnv_result r;
-    check(ctx, sx_site_gl_somatic(ctx, &b[0], &b[1], &forced, &r));
+    check(ctx, isComputeNonSomatic ? sx_site_gl_somatic_callable(ctx, &b[0], &b[1], &forced, &r) : sx_site_gl_somatic(ctx, &b[0], &b[1], &forced, &r));
     ++counters().site_gl_somatic;
     sgtg.ref_gt = r.ref_gt;
     if (!r.is_computed) return;
@@ -208,6 +211,7 @@ inline void site_gl_somatic(const strelka_options& opt, const snp_pos_info& norm
     sgtg.rs.normal_alt_id = r.normal_alt_id;
     sgtg.rs.tumor_alt_id = r.tumor_alt_id;
     sgtg.rs.strandBias = r.strandBias;
+    sgtg.rs.nonsomatic_qphred = r.nonsomatic_qphred;
 }
 
 /// _dopt.sicaller_grid().get_somatic_indel(_opt, _dopt, normal_opt, tumor_opt, indelKey, indelData, NORMAL, TUMOR, is_use_alt_indel = true, sindel)

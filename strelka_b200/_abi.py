@@ -86,7 +86,7 @@ SSNV_RESULT_DT = np.dtype(
         ("from_ntype_qphred", "<i4"),
         ("normal_alt_id", "<u4"),
         ("tumor_alt_id", "<u4"),
-        ("pad", "<u4"),
+        ("nonsomatic_qphred", "<i4"),  # NQSS, callable mode only
     ]
 )
 
@@ -367,7 +367,7 @@ SOMATIC_INDEL_CALL_DT = np.dtype([("locus", "<u4"), ("pad", "<u4"), ("r", SINDEL
 
 class SxSomaticWindowBatch(C.Structure):
     _fields_ = [("sample", SxWindowBatch * 2), ("key_gid", C.c_void_p * 2), ("read_id", C.c_void_p * 2), ("snv_forced_output", C.c_void_p), ("loci", SxIndelLoci),
-                ("sindel_opts", SxSindelOpts), ("err_prob", C.c_void_p), ("n_err", C.c_uint32), ("pad", C.c_uint32)]
+                ("sindel_opts", SxSindelOpts), ("err_prob", C.c_void_p), ("n_err", C.c_uint32), ("is_compute_nonsomatic", C.c_uint32)]
 
 
 class SxSomaticWindowOut(C.Structure):
@@ -478,6 +478,9 @@ SYMBOLS = [
     ("sx_dependent_eprob", C.c_int, [_P, C.POINTER(SxPileupBatch), _P, _P]),
     ("sx_site_gl_somatic", C.c_int, [_P, C.POINTER(SxPileupBatch), C.POINTER(SxPileupBatch), _P, _P]),
     ("sx_site_gl_somatic_dev", C.c_int, [_P, C.POINTER(SxPileupBatch), C.POINTER(SxPileupBatch), _P, _P]),
+    ("sx_site_gl_somatic_callable", C.c_int, [_P, C.POINTER(SxPileupBatch), C.POINTER(SxPileupBatch), _P, _P]),
+    ("sx_site_gl_somatic_callable_dev", C.c_int, [_P, C.POINTER(SxPileupBatch), C.POINTER(SxPileupBatch), _P, _P]),
+    ("sx_somatic_callable_regions_dev", C.c_int, [_P, _P, C.c_uint32, C.c_int32, _P, _P, C.c_uint32, C.POINTER(C.c_uint32)]),
     ("sx_default_score_indels_opts", None, [C.POINTER(SxScoreIndelsOpts)]),
     ("sx_score_indels", C.c_int, [_P, C.POINTER(SxScoreIndelsBatch), _P, C.POINTER(SxScoreIndelsOut)]),
     ("sx_score_indels_dev", C.c_int, [_P, C.POINTER(SxScoreIndelsBatch), _P, C.POINTER(SxScoreIndelsOut)]),

@@ -202,6 +202,28 @@ class Context:
     def site_gl_somatic_dev(self, dn: DevPileupBatch, dt: DevPileupBatch, forced: Optional[DeviceArray], out: DeviceArray) -> None:
         self._chk(self.lib.sx_site_gl_somatic_dev(self.h, C.byref(dn.c), C.byref(dt.c), forced.ptr if forced else None, out.ptr))
 
+    def site_gl_somatic_callable(self, npb: B.PileupBatch, tpb: B.PileupBatch, forced: Optional[np.ndarray] = None,
+                                 out: Optional[np.ndarray] = None) -> np.ndarray:
+        """K2b in callable mode (isComputeNonSomatic): every non-'N' position computed, with its nonsomatic_qphred"""
+        if out is None:
+            out = np.zeros(npb.n_sites, A.SSNV_RESULT_DT)
+        f = None if forced is None else np.ascontiguousarray(forced, np.uint8)
+        self._chk(self.lib.sx_site_gl_somatic_callable(self.h, C.byref(npb.c), C.byref(tpb.c), A.ptr(f), out.ctypes.data))
+        return out
+
+    def site_gl_somatic_callable_dev(self, dn: DevPileupBatch, dt: DevPileupBatch, forced: Optional[DeviceArray], out: DeviceArray) -> None:
+        self._chk(self.lib.sx_site_gl_somatic_callable_dev(self.h, C.byref(dn.c), C.byref(dt.c), forced.ptr if forced else None, out.ptr))
+
+    def somatic_callable_regions_dev(self, site_snv: DeviceArray, n_pos: int, pos_begin: int, region_begin: Optional[DeviceArray],
+                                     region_end: Optional[DeviceArray], cap_regions: int) -> int:
+        """the callable intervals of site_snv[n_pos] into region_begin / region_end (int32 device arrays of cap_regions); returns their number.
+        SX_ERR_CAPACITY raises an SxError whose `totals` holds that number."""
+        n = C.c_uint32(0)
+        rc = self.lib.sx_somatic_callable_regions_dev(self.h, site_snv.ptr if site_snv else None, n_pos, pos_begin, region_begin.ptr if region_begin else None,
+                                                      region_end.ptr if region_end else None, cap_regions, C.byref(n))
+        self._chk_totals(rc, np.array([n.value], np.uint32))
+        return int(n.value)
+
     # ---- K5
     def indel_gl(self, ib: "B.IndelBatch", out=None) -> np.ndarray:
         if out is None:
@@ -804,10 +826,12 @@ class DevSomaticWindow:
     """sx_process_somatic_window_dev on two B.WindowBatch samples (normal, tumor) of one window of positions and the candidate loci: every
     input resident in HBM, every output allocated here.  The samples' per-read and column outputs are DevWindow's (`normal` / `tumor`).
     useTier2Evidence of the pile-up and of K5b is `use_tier2`.  records_only: only the two record lists and the totals come out; every other
-    output (the samples', site_snv, indel) is left NULL, so the pass keeps it in the context's own buffers."""
+    output (the samples', site_snv, indel) is left NULL, so the pass keeps it in the context's own buffers -- except site_snv in callable mode.
+    compute_nonsomatic: K2b runs in callable mode (is_compute_nonsomatic), and callable_regions() gives the pass's callable intervals."""
 
     def __init__(self, ctx: "Context", normal: "B.WindowBatch", tumor: "B.WindowBatch", loci: "B.IndelLoci", key_gid, read_id=None, snv_forced=None,
-                 use_tier2: bool = False, opts: Optional[A.SxSindelOpts] = None, cap_snv_calls=None, cap_indel_calls=None, records_only: bool = False):
+                 use_tier2: bool = False, opts: Optional[A.SxSindelOpts] = None, cap_snv_calls=None, cap_indel_calls=None, records_only: bool = False,
+                 compute_nonsomatic: bool = False):
         assert not normal.do_site_gl and not tumor.do_site_gl, "strelka2 runs no germline site model: build the samples with do_site_gl=False"
         self.ctx, self.loci = ctx, loci
         self.records_only = records_only
@@ -830,7 +854,8 @@ class DevSomaticWindow:
                                         key_gid=(C.c_void_p * 2)(*(x.ptr if x else None for x in ib["key_gid"])),
                                         read_id=(C.c_void_p * 2)(*(x.ptr if x else None for x in ib["read_id"])),
                                         snv_forced_output=ib["snv_forced"].ptr if ib["snv_forced"] else None, loci=self.dloci.c, sindel_opts=self.opts,
-                                        err_prob=A.ptr(self.err_prob), n_err=self.err_prob.size)
+                                        err_prob=A.ptr(self.err_prob), n_err=self.err_prob.size, is_compute_nonsomatic=int(compute_nonsomatic))
+        self.compute_nonsomatic = compute_nonsomatic
         self.cap_snv = max(1, self.n_sites) if cap_snv_calls is None else cap_snv_calls
         self.cap_indel = max(1, n_loci) if cap_indel_calls is None else cap_indel_calls
         self.obufs = {"site_snv": DeviceArray(ctx, (self.n_sites + 1) * A.SSNV_RESULT_DT.itemsize),
@@ -838,7 +863,7 @@ class DevSomaticWindow:
                       "indel": DeviceArray(ctx, (n_loci + 1) * A.SINDEL_RESULT_DT.itemsize),
                       "indel_calls": DeviceArray(ctx, (self.cap_indel + 1) * A.SOMATIC_INDEL_CALL_DT.itemsize), "totals": DeviceArray(ctx, 64)}
         if records_only:
-            for k in ("site_snv", "indel"):
+            for k in ("indel",) if compute_nonsomatic else ("site_snv", "indel"):  # (callable_regions reads site_snv)
                 self.obufs.pop(k).free()
         samples = (A.SxWindowOut * 2)() if records_only else (A.SxWindowOut * 2)(*(dw.out for dw in self.windows))
         self.out = A.SxSomaticWindowOut(sample=samples, cap_snv_calls=self.cap_snv, cap_indel_calls=self.cap_indel, **{k: b.ptr for k, b in self.obufs.items()})
@@ -852,6 +877,19 @@ class DevSomaticWindow:
         ms = np.zeros(A.SX_SWIN_N_STAGES, np.float32)
         ctx.lib.sx_last_somatic_window_timing(ctx.h, ms.ctypes.data)
         return dict(zip(A.SX_SWIN_STAGE_NAMES, (float(x) for x in ms)))
+
+    def callable_regions(self, cap_regions=None):
+        """the callable intervals of the most recent run (callable mode): (begin, end) int32 arrays, half-open, in the positions' coordinates.
+        An interval that touches either end of [report_begin, report_end) may continue in the neighbouring window."""
+        assert self.compute_nonsomatic, "callable_regions needs a DevSomaticWindow made with compute_nonsomatic=True"
+        cap = (self.n_sites + 1) // 2 if cap_regions is None else cap_regions  # (no two intervals are adjacent)
+        rb, re = (DeviceArray(self.ctx, 4 * cap + 64) for _ in range(2))
+        try:
+            n = self.ctx.somatic_callable_regions_dev(self.obufs["site_snv"], self.n_sites, int(self.c.sample[0].report_begin), rb, re, cap)
+            return rb.download(np.int32, n), re.download(np.int32, n)
+        finally:
+            rb.free()
+            re.free()
 
     def download(self):
         """dict: each sample's DevWindow.download(), the per-position and per-locus results, the two record lists and the totals (records_only:

@@ -1544,3 +1544,13 @@ class WindowBatch:
                 {"seq4": pools.used["seq4"], "qual": pools.used["qual"], "ref": int(reg["ref_off"][eb.n_regions - 1]) + int(reg["ref_len"][eb.n_regions - 1])})
         w.enum_opts = eb.opts
         return w
+
+
+# ---- somatic callable regions (sx_somatic_callable_regions_dev's host builder)
+def somatic_callable_regions(site_snv: np.ndarray, pos_begin: int):
+    """SomaticCallableProcessor + RegionProcessor on sx_ssnv_result records of consecutive positions pos_begin, pos_begin + 1, ...: a
+    position is callable unless both qphred < 15 and nonsomatic_qphred < 15; returns the half-open intervals of consecutive callable
+    positions as (begin, end) int32 arrays"""
+    c = ~((site_snv["qphred"] < 15) & (site_snv["nonsomatic_qphred"] < 15))
+    d = np.diff(np.concatenate([[0], c.astype(np.int8), [0]]))
+    return (np.nonzero(d == 1)[0] + pos_begin).astype(np.int32), (np.nonzero(d == -1)[0] + pos_begin).astype(np.int32)

@@ -15,6 +15,11 @@
 // exp() terms summed in the reference's loop order; exp / log / log10 are the reference's libm functions restated
 // (sx_libm_mirror_d.h).  The nine strand-state likelihoods end in a float log-sum (getLogSum<float>: expf, then log1p in double
 // below 0.01f or logf), restated the same way, so they and the strandBias feature are the reference's bits as well.
+//
+// Callable mode (isComputeNonSomatic = true, a template parameter so that the default instantiation is the code it was) drops the two early
+// exits and adds the non-somatic quality of the tier1 view (k2b_nonsomatic.cuh), its 441 states spread over the warp.  This file also holds
+// the callable-region stage (sx_somatic_callable_regions_dev).
+#include "k2b_nonsomatic.cuh"
 #include "sx_libm_mirror.h"
 #include "sx_device_util.cuh"
 #include "sx_internal.h"
@@ -152,6 +157,38 @@ struct k2b_terms
     __device__ __forceinline__ float geno_prior(uint32_t combo) const { return T.geno_prior[combo]; }
 };
 
+// k2bn_nonsomatic_qphred with the states spread over the warp: lane l takes states l, l + 32, ...  Every lane returns the same value.
+__device__ __forceinline__ int nonsomatic_qphred_warp(const float* nl, const float* tl, const uint32_t lane)
+{
+    constexpr uint32_t ROUNDS = (K2BN_STATES + 31) / 32;
+    double m = -INFINITY; // the largest non-NaN state (fmax passes over NaN)
+    for (uint32_t k = 0; k < ROUNDS; ++k)
+    {
+        const uint32_t i = k * 32 + lane;
+        if (i < K2BN_STATES) m = fmax(m, k2bn_pprob(nl, tl, i));
+    }
+#pragma unroll
+    for (int d = 16; d; d >>= 1) m = fmax(m, __shfl_xor_sync(FULL, m, d));
+    const double p0 = k2bn_pprob(nl, tl, 0);
+    const double max = isnan(p0) ? p0 : m, opt_max = p0;
+    // the sum of the non-zero terms in index order, accumulated identically by every lane
+    double sum = 0.0;
+    for (uint32_t k = 0; k < ROUNDS; ++k)
+    {
+        const uint32_t i = k * 32 + lane;
+        const double t = i < K2BN_STATES ? k2bn_term(k2bn_pprob(nl, tl, i), max, opt_max, i) : 0.0;
+        for (unsigned nz = __ballot_sync(FULL, t != 0.0); nz; nz &= nz - 1)
+            sum = d_add(sum, __shfl_sync(FULL, t, __ffs(nz) - 1));
+    }
+    const double inv = d_div(1.0, sum);
+    const uint32_t di = lane * K2BN_DIAG_STRIDE;
+    const double dv = lane < K2BN_GRID ? d_mul(k2bn_term(k2bn_pprob(nl, tl, di), max, opt_max, di), inv) : 0.0;
+    double diag = 0.0;
+    for (uint32_t f = 0; f < K2BN_GRID; ++f) diag = d_add(diag, __shfl_sync(FULL, dv, f));
+    return k2bn_qphred(diag);
+}
+
+template <bool CALLABLE>
 __global__ void __launch_bounds__(K2B_WARPS * 32) k2b_somatic_kernel(const uint32_t* __restrict__ n_off, const uint16_t* __restrict__ n_calls,
                                                                      const uint32_t* __restrict__ n_t2off, const uint16_t* __restrict__ n_t2calls,
                                                                      const uint32_t* __restrict__ t_off, const uint16_t* __restrict__ t_calls,
@@ -217,6 +254,7 @@ __global__ void __launch_bounds__(K2B_WARPS * 32) k2b_somatic_kernel(const uint3
         trs[0] = tier_rs{0, 0, 0, 0, 0, 0, 0.f};
         trs[1] = trs[0];
         bool early = false;
+        int nqss = 0; // callable mode: the tier1 view's NQSS
         for (int tier = 0; tier < 2; ++tier)
         {
             if (tier == 1)
@@ -235,7 +273,7 @@ __global__ void __launch_bounds__(K2B_WARPS * 32) k2b_somatic_kernel(const uint3
             }
             const sample_acc na = accumulate_sample(T, n_off, n_calls, n_t2off, n_t2calls, site, ref_gt, tier == 1, false, lane, ln_one_half);
             const sample_acc ta = accumulate_sample(T, t_off, t_calls, t_t2off, t_t2calls, site, ref_gt, tier == 1, true, lane, ln_one_half);
-            if (tier == 0 && !forced && na.allref && ta.allref)
+            if (!CALLABLE && tier == 0 && !forced && na.allref && ta.allref)
             {
                 early = true; // is_spi_allref(normal) && is_spi_allref(tumor)
                 break;
@@ -244,9 +282,13 @@ __global__ void __launch_bounds__(K2B_WARPS * 32) k2b_somatic_kernel(const uint3
             s_tl[warp][tier][lane] = (lane < 30) ? ta.lh : 0.f;
             __syncwarp();
             result_set_grid(k2b_terms{T}, s_nl[warp][tier], s_tl[warp][tier], s_scr[warp], lane, trs[tier]);
-            // wrapper (strand_grid.cpp:157-226): returns before the strand-bias block when qphred==0 and not forced
+            if constexpr (CALLABLE)
+            {
+                if (tier == 0) nqss = nonsomatic_qphred_warp(s_nl[warp][0], s_tl[warp][0], lane);
+            }
+            // wrapper (strand_grid.cpp:157-226): returns before the strand-bias block when qphred==0, unless forced or in callable mode
             trs[tier].strandBias = 0.f;
-            if (forced || trs[tier].qphred != 0)
+            if (CALLABLE || forced || trs[tier].qphred != 0)
             {
                 float symm = s_tl[warp][tier][3], strand = s_tl[warp][tier][21];
                 for (int k = 4; k < 21; ++k) symm = fmaxf(symm, s_tl[warp][tier][k]);
@@ -257,7 +299,7 @@ __global__ void __launch_bounds__(K2B_WARPS * 32) k2b_somatic_kernel(const uint3
             trs[tier].tumor_alt_id = ta.alt_id;
         }
         if (early) continue;
-        if (!forced)
+        if (!CALLABLE && !forced)
         {
             if ((trs[0].qphred == 0) || (is_tier2 && (trs[1].qphred == 0))) continue;
         }
@@ -291,39 +333,93 @@ __global__ void __launch_bounds__(K2B_WARPS * 32) k2b_somatic_kernel(const uint3
             res->from_ntype_qphred = rs.from_ntype_qphred;
             res->normal_alt_id = rs.normal_alt_id;
             res->tumor_alt_id = rs.tumor_alt_id;
+            if constexpr (CALLABLE) res->nonsomatic_qphred = nqss;
         }
         __syncwarp();
     }
 }
 
+// ---- the callable regions: a per-position flag, run starts -> sx_scan -> interval offsets, a scatter of both ends
+constexpr uint32_t CR_THREADS = 256;
+
+// SomaticCallableProcessor::addToRegion (SomaticCallableProcessor.hh:41-54): callable unless both QSS and NQSS are below 15
+__device__ __forceinline__ bool is_callable(const sx_ssnv_result* __restrict__ r, const uint32_t i)
+{
+    return !(r[i].qphred < 15 && r[i].nonsomatic_qphred < 15);
+}
+
+__global__ void __launch_bounds__(CR_THREADS) k2b_region_mark_kernel(const sx_ssnv_result* __restrict__ r, const uint32_t n, uint32_t* __restrict__ starts)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+        starts[i] = (is_callable(r, i) && (i == 0 || !is_callable(r, i - 1))) ? 1u : 0u;
+}
+
+// off[i] = the number of intervals that start before i (off[n] the total): the interval that starts at i is off[i], and the one that ends
+// at i (inclusive) is off[i + 1] - 1
+__global__ void __launch_bounds__(CR_THREADS) k2b_region_write_kernel(const sx_ssnv_result* __restrict__ r, const uint32_t n, const uint32_t* __restrict__ off,
+                                                                       const int32_t pos_begin, int32_t* __restrict__ rb, int32_t* __restrict__ re, const uint32_t cap)
+{
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    {
+        if (!is_callable(r, i)) continue;
+        if ((i == 0 || !is_callable(r, i - 1)) && off[i] < cap) rb[off[i]] = pos_begin + (int32_t)i;
+        if ((i + 1 == n || !is_callable(r, i + 1)) && off[i + 1] - 1 < cap) re[off[i + 1] - 1] = pos_begin + (int32_t)i + 1;
+    }
+}
+
 } // namespace
 
-int sx_k2b_run(sx_ctx* ctx, const sx_pileup_batch* n, const sx_pileup_batch* t, const uint8_t* forced_dev, sx_ssnv_result* out_dev, unsigned* launches)
+int sx_k2b_run(sx_ctx* ctx, const sx_pileup_batch* n, const sx_pileup_batch* t, const uint8_t* forced_dev, sx_ssnv_result* out_dev, const bool callable,
+               unsigned* launches)
 {
     const int grid = static_cast<int>(std::min<uint32_t>((n->n_sites + K2B_WARPS - 1) / K2B_WARPS, (uint32_t)ctx->sm_count * 8));
-    k2b_somatic_kernel<<<grid, K2B_WARPS * 32, 0, ctx->s_compute>>>(n->site_off, n->calls, n->t2_off, n->t2_calls, t->site_off, t->calls, t->t2_off, t->t2_calls,
-                                                                  n->ref_base, forced_dev, n->n_sites, ctx->d_tables, out_dev);
+    const auto kernel = callable ? k2b_somatic_kernel<true> : k2b_somatic_kernel<false>;
+    kernel<<<grid, K2B_WARPS * 32, 0, ctx->s_compute>>>(n->site_off, n->calls, n->t2_off, n->t2_calls, t->site_off, t->calls, t->t2_off, t->t2_calls, n->ref_base,
+                                                         forced_dev, n->n_sites, ctx->d_tables, out_dev);
     SX_CUDA(ctx, cudaGetLastError());
     *launches += 1;
     return SX_OK;
 }
 
-extern "C" int sx_site_gl_somatic_dev(sx_ctx* ctx, const sx_pileup_batch* n, const sx_pileup_batch* t, const uint8_t* forced_dev, sx_ssnv_result* out_dev)
+int sx_k2b_regions_run(sx_ctx* ctx, const sx_ssnv_result* site_snv, const uint32_t n_pos, const int32_t pos_begin, int32_t* region_begin, int32_t* region_end,
+                       const uint32_t cap, uint32_t* total_host, unsigned* launches)
 {
-    if (!ctx) return SX_ERR_ARG;
-    ctx->timing = sx_timing{};
-    if (!n || !t || !out_dev) return sx_fail(ctx, SX_ERR_ARG, "sx_site_gl_somatic_dev: NULL argument");
-    if (n->n_sites != t->n_sites) return sx_fail(ctx, SX_ERR_ARG, "sx_site_gl_somatic_dev: normal and tumor batches differ in n_sites");
-    if (n->n_sites == 0) return SX_OK;
-    return sx_run_timed(ctx, [&](unsigned* launches) { return sx_k2b_run(ctx, n, t, forced_dev, out_dev, launches); });
+    cudaStream_t st(ctx->s_compute);
+    uint32_t* off(nullptr);
+    int rc;
+    if ((rc = sx_take(ctx, SX_SLOT_K2B_REGION_OFF, (size_t)n_pos + 1, off, 64))) return rc;
+    const int grid = static_cast<int>(std::min<uint32_t>((n_pos + CR_THREADS - 1) / CR_THREADS, (uint32_t)ctx->sm_count * 16));
+    k2b_region_mark_kernel<<<grid, CR_THREADS, 0, st>>>(site_snv, n_pos, off);
+    SX_CUDA(ctx, cudaGetLastError());
+    const sx_scan_set J = {1, {{off, n_pos, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, nullptr}}};
+    if ((rc = sx_scan(ctx, SX_SLOT_K2B_REGION_SUMS, J, launches))) return rc;
+    k2b_region_write_kernel<<<grid, CR_THREADS, 0, st>>>(site_snv, n_pos, off, pos_begin, region_begin, region_end, cap);
+    SX_CUDA(ctx, cudaGetLastError());
+    *launches += 2;
+    SX_CUDA(ctx, cudaMemcpyAsync(total_host, off + n_pos, 4, cudaMemcpyDeviceToHost, st));
+    return SX_OK;
 }
 
-extern "C" int sx_site_gl_somatic(sx_ctx* ctx, const sx_pileup_batch* n, const sx_pileup_batch* t, const uint8_t* forced_host, sx_ssnv_result* out_host)
+namespace
+{
+int site_gl_somatic_dev(sx_ctx* ctx, const char* what, const sx_pileup_batch* n, const sx_pileup_batch* t, const uint8_t* forced_dev, sx_ssnv_result* out_dev,
+                        const bool callable)
 {
     if (!ctx) return SX_ERR_ARG;
     ctx->timing = sx_timing{};
-    if (!n || !t || !out_host) return sx_fail(ctx, SX_ERR_ARG, "sx_site_gl_somatic: NULL argument");
-    if (n->n_sites != t->n_sites) return sx_fail(ctx, SX_ERR_ARG, "sx_site_gl_somatic: normal and tumor batches differ in n_sites");
+    if (!n || !t || !out_dev) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL argument", what);
+    if (n->n_sites != t->n_sites) return sx_fail(ctx, SX_ERR_ARG, "%s: normal and tumor batches differ in n_sites", what);
+    if (n->n_sites == 0) return SX_OK;
+    return sx_run_timed(ctx, [&](unsigned* launches) { return sx_k2b_run(ctx, n, t, forced_dev, out_dev, callable, launches); });
+}
+
+int site_gl_somatic(sx_ctx* ctx, const char* what, const sx_pileup_batch* n, const sx_pileup_batch* t, const uint8_t* forced_host, sx_ssnv_result* out_host,
+                    const bool callable)
+{
+    if (!ctx) return SX_ERR_ARG;
+    ctx->timing = sx_timing{};
+    if (!n || !t || !out_host) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL argument", what);
+    if (n->n_sites != t->n_sites) return sx_fail(ctx, SX_ERR_ARG, "%s: normal and tumor batches differ in n_sites", what);
     if (n->n_sites == 0) return SX_OK;
     SX_CUDA(ctx, cudaSetDevice(ctx->device));
     sx_call_timer tm(ctx);
@@ -337,7 +433,50 @@ extern "C" int sx_site_gl_somatic(sx_ctx* ctx, const sx_pileup_batch* n, const s
     sx_ssnv_result* d_out = nullptr;
     if ((rc = sx_take(ctx, sx_host_slot(22), n->n_sites, d_out, 0))) return rc;
     unsigned launches = 0;
-    if ((rc = sx_k2b_run(ctx, &dn, &dt, d_forced, d_out, &launches))) return rc;
+    if ((rc = sx_k2b_run(ctx, &dn, &dt, d_forced, d_out, callable, &launches))) return rc;
     if ((rc = sx_download(ctx, out_host, d_out, n->n_sites))) return rc;
     return tm.finish(launches);
+}
+} // namespace
+
+extern "C" int sx_site_gl_somatic_dev(sx_ctx* ctx, const sx_pileup_batch* n, const sx_pileup_batch* t, const uint8_t* forced_dev, sx_ssnv_result* out_dev)
+{
+    return site_gl_somatic_dev(ctx, "sx_site_gl_somatic_dev", n, t, forced_dev, out_dev, false);
+}
+
+extern "C" int sx_site_gl_somatic_callable_dev(sx_ctx* ctx, const sx_pileup_batch* n, const sx_pileup_batch* t, const uint8_t* forced_dev, sx_ssnv_result* out_dev)
+{
+    return site_gl_somatic_dev(ctx, "sx_site_gl_somatic_callable_dev", n, t, forced_dev, out_dev, true);
+}
+
+extern "C" int sx_site_gl_somatic(sx_ctx* ctx, const sx_pileup_batch* n, const sx_pileup_batch* t, const uint8_t* forced_host, sx_ssnv_result* out_host)
+{
+    return site_gl_somatic(ctx, "sx_site_gl_somatic", n, t, forced_host, out_host, false);
+}
+
+extern "C" int sx_site_gl_somatic_callable(sx_ctx* ctx, const sx_pileup_batch* n, const sx_pileup_batch* t, const uint8_t* forced_host, sx_ssnv_result* out_host)
+{
+    return site_gl_somatic(ctx, "sx_site_gl_somatic_callable", n, t, forced_host, out_host, true);
+}
+
+extern "C" int sx_somatic_callable_regions_dev(sx_ctx* ctx, const sx_ssnv_result* site_snv, uint32_t n_pos, int32_t pos_begin, int32_t* region_begin,
+                                               int32_t* region_end, uint32_t cap_regions, uint32_t* n_regions_host)
+{
+    if (!ctx) return SX_ERR_ARG;
+    ctx->timing = sx_timing{};
+    const char* what("sx_somatic_callable_regions_dev");
+    if (!n_regions_host) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL n_regions_host", what);
+    *n_regions_host = 0;
+    if (n_pos && !site_snv) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL site_snv", what);
+    if (cap_regions && (!region_begin || !region_end)) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL region array", what);
+    if ((int64_t)pos_begin + (int64_t)n_pos > (int64_t)INT32_MAX) return sx_fail(ctx, SX_ERR_ARG, "%s: pos_begin + n_pos exceeds int32", what);
+    if (n_pos == 0) return SX_OK;
+    uint32_t total(0);
+    const int rc = sx_run_timed(ctx, [&](unsigned* launches) {
+        return sx_k2b_regions_run(ctx, site_snv, n_pos, pos_begin, region_begin, region_end, cap_regions, &total, launches);
+    });
+    if (rc) return rc;
+    *n_regions_host = total;
+    if (total > cap_regions) return sx_fail(ctx, SX_ERR_CAPACITY, "%s: %u callable regions, cap_regions is %u", what, total, cap_regions);
+    return SX_OK;
 }

@@ -93,6 +93,7 @@ enum sx_slot : int
     // stage scratch, owned by the stage's launcher while its launches run
     SX_SLOT_K1_SMEM_NEED = SX_SLOT_HOST_END,
     SX_SLOT_K2A_SCRATCH, SX_SLOT_K2A_MAX_SITE,
+    SX_SLOT_K2B_REGION_OFF, SX_SLOT_K2B_REGION_SUMS,
     SX_SLOT_K2C_COUNTS, SX_SLOT_K2C_REC_OFF, SX_SLOT_K2C_TOTAL, SX_SLOT_K2C_SUMS,
     SX_SLOT_K3_INFO, SX_SLOT_K3_CURSOR, SX_SLOT_K3_ORDER, SX_SLOT_K3_SCRATCH,
     SX_SLOT_K4_SCAN_S, SX_SLOT_K4_SCAN_B, SX_SLOT_K4_TILE_SUMS, SX_SLOT_K4_MAX_CAND,
@@ -349,7 +350,12 @@ size_t sx_k1_region_smem(const sx_region* r0, const sx_region* r1, const sx_aln*
 int sx_k1_run(sx_ctx* ctx, const sx_align_batch* d, double* lnp_dev, unsigned* launches);
 int sx_k1_read_max_run(sx_ctx* ctx, const sx_align_batch* d, const double* lnp_dev, double* max_lnp_dev, uint32_t* max_aln_dev, unsigned* launches);
 int sx_k2a_run(sx_ctx* ctx, const sx_pileup_batch* d, int is_always_test, sx_digt_result* out_dev, unsigned* launches);
-int sx_k2b_run(sx_ctx* ctx, const sx_pileup_batch* n, const sx_pileup_batch* t, const uint8_t* forced_dev, sx_ssnv_result* out_dev, unsigned* launches);
+// `callable`: isComputeNonSomatic (sx_site_gl_somatic_callable_dev)
+int sx_k2b_run(sx_ctx* ctx, const sx_pileup_batch* n, const sx_pileup_batch* t, const uint8_t* forced_dev, sx_ssnv_result* out_dev, bool callable,
+               unsigned* launches);
+// the callable regions of site_snv[n_pos] (n_pos > 0); *total_host (host memory) receives their number once the stream has passed the copy
+int sx_k2b_regions_run(sx_ctx* ctx, const sx_ssnv_result* site_snv, uint32_t n_pos, int32_t pos_begin, int32_t* region_begin, int32_t* region_end,
+                       uint32_t cap, uint32_t* total_host, unsigned* launches);
 int sx_k3_run(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* d, sx_ga_result* res_dev, uint32_t* cigar_dev, unsigned* launches);
 int sx_k4_run(sx_ctx* ctx, const sx_pileup_reads_batch* d, const sx_pileup_columns* out, unsigned* launches);
 int sx_k5_run(sx_ctx* ctx, const sx_indel_batch* d, sx_indel_result* out_dev, unsigned* launches);

@@ -866,7 +866,7 @@ extern "C" int sx_process_somatic_window_dev(sx_ctx* ctx, const sx_somatic_windo
     SX_CUDA(ctx, mark(SX_SWIN_ST_SITE_SNV));
     const char* ref_base(bn.ref + ((int64_t)bn.report_begin - (int64_t)bn.ref_begin));
     const sx_pileup_batch pn(somatic_pileup_of(kept[0].cols, n_sites, ref_base, tier2)), pt(somatic_pileup_of(kept[1].cols, n_sites, ref_base, tier2));
-    if (n_sites && (rc = sx_k2b_run(ctx, &pn, &pt, sb->snv_forced_output, site_snv, &launches))) return rc;
+    if (n_sites && (rc = sx_k2b_run(ctx, &pn, &pt, sb->snv_forced_output, site_snv, sb->is_compute_nonsomatic != 0, &launches))) return rc;
     SX_CUDA(ctx, mark(SX_SWIN_ST_SNV_CALLS));
     if (n_sites && so->snv_calls)
     {
