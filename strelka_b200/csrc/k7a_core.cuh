@@ -176,87 +176,60 @@ K7A_HD uint32_t k7a_read(const k7a_view& v, const uint32_t region, const uint32_
 // ---------------------------------------------------------------------------------------------------------------------------
 #define K7G_MAX_SEGS 64u // path segments of a mapper alignment handled here (longer: the read is left to the caller, gate 0)
 
-struct k7g_path
-{
-    int32_t pos;
-    uint32_t n;
-    sx_aln_seg seg[K7G_MAX_SEGS];
-};
-
 K7A_HD bool k7g_align_match(const unsigned t) { return t == SX_AP_MATCH || t == SX_AP_SEQ_MATCH || t == SX_AP_SEQ_MISMATCH; }
 K7A_HD bool k7g_read_kind(const unsigned t) { return k7g_align_match(t) || t == SX_AP_INSERT || t == SX_AP_SOFT_CLIP; }
 K7A_HD bool k7g_ref_kind(const unsigned t) { return k7g_align_match(t) || t == SX_AP_DELETE || t == SX_AP_SKIP; }
 
-K7A_HD void k7g_ends(const k7g_path& p, uint32_t& first, uint32_t& last) // get_match_edge_segments, align_path.cpp:736-752
+K7A_HD void k7g_ends(const sx_aln_seg* p, const uint32_t n, uint32_t& first, uint32_t& last) // get_match_edge_segments, align_path.cpp:736-752
 {
-    first = last = p.n;
-    for (uint32_t i = 0; i < p.n; ++i)
-        if (k7g_align_match(p.seg[i].kind))
+    first = last = n;
+    for (uint32_t i = 0; i < n; ++i)
+        if (k7g_align_match(p[i].kind))
         {
-            if (first == p.n) first = i;
+            if (first == n) first = i;
             last = i;
         }
 }
 
-// matchify_edge_segment_type, alignment_util.cpp:128-175
-K7A_HD void k7g_matchify(const k7g_path& al, const unsigned segment_type, const bool lead, const bool trail, k7g_path& out)
+// appends ps to out[0 .. n) as matchify_edge_segment_type does (alignment_util.cpp:128-175): a segment that becomes a match (`to_match`)
+// extends a match before it
+K7A_HD void k7g_put(sx_aln_seg* out, uint32_t& n, const sx_aln_seg ps, const bool to_match)
 {
-    uint32_t first, last;
-    k7g_ends(al, first, last);
-    out.pos = al.pos;
-    out.n = 0;
-    for (uint32_t i = 0; i < al.n; ++i)
-    {
-        const sx_aln_seg ps(al.seg[i]);
-        const bool is_lead(i < first), is_trail(i > last);
-        const bool edge_target(((lead && is_lead) || (trail && is_trail)) && ps.kind == segment_type);
-        if (edge_target && is_lead) out.pos -= (int32_t)ps.len;
-        if (edge_target || k7g_align_match(ps.kind))
-        {
-            if (out.n > 0 && k7g_align_match(out.seg[out.n - 1].kind)) out.seg[out.n - 1].len = (uint16_t)(out.seg[out.n - 1].len + ps.len);
-            else
-            {
-                out.seg[out.n] = ps;
-                out.seg[out.n].kind = SX_AP_MATCH;
-                out.n++;
-            }
-        }
-        else out.seg[out.n++] = ps;
-    }
+    if (to_match && n > 0 && out[n - 1].kind == SX_AP_MATCH) out[n - 1].len = (uint16_t)(out[n - 1].len + ps.len);
+    else out[n++] = sx_aln_seg{ps.len, (uint8_t)(to_match ? SX_AP_MATCH : ps.kind), 0};
 }
 
-// returns gate bits; out_pos / out_segs[0 .. n_slots) receive the normalized alignment (+ zero-length HARD_CLIP pads)
+// returns gate bits; out_pos / out_segs[0 .. n_slots) receive the normalized alignment (+ zero-length HARD_CLIP pads).  The tests take the
+// mapper's alignment as it is; only edge-indel removal and the soft-clip matchify rewrite it, straight into out_segs.
 K7A_HD uint32_t k7g_read(const sx_gate_batch& b, const uint32_t region, const uint32_t r, int32_t& out_pos, sx_aln_seg* out_segs)
 {
     const uint32_t s0(b.seg_off[r]), n_slots(b.seg_off[r + 1] - s0);
-    out_pos = b.raw_pos[r];
-    for (uint32_t i = 0; i < n_slots; ++i) out_segs[i] = b.raw_segs[s0 + i];
+    const sx_aln_seg* al(b.raw_segs + s0);
+    const int32_t al_pos(b.raw_pos[r]);
+    out_pos = al_pos;
+    for (uint32_t i = 0; i < n_slots; ++i) out_segs[i] = al[i];
     if (n_slots == 0 || n_slots > K7G_MAX_SEGS) return 0;
-    k7g_path al;
-    al.pos = b.raw_pos[r];
-    al.n = n_slots;
-    for (uint32_t i = 0; i < n_slots; ++i) al.seg[i] = b.raw_segs[s0 + i];
     // ---- is_realignable = !is_overmax, alignment.cpp:34-50
-    for (uint32_t i = 1; i + 1 < al.n; ++i)
-        if ((al.seg[i].kind == SX_AP_INSERT || al.seg[i].kind == SX_AP_DELETE) && al.seg[i].len > b.max_indel_size) return 0;
+    for (uint32_t i = 1; i + 1 < n_slots; ++i)
+        if ((al[i].kind == SX_AP_INSERT || al[i].kind == SX_AP_DELETE) && al[i].len > b.max_indel_size) return 0;
     // ---- check_for_candidate_indel_overlap, :222-283
     {
         uint32_t lead(0), trail(0), asize(0);
-        for (uint32_t i = 0; i < al.n; ++i) // unalignedPrefixSize
+        for (uint32_t i = 0; i < n_slots; ++i) // unalignedPrefixSize
         {
-            const unsigned t(al.seg[i].kind);
+            const unsigned t(al[i].kind);
             if (!(t == SX_AP_INSERT || t == SX_AP_HARD_CLIP || t == SX_AP_SOFT_CLIP)) break;
-            if (k7g_read_kind(t)) lead += al.seg[i].len;
+            if (k7g_read_kind(t)) lead += al[i].len;
         }
-        for (uint32_t i = al.n; i-- > 0;) // unalignedSuffixSize
+        for (uint32_t i = n_slots; i-- > 0;) // unalignedSuffixSize
         {
-            const unsigned t(al.seg[i].kind);
+            const unsigned t(al[i].kind);
             if (!(t == SX_AP_INSERT || t == SX_AP_HARD_CLIP || t == SX_AP_SOFT_CLIP)) break;
-            if (k7g_read_kind(t)) trail += al.seg[i].len;
+            if (k7g_read_kind(t)) trail += al[i].len;
         }
-        for (uint32_t i = 0; i < al.n; ++i)
-            if (k7g_ref_kind(al.seg[i].kind)) asize += al.seg[i].len;
-        const int32_t pb(al.pos - (int32_t)lead), pe(al.pos + (int32_t)asize + (int32_t)trail), len((int32_t)b.read_len[r]);
+        for (uint32_t i = 0; i < n_slots; ++i)
+            if (k7g_ref_kind(al[i].kind)) asize += al[i].len;
+        const int32_t pb(al_pos - (int32_t)lead), pe(al_pos + (int32_t)asize + (int32_t)trail), len((int32_t)b.read_len[r]);
         int32_t zb(pb < pe - len ? pb : pe - len);
         zb = zb > 0 ? zb : 0;
         const int32_t ze(pe > pb + len ? pe : pb + len);
@@ -281,51 +254,60 @@ K7A_HD uint32_t k7g_read(const sx_gate_batch& b, const uint32_t region, const ui
         }
         if (!overlap) return 0;
     }
-    // ---- normalizeInputAlignmentIndels, :2000-2021
+    // ---- normalizeInputAlignmentIndels, :2000-2021: remove_edge_deletions (alignment_util.cpp:89-123) and matchify_edge_insertions, one pass
     const unsigned pins(b.pin_flags ? b.pin_flags[r] : 0u);
     const bool rm_lead(!(pins & 1u)), rm_trail(!(pins & 2u));
-    k7g_path cur(al);
+    uint32_t first, last;
+    k7g_ends(al, n_slots, first, last);
+    bool edge(false); // is_edge_readref_len_segment, align_path.cpp:827-846
     if (rm_lead || rm_trail)
-    {
-        uint32_t first, last;
-        k7g_ends(al, first, last);
-        bool edge(false); // is_edge_readref_len_segment, align_path.cpp:827-846
-        for (uint32_t i = 0; i < al.n; ++i)
+        for (uint32_t i = 0; i < n_slots; ++i)
         {
-            const unsigned t(al.seg[i].kind);
+            const unsigned t(al[i].kind);
             if ((i < first || i > last) && (t == SX_AP_INSERT || t == SX_AP_DELETE || t == SX_AP_SKIP || t == SX_AP_SOFT_CLIP)) edge = true;
         }
-        if (edge)
+    int32_t pos(al_pos);
+    uint32_t n(0);
+    bool soft(false);
+    for (uint32_t i = 0; i < n_slots; ++i)
+    {
+        const sx_aln_seg ps(al[i]);
+        const bool is_lead(i < first), is_trail(i > last), rm((is_lead && rm_lead) || (is_trail && rm_trail));
+        soft = soft || ps.kind == SX_AP_SOFT_CLIP;
+        if (!edge) out_segs[n++] = sx_aln_seg{ps.len, ps.kind, 0};
+        else if (ps.kind == SX_AP_DELETE && rm) // an edge deletion goes
         {
-            k7g_path nodel; // remove_edge_deletions, alignment_util.cpp:89-123
-            nodel.pos = al.pos;
-            nodel.n = 0;
-            for (uint32_t i = 0; i < al.n; ++i)
-            {
-                const bool is_lead(i < first), is_trail(i > last);
-                if (al.seg[i].kind == SX_AP_DELETE && ((is_lead && rm_lead) || (is_trail && rm_trail)))
-                {
-                    if (is_lead) nodel.pos += (int32_t)al.seg[i].len;
-                }
-                else nodel.seg[nodel.n++] = al.seg[i];
-            }
-            k7g_matchify(nodel, SX_AP_INSERT, rm_lead, rm_trail, cur); // matchify_edge_insertions
+            if (is_lead) pos += (int32_t)ps.len;
+        }
+        else // an edge insertion becomes a match (the deletions' removal leaves every other segment on its side of the matches)
+        {
+            const bool target(rm && ps.kind == SX_AP_INSERT);
+            if (target && is_lead) pos -= (int32_t)ps.len;
+            k7g_put(out_segs, n, ps, target || k7g_align_match(ps.kind));
         }
     }
-    // ---- soft clips become matches, :2051-2057
+    // ---- soft clips become matches, :2051-2057: matchify_edge_soft_clip of the path above, in place (it never grows)
     uint32_t gate(SX_GATE_REALIGN);
-    bool soft(false);
-    for (uint32_t i = 0; i < cur.n; ++i) soft = soft || cur.seg[i].kind == SX_AP_SOFT_CLIP;
     if (soft)
     {
         gate |= SX_GATE_SOFT_CLIPPED;
-        k7g_path m;
-        k7g_matchify(cur, SX_AP_SOFT_CLIP, true, true, m);
-        cur = m;
+        k7g_ends(out_segs, n, first, last);
+        const uint32_t m(n);
+        n = 0;
+        for (uint32_t i = 0; i < m; ++i)
+        {
+            const sx_aln_seg ps(out_segs[i]);
+            const bool target((i < first || i > last) && ps.kind == SX_AP_SOFT_CLIP);
+            if (target && i < first) pos -= (int32_t)ps.len;
+            k7g_put(out_segs, n, ps, target || k7g_align_match(ps.kind));
+        }
     }
-    if (cur.pos < 0) return gate & ~SX_GATE_REALIGN; // :2062
-    out_pos = cur.pos;
-    for (uint32_t i = 0; i < cur.n; ++i) out_segs[i] = sx_aln_seg{cur.seg[i].len, cur.seg[i].kind, 0};
-    for (uint32_t i = cur.n; i < n_slots; ++i) out_segs[i] = sx_aln_seg{0, SX_AP_HARD_CLIP, 0};
+    if (pos < 0) // :2062 -- the read keeps its mapper's alignment
+    {
+        for (uint32_t i = 0; i < n_slots; ++i) out_segs[i] = al[i];
+        return gate & ~SX_GATE_REALIGN;
+    }
+    out_pos = pos;
+    for (uint32_t i = n; i < n_slots; ++i) out_segs[i] = sx_aln_seg{0, SX_AP_HARD_CLIP, 0};
     return gate;
 }

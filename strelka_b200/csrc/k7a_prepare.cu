@@ -10,24 +10,19 @@
 
 #include "k7a_core.cuh"
 #include "sx_internal.h"
+#include "sx_read_index.cuh"
 
 #include <algorithm>
+#include <cstring>
 
 namespace
 {
-// byte offset of every read's first packed base: reads of a region are back to back from its seq_off, each on a byte boundary
-__global__ void k7a_read_offsets_kernel(const k7a_view v, unsigned long long* __restrict__ read_byte, uint32_t* __restrict__ read_region)
+// the byte offset of read r's first packed base from the read index's 32-bit offset: the region's 64-bit seq_off plus the read's place in the
+// region (the index's offsets wrap at 4 GiB together with the region's)
+__device__ __forceinline__ uint64_t k7a_read_byte(const k7a_view& v, const uint32_t g, const uint32_t* __restrict__ seq_off, const uint32_t r)
 {
-    for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < v.b.n_regions; g += gridDim.x * blockDim.x)
-    {
-        unsigned long long at(v.regions[g].seq_off);
-        for (uint32_t r = v.b.region_read_off[g]; r < v.b.region_read_off[g + 1]; ++r)
-        {
-            read_byte[r] = at;
-            read_region[r] = g;
-            at += (v.b.read_len[r] + 1u) / 2u;
-        }
-    }
+    const uint64_t b(v.regions[g].seq_off);
+    return b + (uint32_t)(seq_off[r] - (uint32_t)b);
 }
 
 // The reads the gates turned away (about half of a 30x window's) have no keys: with a gate the two passes below run over the DENSE list of the
@@ -37,15 +32,16 @@ __global__ void k7a_read_offsets_kernel(const k7a_view v, unsigned long long* __
 
 // list == NULL: every read (and the per-read defaults are written here); otherwise the listed reads (the defaults were set by the host side).
 // The counts go into in_key_off, which the scan turns into the offsets.
-__global__ void k7a_count_kernel(const k7a_view v, const unsigned long long* __restrict__ read_byte, const uint32_t* __restrict__ read_region,
+__global__ void k7a_count_kernel(const k7a_view v, const uint32_t* __restrict__ seq_off, const uint32_t* __restrict__ read_region,
                                  const uint32_t* __restrict__ list, const uint32_t* __restrict__ n_list, uint16_t* __restrict__ stage, const sx_prep_out o)
 {
     const uint32_t n_work(list ? *n_list : v.b.n_reads);
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_work; i += gridDim.x * blockDim.x)
     {
         const uint32_t r(list ? list[i] : i);
+        const uint32_t g(read_region[r]);
         uint16_t keys[K7A_MAX_KEYS], lead, trail;
-        const uint32_t n(k7a_read(v, read_region[r], r, read_byte[r], keys, lead, trail));
+        const uint32_t n(k7a_read(v, g, r, k7a_read_byte(v, g, seq_off, r), keys, lead, trail));
         o.in_key_off[r] = n;
         o.in_lead_key[r] = lead;
         o.in_trail_key[r] = trail;
@@ -54,7 +50,7 @@ __global__ void k7a_count_kernel(const k7a_view v, const unsigned long long* __r
     }
 }
 
-__global__ void k7a_write_kernel(const k7a_view v, const unsigned long long* __restrict__ read_byte, const uint32_t* __restrict__ read_region, const uint32_t* __restrict__ list,
+__global__ void k7a_write_kernel(const k7a_view v, const uint32_t* __restrict__ seq_off, const uint32_t* __restrict__ read_region, const uint32_t* __restrict__ list,
                                  const uint32_t* __restrict__ n_list, const uint16_t* __restrict__ stage, const sx_prep_out o, int* __restrict__ status)
 {
     if (o.totals[0] > o.cap_keys)
@@ -72,35 +68,29 @@ __global__ void k7a_write_kernel(const k7a_view v, const unsigned long long* __r
             for (uint32_t k = 0; k < n_known; ++k) o.in_keys[at + k] = stage[(size_t)r * K7A_STAGE + k];
             continue;
         }
+        const uint32_t g(read_region[r]);
         uint16_t keys[K7A_MAX_KEYS], lead, trail;
-        const uint32_t n(k7a_read(v, read_region[r], r, read_byte[r], keys, lead, trail));
+        const uint32_t n(k7a_read(v, g, r, k7a_read_byte(v, g, seq_off, r), keys, lead, trail));
         for (uint32_t k = 0; k < n; ++k) o.in_keys[at + k] = keys[k];
     }
 }
 
-__global__ void k7g_gates_kernel(const sx_gate_batch b, const sx_gate_out o, uint32_t* __restrict__ read_region)
+// read_region: the read index's (the window pass), or NULL: a binary search of region_read_off per read (the gates' own entry points)
+__global__ void k7g_gates_kernel(const sx_gate_batch b, const sx_gate_out o, const uint32_t* __restrict__ read_region)
 {
-    // reads of a region are consecutive: a thread finds its read's region by a binary search of region_read_off
     for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < b.n_reads; r += gridDim.x * blockDim.x)
     {
-        uint32_t lo(0), hi(b.n_regions);
-        while (lo + 1 < hi)
-        {
-            const uint32_t mid((lo + hi) / 2);
-            if (b.region_read_off[mid] <= r) lo = mid;
-            else hi = mid;
-        }
+        const uint32_t g(read_region ? read_region[r] : sxi_region_of(b.region_read_off, b.n_regions, r));
         int32_t pos;
-        o.gate[r] = (uint8_t)k7g_read(b, lo, r, pos, o.in_segs + b.seg_off[r]);
+        o.gate[r] = (uint8_t)k7g_read(b, g, r, pos, o.in_segs + b.seg_off[r]);
         o.in_pos[r] = pos;
     }
-    (void)read_region;
 }
 } // namespace
 
 // K7a's launcher
 int sx_k7a_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_region* regions, const uint8_t* seq4, const char* ref, const uint32_t* key_ins_off, const char* key_ins,
-               const sx_prep_out* o, unsigned* launches)
+               const sx_prep_out* o, const uint32_t* read_region, const uint32_t* read_seq_off, unsigned* launches)
 {
     k7a_view v;
     v.b = *d;
@@ -112,14 +102,28 @@ int sx_k7a_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_region* regions, co
     cudaStream_t st(ctx->s_compute);
     const uint32_t n(v.b.n_reads);
     int rc;
-    unsigned long long* read_byte(nullptr);
-    uint32_t* read_region(nullptr);
-    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_READ_WORD, n, read_byte, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K7A_READ_REGION, n, read_region, 16))) return rc;
+    if (!read_region || !read_seq_off) // no window pass in front: the read index's region and packed-base offsets of every read
+    {
+        uint32_t *region(nullptr), *seq_off(nullptr);
+        if ((rc = sx_take(ctx, SX_SLOT_K7A_READ_REGION, n, region, 16))) return rc;
+        if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_READ_WORD, (size_t)n + 1, seq_off, 16))) return rc;
+        sx_read_index_in in;
+        memset(&in, 0, sizeof(in));
+        in.n_regions = v.b.n_regions;
+        in.n_reads = n;
+        in.region_read_off = v.b.region_read_off;
+        in.read_len = v.b.read_len;
+        in.regions = regions;
+        sx_read_index ix;
+        memset(&ix, 0, sizeof(ix));
+        ix.region = region;
+        ix.seq_off = seq_off;
+        if ((rc = sx_read_index_run(ctx, &in, &ix, launches))) return rc;
+        read_region = region;
+        read_seq_off = seq_off;
+    }
     const int cap(ctx->sm_count * 16);
     const auto grid = [cap](const uint32_t m) { return (unsigned)std::max(1, std::min<int>((int)((m + 127) / 128), cap)); };
-    k7a_read_offsets_kernel<<<grid(v.b.n_regions), 128, 0, st>>>(v, read_byte, read_region);
-    SX_CUDA(ctx, cudaGetLastError());
     uint32_t *list(nullptr), *n_list(nullptr);
     uint16_t* stage(nullptr);
     unsigned extra(0);
@@ -135,23 +139,23 @@ int sx_k7a_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_region* regions, co
         if ((rc = sx_k7_active_reads(ctx, n, v.b.gate, list, n_list))) return rc;
         extra = 1;
     }
-    k7a_count_kernel<<<grid(n), 128, 0, st>>>(v, read_byte, read_region, list, n_list, stage, *o);
+    k7a_count_kernel<<<grid(n), 128, 0, st>>>(v, read_seq_off, read_region, list, n_list, stage, *o);
     SX_CUDA(ctx, cudaGetLastError());
-    *launches += 2 + extra;
+    *launches += 1 + extra;
     const sx_scan_set J = {1, {{o->in_key_off, n, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, o->totals}}};
     if ((rc = sx_scan(ctx, SX_SLOT_K7A_K9_SUMS, J, launches))) return rc;
-    k7a_write_kernel<<<grid(n), 128, 0, st>>>(v, read_byte, read_region, list, n_list, stage, *o, ctx->d_status);
+    k7a_write_kernel<<<grid(n), 128, 0, st>>>(v, read_seq_off, read_region, list, n_list, stage, *o, ctx->d_status);
     SX_CUDA(ctx, cudaGetLastError());
     *launches += 1;
     return SX_OK;
 }
 
 // K7g's launcher
-int sx_k7g_run(sx_ctx* ctx, const sx_gate_batch* d, const sx_gate_out* o, unsigned* launches)
+int sx_k7g_run(sx_ctx* ctx, const sx_gate_batch* d, const sx_gate_out* o, const uint32_t* read_region, unsigned* launches)
 {
     if (d->n_reads == 0) return SX_OK;
     const unsigned grid((unsigned)std::max(1, std::min<int>((int)((d->n_reads + 127) / 128), ctx->sm_count * 16)));
-    k7g_gates_kernel<<<grid, 128, 0, ctx->s_compute>>>(*d, *o, nullptr);
+    k7g_gates_kernel<<<grid, 128, 0, ctx->s_compute>>>(*d, *o, read_region);
     SX_CUDA(ctx, cudaGetLastError());
     *launches += 1;
     return SX_OK;
@@ -191,7 +195,7 @@ extern "C" int sx_realign_gates_dev(sx_ctx* ctx, const sx_gate_batch* d, sx_gate
     int rc;
     if ((rc = k7g_check_args(ctx, d, out_dev, "sx_realign_gates_dev"))) return rc;
     if (d->n_reads == 0) return SX_OK;
-    if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k7g_run(ctx, d, out_dev, launches); }))) return rc;
+    if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k7g_run(ctx, d, out_dev, nullptr, launches); }))) return rc;
     return sx_check_status(ctx, "sx_realign_gates");
 }
 
@@ -221,7 +225,7 @@ extern "C" int sx_realign_gates(sx_ctx* ctx, const sx_gate_batch* b, sx_gate_out
     if ((rc = sx_take(ctx, sx_host_slot(11), n, o.in_pos, 16))) return rc;
     if ((rc = sx_take(ctx, sx_host_slot(12), n_segs, o.in_segs, 16))) return rc;
     unsigned launches(0);
-    if ((rc = sx_k7g_run(ctx, &d, &o, &launches))) return rc;
+    if ((rc = sx_k7g_run(ctx, &d, &o, nullptr, &launches))) return rc;
     if ((rc = sx_download(ctx, out_host->gate, o.gate, n))) return rc;
     if ((rc = sx_download(ctx, out_host->in_pos, o.in_pos, n))) return rc;
     if ((rc = sx_download(ctx, out_host->in_segs, o.in_segs, n_segs))) return rc;
@@ -244,7 +248,7 @@ extern "C" int sx_alignment_indels_dev(sx_ctx* ctx, const sx_enum_batch* d, cons
         SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
         return SX_OK;
     }
-    if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k7a_run(ctx, d, regions, seq4, ref, key_ins_off, key_ins, out_dev, launches); }))) return rc;
+    if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k7a_run(ctx, d, regions, seq4, ref, key_ins_off, key_ins, out_dev, nullptr, nullptr, launches); }))) return rc;
     return sx_check_status(ctx, "sx_alignment_indels", SX_ST_K7A_CAP);
 }
 
@@ -290,7 +294,7 @@ extern "C" int sx_alignment_indels(sx_ctx* ctx, const sx_enum_batch* b, const sx
     if ((rc = sx_take(ctx, sx_host_slot(15), n, o.in_lead_key, 16))) return rc;
     if ((rc = sx_take(ctx, sx_host_slot(16), n, o.in_trail_key, 16))) return rc;
     unsigned launches(0);
-    if ((rc = sx_k7a_run(ctx, &d, d_regions, d_seq4, d_ref, d_key_ins_off, d_key_ins, &o, &launches))) return rc;
+    if ((rc = sx_k7a_run(ctx, &d, d_regions, d_seq4, d_ref, d_key_ins_off, d_key_ins, &o, nullptr, nullptr, &launches))) return rc;
     if ((rc = sx_download(ctx, out_host->totals, o.totals, 1))) return rc;
     if ((rc = sx_download(ctx, out_host->in_key_off, o.in_key_off, n + 1))) return rc;
     if ((rc = sx_download(ctx, out_host->in_lead_key, o.in_lead_key, n))) return rc;

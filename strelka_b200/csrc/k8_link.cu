@@ -26,12 +26,6 @@ __global__ void k8_aln_read_kernel(const uint32_t n_reads, const uint32_t* __res
         for (uint32_t a = aln_off[r]; a < aln_off[r + 1]; ++a) aln_read[a] = r;
 }
 
-__global__ void k8_read_region_kernel(const uint32_t n_regions, const uint32_t* __restrict__ region_read_off, uint32_t* __restrict__ read_region)
-{
-    for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < n_regions; g += gridDim.x * blockDim.x)
-        for (uint32_t r = region_read_off[g]; r < region_read_off[g + 1]; ++r) read_region[r] = g;
-}
-
 __global__ void k8_size_kernel(const k8_view v, const uint32_t n_alns, const uint32_t* __restrict__ aln_read, const uint32_t* __restrict__ read_region,
                                uint32_t* __restrict__ seg_n, uint32_t* __restrict__ ins_n, int* __restrict__ status)
 {
@@ -149,14 +143,20 @@ __global__ void k8_pad_kernel(const k8_view v, const uint32_t n_alns, const uint
 
 // K7b's launcher
 int sx_k8_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* e, const uint32_t n_alns, const uint32_t* key_ins_off, const char* key_ins, const sx_link_out* o,
-              unsigned* launches)
+              const uint32_t* read_region, unsigned* launches)
 {
     cudaStream_t st(ctx->s_compute);
     int rc;
-    uint32_t *aln_read(nullptr), *read_region(nullptr), *seg_n(nullptr), *ins_n(nullptr), *reg_seg(nullptr), *reg_ins(nullptr);
+    uint32_t *aln_read(nullptr), *seg_n(nullptr), *ins_n(nullptr), *reg_seg(nullptr), *reg_ins(nullptr);
     const uint32_t nr(d->n_regions);
     if ((rc = sx_take(ctx, SX_SLOT_K8_ALN_READ, n_alns, aln_read, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K8_READ_REGION, d->n_reads, read_region, 16))) return rc;
+    if (!read_region) // no window pass in front: the read index's region of every read
+    {
+        uint32_t* region(nullptr);
+        if ((rc = sx_take(ctx, SX_SLOT_K8_READ_REGION, d->n_reads, region, 16))) return rc;
+        if ((rc = sx_read_region_run(ctx, nr, d->n_reads, d->region_read_off, region, launches))) return rc;
+        read_region = region;
+    }
     if ((rc = sx_take(ctx, SX_SLOT_K8_SEG_N, n_alns, seg_n, 16))) return rc;
     if ((rc = sx_take(ctx, SX_SLOT_K8_INS_N, n_alns, ins_n, 16))) return rc;
     if ((rc = sx_take(ctx, SX_SLOT_K8_REG_SEG, nr, reg_seg, 16))) return rc;
@@ -168,15 +168,13 @@ int sx_k8_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* e, const u
     v.key_ins = key_ins;
     const int cap(ctx->sm_count * 16);
     const auto grid = [cap](const uint32_t n) { return (unsigned)std::max(1, std::min<int>((int)((n + 127) / 128), cap)); };
-    k8_read_region_kernel<<<grid(nr), 128, 0, st>>>(nr, d->region_read_off, read_region);
-    SX_CUDA(ctx, cudaGetLastError());
     k8_aln_read_kernel<<<grid(d->n_reads), 128, 0, st>>>(d->n_reads, e->aln_off, aln_read);
     SX_CUDA(ctx, cudaGetLastError());
     k8_size_kernel<<<grid(n_alns), 128, 0, st>>>(v, n_alns, aln_read, read_region, seg_n, ins_n, ctx->d_status);
     SX_CUDA(ctx, cudaGetLastError());
     k8_region_kernel<<<grid((uint32_t)std::min<uint64_t>((uint64_t)nr * 32u, 0xffffff00u)), 128, 0, st>>>(v, seg_n, ins_n, reg_seg, reg_ins);
     SX_CUDA(ctx, cudaGetLastError());
-    *launches += 4;
+    *launches += 3;
     const sx_scan_set J = {2, {{reg_seg, nr, SX_SCAN_EXCLUSIVE, o->totals}, {reg_ins, nr, SX_SCAN_EXCLUSIVE, o->totals + 1}}};
     if ((rc = sx_scan(ctx, SX_SLOT_K8_SUMS, J, launches))) return rc;
     k8_write_kernel<<<grid(n_alns), 128, 0, st>>>(v, n_alns, aln_read, read_region, seg_n, ins_n, reg_seg, reg_ins, *o);
@@ -208,7 +206,7 @@ extern "C" int sx_link_alignments_dev(sx_ctx* ctx, const sx_enum_batch* d, const
     ctx->timing = sx_timing{};
     int rc;
     if ((rc = k8_check_args(ctx, d, e, key_ins_off, key_ins, out_dev, "sx_link_alignments_dev"))) return rc;
-    if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k8_run(ctx, d, e, n_alns, key_ins_off, key_ins, out_dev, launches); }))) return rc;
+    if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k8_run(ctx, d, e, n_alns, key_ins_off, key_ins, out_dev, nullptr, launches); }))) return rc;
     return sx_check_status(ctx, "sx_link_alignments", SX_ST_K8_NO_KEY | SX_ST_K8_KIND | SX_ST_K8_CAP);
 }
 
@@ -248,7 +246,7 @@ extern "C" int sx_link_alignments(sx_ctx* ctx, const sx_enum_batch* b, const sx_
     if ((rc = sx_take(ctx, sx_host_slot(17), o.cap_ins, o.ins, SX_POOL_SLACK + 16))) return rc;
     if (out_host->k6_segs && (rc = sx_take(ctx, sx_host_slot(18), n_segs, o.k6_segs, 16))) return rc;
     unsigned launches(0);
-    if ((rc = sx_k8_run(ctx, &d, &de, n_alns, d_key_ins_off, d_key_ins, &o, &launches))) return rc;
+    if ((rc = sx_k8_run(ctx, &d, &de, n_alns, d_key_ins_off, d_key_ins, &o, nullptr, &launches))) return rc;
     if ((rc = sx_download(ctx, out_host->totals, o.totals, 2))) return rc;
     if ((rc = sx_download(ctx, out_host->regions, o.regions, nr + 1))) return rc;
     SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));

@@ -3,7 +3,10 @@
 // reads, isTestSoftClippedInputAligned = false), isFirstCandidateAlignmentPreferred :1352-1377, finishRealignment :1411-1450 and
 // starling_read_align_clipper.cpp (get_alignment_ref_map :96-146, mark_ref_map_conflicts :150-225, soft_clip_alignment :255-338,
 // getClippedAlignmentFromTopAlignmentPool :340-424).  The pool is never stored: membership is a comparison, so the alignments are
-// simply walked again.  __host__ __device__: tests/cpp/k9_core_host.cpp runs exactly this code on the CPU against the reference.
+// simply walked again, and so is the reference map: it is piecewise (one type per segment, a MATCH position that is the segment's start
+// plus the read offset), so a member conflicts with it on whole segment overlaps, and the clip walk needs only the 32-position words at the
+// ends that hold the first and the last unconflicted match.  __host__ __device__: tests/cpp/k9_core_host.cpp runs exactly this code on the
+// CPU against the reference.
 #pragma once
 
 #include "strelka_b200.h"
@@ -17,7 +20,7 @@
 #define K9_HD inline
 #endif
 
-#define K9_MAX_READ 1024u // read positions of the reference map (per-thread scratch)
+#define K9_MAX_READ 1024u // read positions of the reference map (longer: SX_REALIGN_ST_LIMIT)
 
 enum // ref_map_type::map_t, starling_read_align_clipper.cpp:44-51
 {
@@ -34,7 +37,7 @@ struct k9_view
     const double* lnp;
 };
 
-struct k9_scratch // per thread
+struct k9_scratch // per thread (no longer read: the map is not stored)
 {
     uint8_t* type; // [K9_MAX_READ]
     int32_t* pos;  // [K9_MAX_READ]
@@ -139,6 +142,104 @@ K9_HD void k9_extend_or_add_sc(k9_writer& w, const uint32_t len) // :229-243
     else k9_push(w, SX_AP_SOFT_CLIP, len);
 }
 
+K9_HD uint32_t k9_ctz(const uint32_t x)
+{
+#if defined(__CUDA_ARCH__)
+    return (uint32_t)(__ffs(x) - 1);
+#else
+    return (uint32_t)__builtin_ctz(x);
+#endif
+}
+K9_HD uint32_t k9_clz(const uint32_t x)
+{
+#if defined(__CUDA_ARCH__)
+    return (uint32_t)__clz(x);
+#else
+    return (uint32_t)__builtin_clz(x);
+#endif
+}
+
+// the next segment of a path that covers read positions (ref_map_type of get_alignment_ref_map): [rb, re), its type and, for a MATCH, its
+// reference position minus its read position
+struct k9_cursor
+{
+    const sx_aln_seg* p;
+    uint32_t s, n, rb, re;
+    int32_t ref, off;
+    uint8_t type;
+};
+K9_HD bool k9_next(k9_cursor& c)
+{
+    c.rb = c.re;
+    for (; c.s < c.n; ++c.s)
+    {
+        const unsigned t(c.p[c.s].kind), len(c.p[c.s].len);
+        if (k9_align_match(t) || t == SX_AP_INSERT || t == SX_AP_SOFT_CLIP)
+        {
+            c.re = c.rb + len;
+            c.type = k9_align_match(t) ? K9_MATCH : (t == SX_AP_INSERT ? K9_INSERT : K9_SOFT_CLIP);
+            c.off = c.ref - (int32_t)c.rb;
+            if (k9_align_match(t)) c.ref += (int32_t)len;
+            ++c.s;
+            return true;
+        }
+        if (t == SX_AP_DELETE || t == SX_AP_SKIP) c.ref += (int32_t)len;
+    }
+    return false;
+}
+K9_HD k9_cursor k9_cursor_of(const k9_view& v, const uint32_t a)
+{
+    k9_cursor c;
+    c.p = v.b.segs + v.b.aln_seg_off[a];
+    c.s = 0;
+    c.n = v.b.aln_seg_off[a + 1] - v.b.aln_seg_off[a];
+    c.rb = c.re = 0;
+    c.ref = v.b.aln_pos[a];
+    c.off = 0;
+    c.type = K9_NONE;
+    return c;
+}
+// bits of [x, y) in the word of read positions w0 .. w0 + 31
+K9_HD uint32_t k9_bits(const uint32_t x, const uint32_t y, const uint32_t w0)
+{
+    const uint32_t lo(x > w0 ? x - w0 : 0u), hi(y - w0 < 32u ? y - w0 : 32u);
+    if (y <= w0 || lo >= hi) return 0u;
+    return (hi == 32u ? 0xFFFFFFFFu : ((1u << hi) - 1u)) & ~((1u << lo) - 1u);
+}
+
+// read positions w0 .. w0 + 31 of the chosen alignment's reference map after mark_ref_map_conflicts (:150-225): its MATCH and SOFT_CLIP
+// positions, and the positions where a member of the pool disagrees with it (another type, or a MATCH at another reference position)
+K9_HD void k9_word(const k9_view& v, const uint32_t a0, const uint32_t a1, const uint32_t best, const double range, const double maxScore, const uint32_t w0,
+                   uint32_t& match, uint32_t& soft, uint32_t& conflict)
+{
+    match = soft = conflict = 0;
+    const uint32_t w1(w0 + 32u);
+    k9_cursor c(k9_cursor_of(v, best));
+    while (k9_next(c) && c.rb < w1)
+    {
+        if (c.type == K9_MATCH) match |= k9_bits(c.rb, c.re, w0);
+        else if (c.type == K9_SOFT_CLIP) soft |= k9_bits(c.rb, c.re, w0);
+    }
+    for (uint32_t a = a0; a < a1; ++a)
+    {
+        if (a == best || v.lnp[a] + range < maxScore) continue;
+        k9_cursor m(k9_cursor_of(v, a)), c2(k9_cursor_of(v, best));
+        bool have(k9_next(c2));
+        while (k9_next(m) && m.rb < w1)
+        {
+            if (m.re <= w0) continue;
+            const uint32_t lo(m.rb > w0 ? m.rb : w0), hi(m.re < w1 ? m.re : w1);
+            while (have && c2.re <= lo) have = k9_next(c2);
+            while (have && c2.rb < hi)
+            {
+                if (c2.type != m.type || (m.type == K9_MATCH && c2.off != m.off)) conflict |= k9_bits(lo > c2.rb ? lo : c2.rb, hi < c2.re ? hi : c2.re, w0);
+                if (c2.re > hi) break;
+                have = k9_next(c2);
+            }
+        }
+    }
+}
+
 // one read.  slots: where its realignment goes (cap of them).  Returns the status byte.
 K9_HD uint32_t k9_read(const k9_view& v, const uint32_t region, const uint32_t r, k9_scratch& S, sx_aln_seg* slots, const uint32_t cap, int32_t& out_pos, uint16_t& out_n,
                        uint32_t& best_aln)
@@ -189,32 +290,21 @@ K9_HD uint32_t k9_read(const k9_view& v, const uint32_t region, const uint32_t r
     bool clip(false);
     if (poolSize > 1)
     {
-        // ---- get_alignment_ref_map of the chosen alignment
+        // ---- get_alignment_ref_map of the chosen alignment: its read length, and the statuses of the walk
+        for (uint32_t s = 0; s < n_path; ++s)
         {
-            int32_t ref_head(b.aln_pos[best]);
-            for (uint32_t s = 0; s < n_path; ++s)
+            const unsigned t(path[s].kind), len(path[s].len);
+            if (k9_align_match(t) || t == SX_AP_INSERT || t == SX_AP_SOFT_CLIP)
             {
-                const unsigned t(path[s].kind), len(path[s].len);
-                if (k9_align_match(t) || t == SX_AP_INSERT || t == SX_AP_SOFT_CLIP)
-                {
-                    if (read_size + len > K9_MAX_READ) return SX_REALIGN_ST_LIMIT;
-                    for (uint32_t j = 0; j < len; ++j)
-                    {
-                        S.type[read_size + j] = k9_align_match(t) ? K9_MATCH : (t == SX_AP_INSERT ? K9_INSERT : K9_SOFT_CLIP);
-                        S.pos[read_size + j] = k9_align_match(t) ? ref_head + (int32_t)j : 0;
-                    }
-                    read_size += len;
-                    if (k9_align_match(t)) ref_head += (int32_t)len;
-                }
-                else if (t == SX_AP_DELETE || t == SX_AP_SKIP) ref_head += (int32_t)len;
-                else if (t != SX_AP_HARD_CLIP) return SX_REALIGN_ST_BADPATH;
+                if (read_size + len > K9_MAX_READ) return SX_REALIGN_ST_LIMIT;
+                read_size += len;
             }
+            else if (!(t == SX_AP_DELETE || t == SX_AP_SKIP || t == SX_AP_HARD_CLIP)) return SX_REALIGN_ST_BADPATH;
         }
-        // ---- mark_ref_map_conflicts for every other member of the pool
+        // ---- the statuses of mark_ref_map_conflicts for every other member of the pool
         for (uint32_t a = a0; a < a1; ++a)
         {
             if (a == best || v.lnp[a] + range < maxScore) continue;
-            int32_t ref_head(b.aln_pos[a]);
             uint32_t read_head(0);
             for (uint32_t s = b.aln_seg_off[a]; s < b.aln_seg_off[a + 1]; ++s)
             {
@@ -222,30 +312,43 @@ K9_HD uint32_t k9_read(const k9_view& v, const uint32_t region, const uint32_t r
                 if (k9_align_match(t) || t == SX_AP_INSERT || t == SX_AP_SOFT_CLIP)
                 {
                     if (read_head + len > read_size) return SX_REALIGN_ST_BADPATH; // the reference would index past its vector
-                    const uint8_t want(k9_align_match(t) ? K9_MATCH : (t == SX_AP_INSERT ? K9_INSERT : K9_SOFT_CLIP));
-                    for (uint32_t j = 0; j < len; ++j)
-                    {
-                        const uint32_t i(read_head + j);
-                        if (S.type[i] == K9_CONFLICT) continue;
-                        if (S.type[i] != want || (want == K9_MATCH && S.pos[i] != ref_head + (int32_t)j)) S.type[i] = K9_CONFLICT;
-                    }
                     read_head += len;
-                    if (k9_align_match(t)) ref_head += (int32_t)len;
                 }
-                else if (t == SX_AP_DELETE || t == SX_AP_SKIP) ref_head += (int32_t)len;
-                else if (t != SX_AP_HARD_CLIP) return SX_REALIGN_ST_BADPATH;
+                else if (!(t == SX_AP_DELETE || t == SX_AP_SKIP || t == SX_AP_HARD_CLIP)) return SX_REALIGN_ST_BADPATH;
             }
         }
-        // ---- from each end: in until a match, then out until a conflict or a soft clip, :384-409
-        for (; lead_clip < read_size; lead_clip++)
-            if (S.type[lead_clip] == K9_MATCH) break;
-        for (; lead_clip > 0; lead_clip--)
-            if (S.type[lead_clip - 1] == K9_CONFLICT || S.type[lead_clip - 1] == K9_SOFT_CLIP) break;
+        // ---- from each end: in until a match, then out until a conflict or a soft clip, :384-409.  Word by word from each end: lead_clip is one
+        // past the last conflict / soft clip before the first unconflicted match, trail_clip the first one after the last (none: 0 / read_size)
+        const uint32_t n_words((read_size + 31u) / 32u);
+        for (uint32_t w = 0; w < n_words; ++w)
+        {
+            uint32_t m, sc, cf;
+            k9_word(v, a0, a1, best, range, maxScore, 32u * w, m, sc, cf);
+            const uint32_t valid(read_size - 32u * w >= 32u ? 0xFFFFFFFFu : (1u << (read_size - 32u * w)) - 1u);
+            const uint32_t free_match(m & ~cf & valid), stop((cf | sc) & valid);
+            if (free_match)
+            {
+                const uint32_t below(stop & ((1u << k9_ctz(free_match)) - 1u));
+                if (below) lead_clip = 32u * w + 32u - k9_clz(below);
+                break;
+            }
+            if (stop) lead_clip = 32u * w + 32u - k9_clz(stop);
+        }
         trail_clip = read_size;
-        for (; trail_clip > 0; trail_clip--)
-            if (S.type[trail_clip - 1] == K9_MATCH) break;
-        for (; trail_clip < read_size; trail_clip++)
-            if (S.type[trail_clip] == K9_CONFLICT || S.type[trail_clip] == K9_SOFT_CLIP) break;
+        for (uint32_t w = n_words; w-- > 0;)
+        {
+            uint32_t m, sc, cf;
+            k9_word(v, a0, a1, best, range, maxScore, 32u * w, m, sc, cf);
+            const uint32_t valid(read_size - 32u * w >= 32u ? 0xFFFFFFFFu : (1u << (read_size - 32u * w)) - 1u);
+            const uint32_t free_match(m & ~cf & valid), stop((cf | sc) & valid);
+            if (free_match)
+            {
+                const uint32_t above(stop & ~((2u << (31u - k9_clz(free_match))) - 1u));
+                if (above) trail_clip = 32u * w + k9_ctz(above);
+                break;
+            }
+            if (stop) trail_clip = 32u * w + k9_ctz(stop);
+        }
         // leading_clip >= trailing_clip: clipping failed, finishRealignment reverts to the chosen alignment (:1432-1435)
         clip = (lead_clip < trail_clip) && (lead_clip != 0 || trail_clip != read_size);
     }

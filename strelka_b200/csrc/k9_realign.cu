@@ -4,26 +4,26 @@
 // (starling_common/starling_read_align.cpp:1573-1741) with finishRealignment :1411-1450 and starling_read_align_clipper.cpp.  Per-read
 // body: k9_core.cuh.
 //
-// Shape of the work: per read two or three passes over its few alignments' segments (arg-max, pool preference, conflict marking) and
-// a per-read-position map of at most 1024 entries kept in local memory (interleaved per lane by the hardware).  Reads in the scores
+// Shape of the work: per read two or three passes over its few alignments' segments (arg-max, pool preference, conflict marking); the
+// conflicts are found on segment overlaps, 32 read positions at a time, so nothing per read position is stored.  Reads in the scores
 // where K1 wrote them and the alignments where K7 wrote them; writes one (pos, path) per read where K4 reads a read's best alignment.
 // HBM-bound by construction (~40 B per alignment in, ~30 B per read out).  Launches: slots per read -> scan -> choose.
 
 #include "k9_core.cuh"
 #include "sx_internal.h"
+#include "sx_read_index.cuh"
 
 #include <algorithm>
 
 namespace
 {
 // the slot counts go into seg_off, which the scan turns into the offsets
-__global__ void k9_slots_kernel(const sx_realign_batch b, uint32_t* __restrict__ cnt, uint32_t* __restrict__ read_region)
+__global__ void k9_slots_kernel(const sx_realign_batch b, uint32_t* __restrict__ cnt)
 {
     for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < b.n_reads; r += gridDim.x * blockDim.x) cnt[r] = k9_slots(b, r);
-    for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < b.n_regions; g += gridDim.x * blockDim.x)
-        for (uint32_t r = b.region_read_off[g]; r < b.region_read_off[g + 1]; ++r) read_region[r] = g;
 }
 
+// read_region: the read index's (the window pass), or NULL: a binary search of region_read_off per read (K9's own entry points)
 __global__ void __launch_bounds__(128) k9_choose_kernel(const k9_view v, const uint32_t* __restrict__ read_region, const sx_realign_out o, int* __restrict__ status)
 {
     if (o.totals[0] > o.cap_segs)
@@ -31,9 +31,7 @@ __global__ void __launch_bounds__(128) k9_choose_kernel(const k9_view v, const u
         if (blockIdx.x == 0 && threadIdx.x == 0) atomicOr(status, SX_ST_K9_CAP);
         return;
     }
-    uint8_t type[K9_MAX_READ];
-    int32_t pos[K9_MAX_READ];
-    k9_scratch S = {type, pos};
+    k9_scratch S = {nullptr, nullptr}; // (the reference map is not stored)
     const uint32_t n(v.b.n_reads);
     for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < n; r += gridDim.x * blockDim.x)
     {
@@ -41,7 +39,8 @@ __global__ void __launch_bounds__(128) k9_choose_kernel(const k9_view v, const u
         int32_t p;
         uint16_t ns;
         uint32_t best;
-        const uint32_t st(k9_read(v, read_region[r], r, S, o.segs + s0, s1 - s0, p, ns, best));
+        const uint32_t g(read_region ? read_region[r] : sxi_region_of(v.b.region_read_off, v.b.n_regions, r));
+        const uint32_t st(k9_read(v, g, r, S, o.segs + s0, s1 - s0, p, ns, best));
         if (!(st & SX_REALIGN_ST_REALIGNED)) k9_fallback(v.b, r, o.segs + s0, s1 - s0, p, ns);
         o.pos[r] = p;
         o.n_seg[r] = ns;
@@ -52,17 +51,15 @@ __global__ void __launch_bounds__(128) k9_choose_kernel(const k9_view v, const u
 } // namespace
 
 // K9's launcher
-int sx_k9_run(sx_ctx* ctx, const sx_realign_batch* d, const double* lnp, const sx_realign_out* o, unsigned* launches)
+int sx_k9_run(sx_ctx* ctx, const sx_realign_batch* d, const double* lnp, const sx_realign_out* o, const uint32_t* read_region, unsigned* launches)
 {
     if (d->n_reads == 0) return SX_OK;
     cudaStream_t st(ctx->s_compute);
     const uint32_t n(d->n_reads);
     int rc;
-    uint32_t* read_region(nullptr);
-    if ((rc = sx_take(ctx, SX_SLOT_K7A_K9_READ_WORD, n, read_region, 16))) return rc;
     const int cap(ctx->sm_count * 16);
     const auto grid = [cap](const uint32_t m) { return (unsigned)std::max(1, std::min<int>((int)((m + 127) / 128), cap)); };
-    k9_slots_kernel<<<grid(std::max(n, d->n_regions)), 128, 0, st>>>(*d, o->seg_off, read_region);
+    k9_slots_kernel<<<grid(n), 128, 0, st>>>(*d, o->seg_off);
     SX_CUDA(ctx, cudaGetLastError());
     *launches += 1;
     const sx_scan_set J = {1, {{o->seg_off, n, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, o->totals}}};
@@ -105,7 +102,7 @@ extern "C" int sx_choose_realignment_dev(sx_ctx* ctx, const sx_realign_batch* d,
         SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
         return SX_OK;
     }
-    if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k9_run(ctx, d, lnp_dev, out_dev, launches); }))) return rc;
+    if ((rc = sx_run_timed(ctx, [&](unsigned* launches) { return sx_k9_run(ctx, d, lnp_dev, out_dev, nullptr, launches); }))) return rc;
     return sx_check_status(ctx, "sx_choose_realignment", SX_ST_K9_CAP);
 }
 
@@ -148,7 +145,7 @@ extern "C" int sx_choose_realignment(sx_ctx* ctx, const sx_realign_batch* b, con
     if ((rc = sx_take(ctx, sx_host_slot(17), n, o.best_aln, 16))) return rc;
     if ((rc = sx_take(ctx, sx_host_slot(18), o.cap_segs, o.segs, 16))) return rc;
     unsigned launches(0);
-    if ((rc = sx_k9_run(ctx, &d, d_lnp, &o, &launches))) return rc;
+    if ((rc = sx_k9_run(ctx, &d, d_lnp, &o, nullptr, &launches))) return rc;
     if ((rc = sx_download(ctx, out_host->totals, o.totals, 1))) return rc;
     if ((rc = sx_download(ctx, out_host->seg_off, o.seg_off, n + 1))) return rc;
     SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));

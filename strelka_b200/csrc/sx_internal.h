@@ -113,12 +113,12 @@ enum sx_slot : int
     SX_SLOT_K7_CLASS, SX_SLOT_K7_HIST, SX_SLOT_K7_ACTIVE_BY_CLASS,
     SX_SLOT_K7A_READ_REGION, SX_SLOT_K7A_STAGE, SX_SLOT_K7A_ACTIVE,
     SX_SLOT_K8_ALN_READ, SX_SLOT_K8_READ_REGION, SX_SLOT_K8_SEG_N, SX_SLOT_K8_INS_N, SX_SLOT_K8_REG_SEG, SX_SLOT_K8_REG_INS, SX_SLOT_K8_SUMS,
-    // per-read scratch shared by K7a and K9: a per-read word (K7a: read byte offset, K9: read region) and the tile sums of their scan.
+    // per-read scratch shared by K7a and K9: a per-read word (K7a's entry: read byte offset, K9's entry: read region) and the tile sums of their scan.
     // These are O(reads) and every context that runs the window pass holds them.  Their lifetimes cannot overlap: K7a's are dead once its
     // write kernel has run, and K9 is enqueued after K7a on the same stream (sx_process_window_dev) or by its own entry point.
     SX_SLOT_K7A_K9_READ_WORD, SX_SLOT_K7A_K9_SUMS,
     // window pass: the intermediates of sx_process_window_dev
-    SX_SLOT_WIN_SEQ_OFF, SX_SLOT_WIN_QUAL_OFF, SX_SLOT_WIN_BPOS, SX_SLOT_WIN_NON_AMBIG, SX_SLOT_WIN_PIN, SX_SLOT_WIN_MAXIMA,
+    SX_SLOT_WIN_READ_REGION, SX_SLOT_WIN_SEQ_OFF, SX_SLOT_WIN_QUAL_OFF, SX_SLOT_WIN_BPOS, SX_SLOT_WIN_NON_AMBIG, SX_SLOT_WIN_PIN, SX_SLOT_WIN_MAXIMA,
     SX_SLOT_WIN_GATE, SX_SLOT_WIN_IN_POS, SX_SLOT_WIN_IN_SEGS,
     SX_SLOT_WIN_KEY_TOTALS, SX_SLOT_WIN_IN_KEY_OFF, SX_SLOT_WIN_IN_KEYS, SX_SLOT_WIN_IN_LEAD, SX_SLOT_WIN_IN_TRAIL,
     SX_SLOT_WIN_ENUM_TOTALS, SX_SLOT_WIN_ALN_OFF, SX_SLOT_WIN_ENUM_STATUS, SX_SLOT_WIN_ALN_POS, SX_SLOT_WIN_ALN_SEG_OFF, SX_SLOT_WIN_SEGS,
@@ -387,12 +387,34 @@ int sx_k6g_run(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* sampl
 // K2c on device arrays: count, scan, write.  totals_host[0] receives the record count (also on SX_ERR_CAPACITY, which leaves site_rec_off
 // written and no record).  One host synchronisation (the count).
 int sx_k2c_run(sx_ctx* ctx, const sx_cont_opts* o, const sx_cont_batch* d, const sx_cont_out* out, uint32_t* totals_host, unsigned* launches);
-int sx_k7g_run(sx_ctx* ctx, const sx_gate_batch* d, const sx_gate_out* o, unsigned* launches);
+// The read index (sx_read_index.cu): one pass, a warp per region.  Every output array is optional (NULL: not computed); seq_off / qual_off
+// (which need read_len and regions) are byte offsets in the pools -- the region's seq_off / qual_off plus the sizes of the reads before it in
+// the region -- closed by [n_reads].
+struct sx_read_index_in
+{
+    uint32_t n_regions, n_reads, qual_bits;
+    const uint32_t* region_read_off;
+    const uint16_t* read_len;
+    const sx_region* regions;
+};
+struct sx_read_index
+{
+    uint32_t* region;   // [n_reads] the read's region
+    uint32_t* seq_off;  // [n_reads + 1] byte offset of its packed bases
+    uint32_t* qual_off; // [n_reads + 1] ... of its qualities (qual_bits 4: packed like the bases; else one byte per base)
+};
+int sx_read_index_run(sx_ctx* ctx, const sx_read_index_in* in, const sx_read_index* o, unsigned* launches);
+// ... only the region of every read (the stages' own entry points)
+int sx_read_region_run(sx_ctx* ctx, uint32_t n_regions, uint32_t n_reads, const uint32_t* region_read_off, uint32_t* region, unsigned* launches);
+// The per-read stages take the region of every read (and K7a the byte offset of its packed bases) from the window's read index.  NULL (a
+// stage's own entry points): K7a and K7b build them with the index's kernel in place of the one launch they always had for it; the gates and
+// K9, which had none, search region_read_off per read.
+int sx_k7g_run(sx_ctx* ctx, const sx_gate_batch* d, const sx_gate_out* o, const uint32_t* read_region, unsigned* launches);
 int sx_k7a_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_region* regions, const uint8_t* seq4, const char* ref, const uint32_t* key_ins_off, const char* key_ins,
-               const sx_prep_out* o, unsigned* launches);
+               const sx_prep_out* o, const uint32_t* read_region, const uint32_t* read_seq_off, unsigned* launches);
 int sx_k7_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* o, unsigned* launches);
 // K7 and K7a: the reads whose gate lets them into the search (SX_GATE_REALIGN) as a dense list, *count of them (one launch)
 int sx_k7_active_reads(sx_ctx* ctx, uint32_t n_reads, const uint8_t* gate, uint32_t* list, uint32_t* count);
 int sx_k8_run(sx_ctx* ctx, const sx_enum_batch* d, const sx_enum_out* e, uint32_t n_alns, const uint32_t* key_ins_off, const char* key_ins, const sx_link_out* o,
-              unsigned* launches);
-int sx_k9_run(sx_ctx* ctx, const sx_realign_batch* d, const double* lnp, const sx_realign_out* o, unsigned* launches);
+              const uint32_t* read_region, unsigned* launches);
+int sx_k9_run(sx_ctx* ctx, const sx_realign_batch* d, const double* lnp, const sx_realign_out* o, const uint32_t* read_region, unsigned* launches);

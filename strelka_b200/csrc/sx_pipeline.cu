@@ -7,10 +7,12 @@
 //
 // Nothing here is a new algorithm: the function owns the buffers between the stages and enqueues the stage launchers (each beside its
 // kernels: sx_k7g_run ... sx_k2a_run) on the context's compute stream.  What crosses to the host between the stages is the handful of totals
-// that size the next stage's buffers and launch; every array stays in HBM.  Three small kernels of its own prepare what no stage
-// produces: per-read byte offsets / buffer positions / 'N' counts (prep), the sub-mapped reads' gate (align_pos :746), and K4's read
-// records from K9's best alignments (pileup_read_segment's preamble :1136-1171).
+// that size the next stage's buffers and launch; every array stays in HBM.  Small kernels of its own prepare what no stage produces: the
+// read index of sx_read_index.cu (per-read regions and byte offsets, which K7g, K7a, K7b and K9 read) and the per-read facts read off it --
+// 'N' counts, buffer positions, pin bits -- with the window entries' longest insert (prep), the sub-mapped reads' gate (align_pos :746),
+// and K4's read records from K9's best alignments (pileup_read_segment's preamble :1136-1171).
 #include "sx_internal.h"
+#include "sx_read_index.cuh"
 
 #include <algorithm>
 #include <cstring>
@@ -19,52 +21,35 @@ namespace
 {
 struct prep_out
 {
-    uint32_t* seq_off;   // [n_reads + 1] byte offset of each read's packed bases (reads of a region back to back, each on a byte boundary)
-    uint32_t* qual_off;  // [n_reads + 1] ... of its qualities (qual_bits 4: packed like the bases; else one byte per base)
-    int32_t* bpos;       // [n_reads] rseg.buffer_pos
-    uint16_t* non_ambig; // [n_reads] bases that are not 'N'
+    uint32_t* region;    // [n_reads] the read's region (this and the two offsets: the read index, sx_read_index.cu)
+    uint32_t* seq_off;   // [n_reads + 1] byte offset of its packed bases (reads of a region back to back, each on a byte boundary),
+    uint32_t* qual_off;  // [n_reads + 1] ... of its qualities (qual_bits 4: packed like the bases; else one byte per base),
+    int32_t* bpos;       // [n_reads] rseg.buffer_pos,
+    uint16_t* non_ambig; // [n_reads] bases that are not 'N',
     uint8_t* pin;        // [n_reads] bit 0 / 1: edge pins
     uint32_t* maxima;    // [4] max insert length of a window entry, max |best pos - buffer pos|, max reference span, (unused)
 };
 
-// one thread per region walks its reads (tens): offsets are a running sum inside the region
-__global__ void sxp_prep_kernel(const sx_window_batch b, const prep_out o)
+// the per-read facts only the window pass reads, from the read index's offsets: 'N' counts (K6), buffer positions (K4), pin bits (K7g, K9)
+__global__ void sxp_read_facts_kernel(const sx_window_batch b, const prep_out o)
 {
-    for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < b.n_regions; g += gridDim.x * blockDim.x)
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < b.n_reads; r += gridDim.x * blockDim.x)
     {
-        unsigned long long sb(b.regions[g].seq_off), qb(b.regions[g].qual_off);
-        for (uint32_t r = b.region_read_off[g]; r < b.region_read_off[g + 1]; ++r)
-        {
-            const uint32_t len(b.read_len[r]), packed((len + 1u) / 2u);
-            o.seq_off[r] = (uint32_t)sb;
-            o.qual_off[r] = (uint32_t)qb;
-            // 'N' count (score_indels :866-875)
-            uint32_t n_amb(0);
-            for (uint32_t i = 0; i < len; ++i) n_amb += (((b.seq4[sb + (i >> 1)] >> ((~i & 1u) << 2)) & 15u) == 15u) ? 1u : 0u;
-            o.non_ambig[r] = (uint16_t)(len - n_amb);
-            // get_alignment_buffer_pos (starling_read_util.cpp:30-35): pos - unalignedPrefixSize
-            uint32_t lead(0);
-            for (uint32_t s = b.raw_seg_off[r]; s < b.raw_seg_off[r + 1]; ++s)
-            {
-                const unsigned t(b.raw_segs[s].kind);
-                if (!(t == SX_AP_INSERT || t == SX_AP_HARD_CLIP || t == SX_AP_SOFT_CLIP)) break;
-                if (t != SX_AP_HARD_CLIP) lead += b.raw_segs[s].len;
-            }
-            o.bpos[r] = b.raw_pos[r] - (int32_t)lead;
-            const unsigned f(b.read_flags[r]);
-            o.pin[r] = (uint8_t)(((f & SX_PRF_PIN_FIRST) ? 1u : 0u) | ((f & SX_PRF_PIN_SECOND) ? 2u : 0u));
-            sb += packed;
-            qb += (b.qual_bits == 4) ? packed : len;
-        }
-        if (g + 1 == b.n_regions)
-        {
-            o.seq_off[b.n_reads] = (uint32_t)sb;
-            o.qual_off[b.n_reads] = (uint32_t)qb;
-        }
+        const uint32_t len(b.read_len[r]);
+        o.non_ambig[r] = (uint16_t)(len - sxi_count_n(b.seq4 + o.seq_off[r], len)); // score_indels :866-875
+        const uint32_t s0(b.raw_seg_off[r]);
+        o.bpos[r] = sxi_buffer_pos(b.raw_pos[r], b.raw_segs + s0, b.raw_seg_off[r + 1] - s0);
+        const unsigned f(b.read_flags[r]);
+        o.pin[r] = (uint8_t)(((f & SX_PRF_PIN_FIRST) ? 1u : 0u) | ((f & SX_PRF_PIN_SECOND) ? 2u : 0u));
     }
+}
+
+// the longest insert of a window entry (sizes K7b's insert pool)
+__global__ void sxp_key_max_kernel(const uint32_t n_keys, const sx_indel_key* __restrict__ keys, uint32_t* __restrict__ maxima)
+{
     uint32_t m(0);
-    for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < b.n_keys; k += gridDim.x * blockDim.x) m = max(m, (uint32_t)b.keys[k].ins_len);
-    if (m) atomicMax(&o.maxima[0], m);
+    for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < n_keys; k += gridDim.x * blockDim.x) m = max(m, (uint32_t)keys[k].ins_len);
+    if (m) atomicMax(&maxima[0], m);
 }
 
 // align_pos :746: only tier1 / tier2 mappings are realigned
@@ -358,6 +343,7 @@ int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint3
     // ---------------------------------------------------------------------------------------------------------------- prep
     SX_CUDA(ctx, mark(SX_WIN_ST_PREP));
     prep_out P;
+    if ((rc = take(ctx, SX_SLOT_WIN_READ_REGION, (size_t)n + 1, P.region))) return rc;
     if ((rc = take(ctx, SX_SLOT_WIN_SEQ_OFF, (size_t)n + 1, P.seq_off))) return rc;
     if ((rc = take(ctx, SX_SLOT_WIN_QUAL_OFF, (size_t)n + 1, P.qual_off))) return rc;
     if ((rc = take(ctx, SX_SLOT_WIN_BPOS, (size_t)n + 1, P.bpos))) return rc;
@@ -368,9 +354,21 @@ int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint3
     uint32_t n_raw_segs(0);
     if (n)
     {
-        sxp_prep_kernel<<<grid(std::max(nr, b->n_keys)), 128, 0, st>>>(*b, P);
+        sx_read_index_in in;
+        memset(&in, 0, sizeof(in));
+        in.n_regions = nr;
+        in.n_reads = n;
+        in.qual_bits = b->qual_bits;
+        in.region_read_off = b->region_read_off;
+        in.read_len = b->read_len;
+        in.regions = b->regions;
+        const sx_read_index ix = {P.region, P.seq_off, P.qual_off};
+        if ((rc = sx_read_index_run(ctx, &in, &ix, &launches))) return rc;
+        sxp_read_facts_kernel<<<grid(n), 128, 0, st>>>(*b, P);
         SX_CUDA(ctx, cudaGetLastError());
-        ++launches;
+        sxp_key_max_kernel<<<grid(b->n_keys), 128, 0, st>>>(b->n_keys, b->keys, P.maxima);
+        SX_CUDA(ctx, cudaGetLastError());
+        launches += 2;
         SX_CUDA(ctx, cudaMemcpyAsync(&n_raw_segs, b->raw_seg_off + n, 4, cudaMemcpyDeviceToHost, st));
     }
     // ---------------------------------------------------------------------------------------------------------------- K7g gates
@@ -399,7 +397,7 @@ int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint3
         gb.pin_flags = P.pin;
         gb.max_indel_size = b->enum_opts.max_indel_size;
         sx_gate_out go = {gate, in_pos, in_segs};
-        if ((rc = sx_k7g_run(ctx, &gb, &go, &launches))) return rc;
+        if ((rc = sx_k7g_run(ctx, &gb, &go, P.region, &launches))) return rc;
         if (n)
         {
             sxp_submapped_gate_kernel<<<grid(n), 128, 0, st>>>(n, b->read_flags, gate);
@@ -445,7 +443,7 @@ int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint3
         po.in_keys = in_keys;
         po.in_lead_key = in_lead;
         po.in_trail_key = in_trail;
-        if ((rc = sx_k7a_run(ctx, &eb, b->regions, b->seq4, b->ref, b->key_ins_off, b->key_ins, &po, &launches))) return rc;
+        if ((rc = sx_k7a_run(ctx, &eb, b->regions, b->seq4, b->ref, b->key_ins_off, b->key_ins, &po, P.region, P.seq_off, &launches))) return rc;
         SX_CUDA(ctx, cudaMemcpyAsync(&n_in_keys, po.totals, 4, cudaMemcpyDeviceToHost, st));
         SX_CUDA(ctx, cudaStreamSynchronize(st));
         if (n_in_keys <= cap_in_keys) break;
@@ -521,7 +519,7 @@ int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint3
     uint32_t link_totals[2] = {0, 0};
     if (n)
     {
-        if ((rc = sx_k8_run(ctx, &eb, &eo, nA, b->key_ins_off, b->key_ins, &lo, &launches))) return rc;
+        if ((rc = sx_k8_run(ctx, &eb, &eo, nA, b->key_ins_off, b->key_ins, &lo, P.region, &launches))) return rc;
         SX_CUDA(ctx, cudaMemcpyAsync(link_totals, lo.totals, 8, cudaMemcpyDeviceToHost, st));
     }
     // ---------------------------------------------------------------------------------------------------------------- K1 scores
@@ -625,7 +623,7 @@ int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint3
         rb.raw_pos = b->raw_pos;
         rb.raw_seg_off = b->raw_seg_off;
         rb.raw_segs = b->raw_segs;
-        if ((rc = sx_k9_run(ctx, &rb, lnp, &ro, &launches))) return rc;
+        if ((rc = sx_k9_run(ctx, &rb, lnp, &ro, P.region, &launches))) return rc;
     }
     // ---------------------------------------------------------------------------------------------------------------- K4 pile-up
     SX_CUDA(ctx, mark(SX_WIN_ST_PILEUP));
