@@ -10,38 +10,20 @@
 //   k6b_locus_table_kernel  id -> locus as a dense table of n_gid words.  A binary search of loci.gid would cost ~20 dependent loads per
 //                           record, twice (count and scatter), against one load here; the table is an eighth of the gid_key array the
 //                           caller already holds, so an id space too sparse for it is too sparse for the ABI.
-//   k6b_count_kernel        one thread per read of either sample: integer atomics on cnt[2 * locus + sample]
-//   scan                    -> pair_off, copied to the scatter's cursors; one 12-byte round trip sizes the pair scratch (and refuses more
-//                           than 2^32 - 1 entries)
-//   k6b_scatter_kernel      (read id, record, read) triples at atomic cursors: the order inside a (locus, sample) segment is arbitrary here
-//   k6b_sort_kernel         one warp per locus: each segment sorted by read id (k6b_sort_by_key, in shared memory up to K6B_SMEM_SORT
-//                           entries, in the global scratch itself beyond -- no depth cap), equal neighbours = a duplicate id; the
-//                           alternates' ids gathered into an ascending set of at most 16.  Read ids of an unflagged segment are distinct,
-//                           so the sorted order -- and with it every output byte -- is the same whatever order the atomics ran in.
+//   the list builder        (k6_lists.cuh) count, scan, scatter and sort into segments 2 * locus + sample, one warp per locus in the sort;
+//                           its hook (k6b_hook) gathers the alternates' ids into an ascending set of at most 16 and writes each locus's status
 //   scan                    of the unflagged loci's counts, in place in read_off and alt_off, -> totals; one 8-byte round trip checks
 //                           the capacities
 //   k6b_write_kernel        one warp per locus: the table rows from gid_key, and every entry (k6b_entry) at its sorted place
 // The body is k6b_core.cuh.
-#include "k6b_core.cuh"
-#include "sx_internal.h"
-
-#include <algorithm>
+#include "k6_lists.cuh"
 
 namespace
 {
 constexpr int K6B_THREADS = 128;
 constexpr int K6B_WARPS = K6B_THREADS / 32;
-constexpr uint32_t K6B_SMEM_SORT = 512; // entries of one (locus, sample) segment sorted in shared memory: 4 KiB per warp
 constexpr unsigned FULL = 0xffffffffu;
 static_assert(SX_ST_INDEL_READS_DUP == SX_INDEL_READS_ST_DUP_READ, "the per-locus duplicate status of K6b is its status bit");
-
-struct k6b_pairs // the scatter's output, segment (locus, sample) at pair_off[2 * locus + sample]
-{
-    uint32_t* id;    // read id (sorted in place on the deep path)
-    uint32_t* rec;   // record index in the sample's recs
-    uint32_t* read;  // read index in the sample
-    uint32_t* order; // order[i] = which of the segment's triples is i-th by read id
-};
 
 __global__ void k6b_locus_table_kernel(const sx_indel_loci loci, uint32_t* __restrict__ locus_of, int* __restrict__ status)
 {
@@ -53,106 +35,56 @@ __global__ void k6b_locus_table_kernel(const sx_indel_loci loci, uint32_t* __res
     }
 }
 
-// `total` is the 64-bit count of what the 32-bit counts and their scan hold: the launcher refuses a batch whose entries do not fit 32 bits
-__global__ void __launch_bounds__(K6B_THREADS) k6b_count_kernel(const k6b_view v, uint32_t* __restrict__ cnt, unsigned long long* __restrict__ total, int* __restrict__ status)
+// K6b's part of the list builder's sort: each locus's ascending alternate ids (alt_ids[16 * locus ..]), its status, and the counts the second
+// scan runs over (read_off[2 * locus + sample], alt_off[locus]; 0 for a flagged locus)
+struct k6b_hook
 {
-    const uint32_t n0(v.s[0].n_reads), n(n0 + v.s[1].n_reads);
-    uint32_t st(0);
-    unsigned long long mine(0);
-    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x)
+    static constexpr uint32_t n_samples = 2;
+    struct warp_smem
     {
-        const uint32_t sample(t < n0 ? 0u : 1u);
-        st |= k6b_for_each_entry(v, sample, t - (sample ? n0 : 0u), [&](const uint32_t l, uint32_t) {
-            atomicAdd(cnt + 2 * l + sample, 1u);
-            ++mine;
-        });
-    }
-    for (int d = 16; d > 0; d >>= 1) mine += __shfl_down_sync(FULL, mine, d);
-    if ((threadIdx.x & 31) == 0 && mine) atomicAdd(total, mine);
-    if (st) atomicOr(status, SX_ST_K6B_ID);
-}
+        uint32_t set[SX_SINDEL_MAX_ALTS], n, over;
+    };
+    k6b_view v;
+    uint32_t* alt_ids;
+    sx_indel_reads_out o;
 
-__global__ void __launch_bounds__(K6B_THREADS) k6b_scatter_kernel(const k6b_view v, uint32_t* __restrict__ cursor, const k6b_pairs P)
-{
-    const uint32_t n0(v.s[0].n_reads), n(n0 + v.s[1].n_reads);
-    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x)
+    __device__ void begin(warp_smem& w, const uint32_t lane) const
     {
-        const uint32_t sample(t < n0 ? 0u : 1u), r(t - (sample ? n0 : 0u));
-        const uint32_t id(k6b_read_id(v.s[sample], r));
-        k6b_for_each_entry(v, sample, r, [&](const uint32_t l, const uint32_t i) {
-            const uint32_t at(atomicAdd(cursor + 2 * l + sample, 1u));
-            P.id[at] = id;
-            P.rec[at] = i;
-            P.read[at] = r;
-        });
-    }
-}
-
-// one warp per locus: P.order of both segments, the locus's status, its ascending alternate ids (alt_ids[16 * locus ..]) and the counts
-// the second scan runs over (read_off[2 * locus + sample], alt_off[locus]; 0 for a flagged locus)
-__global__ void __launch_bounds__(K6B_THREADS) k6b_sort_kernel(const k6b_view v, const uint32_t* __restrict__ pair_off, const k6b_pairs P, uint32_t* __restrict__ alt_ids,
-                                                              const sx_indel_reads_out o, int* __restrict__ status)
-{
-    __shared__ uint32_t s_key[K6B_WARPS][K6B_SMEM_SORT], s_val[K6B_WARPS][K6B_SMEM_SORT];
-    __shared__ uint32_t s_set[K6B_WARPS][SX_SINDEL_MAX_ALTS], s_n[K6B_WARPS], s_over[K6B_WARPS];
-    const uint32_t lane(threadIdx.x & 31), warp(threadIdx.x >> 5);
-    const auto sync = [] { __syncwarp(); };
-    uint32_t bad(0);
-    for (uint32_t l = blockIdx.x * K6B_WARPS + warp; l < v.loci.n_loci; l += gridDim.x * K6B_WARPS)
-    {
-        if (lane == 0) s_n[warp] = s_over[warp] = 0;
+        if (lane == 0) w.n = w.over = 0;
         __syncwarp();
-        bool dup(false);
-        for (uint32_t sample = 0; sample < 2; ++sample)
+    }
+    // the ids this segment's entries name as alternates, into the locus's set (lane 0 inserts, one new id per round)
+    __device__ uint32_t segment(warp_smem& w, uint32_t, const uint32_t sample, const uint32_t base, const uint32_t n, const k6l_pairs& P, const uint32_t lane) const
+    {
+        const sx_indel_reads_sample& s(v.s[sample]);
+        uint32_t bad(0);
+        for (uint32_t i0 = 0; i0 < n && !w.over; i0 += 32)
         {
-            const sx_indel_reads_sample& s(v.s[sample]);
-            const uint32_t base(pair_off[2 * l + sample]), n(pair_off[2 * l + sample + 1] - base);
-            const uint32_t* key(P.id + base);
-            if (n <= K6B_SMEM_SORT)
+            uint32_t ids[2] = {K6B_NONE, K6B_NONE};
+            if (i0 + lane < n)
             {
-                for (uint32_t i = lane; i < n; i += 32)
+                const sx_read_indel_score& rec(s.recs[P.rec[base + i0 + lane]]);
+                if (rec.n_alt) k6b_alt_ids(s, v.loci.n_gid, k6b_region_of(s, P.read[base + i0 + lane]), rec, ids, bad);
+            }
+            for (uint32_t a = 0; a < 2; ++a)
+                for (;;)
                 {
-                    s_key[warp][i] = P.id[base + i];
-                    s_val[warp][i] = i;
+                    bool need(ids[a] != K6B_NONE && !w.over);
+                    for (uint32_t k = 0; need && k < w.n; ++k) need = w.set[k] != ids[a];
+                    const unsigned m(__ballot_sync(FULL, need));
+                    if (!m) break;
+                    const uint32_t id(__shfl_sync(FULL, ids[a], __ffs(m) - 1));
+                    if (lane == 0 && !k6b_set_insert(w.set, w.n, id)) w.over = 1;
+                    __syncwarp();
                 }
-                __syncwarp();
-                k6b_sort_by_key(s_key[warp], s_val[warp], n, lane, 32u, sync);
-                for (uint32_t i = lane; i < n; i += 32) P.order[base + i] = s_val[warp][i];
-                key = s_key[warp];
-            }
-            else
-            {
-                for (uint32_t i = lane; i < n; i += 32) P.order[base + i] = i;
-                __syncwarp();
-                k6b_sort_by_key(P.id + base, P.order + base, n, lane, 32u, sync);
-            }
-            for (uint32_t i = lane; i + 1 < n; i += 32) dup |= key[i] == key[i + 1];
-            // the ids this segment's entries name as alternates, into the locus's set (lane 0 inserts, one new id per round)
-            for (uint32_t i0 = 0; i0 < n && !s_over[warp]; i0 += 32)
-            {
-                uint32_t ids[2] = {K6B_NONE, K6B_NONE};
-                if (i0 + lane < n)
-                {
-                    const sx_read_indel_score& rec(s.recs[P.rec[base + i0 + lane]]);
-                    if (rec.n_alt) k6b_alt_ids(s, v.loci.n_gid, k6b_region_of(s, P.read[base + i0 + lane]), rec, ids, bad);
-                }
-                for (uint32_t a = 0; a < 2; ++a)
-                    for (;;)
-                    {
-                        bool need(ids[a] != K6B_NONE && !s_over[warp]);
-                        for (uint32_t k = 0; need && k < s_n[warp]; ++k) need = s_set[warp][k] != ids[a];
-                        const unsigned m(__ballot_sync(FULL, need));
-                        if (!m) break;
-                        const uint32_t id(__shfl_sync(FULL, ids[a], __ffs(m) - 1));
-                        if (lane == 0 && !k6b_set_insert(s_set[warp], s_n[warp], id)) s_over[warp] = 1;
-                        __syncwarp();
-                    }
-            }
-            __syncwarp(); // s_key is loaded again for the tumor segment
         }
-        const uint32_t st((__any_sync(FULL, dup) ? SX_INDEL_READS_ST_DUP_READ : 0u) | (s_over[warp] ? SX_SINDEL_ST_CAP : 0u));
-        const uint32_t n_alts(st ? 0u : s_n[warp]);
-        if (lane < n_alts) alt_ids[(size_t)SX_SINDEL_MAX_ALTS * l + lane] = s_set[warp][lane];
+        return bad;
+    }
+    __device__ void end(warp_smem& w, const uint32_t l, const bool dup, const uint32_t* pair_off, const uint32_t lane) const
+    {
+        const uint32_t st((dup ? SX_INDEL_READS_ST_DUP_READ : 0u) | (w.over ? SX_SINDEL_ST_CAP : 0u));
+        const uint32_t n_alts(st ? 0u : w.n);
+        if (lane < n_alts) alt_ids[(size_t)SX_SINDEL_MAX_ALTS * l + lane] = w.set[lane];
         if (lane < 2) o.read_off[2 * l + lane] = st ? 0u : pair_off[2 * l + lane + 1] - pair_off[2 * l + lane];
         if (lane == 0)
         {
@@ -161,10 +93,9 @@ __global__ void __launch_bounds__(K6B_THREADS) k6b_sort_kernel(const k6b_view v,
         }
         __syncwarp();
     }
-    if (bad) atomicOr(status, SX_ST_K6B_ID);
-}
+};
 
-__global__ void __launch_bounds__(K6B_THREADS) k6b_write_kernel(const k6b_view v, const uint32_t* __restrict__ pair_off, const k6b_pairs P, const uint32_t* __restrict__ alt_ids,
+__global__ void __launch_bounds__(K6B_THREADS) k6b_write_kernel(const k6b_view v, const uint32_t* __restrict__ pair_off, const k6l_pairs P, const uint32_t* __restrict__ alt_ids,
                                                                const sx_indel_reads_out o)
 {
     const uint32_t lane(threadIdx.x & 31), warp(threadIdx.x >> 5);
@@ -235,13 +166,13 @@ int sx_k6b_check_loci(sx_ctx* ctx, const char* what, const sx_indel_loci* loci)
 }
 
 // The stage's launcher, beside its kernels like sx_k6_run: everything is enqueued on the compute stream, with two small round trips (the
-// pair total, then the output totals).  own_out: the entry and table arrays are taken from the context's SX_SLOT_K6B_OUT_* buffers once
+// list builder's, then the output totals).  own_out: the entry and table arrays are taken from the context's SX_SLOT_K6B_OUT_* buffers once
 // the totals are known, instead of checked against the caller's capacities.
 int sx_k6b_run(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* normal, const sx_indel_reads_sample* tumor, const sx_indel_loci* loci, sx_indel_reads_out* o,
             uint32_t* totals_host, const bool own_out, unsigned* launches)
 {
     cudaStream_t st(ctx->s_compute);
-    const uint32_t n_loci(loci->n_loci), n2(2 * n_loci), n_reads(normal->n_reads + tumor->n_reads);
+    const uint32_t n_loci(loci->n_loci), n2(2 * n_loci);
     uint32_t h_totals[2] = {0, 0};
     int rc;
     if (n_loci == 0)
@@ -253,14 +184,9 @@ int sx_k6b_run(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* norma
         return SX_OK;
     }
     if (!o->status) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL output array", what);
-    uint32_t *locus_of(nullptr), *pair_off(nullptr), *cursor(nullptr), *alt_ids(nullptr);
+    uint32_t *locus_of(nullptr), *alt_ids(nullptr);
     if ((rc = sx_take(ctx, SX_SLOT_K6B_LOCUS_OF, loci->n_gid, locus_of, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K6B_PAIR_OFF, (size_t)n2 + 1, pair_off, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K6B_CURSOR, (size_t)n2 + 2, cursor, 0))) return rc;
     if ((rc = sx_take(ctx, SX_SLOT_K6B_ALT_IDS, (size_t)SX_SINDEL_MAX_ALTS * n_loci, alt_ids, 16))) return rc;
-    unsigned long long* total64(reinterpret_cast<unsigned long long*>(cursor + n2)); // (past the cursors; n2 is even, so 8-byte aligned)
-    const int cap(ctx->sm_count * 16);
-    const auto grid = [cap](const uint32_t m, const uint32_t per) { return (unsigned)std::max(1, std::min<int>((int)((m + per - 1) / per), cap)); };
 
     k6b_view v;
     v.s[0] = *normal;
@@ -268,35 +194,13 @@ int sx_k6b_run(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* norma
     v.loci = *loci;
     v.locus_of = locus_of;
     SX_CUDA(ctx, cudaMemsetAsync(locus_of, 0xFF, (size_t)loci->n_gid * 4, st));
-    SX_CUDA(ctx, cudaMemsetAsync(pair_off, 0, (size_t)n2 * 4, st));
-    k6b_locus_table_kernel<<<grid(n_loci, 256), 256, 0, st>>>(*loci, locus_of, ctx->d_status);
+    k6b_locus_table_kernel<<<k6l_grid(ctx, n_loci, 256), 256, 0, st>>>(*loci, locus_of, ctx->d_status);
     SX_CUDA(ctx, cudaGetLastError());
-    SX_CUDA(ctx, cudaMemsetAsync(total64, 0, 8, st));
-    k6b_count_kernel<<<grid(n_reads, K6B_THREADS), K6B_THREADS, 0, st>>>(v, pair_off, total64, ctx->d_status);
-    SX_CUDA(ctx, cudaGetLastError());
-    *launches += 2;
-    const sx_scan_set pairs = {1, {{pair_off, n2, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, nullptr}}};
-    if ((rc = sx_scan(ctx, SX_SLOT_K6B_SUMS, pairs, launches))) return rc;
-    SX_CUDA(ctx, cudaMemcpyAsync(cursor, pair_off, (size_t)n2 * 4, cudaMemcpyDeviceToDevice, st));
-    uint32_t n_pairs(0);
-    unsigned long long n_pairs64(0);
-    SX_CUDA(ctx, cudaMemcpyAsync(&n_pairs, pair_off + n2, 4, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaMemcpyAsync(&n_pairs64, total64, 8, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaStreamSynchronize(st));
-    if (n_pairs64 != n_pairs) return sx_fail(ctx, SX_ERR_RANGE, "%s: %llu entries: the offsets are 32-bit", what, n_pairs64);
-
-    k6b_pairs P;
-    if ((rc = sx_take(ctx, SX_SLOT_K6B_PAIR_ID, n_pairs, P.id, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K6B_PAIR_REC, n_pairs, P.rec, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K6B_PAIR_READ, n_pairs, P.read, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K6B_PAIR_ORDER, n_pairs, P.order, 16))) return rc;
-    k6b_scatter_kernel<<<grid(n_reads, K6B_THREADS), K6B_THREADS, 0, st>>>(v, cursor, P);
-    SX_CUDA(ctx, cudaGetLastError());
-    k6b_sort_kernel<<<grid(n_loci, K6B_WARPS), K6B_THREADS, 0, st>>>(v, pair_off, P, alt_ids, *o, ctx->d_status);
-    SX_CUDA(ctx, cudaGetLastError());
-    *launches += 2;
+    *launches += 1;
+    k6l_lists L;
+    if ((rc = k6l_build(ctx, what, v, n_loci, k6b_hook{v, alt_ids, *o}, &L, launches))) return rc;
     const sx_scan_set out = {2, {{o->read_off, n2, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, o->totals}, {o->alt_off, n_loci, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, o->totals + 1}}};
-    if ((rc = sx_scan(ctx, SX_SLOT_K6B_SUMS, out, launches))) return rc;
+    if ((rc = sx_scan(ctx, SX_SLOT_K6L_SUMS, out, launches))) return rc;
     SX_CUDA(ctx, cudaMemcpyAsync(h_totals, o->totals, 8, cudaMemcpyDeviceToHost, st));
     SX_CUDA(ctx, cudaStreamSynchronize(st));
     if (totals_host)
@@ -314,7 +218,7 @@ int sx_k6b_run(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* norma
     if (h_totals[0] > o->cap_reads || h_totals[1] > o->cap_alts)
         return sx_fail(ctx, SX_ERR_CAPACITY, "%s: output capacity too small: %u entries, %u alternates needed", what, h_totals[0], h_totals[1]);
     if ((h_totals[0] && !o->reads) || (h_totals[1] && !o->alts)) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL output array", what);
-    k6b_write_kernel<<<grid(n_loci, K6B_WARPS), K6B_THREADS, 0, st>>>(v, pair_off, P, alt_ids, *o);
+    k6b_write_kernel<<<k6l_grid(ctx, n_loci, K6B_WARPS), K6B_THREADS, 0, st>>>(v, L.off, L.P, alt_ids, *o);
     SX_CUDA(ctx, cudaGetLastError());
     *launches += 1;
     return SX_OK;
@@ -360,20 +264,7 @@ extern "C" int sx_link_indel_reads_dev(sx_ctx* ctx, const sx_indel_reads_sample*
     int rc;
     if ((rc = k6b_check(ctx, what, normal, tumor, loci)) || (rc = k6b_check_out(ctx, what, out_dev))) return rc;
     sx_indel_reads_out o(*out_dev);
-    bool ran(false);
-    int rc_link(SX_OK);
-    rc = sx_run_timed(ctx, [&](unsigned* launches) {
-        ran = true;
-        rc_link = sx_k6b_run(ctx, what, normal, tumor, loci, &o, totals_host, false, launches);
-        return SX_OK; // (the timer finishes whatever the link returns: its totals stand even when a capacity is too small)
-    });
-    if (!ran) return rc; // (the device could not be set)
-    if (rc_link == SX_ERR_CAPACITY || rc_link == SX_OK)
-    {
-        const int rc3(sx_check_status(ctx, what, SX_ST_K6B_ID)); // (a bad id outranks the capacity it may have inflated)
-        if (rc3) return rc3;
-    }
-    return rc_link ? rc_link : rc;
+    return k6l_link_dev(ctx, what, SX_ST_K6B_ID, [&](unsigned* launches) { return sx_k6b_run(ctx, what, normal, tumor, loci, &o, totals_host, false, launches); });
 }
 
 extern "C" int sx_link_indel_reads(sx_ctx* ctx, const sx_indel_reads_sample* normal, const sx_indel_reads_sample* tumor, const sx_indel_loci* loci,

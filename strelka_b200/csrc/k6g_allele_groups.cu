@@ -9,14 +9,8 @@
 // (tools/germline_indel_leg.py counts them).  A CSR producer like K6b: count -> scan (sx_scan) -> write, with a sort between.
 //   k6g_mark_kernel         one thread per group: the group's checks, and list_of[id] = id for every id it names (a dense table of n_gid
 //                           words, as K6b's id -> locus table; several groups store the same value to one word)
-//   k6g_count_kernel        one thread per read: integer atomics on cnt[id], through K6b's record walk (k6b_for_each_entry)
-//   scan                    -> list_off, copied to the scatter's cursors; one 12-byte round trip sizes the triples (and refuses more
-//                           than 2^32 - 1)
-//   k6g_scatter_kernel      (read id, record, read) triples at atomic cursors: the order inside a list is arbitrary here
-//   k6g_sort_kernel         one warp per named id: its list sorted by read id (k6b_sort_by_key, in shared memory up to K6G_SMEM_SORT
-//                           entries, in the global scratch itself beyond -- no depth cap); equal neighbours = a duplicate id.  The read
-//                           ids of an unflagged list are distinct, so the sorted order -- and every output byte -- does not depend on the
-//                           order the atomics ran in.
+//   the list builder        (k6_lists.cuh) count, scan, scatter and sort into one list per id, one warp per id in the sort; its hook
+//                           (k6g_hook) marks a list that holds a read id twice (dup[id])
 //   k6g_group_count_kernel  one warp per group: its status, and its supporting reads counted 32 entries of the first allele's list at a time
 //                           (binary searches in the other alleles' lists)
 //   scan                    of the unflagged groups' read and float counts, in place in read_off and lnp_off, -> totals; one 12-byte round
@@ -24,27 +18,16 @@
 //   k6g_write_kernel        one warp per group: ploidy and the alleles' lengths, then every supporting read's A+1 floats and fields at its
 //                           rank among the supporting entries (ballot + popc)
 // The body is k6g_core.cuh.
+#include "k6_lists.cuh"
 #include "k6g_core.cuh"
-#include "sx_internal.h"
-
-#include <algorithm>
 
 namespace
 {
 constexpr int K6G_THREADS = 128;
 constexpr int K6G_WARPS = K6G_THREADS / 32;
-constexpr uint32_t K6G_SMEM_SORT = 512; // entries of one id's list sorted in shared memory: 4 KiB per warp
 constexpr unsigned FULL = 0xffffffffu;
 
-struct k6g_pairs // the scatter's output, id x's list at list_off[x]
-{
-    uint32_t* id;    // read id (sorted in place by k6g_sort_kernel)
-    uint32_t* rec;   // record index in the sample's recs
-    uint32_t* read;  // read index in the sample
-    uint32_t* order; // order[p] = which of the list's triples is p-th by read id
-};
-
-k6g_lists k6g_lists_of(const uint32_t* list_off, const k6g_pairs& P) { return k6g_lists{list_off, P.id, P.order, P.rec, P.read}; }
+k6g_lists k6g_lists_of(const k6l_lists& L) { return k6g_lists{L.off, L.P.id, L.P.order, L.P.rec, L.P.read}; }
 
 __global__ void k6g_mark_kernel(const sx_allele_groups G, uint32_t* __restrict__ list_of, int* __restrict__ status)
 {
@@ -62,77 +45,22 @@ __global__ void k6g_mark_kernel(const sx_allele_groups G, uint32_t* __restrict__
     if (bad) atomicOr(status, SX_ST_K6G_GROUP);
 }
 
-// `total` is the 64-bit count of what the 32-bit counts and their scan hold: the launcher refuses a sample whose triples do not fit 32 bits
-__global__ void __launch_bounds__(K6G_THREADS) k6g_count_kernel(const k6b_view v, uint32_t* __restrict__ cnt, unsigned long long* __restrict__ total, int* __restrict__ status)
+// K6g's part of the list builder's sort: dup[x] = a read id twice in id x's list
+struct k6g_hook
 {
-    uint32_t st(0);
-    unsigned long long mine(0);
-    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < v.s[0].n_reads; r += gridDim.x * blockDim.x)
-        st |= k6b_for_each_entry(v, 0u, r, [&](const uint32_t x, uint32_t) {
-            atomicAdd(cnt + x, 1u);
-            ++mine;
-        });
-    for (int d = 16; d > 0; d >>= 1) mine += __shfl_down_sync(FULL, mine, d);
-    if ((threadIdx.x & 31) == 0 && mine) atomicAdd(total, mine);
-    if (st) atomicOr(status, SX_ST_K6B_ID);
-}
-
-__global__ void __launch_bounds__(K6G_THREADS) k6g_scatter_kernel(const k6b_view v, uint32_t* __restrict__ cursor, const k6g_pairs P)
-{
-    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < v.s[0].n_reads; r += gridDim.x * blockDim.x)
+    static constexpr uint32_t n_samples = 1;
+    struct warp_smem
     {
-        const uint32_t id(k6b_read_id(v.s[0], r));
-        k6b_for_each_entry(v, 0u, r, [&](const uint32_t x, const uint32_t i) {
-            const uint32_t at(atomicAdd(cursor + x, 1u));
-            P.id[at] = id;
-            P.rec[at] = i;
-            P.read[at] = r;
-        });
-    }
-}
+    };
+    uint32_t* dup;
 
-// one warp per id: the list sorted by read id (P.id in sorted order, P.order beside it) and dup[x] = a read id twice in it
-__global__ void __launch_bounds__(K6G_THREADS) k6g_sort_kernel(const uint32_t n_gid, const uint32_t* __restrict__ list_off, const k6g_pairs P, uint32_t* __restrict__ dup)
-{
-    __shared__ uint32_t s_key[K6G_WARPS][K6G_SMEM_SORT], s_val[K6G_WARPS][K6G_SMEM_SORT];
-    const uint32_t lane(threadIdx.x & 31), warp(threadIdx.x >> 5);
-    const auto sync = [] { __syncwarp(); };
-    for (uint32_t x = blockIdx.x * K6G_WARPS + warp; x < n_gid; x += gridDim.x * K6G_WARPS)
+    __device__ void begin(warp_smem&, uint32_t) const {}
+    __device__ uint32_t segment(warp_smem&, uint32_t, uint32_t, uint32_t, uint32_t, const k6l_pairs&, uint32_t) const { return 0u; }
+    __device__ void end(warp_smem&, const uint32_t x, const bool d, const uint32_t*, const uint32_t lane) const
     {
-        const uint32_t base(list_off[x]), n(list_off[x + 1] - base);
-        if (n < 2)
-        {
-            if (n == 1 && lane == 0) P.order[base] = 0;
-            continue;
-        }
-        if (n <= K6G_SMEM_SORT)
-        {
-            for (uint32_t i = lane; i < n; i += 32)
-            {
-                s_key[warp][i] = P.id[base + i];
-                s_val[warp][i] = i;
-            }
-            __syncwarp();
-            k6b_sort_by_key(s_key[warp], s_val[warp], n, lane, 32u, sync);
-            for (uint32_t i = lane; i < n; i += 32)
-            {
-                P.id[base + i] = s_key[warp][i];
-                P.order[base + i] = s_val[warp][i];
-            }
-        }
-        else
-        {
-            for (uint32_t i = lane; i < n; i += 32) P.order[base + i] = i;
-            __syncwarp();
-            k6b_sort_by_key(P.id + base, P.order + base, n, lane, 32u, sync);
-        }
-        __syncwarp();
-        bool d(false);
-        for (uint32_t i = lane; i + 1 < n; i += 32) d |= P.id[base + i] == P.id[base + i + 1];
-        if (__any_sync(FULL, d) && lane == 0) dup[x] = 1u;
-        __syncwarp(); // (s_key is loaded again for the next id)
+        if (d && lane == 0) dup[x] = 1u;
     }
-}
+};
 
 // a group's status: SX_INDEL_READS_ST_DUP_READ when a list it names holds a read id twice
 __device__ uint32_t k6g_group_status(const sx_allele_groups& G, const uint32_t g, const uint32_t* dup, const uint32_t lane)
@@ -260,7 +188,7 @@ int sx_k6g_run(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* sampl
                const bool own_out, unsigned* launches)
 {
     cudaStream_t st(ctx->s_compute);
-    const uint32_t n_groups(groups->n_groups), n_gid(groups->n_gid), n_reads(sample->n_reads);
+    const uint32_t n_groups(groups->n_groups), n_gid(groups->n_gid);
     int rc;
     if (n_groups == 0)
     {
@@ -271,57 +199,33 @@ int sx_k6g_run(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* sampl
         if (totals_host) totals_host[0] = totals_host[1] = 0;
         return SX_OK;
     }
-    uint32_t *list_of(nullptr), *list_off(nullptr), *cursor(nullptr), *dup(nullptr);
-    unsigned long long* total64(nullptr); // [0] triples, [1] allele_lnp floats
+    uint32_t *list_of(nullptr), *dup(nullptr);
+    unsigned long long* lnp64(nullptr); // allele_lnp floats
     if ((rc = sx_take(ctx, SX_SLOT_K6G_LIST_OF, n_gid, list_of, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K6G_LIST_OFF, (size_t)n_gid + 1, list_off, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K6G_CURSOR, n_gid, cursor, 16))) return rc;
     if ((rc = sx_take(ctx, SX_SLOT_K6G_DUP, n_gid, dup, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K6G_TOTAL64, 2, total64, 0))) return rc;
-    const int cap(ctx->sm_count * 16);
-    const auto grid = [cap](const uint32_t m, const uint32_t per) { return (unsigned)std::max(1, std::min<int>((int)((m + per - 1) / per), cap)); };
+    if ((rc = sx_take(ctx, SX_SLOT_K6G_LNP64, 1, lnp64, 0))) return rc;
 
     const k6b_view v(k6g_view(*sample, n_gid, list_of));
     SX_CUDA(ctx, cudaMemsetAsync(list_of, 0xFF, (size_t)n_gid * 4, st));
-    SX_CUDA(ctx, cudaMemsetAsync(list_off, 0, (size_t)n_gid * 4, st));
     SX_CUDA(ctx, cudaMemsetAsync(dup, 0, (size_t)n_gid * 4, st));
-    SX_CUDA(ctx, cudaMemsetAsync(total64, 0, 16, st));
-    k6g_mark_kernel<<<grid(n_groups, 256), 256, 0, st>>>(*groups, list_of, ctx->d_status);
+    SX_CUDA(ctx, cudaMemsetAsync(lnp64, 0, 8, st));
+    k6g_mark_kernel<<<k6l_grid(ctx, n_groups, 256), 256, 0, st>>>(*groups, list_of, ctx->d_status);
     SX_CUDA(ctx, cudaGetLastError());
-    k6g_count_kernel<<<grid(n_reads, K6G_THREADS), K6G_THREADS, 0, st>>>(v, list_off, total64, ctx->d_status);
+    *launches += 1;
+    k6l_lists lists;
+    if ((rc = k6l_build(ctx, what, v, n_gid, k6g_hook{dup}, &lists, launches))) return rc;
+    const k6g_lists L(k6g_lists_of(lists));
+    k6g_group_count_kernel<<<k6l_grid(ctx, n_groups, K6G_WARPS), K6G_THREADS, 0, st>>>(*sample, *groups, L, dup, *o, lnp64);
     SX_CUDA(ctx, cudaGetLastError());
-    *launches += 2;
-    const sx_scan_set lists = {1, {{list_off, n_gid, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, nullptr}}};
-    if ((rc = sx_scan(ctx, SX_SLOT_K6G_SUMS, lists, launches))) return rc;
-    SX_CUDA(ctx, cudaMemcpyAsync(cursor, list_off, (size_t)n_gid * 4, cudaMemcpyDeviceToDevice, st));
-    uint32_t n_pairs(0);
-    unsigned long long n_pairs64(0);
-    SX_CUDA(ctx, cudaMemcpyAsync(&n_pairs, list_off + n_gid, 4, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaMemcpyAsync(&n_pairs64, total64, 8, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaStreamSynchronize(st));
-    if (n_pairs64 != n_pairs) return sx_fail(ctx, SX_ERR_RANGE, "%s: %llu list entries: the offsets are 32-bit", what, n_pairs64);
-
-    k6g_pairs P;
-    if ((rc = sx_take(ctx, SX_SLOT_K6G_PAIR_ID, n_pairs, P.id, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K6G_PAIR_REC, n_pairs, P.rec, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K6G_PAIR_READ, n_pairs, P.read, 16))) return rc;
-    if ((rc = sx_take(ctx, SX_SLOT_K6G_PAIR_ORDER, n_pairs, P.order, 16))) return rc;
-    const k6g_lists L(k6g_lists_of(list_off, P));
-    k6g_scatter_kernel<<<grid(n_reads, K6G_THREADS), K6G_THREADS, 0, st>>>(v, cursor, P);
-    SX_CUDA(ctx, cudaGetLastError());
-    k6g_sort_kernel<<<grid(n_gid, K6G_WARPS), K6G_THREADS, 0, st>>>(n_gid, list_off, P, dup);
-    SX_CUDA(ctx, cudaGetLastError());
-    k6g_group_count_kernel<<<grid(n_groups, K6G_WARPS), K6G_THREADS, 0, st>>>(*sample, *groups, L, dup, *o, total64 + 1);
-    SX_CUDA(ctx, cudaGetLastError());
-    *launches += 3;
+    *launches += 1;
     SX_CUDA(ctx, cudaMemcpyAsync(o->allele_off, groups->allele_off, ((size_t)n_groups + 1) * 4, cudaMemcpyDeviceToDevice, st));
     const sx_scan_set out = {2, {{o->read_off, n_groups, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, o->totals}, {o->lnp_off, n_groups, SX_SCAN_EXCLUSIVE | SX_SCAN_CLOSE, o->totals + 1}}};
-    if ((rc = sx_scan(ctx, SX_SLOT_K6G_SUMS, out, launches))) return rc;
+    if ((rc = sx_scan(ctx, SX_SLOT_K6L_SUMS, out, launches))) return rc;
     uint32_t h[3] = {0, 0, 0}; // reads, floats, alleles
     unsigned long long n_lnp64(0);
     SX_CUDA(ctx, cudaMemcpyAsync(h, o->totals, 8, cudaMemcpyDeviceToHost, st));
     SX_CUDA(ctx, cudaMemcpyAsync(h + 2, o->allele_off + n_groups, 4, cudaMemcpyDeviceToHost, st));
-    SX_CUDA(ctx, cudaMemcpyAsync(&n_lnp64, total64 + 1, 8, cudaMemcpyDeviceToHost, st));
+    SX_CUDA(ctx, cudaMemcpyAsync(&n_lnp64, lnp64, 8, cudaMemcpyDeviceToHost, st));
     SX_CUDA(ctx, cudaStreamSynchronize(st));
     if (n_lnp64 != h[1]) return sx_fail(ctx, SX_ERR_RANGE, "%s: %llu allele log-likelihoods: the offsets are 32-bit", what, n_lnp64);
     if (totals_host)
@@ -343,7 +247,7 @@ int sx_k6g_run(sx_ctx* ctx, const char* what, const sx_indel_reads_sample* sampl
     if (h[0] > o->cap_reads || h[1] > o->cap_lnp)
         return sx_fail(ctx, SX_ERR_CAPACITY, "%s: output capacity too small: %u reads, %u allele log-likelihoods needed", what, h[0], h[1]);
     if ((h[0] && (!o->read_length || !o->non_ambig || !o->is_fwd)) || (h[1] && !o->allele_lnp)) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL output array", what);
-    k6g_write_kernel<<<grid(n_groups, K6G_WARPS), K6G_THREADS, 0, st>>>(*sample, *groups, L, *o);
+    k6g_write_kernel<<<k6l_grid(ctx, n_groups, K6G_WARPS), K6G_THREADS, 0, st>>>(*sample, *groups, L, *o);
     SX_CUDA(ctx, cudaGetLastError());
     *launches += 1;
     return SX_OK;
@@ -358,20 +262,7 @@ extern "C" int sx_link_allele_groups_dev(sx_ctx* ctx, const sx_indel_reads_sampl
     int rc;
     if ((rc = k6g_check(ctx, what, sample, groups)) || (rc = k6g_check_out(ctx, what, out_dev, groups->n_groups))) return rc;
     sx_allele_group_reads_out o(*out_dev);
-    bool ran(false);
-    int rc_link(SX_OK);
-    rc = sx_run_timed(ctx, [&](unsigned* launches) {
-        ran = true;
-        rc_link = sx_k6g_run(ctx, what, sample, groups, &o, totals_host, false, launches);
-        return SX_OK; // (the timer finishes whatever the link returns: its totals stand even when a capacity is too small)
-    });
-    if (!ran) return rc;
-    if (rc_link == SX_ERR_CAPACITY || rc_link == SX_OK)
-    {
-        const int rc3(sx_check_status(ctx, what, SX_ST_K6G_GROUP | SX_ST_K6B_ID)); // (a bad group or id outranks the capacity it may have inflated)
-        if (rc3) return rc3;
-    }
-    return rc_link ? rc_link : rc;
+    return k6l_link_dev(ctx, what, SX_ST_K6G_GROUP | SX_ST_K6B_ID, [&](unsigned* launches) { return sx_k6g_run(ctx, what, sample, groups, &o, totals_host, false, launches); });
 }
 
 extern "C" int sx_link_allele_groups(sx_ctx* ctx, const sx_indel_reads_sample* sample, const sx_allele_groups* groups, sx_allele_group_reads_out* out_host,

@@ -98,13 +98,14 @@ enum sx_slot : int
     SX_SLOT_K3_INFO, SX_SLOT_K3_CURSOR, SX_SLOT_K3_ORDER, SX_SLOT_K3_SCRATCH,
     SX_SLOT_K4_SCAN_S, SX_SLOT_K4_SCAN_B, SX_SLOT_K4_TILE_SUMS, SX_SLOT_K4_MAX_CAND,
     SX_SLOT_K6_MAX, SX_SLOT_K6_LIST, SX_SLOT_K6_ARENA, SX_SLOT_K6_CLASS, SX_SLOT_K6_HIST, SX_SLOT_K6_LIST_BY_CLASS,
-    SX_SLOT_K6B_LOCUS_OF, SX_SLOT_K6B_PAIR_OFF, SX_SLOT_K6B_CURSOR, SX_SLOT_K6B_SUMS, SX_SLOT_K6B_ALT_IDS,
-    SX_SLOT_K6B_PAIR_ID, SX_SLOT_K6B_PAIR_REC, SX_SLOT_K6B_PAIR_READ, SX_SLOT_K6B_PAIR_ORDER,
+    // the list builder of K6b and K6g (k6_lists.cuh), and the tile sums of both links' second scan.  Each link's scratch is dead once its
+    // write kernel is enqueued, and both links run on the compute stream, so their lifetimes cannot overlap.
+    SX_SLOT_K6L_OFF, SX_SLOT_K6L_CURSOR, SX_SLOT_K6L_TOTAL64, SX_SLOT_K6L_SUMS, SX_SLOT_K6L_ID, SX_SLOT_K6L_REC, SX_SLOT_K6L_READ, SX_SLOT_K6L_ORDER,
+    SX_SLOT_K6B_LOCUS_OF, SX_SLOT_K6B_ALT_IDS,
     // K6b's output where the library owns it: the sx_sindel_batch between the link and K5b (sx_somatic_indel_from_records_dev), and the
     // device side of sx_link_indel_reads
     SX_SLOT_K6B_OUT_ALT_OFF, SX_SLOT_K6B_OUT_ALTS, SX_SLOT_K6B_OUT_READ_OFF, SX_SLOT_K6B_OUT_READS, SX_SLOT_K6B_OUT_STATUS, SX_SLOT_K6B_OUT_TOTALS,
-    SX_SLOT_K6G_LIST_OF, SX_SLOT_K6G_LIST_OFF, SX_SLOT_K6G_CURSOR, SX_SLOT_K6G_DUP, SX_SLOT_K6G_SUMS, SX_SLOT_K6G_TOTAL64,
-    SX_SLOT_K6G_PAIR_ID, SX_SLOT_K6G_PAIR_REC, SX_SLOT_K6G_PAIR_READ, SX_SLOT_K6G_PAIR_ORDER,
+    SX_SLOT_K6G_LIST_OF, SX_SLOT_K6G_DUP, SX_SLOT_K6G_LNP64,
     // K6g's output where the library owns it: the sx_indel_batch between the link and K5 (sx_indel_gl_from_records_dev)
     SX_SLOT_K6G_OUT_READ_OFF, SX_SLOT_K6G_OUT_LNP_OFF, SX_SLOT_K6G_OUT_ALLELE_OFF, SX_SLOT_K6G_OUT_PLOIDY, SX_SLOT_K6G_OUT_DEL_LEN, SX_SLOT_K6G_OUT_INS_LEN,
     SX_SLOT_K6G_OUT_LNP, SX_SLOT_K6G_OUT_READ_LENGTH, SX_SLOT_K6G_OUT_NON_AMBIG, SX_SLOT_K6G_OUT_IS_FWD, SX_SLOT_K6G_OUT_STATUS, SX_SLOT_K6G_OUT_TOTALS,

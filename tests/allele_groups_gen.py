@@ -20,7 +20,6 @@ from strelka_b200 import batch as B
 
 ROOT = G.ROOT
 ORACLE_SO = os.path.join(ROOT, "oracle", "liballele_groups_oracle.so")
-SMEM_SORT = 512  # K6G_SMEM_SORT of k6g_allele_groups.cu
 _libs: dict = {}
 _ARGS = [C.POINTER(A.SxIndelReadsSample), C.POINTER(A.SxAlleleGroups), C.POINTER(A.SxAlleleGroupReadsOut)]
 
@@ -58,7 +57,7 @@ def ox_link(sample, groups, cap_reads=None, cap_lnp=None):
     return _run(oracle().ox_link_allele_groups, sample, groups, cap_reads, cap_lnp)
 
 
-def core_link(sample, groups, cap_reads=None, cap_lnp=None, smem_sort=SMEM_SORT):
+def core_link(sample, groups, cap_reads=None, cap_lnp=None, smem_sort=G.SMEM_SORT):
     """(rc, AlleleGroupReadsOut) of the host-compiled kernel body."""
     return _run(host_body().k6gcore_run, sample, groups, cap_reads, cap_lnp, smem_sort)
 

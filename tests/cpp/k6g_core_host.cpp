@@ -1,15 +1,13 @@
 // tests/cpp/k6g_core_host.cpp -- TEST ONLY.  Compiles the body of K6g (strelka_b200/csrc/k6g_core.cuh, __host__ __device__) with g++ and
-// runs it the way the kernels of k6g_allele_groups.cu do: mark, count, scan, scatter, sort, group count, scan, write.  The scatter visits the
-// reads BACKWARDS, so the lists reach the sort in an order the device never produces: the output must not depend on it.  `smem_sort` is the
-// depth up to which a list is sorted in a side buffer (the kernel's shared memory), beyond it in the scratch itself.
+// runs it the way the kernels of k6g_allele_groups.cu do: mark, the list builder (k6_lists_host.h: count, scan, backwards scatter, sort at
+// depth `smem_sort`), group count, scan, write.
+#include "k6_lists_host.h"
 #include "k6g_core.cuh"
-
-#include <vector>
 
 extern "C" int k6gcore_run(const sx_indel_reads_sample* sample, const sx_allele_groups* G, sx_allele_group_reads_out* o, uint32_t smem_sort)
 {
     const uint32_t n_gid(G->n_gid), n_groups(G->n_groups);
-    std::vector<uint32_t> list_of(n_gid, K6B_NONE), list_off(n_gid + 1, 0), dup(n_gid, 0);
+    std::vector<uint32_t> list_of(n_gid, K6B_NONE);
     for (uint32_t g = 0; g < n_groups; ++g)
     {
         if (!k6g_group_ok(*G, g)) return SX_ERR_ARG;
@@ -22,50 +20,17 @@ extern "C" int k6gcore_run(const sx_indel_reads_sample* sample, const sx_allele_
         return SX_OK;
     }
     const k6b_view v(k6g_view(*sample, n_gid, list_of.data()));
-    uint32_t bad(0);
-    for (uint32_t r = 0; r < sample->n_reads; ++r) bad |= k6b_for_each_entry(v, 0u, r, [&](uint32_t x, uint32_t) { ++list_off[x + 1]; });
-    if (bad) return SX_ERR_ARG;
-    for (uint32_t i = 0; i < n_gid; ++i) list_off[i + 1] += list_off[i];
-    const uint32_t n_pairs(list_off[n_gid]);
-    std::vector<uint32_t> cursor(list_off.begin(), list_off.end() - 1), id(n_pairs), rec(n_pairs), read(n_pairs), order(n_pairs), key, val;
-    for (uint32_t r = sample->n_reads; r-- > 0;)
-        k6b_for_each_entry(v, 0u, r, [&](uint32_t x, uint32_t i) {
-            const uint32_t at(cursor[x]++);
-            id[at] = k6b_read_id(*sample, r);
-            rec[at] = i;
-            read[at] = r;
-        });
-    for (uint32_t x = 0; x < n_gid; ++x)
-    {
-        const uint32_t base(list_off[x]), n(list_off[x + 1] - base);
-        if (n <= smem_sort)
-        {
-            key.assign(id.begin() + base, id.begin() + base + n);
-            val.resize(n);
-            for (uint32_t i = 0; i < n; ++i) val[i] = i;
-            k6b_sort_by_key(key.data(), val.data(), n, 0u, 1u, [] {});
-            for (uint32_t i = 0; i < n; ++i)
-            {
-                id[base + i] = key[i];
-                order[base + i] = val[i];
-            }
-        }
-        else
-        {
-            for (uint32_t i = 0; i < n; ++i) order[base + i] = i;
-            k6b_sort_by_key(id.data() + base, order.data() + base, n, 0u, 1u, [] {});
-        }
-        for (uint32_t i = 0; i + 1 < n; ++i) dup[x] |= id[base + i] == id[base + i + 1];
-    }
-    const k6g_lists L{list_off.data(), id.data(), order.data(), rec.data(), read.data()};
+    k6l_host_lists lists;
+    if (k6l_host_build(v, 1, n_gid, smem_sort, lists)) return SX_ERR_ARG;
+    const k6g_lists L{lists.off.data(), lists.id.data(), lists.order.data(), lists.rec.data(), lists.read.data()};
     uint32_t n_reads(0), n_lnp(0);
     for (uint32_t g = 0; g < n_groups; ++g)
     {
         const uint32_t a0(G->allele_off[g]), A(G->allele_off[g + 1] - a0);
         const uint32_t* agid(G->allele_gid + a0);
         bool d(false);
-        for (uint32_t i = a0; i < a0 + A; ++i) d |= dup[G->allele_gid[i]] != 0;
-        for (uint32_t i = G->contrast_off[g]; i < G->contrast_off[g + 1]; ++i) d |= dup[G->contrast_gid[i]] != 0;
+        for (uint32_t i = a0; i < a0 + A; ++i) d |= lists.dup[G->allele_gid[i]] != 0;
+        for (uint32_t i = G->contrast_off[g]; i < G->contrast_off[g + 1]; ++i) d |= lists.dup[G->contrast_gid[i]] != 0;
         uint32_t n(0);
         if (!d)
             for (uint32_t p = L.off[agid[0]]; p < L.off[agid[0] + 1]; ++p) n += k6g_supports(*sample, L, agid, A, p) ? 1u : 0u;

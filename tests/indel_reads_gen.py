@@ -23,7 +23,7 @@ from strelka_b200 import batch as B
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ORACLE_SO = os.path.join(ROOT, "oracle", "libindel_reads_oracle.so")
-SMEM_SORT = 512  # K6B_SMEM_SORT of k6b_indel_reads.cu
+SMEM_SORT = 512  # K6L_SMEM_SORT of k6_lists.cuh, the list builder of K6b and K6g
 _libs: dict = {}
 _ARGS = [C.POINTER(A.SxIndelReadsSample), C.POINTER(A.SxIndelReadsSample), C.POINTER(A.SxIndelLoci), C.POINTER(A.SxIndelReadsOut)]
 

@@ -63,7 +63,7 @@ def test_struct_layouts(tmp_path):
 def test_oracle_host_builder_and_kernel_body_agree(cases, oracle_out, i):
     sample, groups = cases[i]
     AG.same(oracle_out[i], B.link_allele_groups(sample, groups))
-    for smem_sort in (AG.SMEM_SORT, 0, 1 << 20):  # the sort is the same network whichever memory it runs in
+    for smem_sort in (G.SMEM_SORT, 0, 1 << 20):  # the sort is the same network whichever memory it runs in
         rc, core = AG.core_link(sample, groups, smem_sort=smem_sort)
         assert rc == 0
         AG.same(oracle_out[i], core)
@@ -121,7 +121,7 @@ def test_cases_reach_every_branch(cases, oracle_out):
                     hit.add("suboverlap records on a named id")
         if any(k > 1 for k in seen.values()):
             hit.add("ids shared between groups")
-        if max(len(scored.get(x, {})) for x in seen) > AG.SMEM_SORT:
+        if max(len(scored.get(x, {})) for x in seen) > G.SMEM_SORT:
             hit.add("list deeper than the shared-memory sort")
     want = {f"A={a} ploidy={p}" for a in range(1, 5) for p in (1, 2)} | {
         "duplicate read id flagged", "group without a supporting read", "no contrast", "one contrast", "several contrasts", "tier-2 read excluded",
