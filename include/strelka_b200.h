@@ -432,7 +432,9 @@ int sx_indel_gl_dev(sx_ctx* ctx, const sx_indel_batch* batch_dev, sx_indel_resul
  * in the order the reference piles them up (read-buffer order: see buffer_pos below).  Output: for every position of the report range the
  * column of base_call words in exactly that order -- the tier1 buffer (`calls`) and the tier2 buffer (`t2_calls`) of
  * pos_basecall_buffer::insert_pos_basecall -- i.e. an sx_pileup_batch ready for K2, plus the spanning-deletion and
- * sub-mapped read counts of each position.  Not produced: MAPQ tallies and the EVS feature accumulators (out of scope).
+ * sub-mapped read counts of each position.  The MAPQ tallies and the germline / somatic scoring-metric accumulators of the same bases are
+ * K4m's (sx_pileup_metrics, below).  What stays with the caller: the EVS feature derivation from those records (RMS and MQ0 fraction of the
+ * merged samples, safeFrac, the strand bias, the random forest itself) and the VCF / gVCF text.
  * ======================================================================================== */
 enum { SX_SEG_DELETE = 5, SX_SEG_SKIP = 6 }; /* K4 paths keep DELETE and SKIP apart: only a DELETE is a spanning deletion */
 
@@ -509,6 +511,67 @@ void sx_default_pileup_opts(sx_pileup_opts* o);
 /* SX_ERR_NOMEM if a capacity is too small (site_off / t2_off are still filled, so the caller can size and retry) */
 int sx_pileup_reads(sx_ctx* ctx, const sx_pileup_reads_batch* batch_host, sx_pileup_columns* out_host);
 int sx_pileup_reads_dev(sx_ctx* ctx, const sx_pileup_reads_batch* batch_dev, sx_pileup_columns* out_dev);
+
+/* ==========================================================================================
+ * K4m  pileup_metrics   (the per-position accumulators pileup_read_segment fills beside the base calls)
+ *   replaces  the insert_mapq_count / updateGermlineScoringMetrics / updateSomaticScoringMetrics calls of pileup_read_segment
+ *   (starling_common/starling_pos_processor_base.cpp:1345-1362, pos_basecall_buffer.cpp:45-70, :984-1000) and the read-out of each
+ *   snp_pos_info through get_z_stat, getExpectedCategory2Value, MeanTracker::mean and median (position_somatic_snv_strand_grid_vcf.cpp:159-189).
+ *
+ * The bases are K4's: matched segments, inside [read_begin, read_end) after ambiguous-end trimming (and minDistanceFromReadEdge), inside the
+ *   report range, of every read without SX_PRF_SKIP -- sub-mapped reads and filtered calls included, as the reference updates the metrics
+ *   before it splits them off.  is_ref of a base is ref_char == id_to_base(call_id), so an 'N' call at an 'N' reference position is reference.
+ * Per position, by mode (one mode per call; a caller with several samples runs one call per sample):
+ *   SX_PM_MAPQ      MapqTracker.add(mapq) for every base
+ *   SX_PM_GERMLINE  the MAPQ tallies; mq_ranksum(is_ref, mapq) for every base; for bases of tier1/tier2 reads: baseq_ranksum(is_ref, qscore)
+ *                   on K4's MAPQ-adjusted qscore, readPositionRankSum(is_ref, align_strand_read_pos) and, for non-reference bases,
+ *                   distanceFromReadEdge += min(20, distance from the edge of the FULL read)  (the germline caller: is_compute_germline_scoring_metrics)
+ *   SX_PM_SOMATIC   the MAPQ tallies; for bases of tier1 reads whose current_call_filter is false: readPositionRankSum(is_ref, read_pos) on the
+ *                   un-flipped read position, and for non-reference bases the (read_pos, read_size) alt list  (strelka2's tumor sample; its normal
+ *                   sample takes SX_PM_MAPQ, as the reference applies the somatic metrics to sample index != 0 only)
+ * Every output is order-free -- integer counts, exact integer sums in doubles, half-integer rank weights, correctly rounded sqrt and
+ *   divisions, order statistics -- so each record has the reference's bits (tests/golden/pileup_metrics_ref.npz: the reference's own
+ *   pileup_read_segment with the metrics on).  Fields a mode does not fill are 0; every byte is written.
+ *   Callers merge the MAPQ tallies of several samples themselves (MapqTracker::merge is an exact sum).
+ * ======================================================================================== */
+enum { SX_PM_MAPQ = 1, SX_PM_GERMLINE = 2, SX_PM_SOMATIC = 3 };
+
+/* sx_pileup_metrics_rec.status: getMannWhitneyZScore's int product n1 * (n1 + n2 + 1) would overflow (about 46k observations at one position
+ * with balanced categories): the reference's value is undefined there, the ranksum field is 0 and its bit is set */
+#define SX_PM_ST_MQ_OVERFLOW 0x1u
+#define SX_PM_ST_BASEQ_OVERFLOW 0x2u
+#define SX_PM_ST_READ_POS_OVERFLOW 0x4u
+
+typedef struct sx_pileup_metrics_opts {
+    uint32_t mode;            /* SX_PM_*; anything else is SX_ERR_ARG */
+    uint32_t reserved_;       /* 0 */
+    const uint16_t* full_len; /* [n_reads] rseg.full_read_size(), or NULL: the read's own length (only RNA segments differ).  Same memory
+                                 space as the batch's arrays; the window passes take NULL (their reads are whole reads). */
+    const uint16_t* full_off; /* [n_reads] rseg.full_read_offset(), or NULL: 0 */
+} sx_pileup_metrics_opts;
+
+/* One position's record, 80 bytes, 8-aligned.  (C gives a type and a function one name space, hence _rec.) */
+typedef struct sx_pileup_metrics_rec {
+    double mapq_sum_sq;        /* MapqTracker.sumSquare */
+    double read_pos_ranksum;   /* readPositionRankSum.get_z_stat(): ReadPosRankSum (germline), TumorSampleReadPosRankSum (somatic) */
+    double mq_ranksum;         /* mq_ranksum.get_z_stat(): MQRankSum (germline) */
+    double baseq_ranksum;      /* baseq_ranksum.get_z_stat(): BaseQRankSum (germline) */
+    double raw_pos;            /* readPositionRankSum.getExpectedCategory2Value(): rawPos (germline) */
+    double raw_baseq;          /* baseq_ranksum.getExpectedCategory2Value(): avgBaseQ (germline) */
+    double mean_edge_distance; /* distanceFromReadEdge.mean(): meanDistanceFromReadEdge (germline) */
+    uint32_t mapq_count;       /* MapqTracker.count */
+    uint32_t mapq_zero;        /* MapqTracker.zeroCount */
+    uint32_t n_alt_read_pos;   /* altAlleleReadPositionInfo.size() (somatic) */
+    uint16_t median_read_pos;  /* medianReadPos: min(median(readPos), median(readLength - readPos)); 0 without alt entries (somatic) */
+    uint16_t median_read_pos_var; /* medianReadPosVar: median(|readPos - median(readPos)|) with 3 or more entries, else 0 (somatic) */
+    uint32_t status;           /* SX_PM_ST_* */
+    uint32_t pad;
+} sx_pileup_metrics_rec;
+
+/* out: [report_end - report_begin] records.  The batch is K4's (its opts and order key included; the columns are not needed).  Reads longer
+ * than 1024 bases or with more than 64 segments are refused as K4 refuses them. */
+int sx_pileup_metrics(sx_ctx* ctx, const sx_pileup_reads_batch* batch_host, const sx_pileup_metrics_opts* opts, sx_pileup_metrics_rec* out_host);
+int sx_pileup_metrics_dev(sx_ctx* ctx, const sx_pileup_reads_batch* batch_dev, const sx_pileup_metrics_opts* opts, sx_pileup_metrics_rec* out_dev);
 
 /* ==========================================================================================
  * K6  score_indels   (SURVEY 8f2: the consumer of K1's scores)
@@ -1236,6 +1299,17 @@ int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* batch_dev, sx_wind
 int sx_process_window(sx_ctx* ctx, const sx_window_batch* batch_host, sx_window_out* out_host, uint32_t* totals_host);
 /* device time of each stage of the most recent sx_process_window_dev on ctx (CUDA events on the compute stream), ms[SX_WIN_N_STAGES] */
 int sx_last_window_timing(const sx_ctx* ctx, float* ms);
+/* sx_process_window_dev plus K4m (sx_pileup_metrics_dev) on the pass's own pile-up batch -- its best alignments, buffer order, bases and
+ * qualities, reference, cand_snv and pileup_opts -- after the last stage, into metrics_dev[report_end - report_begin] (device memory).
+ * mopts->full_len / full_off must be NULL.  Every other output is sx_process_window_dev's, byte for byte.  metrics_dev NULL: this IS
+ * sx_process_window_dev (same launches, same bytes; mopts is not read).  The K4m stage waits once on the host for its word total (4 bytes), so
+ * its stage time includes that round trip. */
+#define SX_WIN_ST_METRICS SX_WIN_N_STAGES
+int sx_process_window_metrics_dev(sx_ctx* ctx, const sx_window_batch* batch_dev, sx_window_out* out_dev, uint32_t* totals_host,
+                                  const sx_pileup_metrics_opts* mopts, sx_pileup_metrics_rec* metrics_dev);
+/* the stage times of the most recent window pass, ms[SX_WIN_N_STAGES + 1]: sx_last_window_timing's, then ms[SX_WIN_ST_METRICS], the K4m
+ * stage of the most recent sx_process_window_metrics_dev that ran it */
+int sx_last_window_metrics_timing(const sx_ctx* ctx, float* ms);
 
 /* ==========================================================================================
  * process_somatic_window   (strelka2's per-position path for a window of positions: the normal and the tumor sample through process_window's
@@ -1314,6 +1388,16 @@ int sx_process_somatic_window_dev(sx_ctx* ctx, const sx_somatic_window_batch* ba
 /* device time of each stage of the most recent sx_process_somatic_window_dev on ctx (CUDA events on the compute stream), ms[SX_SWIN_N_STAGES];
  * sx_last_window_timing then reports the tumor sample's pass */
 int sx_last_somatic_window_timing(const sx_ctx* ctx, float* ms);
+/* sx_process_somatic_window_dev plus K4m on each sample's own pile-up batch at the end of its pass (as sx_process_window_metrics_dev):
+ * sample s gets mopts[s] into metrics_dev[s][report_end - report_begin] (device memory), or no metrics when metrics_dev (or metrics_dev[s])
+ * is NULL.  strelka2's reading: mopts[0]->mode = SX_PM_MAPQ (normal), mopts[1]->mode = SX_PM_SOMATIC (tumor).  The records and every other
+ * output are sx_process_somatic_window_dev's, byte for byte. */
+#define SX_SWIN_ST_METRICS SX_SWIN_N_STAGES
+int sx_process_somatic_window_metrics_dev(sx_ctx* ctx, const sx_somatic_window_batch* batch_dev, sx_somatic_window_out* out_dev, uint32_t* totals_host,
+                                          const sx_pileup_metrics_opts* const mopts[2], sx_pileup_metrics_rec* const metrics_dev[2]);
+/* ms[SX_SWIN_N_STAGES + 1]: sx_last_somatic_window_timing's, then ms[SX_SWIN_ST_METRICS], the two samples' K4m stages (inside their passes'
+ * stage times) of the most recent sx_process_somatic_window_metrics_dev */
+int sx_last_somatic_window_metrics_timing(const sx_ctx* ctx, float* ms);
 
 /* ==========================================================================================
  * K2c  site_continuous

@@ -247,6 +247,19 @@ def default_pileup_opts() -> SxPileupOpts:
     return SxPileupOpts(1, 17, 20, 2, 0, 10, 0, 0)
 
 
+# K4m pileup_metrics
+SX_PM_MAPQ, SX_PM_GERMLINE, SX_PM_SOMATIC = 1, 2, 3
+SX_PM_ST_MQ_OVERFLOW, SX_PM_ST_BASEQ_OVERFLOW, SX_PM_ST_READ_POS_OVERFLOW = 1, 2, 4
+PILEUP_METRICS_DT = np.dtype([("mapq_sum_sq", "<f8"), ("read_pos_ranksum", "<f8"), ("mq_ranksum", "<f8"), ("baseq_ranksum", "<f8"), ("raw_pos", "<f8"),
+                              ("raw_baseq", "<f8"), ("mean_edge_distance", "<f8"), ("mapq_count", "<u4"), ("mapq_zero", "<u4"), ("n_alt_read_pos", "<u4"),
+                              ("median_read_pos", "<u2"), ("median_read_pos_var", "<u2"), ("status", "<u4"), ("pad", "<u4")])  # sx_pileup_metrics_rec
+assert PILEUP_METRICS_DT.itemsize == 80
+
+
+class SxPileupMetricsOpts(C.Structure):
+    _fields_ = [("mode", C.c_uint32), ("reserved_", C.c_uint32), ("full_len", C.c_void_p), ("full_off", C.c_void_p)]
+
+
 # K6 score_indels
 SX_INDEL_TYPE_INDEL, SX_INDEL_TYPE_MISMATCH = 0, 1
 SX_IKF_CANDIDATE = 1
@@ -377,6 +390,7 @@ class SxSomaticWindowOut(C.Structure):
 
 SX_SWIN_TOTALS, SX_SWIN_N_STAGES = 4, 7
 SX_SWIN_STAGE_NAMES = ("normal", "tumor", "k2b_site_snv", "snv_calls", "k6b_link", "k5b_indel", "indel_calls")
+SX_WIN_ST_METRICS, SX_SWIN_ST_METRICS = SX_WIN_N_STAGES, SX_SWIN_N_STAGES
 
 
 class SxGateOut(C.Structure):
@@ -510,12 +524,19 @@ SYMBOLS = [
     ("sx_default_pileup_opts", None, [C.POINTER(SxPileupOpts)]),
     ("sx_pileup_reads", C.c_int, [_P, C.POINTER(SxPileupReadsBatch), C.POINTER(SxPileupColumns)]),
     ("sx_pileup_reads_dev", C.c_int, [_P, C.POINTER(SxPileupReadsBatch), C.POINTER(SxPileupColumns)]),
+    ("sx_pileup_metrics", C.c_int, [_P, C.POINTER(SxPileupReadsBatch), C.POINTER(SxPileupMetricsOpts), _P]),
+    ("sx_pileup_metrics_dev", C.c_int, [_P, C.POINTER(SxPileupReadsBatch), C.POINTER(SxPileupMetricsOpts), _P]),
     ("sx_default_window_opts", None, [C.POINTER(SxWindowBatch)]),
     ("sx_process_window_dev", C.c_int, [_P, C.POINTER(SxWindowBatch), C.POINTER(SxWindowOut), _P]),
     ("sx_process_window", C.c_int, [_P, C.POINTER(SxWindowBatch), C.POINTER(SxWindowOut), _P]),
     ("sx_last_window_timing", C.c_int, [_P, _P]),
     ("sx_process_somatic_window_dev", C.c_int, [_P, C.POINTER(SxSomaticWindowBatch), C.POINTER(SxSomaticWindowOut), _P]),
     ("sx_last_somatic_window_timing", C.c_int, [_P, _P]),
+    ("sx_process_window_metrics_dev", C.c_int, [_P, C.POINTER(SxWindowBatch), C.POINTER(SxWindowOut), _P, C.POINTER(SxPileupMetricsOpts), _P]),
+    ("sx_last_window_metrics_timing", C.c_int, [_P, _P]),
+    ("sx_process_somatic_window_metrics_dev", C.c_int, [_P, C.POINTER(SxSomaticWindowBatch), C.POINTER(SxSomaticWindowOut), _P, C.POINTER(C.c_void_p * 2),
+                                                        C.POINTER(C.c_void_p * 2)]),
+    ("sx_last_somatic_window_metrics_timing", C.c_int, [_P, _P]),
     ("sx_default_cont_opts", None, [C.POINTER(SxContOpts)]),
     ("sx_site_continuous", C.c_int, [_P, C.POINTER(SxContOpts), C.POINTER(SxContBatch), C.POINTER(SxContOut), _P]),
     ("sx_site_continuous_dev", C.c_int, [_P, C.POINTER(SxContOpts), C.POINTER(SxContBatch), C.POINTER(SxContOut), _P]),

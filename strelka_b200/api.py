@@ -252,6 +252,37 @@ class Context:
         self._chk(self.lib.sx_pileup_reads(self.h, C.byref(pb.c), C.byref(out.c)))
         return out.trimmed()
 
+    # ---- K4m
+    def pileup_metrics(self, pb: B.PileupReadsBatch, mode: int, full_len=None, full_off=None) -> np.ndarray:
+        """K4m: the per-position MAPQ tallies and scoring metrics of a read batch (host buffers in, PILEUP_METRICS_DT records out)."""
+        o, keep = self._metrics_opts(mode, full_len, full_off)
+        out = np.zeros(pb.n_sites, A.PILEUP_METRICS_DT)
+        self._chk(self.lib.sx_pileup_metrics(self.h, C.byref(pb.c), C.byref(o), out.ctypes.data))
+        return out
+
+    def pileup_metrics_dev(self, pb: B.PileupReadsBatch, mode: int, full_len=None, full_off=None) -> np.ndarray:
+        """K4m through sx_pileup_metrics_dev: the batch's arrays uploaded, the records written to device memory and downloaded."""
+        o, keep = self._metrics_opts(mode, full_len, full_off)
+        d, bufs = _device_twin(self, pb.c, pb, 64)
+        for k in ("full_len", "full_off"):
+            if keep.get(k) is not None:
+                bufs[k] = DeviceArray(self, keep[k].nbytes + 64).upload(keep[k])
+                setattr(o, k, bufs[k].ptr)
+        out = DeviceArray(self, (pb.n_sites + 1) * A.PILEUP_METRICS_DT.itemsize)
+        try:
+            self._chk(self.lib.sx_pileup_metrics_dev(self.h, C.byref(d), C.byref(o), out.ptr))
+            return out.download(A.PILEUP_METRICS_DT, pb.n_sites)
+        finally:
+            out.free()
+            for x in bufs.values():
+                x.free()
+
+    @staticmethod
+    def _metrics_opts(mode: int, full_len, full_off):
+        keep = {"full_len": None if full_len is None else np.ascontiguousarray(full_len, np.uint16),
+                "full_off": None if full_off is None else np.ascontiguousarray(full_off, np.uint16)}
+        return A.SxPileupMetricsOpts(mode=mode, full_len=A.ptr(keep["full_len"]), full_off=A.ptr(keep["full_off"])), keep
+
     # ---- K6
     def score_indels(self, sb: B.ScoreIndelsBatch, lnp: np.ndarray):
         """K6: the arg-max epilogue of scoreCandidateAlignments + score_indels (host buffers in, host records out).
@@ -746,8 +777,12 @@ class DevWindow:
     """sx_process_window_dev on a B.WindowBatch: every input array resident in HBM, every output array the caller may want to read
     back allocated here (tests download them; bench.py leaves them where they are)."""
 
-    def __init__(self, ctx: "Context", w: "B.WindowBatch", keep_outputs: bool = True, cap_best_segs=None):
+    def __init__(self, ctx: "Context", w: "B.WindowBatch", keep_outputs: bool = True, cap_best_segs=None, metrics: Optional[int] = None):
+        """metrics: an SX_PM_* mode -- run() goes through sx_process_window_metrics_dev and metrics() gives the per-position records"""
         self.ctx, self.w = ctx, w
+        self.metrics_mode = metrics
+        self.mbuf = DeviceArray(ctx, (w.n_sites + 1) * A.PILEUP_METRICS_DT.itemsize) if metrics is not None else None
+        self.mopts = A.SxPileupMetricsOpts(mode=metrics or 0)
         c = A.SxWindowBatch()
         ctx.lib.sx_default_window_opts(C.byref(c))
         c.n_regions, c.n_reads, c.n_keys = w.n_regions, w.n_reads, w.n_keys
@@ -795,10 +830,19 @@ class DevWindow:
     def run(self):
         """one pass; returns the per-stage device times (ms)"""
         ctx = self.ctx
-        ctx._chk(ctx.lib.sx_process_window_dev(ctx.h, C.byref(self.c), C.byref(self.out), self.totals.ctypes.data))
-        ms = np.zeros(A.SX_WIN_N_STAGES, np.float32)
-        ctx.lib.sx_last_window_timing(ctx.h, ms.ctypes.data)
-        return dict(zip(A.SX_WIN_STAGE_NAMES, (float(x) for x in ms)))
+        if self.mbuf is None:
+            ctx._chk(ctx.lib.sx_process_window_dev(ctx.h, C.byref(self.c), C.byref(self.out), self.totals.ctypes.data))
+            ms = np.zeros(A.SX_WIN_N_STAGES, np.float32)
+            ctx.lib.sx_last_window_timing(ctx.h, ms.ctypes.data)
+            return dict(zip(A.SX_WIN_STAGE_NAMES, (float(x) for x in ms)))
+        ctx._chk(ctx.lib.sx_process_window_metrics_dev(ctx.h, C.byref(self.c), C.byref(self.out), self.totals.ctypes.data, C.byref(self.mopts), self.mbuf.ptr))
+        ms = np.zeros(A.SX_WIN_N_STAGES + 1, np.float32)
+        ctx.lib.sx_last_window_metrics_timing(ctx.h, ms.ctypes.data)
+        return dict(zip(A.SX_WIN_STAGE_NAMES + ("k4m_metrics",), (float(x) for x in ms)))
+
+    def metrics(self) -> np.ndarray:
+        """the K4m records of the most recent run (made with metrics=mode)"""
+        return self.mbuf.download(A.PILEUP_METRICS_DT, self.w.n_sites)
 
     def download(self):
         """dict of the host copies of every output (keep_outputs only)"""
@@ -818,7 +862,7 @@ class DevWindow:
         return d
 
     def free(self):
-        for x in list(self.bufs.values()) + list(self.obufs.values()):
+        for x in list(self.bufs.values()) + list(self.obufs.values()) + ([self.mbuf] if self.mbuf is not None else []):
             x.free()
 
 
@@ -831,7 +875,7 @@ class DevSomaticWindow:
 
     def __init__(self, ctx: "Context", normal: "B.WindowBatch", tumor: "B.WindowBatch", loci: "B.IndelLoci", key_gid, read_id=None, snv_forced=None,
                  use_tier2: bool = False, opts: Optional[A.SxSindelOpts] = None, cap_snv_calls=None, cap_indel_calls=None, records_only: bool = False,
-                 compute_nonsomatic: bool = False):
+                 compute_nonsomatic: bool = False, metrics: bool = False):
         assert not normal.do_site_gl and not tumor.do_site_gl, "strelka2 runs no germline site model: build the samples with do_site_gl=False"
         self.ctx, self.loci = ctx, loci
         self.records_only = records_only
@@ -868,15 +912,30 @@ class DevSomaticWindow:
         samples = (A.SxWindowOut * 2)() if records_only else (A.SxWindowOut * 2)(*(dw.out for dw in self.windows))
         self.out = A.SxSomaticWindowOut(sample=samples, cap_snv_calls=self.cap_snv, cap_indel_calls=self.cap_indel, **{k: b.ptr for k, b in self.obufs.items()})
         self.totals = np.zeros(A.SX_SWIN_TOTALS, np.uint32)
+        # metrics: K4m on each sample's pass, strelka2's reading -- the normal sample SX_PM_MAPQ, the tumor sample SX_PM_SOMATIC
+        self.mbufs = [DeviceArray(ctx, (self.n_sites + 1) * A.PILEUP_METRICS_DT.itemsize) for _ in range(2)] if metrics else None
+        self.mopts = [A.SxPileupMetricsOpts(mode=A.SX_PM_MAPQ), A.SxPileupMetricsOpts(mode=A.SX_PM_SOMATIC)]
 
     def run(self):
         """one pass; returns the per-stage device times (ms).  SX_ERR_CAPACITY leaves the totals in the SxError's `totals`."""
         ctx = self.ctx
-        rc = ctx.lib.sx_process_somatic_window_dev(ctx.h, C.byref(self.c), C.byref(self.out), self.totals.ctypes.data)
+        if self.mbufs is None:
+            rc = ctx.lib.sx_process_somatic_window_dev(ctx.h, C.byref(self.c), C.byref(self.out), self.totals.ctypes.data)
+            ctx._chk_totals(rc, self.totals)
+            ms = np.zeros(A.SX_SWIN_N_STAGES, np.float32)
+            ctx.lib.sx_last_somatic_window_timing(ctx.h, ms.ctypes.data)
+            return dict(zip(A.SX_SWIN_STAGE_NAMES, (float(x) for x in ms)))
+        mo = (C.c_void_p * 2)(*(C.addressof(o) for o in self.mopts))
+        mb = (C.c_void_p * 2)(*(b.ptr for b in self.mbufs))
+        rc = ctx.lib.sx_process_somatic_window_metrics_dev(ctx.h, C.byref(self.c), C.byref(self.out), self.totals.ctypes.data, C.byref(mo), C.byref(mb))
         ctx._chk_totals(rc, self.totals)
-        ms = np.zeros(A.SX_SWIN_N_STAGES, np.float32)
-        ctx.lib.sx_last_somatic_window_timing(ctx.h, ms.ctypes.data)
-        return dict(zip(A.SX_SWIN_STAGE_NAMES, (float(x) for x in ms)))
+        ms = np.zeros(A.SX_SWIN_N_STAGES + 1, np.float32)
+        ctx.lib.sx_last_somatic_window_metrics_timing(ctx.h, ms.ctypes.data)
+        return dict(zip(A.SX_SWIN_STAGE_NAMES + ("k4m_metrics",), (float(x) for x in ms)))
+
+    def metrics(self):
+        """(normal, tumor) K4m records of the most recent run (made with metrics=True)"""
+        return tuple(b.download(A.PILEUP_METRICS_DT, self.n_sites) for b in self.mbufs)
 
     def callable_regions(self, cap_regions=None):
         """the callable intervals of the most recent run (callable mode): (begin, end) int32 arrays, half-open, in the positions' coordinates.
@@ -908,5 +967,6 @@ class DevSomaticWindow:
         for dw in self.windows:
             dw.free()
         bufs = list(self.obufs.values()) + list(self.dloci.bufs.values()) + [x for x in self.inbufs["key_gid"] + self.inbufs["read_id"] + [self.inbufs["snv_forced"]] if x]
+        bufs += self.mbufs or []
         for x in bufs:
             x.free()

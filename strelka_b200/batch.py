@@ -13,6 +13,7 @@ everything that function looks up in host-only containers (``getMatchingIndelKey
 from __future__ import annotations
 
 import ctypes as C
+import math
 from dataclasses import dataclass, field
 from typing import List, Optional, Sequence, Tuple
 
@@ -1554,3 +1555,189 @@ def somatic_callable_regions(site_snv: np.ndarray, pos_begin: int):
     c = ~((site_snv["qphred"] < 15) & (site_snv["nonsomatic_qphred"] < 15))
     d = np.diff(np.concatenate([[0], c.astype(np.int8), [0]]))
     return (np.nonzero(d == 1)[0] + pos_begin).astype(np.int32), (np.nonzero(d == -1)[0] + pos_begin).astype(np.int32)
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# K4m pileup_metrics
+# ---------------------------------------------------------------------------------------------------------------------------
+def _mapped_qscore_table() -> np.ndarray:
+    """qphred_cache::mappedq[mapq 0..90][basecall q 0..70] (blt_util/qscore_cache.cpp:44-47)"""
+    t = np.zeros((91, 71), np.uint8)
+    for j in range(91):
+        me = math.pow(10.0, -float(j) / 10.0)
+        for i in range(71):
+            be = math.pow(10.0, -float(i) / 10.0)
+            p = ((1.0 - me) * be) + (me * 0.75)
+            t[j, i] = int(math.floor(-10.0 * max(-307.0, math.log10(p)) + 0.5))
+    return t
+
+
+def _z_stat(vals: np.ndarray, is_ref: np.ndarray):
+    """fastRanksum::get_z_stat of (is_ref, value) observations in closed form: (z, overflow, N2, sum of the category-2 values)"""
+    n1, n2 = int(is_ref.sum()), int((~is_ref).sum())
+    if n1 + n2 == 0:
+        return 0.0, False, 0, 0
+    uniq, inv, cnt = np.unique(vals.astype(np.int64), return_inverse=True, return_counts=True)
+    before = np.concatenate([[0], np.cumsum(cnt)[:-1]])
+    wx2 = 2 * before[inv] + cnt[inv] + 1  # twice the mean rank of each observation's value
+    R1, R2 = int(wx2[is_ref].sum()) * 0.5, int(wx2[~is_ref].sum()) * 0.5
+    a, b, w1 = (n2, n1, R2) if R1 > R2 else (n1, n2, R1)
+    prod = a * (a + b + 1)
+    if prod > 2147483647:
+        return 0.0, True, n2, int(vals[~is_ref].astype(np.int64).sum())
+    mean = float(prod) / 2.0
+    var = math.sqrt(float(b) * mean / 6.0)
+    z = 0.0 if abs(var) < 0.0001 else (w1 - mean) / var
+    return z, False, n2, int(vals[~is_ref].astype(np.int64).sum())
+
+
+def pileup_metrics(pb: PileupReadsBatch, mode: int, full_len=None, full_off=None, observations: Optional[list] = None) -> np.ndarray:
+    """The host restatement of K4m (sx_pileup_metrics) in numpy: every visited base's observation, then each position's statistics in closed
+    form.  full_len / full_off: rseg.full_read_size() / full_read_offset() of every read (None: its own length / 0).  observations: a list
+    that receives, per position, the (mapq, qscore, is_ref, submapped, somatic, edge, cycle, read_pos, read_size) tuples of its bases."""
+    assert mode in (A.SX_PM_MAPQ, A.SX_PM_GERMLINE, A.SX_PM_SOMATIC)
+    o = pb.opts
+    rb, re = int(pb.c.report_begin), int(pb.c.report_end)
+    ref_begin, ref = int(pb.c.ref_begin), bytes(pb.ref[: int(pb.c.ref_len)])
+    ref_at = lambda pos: chr(ref[pos - ref_begin]) if 0 <= pos - ref_begin < len(ref) else "N"
+    mq = _mapped_qscore_table()
+    cand = set(int(k) for k in pb.cand_snv[: int(pb.c.n_cand_snv)])
+    qual_bits = int(pb.c.qual_bits)
+    qdict = list(pb.c.qual_dict)
+    chars = "=AC" + "N" + "G" + "NNN" + "T" + "N" * 7
+    ids = [4, 0, 1, 5, 2, 5, 5, 5, 3, 5, 5, 5, 5, 5, 5, 4]
+    obs = [[] for _ in range(re - rb)]  # per site: (mapq, qscore, is_ref, submapped, somatic, edge, cycle, read_pos, read_size)
+    reads, segs = pb.reads, pb.segs
+    for r in range(pb.n_reads):
+        rd = reads[r]
+        flags, n, pos0, mapq = int(rd["flags"]), int(rd["len"]), int(rd["pos"]), int(rd["mapq"])
+        if flags & A.SX_PRF_SKIP:
+            continue
+        path = [(int(s["kind"]), int(s["len"])) for s in segs[int(rd["seg_off"]): int(reads[r + 1]["seg_off"])]]
+        so = int(rd["seq_off"])
+        code = lambda i: (int(pb.seq4[so + (i >> 1)]) >> (4 if i % 2 == 0 else 0)) & 15
+        qo = int(rd["qual_off"])
+        qual = (lambda i: qdict[(int(pb.qual[qo + (i >> 1)]) >> (4 if i % 2 == 0 else 0)) & 15]) if qual_bits == 4 else (lambda i: int(pb.qual[qo + i]))
+        span = sum(ln for k, ln in path if k in (A.SX_SEG_MATCH, A.SX_SEG_DELETE, A.SX_SEG_SKIP))
+        if pos0 >= re or pos0 + span <= rb:
+            continue
+        fwd = bool(flags & A.SX_PRF_FWD)
+        amb = 0
+        if fwd:
+            while amb < n and code(n - 1 - amb) == 15:
+                amb += 1
+        else:
+            while amb < n and code(amb) == 15:
+                amb += 1
+        b, e = (0, n - amb) if fwd else (amb, n)
+        if o.minDistanceFromReadEdge > 0:
+            b += o.minDistanceFromReadEdge
+            e = e - o.minDistanceFromReadEdge if o.minDistanceFromReadEdge <= e else 0
+            if e <= b:
+                continue
+        submapped, tier1 = not (flags & A.SX_PRF_TIER1OR2), bool(flags & A.SX_PRF_TIER1)
+        amq = max(5, mapq)
+        adjust = o.isBasecallQualAdjustedForMapq and amq <= 80
+        fo = 0 if full_off is None else int(full_off[r])
+        fl = n if full_len is None else int(full_len[r])
+        matches = [i for i, (k, _) in enumerate(path) if k == A.SX_SEG_MATCH]
+        first, last = (matches[0], matches[-1]) if matches else (len(path), len(path))
+        filt = None
+        if mode == A.SX_PM_SOMATIC and tier1 and not submapped and o.mismatchDensityFilterFlankSize > 0:
+            fs = o.mismatchDensityFilterFlankSize
+            ds = max(1 + 2 * fs, n) - 2 * fs
+            delta = np.zeros(ds + 1, np.int64)
+
+            def inc(start, length):
+                delta[max(2 * fs, start) - 2 * fs] += 1
+                if start + length < ds:
+                    delta[start + length] -= 1
+
+            rp, fp = 0, pos0
+            for i, (k, ln) in enumerate(path):
+                edge = i < first or i > last
+                if k == A.SX_SEG_INSERT and not edge:
+                    inc(rp, ln)
+                elif k == A.SX_SEG_DELETE and not edge:
+                    inc(rp, 0)
+                elif k == A.SX_SEG_MATCH:
+                    for p in range(max(rp, b), min(rp + ln, e)):
+                        c = code(p)
+                        if chars[c] == ref_at(fp + p - rp):
+                            continue
+                        rel = fp + p - rp - rb
+                        if ids[c] < 4 and 0 <= rel < (1 << 30) and ((rel << 2) | ids[c]) in cand:
+                            continue
+                        inc(p, 1)
+                if k in (A.SX_SEG_MATCH, A.SX_SEG_INSERT, A.SX_SEG_SOFTCLIP):
+                    rp += ln
+                if k in (A.SX_SEG_MATCH, A.SX_SEG_DELETE, A.SX_SEG_SKIP):
+                    fp += ln
+            tot = np.cumsum(delta[:ds])
+            filt = lambda p: int(o.mismatchDensityFilterMaxMismatchCount) < int(tot[min(ds - 1, max(fs, p) - fs)])
+        rp, fp = 0, pos0
+        for k, ln in path:
+            if k == A.SX_SEG_MATCH:
+                for p in range(max(rp, b), min(rp + ln, e)):
+                    pos = fp + p - rp
+                    if pos < rb or pos >= re:
+                        continue
+                    c = code(p)
+                    cid = ids[c]
+                    if cid > 4:
+                        raise ValueError("unknown base code")
+                    q = qual(p)
+                    if adjust:
+                        if q > 70:
+                            raise ValueError("qscore above 70")
+                        q = int(mq[min(amq, 90), q])
+                    is_ref = ref_at(pos) == "ACGTN"[cid]
+                    som = False
+                    if mode == A.SX_PM_SOMATIC and tier1 and not submapped:
+                        f = c == 15 or q < o.minBasecallErrorPhredProb
+                        if not f and filt is not None:
+                            f = filt(p)
+                        som = not f
+                    fpos = p + fo
+                    d = min(fpos, (fl - (fpos + 1)) & 0xFFFFFFFF)
+                    obs[pos - rb].append((mapq, q, is_ref, submapped, som, min(20, d), p if fwd else n - (p + 1), p, n))
+            if k in (A.SX_SEG_MATCH, A.SX_SEG_INSERT, A.SX_SEG_SOFTCLIP):
+                rp += ln
+            if k in (A.SX_SEG_MATCH, A.SX_SEG_DELETE, A.SX_SEG_SKIP):
+                fp += ln
+    if observations is not None:
+        observations.extend(obs)
+    out = np.zeros(re - rb, A.PILEUP_METRICS_DT)
+    for s, ob in enumerate(obs):
+        rec = out[s]
+        if not ob:
+            continue
+        a = np.array(ob, dtype=np.int64)
+        mapq, q, isr, sub, som, edge, cyc, rpos, rsize = (a[:, i] for i in range(9))
+        isr, sub, som = isr.astype(bool), sub.astype(bool), som.astype(bool)
+        rec["mapq_count"], rec["mapq_zero"], rec["mapq_sum_sq"] = len(ob), int((mapq == 0).sum()), float(int((mapq * mapq).sum()))
+        st = 0
+        if mode == A.SX_PM_GERMLINE:
+            z, ov, _, _ = _z_stat(mapq, isr)
+            rec["mq_ranksum"], st = z, st | (A.SX_PM_ST_MQ_OVERFLOW if ov else 0)
+            m = ~sub
+            z, ov, n2, s2 = _z_stat(q[m], isr[m])
+            rec["baseq_ranksum"], rec["raw_baseq"], st = z, (s2 / float(n2) if n2 else 0.0), st | (A.SX_PM_ST_BASEQ_OVERFLOW if ov else 0)
+            z, ov, n2, s2 = _z_stat(cyc[m], isr[m])
+            rec["read_pos_ranksum"], rec["raw_pos"], st = z, (s2 / float(n2) if n2 else 0.0), st | (A.SX_PM_ST_READ_POS_OVERFLOW if ov else 0)
+            alt = m & ~isr
+            rec["mean_edge_distance"] = int(edge[alt].sum()) / float(int(alt.sum())) if alt.any() else 0.0
+        elif mode == A.SX_PM_SOMATIC:
+            z, ov, _, _ = _z_stat(rpos[som], isr[som])
+            rec["read_pos_ranksum"], st = z, st | (A.SX_PM_ST_READ_POS_OVERFLOW if ov else 0)
+            alt = som & ~isr
+            na = int(alt.sum())
+            rec["n_alt_read_pos"] = na
+            if na:
+                p = np.sort(rpos[alt])
+                pm, lm = int(p[na // 2]), int(np.sort(rsize[alt] - rpos[alt])[na // 2])
+                rec["median_read_pos"] = min(pm, lm)
+                if na >= 3:
+                    rec["median_read_pos_var"] = int(np.sort(np.abs(p - pm))[na // 2])
+        rec["status"] = st
+    return out

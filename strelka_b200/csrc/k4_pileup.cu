@@ -25,6 +25,7 @@
 //      loaded a read ahead, the path's offsets are warp scans, the bases, qualities and reference are staged by one batch of loads,
 //      and the candidate-SNV look-ups search the window's slice of cand_snv, staged in shared memory (pass 1 sizes it).
 // Everything is integer/byte work; the only table is qphred_cache::mappedq, built on the host (sx_context.cu).
+#include "k4_read.cuh"
 #include "sx_internal.h"
 
 #include <algorithm>
@@ -60,19 +61,8 @@ struct k4_args
     sx_pileup_opts opt;
 };
 
-__device__ __forceinline__ uint32_t code_at(const uint8_t* seq, uint32_t i) { return (seq[i >> 1] >> ((~i & 1u) << 2)) & 15u; }
 __device__ __forceinline__ bool kind_ref(uint32_t k) { return k == SX_SEG_MATCH || k == SX_SEG_DELETE || k == SX_SEG_SKIP; }
 __device__ __forceinline__ bool kind_read(uint32_t k) { return k == SX_SEG_MATCH || k == SX_SEG_INSERT || k == SX_SEG_SOFTCLIP; }
-
-// bam_seq code -> base_call id (0..3 ACGT, 4 for '=' / 'N', 5 = bam_seq_code_to_id would throw) and -> bam_seq::get_char, as nibble /
-// byte look-ups in 64-bit literals: a branch per base value makes the compiler duplicate the whole loop body per branch
-__device__ __forceinline__ uint32_t id_of_code(uint32_t c) { return static_cast<uint32_t>(0x4555555355525104ull >> (4u * c)) & 15u; }
-__device__ __forceinline__ char char_of_code(uint32_t c)
-{
-    // codes 0..7: '=', 'A', 'C', 'N', 'G', 'N', 'N', 'N'; codes 8..15: 'T', 'N' x 7
-    const unsigned long long lut = c < 8u ? 0x4e4e4e474e43413dull : 0x4e4e4e4e4e4e4e54ull;
-    return static_cast<char>((lut >> (8u * (c & 7u))) & 0xffu);
-}
 
 __device__ __forceinline__ int32_t bpos_of(const k4_args& A, uint32_t r) { return A.bpos ? A.bpos[r] : A.reads[r].pos; }
 
@@ -87,43 +77,10 @@ __device__ __forceinline__ void diff_add(int* d, int64_t a, int64_t b, uint32_t 
     if (b < static_cast<int64_t>(n)) atomicAdd(&d[b], -1);
 }
 
-// the per-read preamble of pileup_read_segment (:1175-1233): false = the read contributes nothing
-struct read_window
-{
-    uint32_t read_begin, read_end, ref_span;
-};
+// the per-read preamble of pileup_read_segment (k4_read.cuh): false = the read contributes nothing
 template <typename CodeFn> __device__ __forceinline__ bool read_preamble(const k4_args& A, const sx_pileup_read& rd, uint32_t ref_span, CodeFn code, read_window& w)
 {
-    if (rd.pos >= A.report_end) return false;
-    if (static_cast<int64_t>(rd.pos) + ref_span <= A.report_begin) return false;
-    const uint32_t read_size = rd.len;
-    uint32_t ambig = 0; // getReadAmbiguousEndLength: the run of 'N' (code 15) at the 3' end of the read as sequenced
-    if (rd.flags & SX_PRF_FWD)
-    {
-        uint32_t e = read_size;
-        while (e > 0 && code(e - 1) == 15u) --e;
-        ambig = read_size - e;
-    }
-    else
-    {
-        while (ambig < read_size && code(ambig) == 15u) ++ambig;
-    }
-    w.read_begin = 0;
-    w.read_end = read_size;
-    if (ambig > 0)
-    {
-        if (rd.flags & SX_PRF_FWD) w.read_end -= ambig;
-        else w.read_begin += ambig;
-    }
-    if (A.opt.minDistanceFromReadEdge > 0)
-    {
-        w.read_begin += A.opt.minDistanceFromReadEdge;
-        if (A.opt.minDistanceFromReadEdge <= w.read_end) w.read_end -= A.opt.minDistanceFromReadEdge;
-        else w.read_end = 0;
-        if (w.read_end <= w.read_begin) return false;
-    }
-    w.ref_span = ref_span;
-    return true;
+    return k4_trim_read(A.opt, A.report_begin, A.report_end, rd, ref_span, code, w);
 }
 
 // the cand_snv keys ((site << 2) | base id) of the sites a window's reads can reach: sites [(c-2) W, (c+1) W), cut to [0, 2^30 - 1)
@@ -133,18 +90,6 @@ __device__ __forceinline__ void cand_key_range(const k4_args& A, uint32_t c, uin
     const int64_t s0 = (static_cast<int64_t>(c) - 2) * A.W, s1 = s0 + 3 * static_cast<int64_t>(A.W), top = (1 << 30) - 1;
     key_lo = static_cast<uint32_t>(i64min(i64max(s0, 0), top)) << 2;
     key_hi = static_cast<uint32_t>(i64min(i64max(s1, 0), top)) << 2;
-}
-
-__device__ __forceinline__ uint32_t lower_bound_key(const uint32_t* keys, uint32_t n, uint32_t key)
-{
-    uint32_t lo = 0, hi = n;
-    while (lo < hi)
-    {
-        const uint32_t mid = (lo + hi) >> 1;
-        if (keys[mid] < key) lo = mid + 1;
-        else hi = mid;
-    }
-    return lo;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

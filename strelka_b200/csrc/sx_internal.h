@@ -97,6 +97,7 @@ enum sx_slot : int
     SX_SLOT_K2C_COUNTS, SX_SLOT_K2C_REC_OFF, SX_SLOT_K2C_TOTAL, SX_SLOT_K2C_SUMS,
     SX_SLOT_K3_INFO, SX_SLOT_K3_CURSOR, SX_SLOT_K3_ORDER, SX_SLOT_K3_SCRATCH,
     SX_SLOT_K4_SCAN_S, SX_SLOT_K4_SCAN_B, SX_SLOT_K4_TILE_SUMS, SX_SLOT_K4_MAX_CAND,
+    SX_SLOT_K4M_OFF, SX_SLOT_K4M_CURSOR, SX_SLOT_K4M_SUMS, SX_SLOT_K4M_WORDS,
     SX_SLOT_K6_MAX, SX_SLOT_K6_LIST, SX_SLOT_K6_ARENA, SX_SLOT_K6_CLASS, SX_SLOT_K6_HIST, SX_SLOT_K6_LIST_BY_CLASS,
     // the list builder of K6b and K6g (k6_lists.cuh), and the tile sums of both links' second scan.  Each link's scratch is dead once its
     // write kernel is enqueued, and both links run on the compute stream, so their lifetimes cannot overlap.
@@ -359,6 +360,8 @@ int sx_k2b_regions_run(sx_ctx* ctx, const sx_ssnv_result* site_snv, uint32_t n_p
                        uint32_t cap, uint32_t* total_host, unsigned* launches);
 int sx_k3_run(sx_ctx* ctx, const sx_ga_scores* sc, const sx_ga_batch* d, sx_ga_result* res_dev, uint32_t* cigar_dev, unsigned* launches);
 int sx_k4_run(sx_ctx* ctx, const sx_pileup_reads_batch* d, const sx_pileup_columns* out, unsigned* launches);
+// K4m on K4's batch: count, scans, one 4-byte round trip (the word total), walk, reduce into out_dev[report_end - report_begin]
+int sx_k4m_run(sx_ctx* ctx, const sx_pileup_reads_batch* d, const sx_pileup_metrics_opts* o, sx_pileup_metrics_rec* out_dev, unsigned* launches);
 int sx_k5_run(sx_ctx* ctx, const sx_indel_batch* d, sx_indel_result* out_dev, unsigned* launches);
 int sx_k5b_run(sx_ctx* ctx, const sx_sindel_opts* o, const sx_sindel_batch* d, const double* err_prob, uint32_t n_err, sx_sindel_result* out_dev, unsigned* launches);
 // K5b's argument checks, reported under `what` (the K5b entries, and sx_somatic_indel_from_records_dev before its K5b run)

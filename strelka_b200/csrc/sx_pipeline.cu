@@ -314,7 +314,14 @@ extern "C" int sx_last_window_timing(const sx_ctx* ctx, float* ms)
 namespace
 {
 // the window pass of sx_process_window_dev, which sx_process_window runs on the window it has uploaded
-int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint32_t* totals_host, const win_slots& S = WIN_SLOTS, win_kept* kept = nullptr)
+// metrics: K4m on the pass's own pile-up batch after the last stage (sx_process_window_metrics_dev), NULL: not run
+struct win_metrics
+{
+    const sx_pileup_metrics_opts* opts;
+    sx_pileup_metrics_rec* out;
+};
+int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint32_t* totals_host, const win_slots& S = WIN_SLOTS, win_kept* kept = nullptr,
+                const win_metrics& M = win_metrics{nullptr, nullptr})
 {
     if (!ctx) return SX_ERR_ARG;
     ctx->timing = sx_timing{};
@@ -329,7 +336,7 @@ int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint3
         return sx_fail(ctx, SX_ERR_UNSUPPORTED, "sx_process_window_dev: isRetainOptimalSoftClipping (the RNA workflow's soft-clip retention test) is outside the accelerated path");
     SX_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t st(ctx->s_compute);
-    for (int i = 0; i <= SX_WIN_N_STAGES; ++i)
+    for (int i = 0; i <= SX_WIN_N_STAGES + (M.out ? 1 : 0); ++i)
         if (!ctx->ev_win[i]) SX_CUDA(ctx, cudaEventCreate(&ctx->ev_win[i]));
     const uint32_t n(b->n_reads), nr(b->n_regions);
     const uint32_t n_sites((uint32_t)(b->report_end - b->report_begin));
@@ -630,6 +637,8 @@ int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint3
     sx_pileup_read* preads(nullptr);
     if ((rc = take(ctx, SX_SLOT_WIN_PILEUP_READS, (size_t)n + 2, preads))) return rc;
     sx_pileup_columns cols(out->cols);
+    sx_pileup_reads_batch pb;
+    memset(&pb, 0, sizeof(pb));
     uint64_t total_bases(0);
     int st_word(0);
     if (n)
@@ -667,8 +676,6 @@ int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint3
         if ((rc = pick(ctx, S.t2_calls, (size_t)cap_t2 + 16, out->cols.t2_calls, cols.t2_calls))) return rc;
         cols.calls_capacity = cap_calls;
         cols.t2_capacity = cap_t2;
-        sx_pileup_reads_batch pb;
-        memset(&pb, 0, sizeof(pb));
         pb.n_reads = n;
         pb.n_segs = totals[5];
         pb.reads = preads;
@@ -720,6 +727,12 @@ int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint3
     else if (out->variant_sites)
         return sx_fail(ctx, SX_ERR_ARG, "sx_process_window_dev: variant_sites needs do_site_gl");
     SX_CUDA(ctx, mark(SX_WIN_N_STAGES));
+    // ---------------------------------------------------------------------------------------------------------------- K4m metrics (the metrics entries)
+    if (M.out)
+    {
+        if ((rc = sx_k4m_run(ctx, &pb, M.opts, M.out, &launches))) return rc;
+        SX_CUDA(ctx, mark(SX_WIN_ST_METRICS + 1));
+    }
     // ---------------------------------------------------------------------------------------------------------------- the end: one wait, the totals, the status
     uint32_t call_totals[2] = {0, 0};
     SX_CUDA(ctx, cudaMemcpyAsync(&call_totals[0], cols.site_off + n_sites, 4, cudaMemcpyDeviceToHost, st));
@@ -737,6 +750,13 @@ int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint3
         ctx->win_ms[i] = ms;
         sum += ms;
     }
+    if (M.out)
+    {
+        float ms(0);
+        cudaEventElapsedTime(&ms, ctx->ev_win[SX_WIN_ST_METRICS], ctx->ev_win[SX_WIN_ST_METRICS + 1]);
+        ctx->win_ms[SX_WIN_ST_METRICS] = ms;
+        sum += ms;
+    }
     ctx->timing.kernel_ms = sum;
     ctx->timing.launches = launches;
     ctx->total_launches += launches;
@@ -750,6 +770,35 @@ int window_pass(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint3
 extern "C" int sx_process_window_dev(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint32_t* totals_host)
 {
     return window_pass(ctx, b, out, totals_host);
+}
+
+namespace
+{
+int check_window_metrics(sx_ctx* ctx, const char* what, const sx_pileup_metrics_opts* o)
+{
+    if (!o) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL metrics options", what);
+    if (o->mode != SX_PM_MAPQ && o->mode != SX_PM_GERMLINE && o->mode != SX_PM_SOMATIC)
+        return sx_fail(ctx, SX_ERR_ARG, "%s: mode %u is not SX_PM_MAPQ, SX_PM_GERMLINE or SX_PM_SOMATIC", what, o->mode);
+    if (o->full_len || o->full_off) return sx_fail(ctx, SX_ERR_ARG, "%s: full_len / full_off must be NULL (the window's reads are whole reads)", what);
+    return SX_OK;
+}
+} // namespace
+
+extern "C" int sx_process_window_metrics_dev(sx_ctx* ctx, const sx_window_batch* b, sx_window_out* out, uint32_t* totals_host, const sx_pileup_metrics_opts* mopts,
+                                             sx_pileup_metrics_rec* metrics_dev)
+{
+    if (!ctx) return SX_ERR_ARG;
+    if (!metrics_dev) return window_pass(ctx, b, out, totals_host);
+    int rc;
+    if ((rc = check_window_metrics(ctx, "sx_process_window_metrics_dev", mopts))) return rc;
+    return window_pass(ctx, b, out, totals_host, WIN_SLOTS, nullptr, win_metrics{mopts, metrics_dev});
+}
+
+extern "C" int sx_last_window_metrics_timing(const sx_ctx* ctx, float* ms)
+{
+    if (!ctx || !ms) return SX_ERR_ARG;
+    for (int i = 0; i <= SX_WIN_ST_METRICS; ++i) ms[i] = ctx->win_ms[i];
+    return SX_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------------------
@@ -800,11 +849,14 @@ sx_pileup_batch somatic_pileup_of(const sx_pileup_columns& c, const uint32_t n_s
 }
 } // namespace
 
-extern "C" int sx_process_somatic_window_dev(sx_ctx* ctx, const sx_somatic_window_batch* sb, sx_somatic_window_out* so, uint32_t* totals_host)
+namespace
+{
+// the somatic window pass; M[s].out non-NULL: K4m on sample s's pile-up batch at the end of its pass
+int somatic_window_pass(sx_ctx* ctx, const sx_somatic_window_batch* sb, sx_somatic_window_out* so, uint32_t* totals_host, const char* what,
+                        const win_metrics (&M)[2])
 {
     if (!ctx) return SX_ERR_ARG;
     ctx->timing = sx_timing{};
-    const char* what("sx_process_somatic_window_dev");
     if (!sb || !so) return sx_fail(ctx, SX_ERR_ARG, "%s: NULL argument", what);
     const sx_window_batch &bn(sb->sample[0]), &bt(sb->sample[1]);
     for (int s = 0; s < 2; ++s)
@@ -842,6 +894,7 @@ extern "C" int sx_process_somatic_window_dev(sx_ctx* ctx, const sx_somatic_windo
         if (!ctx->ev_swin[i]) SX_CUDA(ctx, cudaEventCreate(&ctx->ev_swin[i]));
     auto mark = [&](int i) { return cudaEventRecord(ctx->ev_swin[i], st); };
     unsigned launches(0), pass_launches(0); // (the passes add theirs to ctx->total_launches themselves)
+    float metrics_ms(0);                    // (the metrics stages, inside the samples' passes)
     uint32_t totals[SX_SWIN_TOTALS] = {0, 0, 0, 0};
 
     // ---------------------------------------------------------------------------------------------------------------- the two chains
@@ -851,7 +904,8 @@ extern "C" int sx_process_somatic_window_dev(sx_ctx* ctx, const sx_somatic_windo
     // sx_process_window_dev's totals_host would.
     const auto sample_pass = [&](const int s, const win_slots& slots) -> int {
         uint32_t wt[SX_WIN_TOTALS] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-        const int r(window_pass(ctx, &sb->sample[s], &so->sample[s], wt, slots, &kept[s]));
+        const int r(window_pass(ctx, &sb->sample[s], &so->sample[s], wt, slots, &kept[s], M[s]));
+        if (M[s].out) metrics_ms += ctx->win_ms[SX_WIN_ST_METRICS];
         if (r == SX_ERR_CAPACITY && so->sample[s].totals) cudaMemcpy(so->sample[s].totals, wt, sizeof(wt), cudaMemcpyHostToDevice);
         pass_launches += ctx->timing.launches;
         return r;
@@ -900,6 +954,7 @@ extern "C" int sx_process_somatic_window_dev(sx_ctx* ctx, const sx_somatic_windo
         ctx->swin_ms[i] = ms;
         sum += ms;
     }
+    ctx->swin_ms[SX_SWIN_ST_METRICS] = metrics_ms;
     ctx->timing.kernel_ms = sum;
     ctx->timing.launches = pass_launches + launches;
     ctx->total_launches += launches;
@@ -908,6 +963,38 @@ extern "C" int sx_process_somatic_window_dev(sx_ctx* ctx, const sx_somatic_windo
         return sx_fail(ctx, SX_ERR_CAPACITY, "%s: %u somatic SNV records, cap_snv_calls is %u", what, totals[0], so->cap_snv_calls);
     if (so->indel_calls && totals[1] > so->cap_indel_calls)
         return sx_fail(ctx, SX_ERR_CAPACITY, "%s: %u somatic indel records, cap_indel_calls is %u", what, totals[1], so->cap_indel_calls);
+    return SX_OK;
+}
+
+} // namespace
+
+extern "C" int sx_process_somatic_window_dev(sx_ctx* ctx, const sx_somatic_window_batch* sb, sx_somatic_window_out* so, uint32_t* totals_host)
+{
+    const win_metrics none[2] = {{nullptr, nullptr}, {nullptr, nullptr}};
+    return somatic_window_pass(ctx, sb, so, totals_host, "sx_process_somatic_window_dev", none);
+}
+
+extern "C" int sx_process_somatic_window_metrics_dev(sx_ctx* ctx, const sx_somatic_window_batch* sb, sx_somatic_window_out* so, uint32_t* totals_host,
+                                                     const sx_pileup_metrics_opts* const mopts[2], sx_pileup_metrics_rec* const metrics_dev[2])
+{
+    if (!ctx) return SX_ERR_ARG;
+    const char* what("sx_process_somatic_window_metrics_dev");
+    win_metrics M[2] = {{nullptr, nullptr}, {nullptr, nullptr}};
+    for (int s = 0; s < 2 && metrics_dev; ++s)
+    {
+        if (!metrics_dev[s]) continue;
+        int rc;
+        if ((rc = check_window_metrics(ctx, what, mopts ? mopts[s] : nullptr))) return rc;
+        M[s] = win_metrics{mopts[s], metrics_dev[s]};
+    }
+    ctx->swin_ms[SX_SWIN_ST_METRICS] = 0;
+    return somatic_window_pass(ctx, sb, so, totals_host, what, M);
+}
+
+extern "C" int sx_last_somatic_window_metrics_timing(const sx_ctx* ctx, float* ms)
+{
+    if (!ctx || !ms) return SX_ERR_ARG;
+    for (int i = 0; i <= SX_SWIN_ST_METRICS; ++i) ms[i] = ctx->swin_ms[i];
     return SX_OK;
 }
 
