@@ -9,114 +9,19 @@
 // parallelism is across pairs.  The addends come from a 143-row table built on the host with the host libm
 // (sx_context.cu), so there is no transcendental on the device.
 //
-// Data movement: one CTA per region.  Every pool slice of the region (packed bases, qualities, reference window,
-// alignment headers, segments, inserted bases, the term table) is pulled into shared memory by TMA bulk copies
-// (cp.async.bulk ... mbarrier::complete_tx) issued by one thread; each read is then expanded ONCE into a 16-bit
-// (table-row | one-hot base) entry that all of its H alignments share, so HBM sees every read byte exactly once.
-#include "sx_internal.h"
-#include "k1q_layout.cuh"
+// Data movement: one CTA per region.  The term table and every pool slice of the region are staged in shared memory as
+// k1_stage.cuh describes; each read is then expanded ONCE into a 16-bit (table-row | one-hot base) entry that all of its H
+// alignments share, so HBM sees every read byte exactly once.
+#include "k1_stage.cuh"
 
 #include <algorithm>
 #include <cstring>
 
 namespace
 {
-constexpr int K1_THREADS = 128;
-constexpr int K1_TAB_BYTES = SX_K1_ROWS * 16;
+using namespace k1;
+
 constexpr int K1_CHUNK = 8;
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count)
-{
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes)
-{
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t phase)
-{
-    asm volatile(
-        "{\n"
-        ".reg .pred P1;\n"
-        "LAB_WAIT:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n"
-        "@P1 bra DONE;\n"
-        "bra LAB_WAIT;\n"
-        "DONE:\n"
-        "}\n" ::"r"(smem_u32(bar)),
-        "r"(phase)
-        : "memory");
-}
-// TMA 1-D bulk copy global -> shared, completion counted in bytes on an mbarrier.  16-byte aligned src/dst/size.
-__device__ __forceinline__ void tma_bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst_smem)), "l"(src_gmem),
-                 "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
-
-// 8-byte shared-memory load from a shared-window address
-__device__ __forceinline__ double lds_f64(uint32_t saddr)
-{
-    double v;
-    asm("ld.shared.f64 %0, [%1];" : "=d"(v) : "r"(saddr));
-    return v;
-}
-
-__host__ __device__ __forceinline__ uint32_t pad16(uint32_t x) { return (x + 15u) & ~15u; }
-
-struct k1_layout
-{
-    uint32_t tab, alns, segs, ref, refp, ins, seq, qual, rlen, boff, soff, eoff, desc, ent, total;
-    uint32_t n_reads, n_alns, seg_bytes, ref_bytes, refp_bytes, ins_bytes, seq_bytes, qual_bytes;
-};
-
-__host__ __device__ __forceinline__ k1_layout k1_make_layout(const sx_region& r0, const sx_region& r1, uint32_t fmt)
-{
-    k1_layout L;
-    L.n_reads = r1.read_begin - r0.read_begin;
-    L.n_alns = r1.aln_begin - r0.aln_begin;
-    L.seg_bytes = pad16((r1.seg_begin - r0.seg_begin) * ((fmt & SX_FMT_SEG2) ? 2u : 4u));
-    L.ref_bytes = pad16(r0.ref_len);
-    L.ins_bytes = pad16(r1.ins_begin - r0.ins_begin);
-    L.seq_bytes = pad16(static_cast<uint32_t>(r1.seq_off - r0.seq_off));
-    L.qual_bytes = (fmt & SX_FMT_BASEQ) ? 0u : pad16(static_cast<uint32_t>(r1.qual_off - r0.qual_off));
-    L.refp_bytes = (fmt & SX_FMT_REF4) ? pad16((r0.ref_len + 1u) / 2u) : 0u;
-    uint32_t o = 16; // mbarrier
-    L.tab = o;
-    o += K1_TAB_BYTES;
-    L.alns = o;
-    o += k1q::aln_slice_bytes(r0.aln_begin, L.n_alns, fmt);
-    L.segs = o;
-    o += L.seg_bytes;
-    L.ref = o;
-    o += L.ref_bytes;
-    L.refp = o;
-    o += L.refp_bytes;
-    L.ins = o;
-    o += L.ins_bytes;
-    L.seq = o;
-    o += L.seq_bytes;
-    L.qual = o;
-    o += L.qual_bytes;
-    L.rlen = o;
-    o += pad16(L.n_reads * 2u);
-    L.boff = o;
-    o += pad16((L.n_reads + 1) * 4u);
-    L.soff = o;
-    o += pad16((L.n_reads + 1) * 4u);
-    L.eoff = 0;
-    L.desc = o;
-    o += 64 + 16; // 16 nibble descriptors + the 16-entry quality dictionary
-    L.ent = o;
-    // entries: 2 bytes per base, every read padded to an even count; + slack: the uniform chunk loop may load (and discard) up to
-    // K1_CHUNK-1 entries past a read
-    o += L.seq_bytes * 4u + 32u;
-    L.total = o;
-    return L;
-}
 
 // reference base (ASCII) -> one-hot nibble; everything that is not ACGT (N, '=', IUPAC) -> 0, which ANDs to "mismatch" with every
 // read nibble.  (get_bam_seq_code maps such characters to ANY=15; a read nibble of 15 never reaches the compare, and 15 equals no
@@ -126,19 +31,19 @@ __device__ __forceinline__ uint8_t onehot_of_char(uint8_t c)
     return c == 'A' ? 1 : c == 'C' ? 2 : c == 'G' ? 4 : c == 'T' ? 8 : 0;
 }
 
-__global__ void __launch_bounds__(K1_THREADS) k1_score_kernel(const sx_region* __restrict__ regions, const uint16_t* __restrict__ read_len,
-                                                              const uint8_t* __restrict__ seq4, const uint8_t* __restrict__ qual,
-                                                              const char* __restrict__ ref, const sx_aln* __restrict__ alns,
-                                                              const sx_aln_seg* __restrict__ segs, const char* __restrict__ ins,
-                                                              const sx_tables* __restrict__ tables, uint32_t region_begin, double* __restrict__ lnp_out,
-                                                              int* __restrict__ status, uint32_t smem_bytes, uint32_t qual_bits, uint4 qual_dict, uint32_t fmt,
-                                                              const uint32_t* __restrict__ exc_off, const uint32_t* __restrict__ exc)
+__global__ void __launch_bounds__(THREADS) k1_score_kernel(const sx_region* __restrict__ regions, const uint16_t* __restrict__ read_len,
+                                                          const uint8_t* __restrict__ seq4, const uint8_t* __restrict__ qual,
+                                                          const char* __restrict__ ref, const sx_aln* __restrict__ alns,
+                                                          const sx_aln_seg* __restrict__ segs, const char* __restrict__ ins,
+                                                          const sx_tables* __restrict__ tables, uint32_t region_begin, double* __restrict__ lnp_out,
+                                                          int* __restrict__ status, uint32_t smem_bytes, uint32_t qual_bits, uint4 qual_dict, uint32_t fmt,
+                                                          const uint32_t* __restrict__ exc_off, const uint32_t* __restrict__ exc)
 {
     extern __shared__ __align__(128) unsigned char smem[];
     const uint32_t ri = region_begin + blockIdx.x;
     const sx_region r0 = regions[ri];
     const sx_region r1 = regions[ri + 1];
-    const k1_layout L = k1_make_layout(r0, r1, fmt);
+    const layout L = make_layout(slices_of(r0, r1, fmt));
     if (L.n_alns == 0) return;
     if (L.total > smem_bytes)
     {
@@ -147,33 +52,8 @@ __global__ void __launch_bounds__(K1_THREADS) k1_score_kernel(const sx_region* _
     }
     uint64_t* bar = reinterpret_cast<uint64_t*>(smem);
     const double* tab = reinterpret_cast<const double*>(smem + L.tab);
-    // alignment headers and segments, read through accessors that hide the wire format (sx_aln / sx_aln8, sx_aln_seg / sx_aln_seg2)
     const bool aln8 = fmt & SX_FMT_ALN8, seg2 = fmt & SX_FMT_SEG2, baseq = fmt & SX_FMT_BASEQ, ref4 = fmt & SX_FMT_REF4;
-    const uint32_t aln_skew = aln8 ? (r0.aln_begin & 1u) : 0u; // the sx_aln8 slice is staged from a 16-byte boundary
-    const uint32_t n_segs_region = r1.seg_begin - r0.seg_begin;
-    const unsigned char* alns_raw = smem + L.alns;
-    const unsigned char* segs_raw = smem + L.segs;
-    auto aln_at = [&](uint32_t a) -> uint4 { // region-relative: x read, y first reference position, z first segment, w first inserted base
-        if (aln8)
-        {
-            const uint2 v = reinterpret_cast<const uint2*>(alns_raw)[a + aln_skew];
-            return make_uint4(v.x & 0xffffu, static_cast<uint32_t>(static_cast<int32_t>(v.x) >> 16), v.y & 0xffffu, v.y >> 16);
-        }
-        const uint4 h = reinterpret_cast<const uint4*>(alns_raw)[a];
-        return make_uint4(h.x - r0.read_begin, h.y - static_cast<uint32_t>(r0.ref_begin), h.z - r0.seg_begin, h.w - r0.ins_begin);
-    };
-    auto seg_end_of = [&](uint32_t a) -> uint32_t {
-        if (aln8) return a + 1 < L.n_alns ? aln_at(a + 1).z : n_segs_region;
-        return reinterpret_cast<const uint4*>(alns_raw)[a + 1].z - r0.seg_begin;
-    };
-    auto seg_at = [&](uint32_t s) -> uint32_t { // len | kind << 16 | flags << 24
-        if (seg2)
-        {
-            const uint32_t v = reinterpret_cast<const uint16_t*>(segs_raw)[s];
-            return (v & 0xfffu) | (((v >> 12) & 7u) << 16) | ((v >> 15) << 24);
-        }
-        return reinterpret_cast<const uint32_t*>(segs_raw)[s];
-    };
+    const aln_reader rd(smem, L, r0, aln8, seg2);
     uint8_t* ref_s = smem + L.ref;
     uint8_t* ins_s = smem + L.ins;
     const uint8_t* seq_s = smem + L.seq;
@@ -184,7 +64,7 @@ __global__ void __launch_bounds__(K1_THREADS) k1_score_kernel(const sx_region* _
     uint32_t* desc_s = reinterpret_cast<uint32_t*>(smem + L.desc);
     uint16_t* ent_s = reinterpret_cast<uint16_t*>(smem + L.ent);
     const uint32_t tab_saddr = smem_u32(tab); // shared-window address of the term table
-    if (tab_saddr + K1_TAB_BYTES > 0xfff0u || (tab_saddr & 15u))
+    if (tab_saddr + TAB_BYTES > 0xfff0u || (tab_saddr & 15u))
     {
         if (threadIdx.x == 0) atomicOr(status, SX_ST_TILE);
         return;
@@ -209,24 +89,9 @@ __global__ void __launch_bounds__(K1_THREADS) k1_score_kernel(const sx_region* _
         desc_s[code] = d + tab_saddr;
     }
 
-    if (threadIdx.x == 0)
-    {
-        mbar_init(bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        const uint32_t aln_bytes = k1q::aln_slice_bytes(r0.aln_begin, L.n_alns, fmt);
-        const uint32_t ref_tx = ref4 ? L.refp_bytes : L.ref_bytes;
-        const uint32_t tx = K1_TAB_BYTES + aln_bytes + L.seg_bytes + ref_tx + L.ins_bytes + L.seq_bytes + L.qual_bytes;
-        mbar_expect_tx(bar, tx);
-        tma_bulk_g2s(smem + L.tab, tables->k1_tab, K1_TAB_BYTES, bar);
-        tma_bulk_g2s(smem + L.alns, reinterpret_cast<const unsigned char*>(alns) + (aln8 ? (size_t)(r0.aln_begin & ~1u) * 8u : (size_t)r0.aln_begin * 16u), aln_bytes, bar);
-        if (L.seg_bytes) tma_bulk_g2s(smem + L.segs, reinterpret_cast<const unsigned char*>(segs) + (size_t)r0.seg_begin * (seg2 ? 2u : 4u), L.seg_bytes, bar);
-        if (ref_tx) tma_bulk_g2s(smem + (ref4 ? L.refp : L.ref), ref + r0.ref_off, ref_tx, bar);
-        if (L.ins_bytes) tma_bulk_g2s(smem + L.ins, ins + r0.ins_begin, L.ins_bytes, bar);
-        if (L.seq_bytes) tma_bulk_g2s(smem + L.seq, seq4 + r0.seq_off, L.seq_bytes, bar);
-        if (L.qual_bytes) tma_bulk_g2s(smem + L.qual, qual + r0.qual_off, L.qual_bytes, bar);
-    }
+    if (threadIdx.x == 0) issue_copies(smem, L, r0, aln8, seg2, ref4, alns, segs, ref, ins, seq4, qual, L.tab, tables->k1_tab, TAB_BYTES);
     // read lengths: tiny, plain coalesced loads (their offset has no 16-byte alignment guarantee)
-    for (uint32_t r = threadIdx.x; r < L.n_reads; r += K1_THREADS) rlen_s[r] = read_len[r0.read_begin + r];
+    for (uint32_t r = threadIdx.x; r < L.n_reads; r += THREADS) rlen_s[r] = read_len[r0.read_begin + r];
     __syncthreads(); // rlen visible, mbarrier initialised
     // per-read base / packed-byte offsets: warp 0, shuffle scan
     if (threadIdx.x < 32)
@@ -275,7 +140,7 @@ __global__ void __launch_bounds__(K1_THREADS) k1_score_kernel(const sx_region* _
     {
         const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
         uint32_t qmax = 0; // largest quality seen on a non-N base: the reference only looks at those (score.cpp:125-126,158-159)
-        for (uint32_t r = warp; r < L.n_reads; r += K1_THREADS / 32)
+        for (uint32_t r = warp; r < L.n_reads; r += THREADS / 32)
         {
             const uint32_t len = rlen_s[r];
             const uint8_t* sq = seq_s + soff_s[r];
@@ -323,7 +188,7 @@ __global__ void __launch_bounds__(K1_THREADS) k1_score_kernel(const sx_region* _
         {
             // the bases that are not A/C/G/T: rebuild their entries from the real code (the nibble kept the quality code)
             __syncthreads();
-            for (uint32_t i = exc_off[ri] + threadIdx.x; i < exc_off[ri + 1]; i += K1_THREADS)
+            for (uint32_t i = exc_off[ri] + threadIdx.x; i < exc_off[ri + 1]; i += THREADS)
             {
                 const uint32_t v = exc[i], pos = v & 0xffffffu, d = desc_s[(v >> 24) & 15u];
                 if (pos >= 2u * soff_s[L.n_reads])
@@ -338,15 +203,15 @@ __global__ void __launch_bounds__(K1_THREADS) k1_score_kernel(const sx_region* _
         if (ref4)
         {
             const uint8_t* rp = smem + L.refp; // packed BAM codes -> one-hot codes, two per packed byte
-            for (uint32_t i = threadIdx.x; i < L.ref_bytes; i += K1_THREADS)
+            for (uint32_t i = threadIdx.x; i < L.ref_bytes; i += THREADS)
             {
                 const uint32_t b = (i >> 1) < L.refp_bytes ? rp[i >> 1] : 0xffu, c = (i & 1u) ? (b & 15u) : (b >> 4);
                 ref_s[i] = static_cast<uint8_t>((c == 1u || c == 2u || c == 4u || c == 8u) ? c : 0u);
             }
         }
         else
-        for (uint32_t i = threadIdx.x; i < L.ref_bytes; i += K1_THREADS) ref_s[i] = onehot_of_char(ref_s[i]);
-        for (uint32_t i = threadIdx.x; i < L.ins_bytes; i += K1_THREADS) ins_s[i] = onehot_of_char(ins_s[i]);
+        for (uint32_t i = threadIdx.x; i < L.ref_bytes; i += THREADS) ref_s[i] = onehot_of_char(ref_s[i]);
+        for (uint32_t i = threadIdx.x; i < L.ins_bytes; i += THREADS) ins_s[i] = onehot_of_char(ins_s[i]);
     }
     __syncthreads();
 
@@ -355,9 +220,9 @@ __global__ void __launch_bounds__(K1_THREADS) k1_score_kernel(const sx_region* _
     const uint32_t zero_entry = (SX_K1_ROW_ZERO << 4) + tab_saddr; // the all-zero table row: adds +0.0
     const int ref_len = static_cast<int>(r0.ref_len);
 
-    for (uint32_t a = threadIdx.x; a < L.n_alns; a += K1_THREADS)
+    for (uint32_t a = threadIdx.x; a < L.n_alns; a += THREADS)
     {
-        const uint4 h = aln_at(a);
+        const uint4 h = rd.aln_at(a);
         const uint32_t rl = h.x;
         if (rl >= L.n_reads)
         {
@@ -369,7 +234,7 @@ __global__ void __launch_bounds__(K1_THREADS) k1_score_kernel(const sx_region* _
         int refp = static_cast<int>(h.y);
         const uint8_t* insp = ins_s + h.w;
         uint32_t s = h.z;
-        const uint32_t s_end = seg_end_of(a);
+        const uint32_t s_end = rd.seg_end(a);
         double lnp = 0.0;
         int rem = 0;
         bool pend = false;
@@ -389,7 +254,7 @@ __global__ void __launch_bounds__(K1_THREADS) k1_score_kernel(const sx_region* _
                     done = true;
                     break;
                 }
-                const uint32_t seg = seg_at(s++);
+                const uint32_t seg = rd.seg_at(s++);
                 const int len = static_cast<int>(seg & 0xffffu);
                 const uint32_t kind = (seg >> 16) & 0xffu;
                 pend = (seg >> 24) & SX_SEGF_NONCANDIDATE;
@@ -475,8 +340,9 @@ __global__ void k1_smem_need_kernel(const sx_region* __restrict__ regions, uint3
     for (uint32_t i = begin + blockIdx.x * blockDim.x + threadIdx.x; i < end; i += gridDim.x * blockDim.x)
     {
         const sx_region a = regions[i], b = regions[i + 1];
-        m = max(m, k1_make_layout(a, b, fmt).total);
-        mq = max(mq, k1q::make_layout(a, b, fmt).total);
+        const footprint f = footprint_of(a, b, fmt);
+        m = max(m, f.general);
+        mq = max(mq, f.fast);
     }
     for (int d = 16; d; d >>= 1)
     {
@@ -570,16 +436,11 @@ int k1_smem_need_dev(sx_ctx* ctx, const sx_region* regions_dev, uint32_t begin, 
 }
 } // namespace
 
-size_t sx_k1_region_smem(const sx_region* r0, const sx_region* r1, const sx_aln*)
-{
-    return k1_make_layout(*r0, *r1, 0).total;
-}
-
 // smem_bytes: largest region footprint of the general kernel; smem_fast: of the 4-bit fast path (0: not computed)
 int sx_k1_launch(sx_ctx* ctx, const sx_align_batch* d, uint32_t region_begin, uint32_t region_end, double* lnp_dev, size_t smem_bytes, size_t smem_fast, cudaStream_t st)
 {
     if (region_end <= region_begin) return SX_OK;
-    if ((d->qual_bits == 4 || d->qual_bits == 2) && smem_fast && smem_fast <= k1q::KQ_MAX_SMEM) return sx_k1q_launch(ctx, d, region_begin, region_end, lnp_dev, smem_fast, st);
+    if ((d->qual_bits == 4 || d->qual_bits == 2) && smem_fast && smem_fast <= k1::KQ_MAX_SMEM) return sx_k1q_launch(ctx, d, region_begin, region_end, lnp_dev, smem_fast, st);
     if (smem_bytes > ctx->smem_optin)
         return sx_fail(ctx, SX_ERR_ARG, "sx_score_alignments: a region needs %zu bytes of shared memory (limit %zu); split it into smaller regions", smem_bytes,
                        ctx->smem_optin);
@@ -588,8 +449,8 @@ int sx_k1_launch(sx_ctx* ctx, const sx_align_batch* d, uint32_t region_begin, ui
         SX_CUDA(ctx, cudaFuncSetAttribute(k1_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(ctx->smem_optin)));
     uint4 qd;
     memcpy(&qd, d->qual_dict, 16);
-    k1_score_kernel<<<region_end - region_begin, K1_THREADS, smem_bytes, st>>>(d->regions, d->read_len, d->seq4, d->qual, d->ref, d->alns, d->segs, d->ins,
-                                                                              ctx->d_tables, region_begin, lnp_dev, ctx->d_status, static_cast<uint32_t>(smem_bytes), d->qual_bits == 4 ? 4u : d->qual_bits == 2 ? 2u : 8u, qd, d->format, d->exc_off, d->exc);
+    k1_score_kernel<<<region_end - region_begin, THREADS, smem_bytes, st>>>(d->regions, d->read_len, d->seq4, d->qual, d->ref, d->alns, d->segs, d->ins,
+                                                                           ctx->d_tables, region_begin, lnp_dev, ctx->d_status, static_cast<uint32_t>(smem_bytes), d->qual_bits == 4 ? 4u : d->qual_bits == 2 ? 2u : 8u, qd, d->format, d->exc_off, d->exc);
     SX_CUDA(ctx, cudaGetLastError());
     return SX_OK;
 }
@@ -641,8 +502,9 @@ static int validate_host_batch(sx_ctx* ctx, const sx_align_batch* b, size_t* max
         if (n.read_begin < r.read_begin || n.aln_begin < r.aln_begin || n.seg_begin < r.seg_begin || n.ins_begin < r.ins_begin || n.seq_off < r.seq_off ||
             n.qual_off < r.qual_off)
             return sx_fail(ctx, SX_ERR_ARG, "sx_score_alignments: region table is not monotone at region %u", i);
-        m = std::max<size_t>(m, k1_make_layout(r, n, b->format).total);
-        mq = std::max<size_t>(mq, k1q::make_layout(r, n, b->format).total);
+        const k1::footprint f = k1::footprint_of(r, n, b->format);
+        m = std::max<size_t>(m, f.general);
+        mq = std::max<size_t>(mq, f.fast);
     }
     if (b->n_regions)
     {

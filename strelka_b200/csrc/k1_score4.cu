@@ -17,49 +17,18 @@
 //     PRMT funnels fetch the 8 entries and 8 reference codes, six logic ops per 4 cells produce the table addresses (including the
 //     substitution of the zero page for the cells past a run's end), and a cell is PRMT + LDS.64 + DADD.
 // Regions that do not fit the 16-bit shared-window addresses used here (KQ_MAX_SMEM) are scored by the general kernel.
-#include "k1q_layout.cuh"
+#include "k1_stage.cuh"
 
 #include <cstring>
 
 namespace
 {
-using namespace k1q;
+using namespace k1;
 
 constexpr uint32_t PAGE_BASE = 0, PAGE_EQ = 1, PAGE_ZERO = 2, PAGE_NOMATCH = 3;
 constexpr uint32_t REF_OTHER = 4;
 constexpr uint32_t ENTRY_BAD = (PAGE_ZERO << 2) | 3u; // low nibble of an entry whose quality is out of range (scores as zero; flagged)
 enum { REC_RUN = 0, REC_SOFT = 1, REC_OOW = 2, REC_END = 3 };
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count)
-{
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes)
-{
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t phase)
-{
-    asm volatile(
-        "{\n"
-        ".reg .pred P1;\n"
-        "KQ_WAIT:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n"
-        "@P1 bra KQ_DONE;\n"
-        "bra KQ_WAIT;\n"
-        "KQ_DONE:\n"
-        "}\n" ::"r"(smem_u32(bar)),
-        "r"(phase)
-        : "memory");
-}
-// TMA 1-D bulk copy global -> shared, completion counted in bytes on an mbarrier.  16-byte aligned src/dst/size.
-__device__ __forceinline__ void tma_bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst_smem)), "l"(src_gmem),
-                 "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
 
 // shared-window loads by 32-bit address
 __device__ __forceinline__ uint32_t lds_u8(uint32_t a)
@@ -78,12 +47,6 @@ __device__ __forceinline__ uint2 lds_u64(uint32_t a)
 {
     uint2 v;
     asm("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(a));
-    return v;
-}
-__device__ __forceinline__ double lds_f64(uint32_t a)
-{
-    double v;
-    asm("ld.shared.f64 %0, [%1];" : "=d"(v) : "r"(a));
     return v;
 }
 // run records are written and read back by the same thread: keep both in program order
@@ -109,19 +72,19 @@ __device__ __forceinline__ uint32_t dict_at(const uint4& qd, uint32_t c)
     return (w >> ((c & 3u) * 8u)) & 0xffu;
 }
 
-__global__ void __launch_bounds__(KQ_THREADS) k1q_score_kernel(const sx_region* __restrict__ regions, const uint16_t* __restrict__ read_len,
-                                                               const uint8_t* __restrict__ seq4, const uint8_t* __restrict__ qual4,
-                                                               const char* __restrict__ ref, const sx_aln* __restrict__ alns,
-                                                               const sx_aln_seg* __restrict__ segs, const char* __restrict__ ins,
-                                                               const sx_tables* __restrict__ tables, uint32_t region_begin, double* __restrict__ lnp_out,
-                                                               int* __restrict__ status, uint32_t smem_bytes, uint4 qual_dict, uint32_t fmt, uint32_t qual_bits,
-                                                               const uint32_t* __restrict__ exc_off, const uint32_t* __restrict__ exc)
+__global__ void __launch_bounds__(THREADS) k1q_score_kernel(const sx_region* __restrict__ regions, const uint16_t* __restrict__ read_len,
+                                                            const uint8_t* __restrict__ seq4, const uint8_t* __restrict__ qual4,
+                                                            const char* __restrict__ ref, const sx_aln* __restrict__ alns,
+                                                            const sx_aln_seg* __restrict__ segs, const char* __restrict__ ins,
+                                                            const sx_tables* __restrict__ tables, uint32_t region_begin, double* __restrict__ lnp_out,
+                                                            int* __restrict__ status, uint32_t smem_bytes, uint4 qual_dict, uint32_t fmt, uint32_t qual_bits,
+                                                            const uint32_t* __restrict__ exc_off, const uint32_t* __restrict__ exc)
 {
     extern __shared__ __align__(128) unsigned char smem[];
     const uint32_t ri = region_begin + blockIdx.x;
     const sx_region r0 = regions[ri];
     const sx_region r1 = regions[ri + 1];
-    const layout L = make_layout(r0, r1, fmt);
+    const qlayout L = make_qlayout(slices_of(r0, r1, fmt));
     if (L.n_alns == 0) return;
     const uint32_t sbase = smem_u32(smem);
     const uint32_t tab_saddr = (sbase + L.tab + 1023u) & ~1023u; // 1 KB-aligned in the shared window: a cell's address is two PRMT'd bytes
@@ -135,35 +98,8 @@ __global__ void __launch_bounds__(KQ_THREADS) k1q_score_kernel(const sx_region* 
     uint2* lut = reinterpret_cast<uint2*>(smem + L.lut);
     uint8_t* e8 = smem + L.e8;
     double* tab = reinterpret_cast<double*>(smem + (tab_saddr - sbase)); // [4 pages][16 quality codes][match, mismatch]
-    // alignment headers and segments, read through accessors that hide the wire format (sx_aln / sx_aln8, sx_aln_seg / sx_aln_seg2)
     const bool aln8 = fmt & SX_FMT_ALN8, seg2 = fmt & SX_FMT_SEG2, baseq = fmt & SX_FMT_BASEQ, ref4 = fmt & SX_FMT_REF4;
-    const uint32_t aln_skew = aln8 ? (r0.aln_begin & 1u) : 0u; // the sx_aln8 slice is staged from a 16-byte boundary
-    const unsigned char* alns_raw = smem + L.alns;
-    const unsigned char* segs_raw = smem + L.segs;
-    // region-relative header of alignment a: x read, y first reference position, z first segment, w first inserted base
-    auto aln_at = [&](uint32_t a) -> uint4 {
-        if (aln8)
-        {
-            const uint2 v = reinterpret_cast<const uint2*>(alns_raw)[a + aln_skew];
-            return make_uint4(v.x & 0xffffu, static_cast<uint32_t>(static_cast<int32_t>(v.x) >> 16), v.y & 0xffffu, v.y >> 16);
-        }
-        const uint4 h = reinterpret_cast<const uint4*>(alns_raw)[a];
-        return make_uint4(h.x - r0.read_begin, h.y - static_cast<uint32_t>(r0.ref_begin), h.z - r0.seg_begin, h.w - r0.ins_begin);
-    };
-    // end of alignment a's segment list
-    auto seg_end_of = [&](uint32_t a) -> uint32_t {
-        if (aln8) return a + 1 < L.n_alns ? aln_at(a + 1).z : L.n_segs;
-        return reinterpret_cast<const uint4*>(alns_raw)[a + 1].z - r0.seg_begin;
-    };
-    // segment s as len | kind << 16 | flags << 24
-    auto seg_at = [&](uint32_t s) -> uint32_t {
-        if (seg2)
-        {
-            const uint32_t v = reinterpret_cast<const uint16_t*>(segs_raw)[s];
-            return (v & 0xfffu) | (((v >> 12) & 7u) << 16) | ((v >> 15) << 24);
-        }
-        return reinterpret_cast<const uint32_t*>(segs_raw)[s];
-    };
+    const aln_reader rd(smem, L, r0, aln8, seg2);
     uint8_t* ref_s = smem + L.ref;
     uint8_t* ins_s = smem + L.ins;
     uint16_t* rlen_s = reinterpret_cast<uint16_t*>(smem + L.rlen);
@@ -177,7 +113,7 @@ __global__ void __launch_bounds__(KQ_THREADS) k1q_score_kernel(const sx_region* 
         tab[2 * tid + 0] = page == PAGE_ZERO ? 0.0 : page == PAGE_NOMATCH ? x : m;
         tab[2 * tid + 1] = page == PAGE_ZERO ? 0.0 : page == PAGE_EQ ? m : x;
     }
-    for (uint32_t idx = tid; idx < 256; idx += KQ_THREADS)
+    for (uint32_t idx = tid; idx < 256; idx += THREADS)
     {
         // (read nibble << 4 | quality code) -> entry.  bam_seq::get_code nibbles: 0 '=', 1 A, 2 C, 4 G, 8 T, 15 N, others IUPAC.
         const uint32_t nib = idx >> 4, qc = idx & 15u;
@@ -197,24 +133,8 @@ __global__ void __launch_bounds__(KQ_THREADS) k1q_score_kernel(const sx_region* 
         lut[tid] = make_uint2(lo, hi);
     }
 
-    if (tid == 0)
-    {
-        mbar_init(bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        const uint32_t aln_bytes = aln_slice_bytes(r0.aln_begin, L.n_alns, fmt);
-        const uint32_t ref_tx = ref4 ? L.refp_bytes : L.ref_bytes;
-        const uint32_t tx = aln_bytes + L.seg_bytes + ref_tx + L.ins_bytes + L.seq_bytes + L.qual_bytes;
-        mbar_expect_tx(bar, tx);
-        const unsigned char* aln_src = reinterpret_cast<const unsigned char*>(alns) + (aln8 ? (size_t)(r0.aln_begin & ~1u) * 8u : (size_t)r0.aln_begin * 16u);
-        const unsigned char* seg_src = reinterpret_cast<const unsigned char*>(segs) + (size_t)r0.seg_begin * (seg2 ? 2u : 4u);
-        tma_bulk_g2s(smem + L.alns, aln_src, aln_bytes, bar);
-        if (L.seg_bytes) tma_bulk_g2s(smem + L.segs, seg_src, L.seg_bytes, bar);
-        if (ref_tx) tma_bulk_g2s(smem + (ref4 ? L.refp : L.ref), ref + r0.ref_off, ref_tx, bar);
-        if (L.ins_bytes) tma_bulk_g2s(smem + L.ins, ins + r0.ins_begin, L.ins_bytes, bar);
-        if (L.seq_bytes) tma_bulk_g2s(smem + L.seq, seq4 + r0.seq_off, L.seq_bytes, bar);
-        if (L.qual_bytes) tma_bulk_g2s(smem + L.qual, qual4 + r0.qual_off, L.qual_bytes, bar);
-    }
-    for (uint32_t r = tid; r < L.n_reads; r += KQ_THREADS) rlen_s[r] = read_len[r0.read_begin + r];
+    if (tid == 0) issue_copies(smem, L, r0, aln8, seg2, ref4, alns, segs, ref, ins, seq4, qual4);
+    for (uint32_t r = tid; r < L.n_reads; r += THREADS) rlen_s[r] = read_len[r0.read_begin + r];
     __syncthreads(); // rlen, tables visible; mbarrier initialised
     // packed-byte offset of every read (reads lie back to back, each padded to a whole byte): warp 0, shuffle scan
     if (tid < 32)
@@ -255,7 +175,7 @@ __global__ void __launch_bounds__(KQ_THREADS) k1q_score_kernel(const sx_region* 
         {
             // one nibble per base, (base << 2) | quality code: the entry (code << 4 | page 0 << 2 | base) is a bit shuffle, no lookup;
             // the host guarantees every dictionary quality <= 70 in this format
-            for (uint32_t w = tid; w < nw; w += KQ_THREADS)
+            for (uint32_t w = tid; w < nw; w += THREADS)
             {
                 const uint32_t s = seq32[w];
                 const uint32_t h = (s >> 4) & 0x0f0f0f0fu, l = s & 0x0f0f0f0fu;  // first / second bases of the four packed bytes
@@ -269,7 +189,7 @@ __global__ void __launch_bounds__(KQ_THREADS) k1q_score_kernel(const sx_region* 
             {
                 __syncthreads();
                 uint8_t* ent8 = smem + L.ent;
-                for (uint32_t i = x0 + tid; i < x1; i += KQ_THREADS)
+                for (uint32_t i = x0 + tid; i < x1; i += THREADS)
                 {
                     const uint32_t v = exc[i], pos = v & 0xffffffu, code = v >> 24;
                     if (pos >= 2u * soff_s[L.n_reads])
@@ -283,7 +203,7 @@ __global__ void __launch_bounds__(KQ_THREADS) k1q_score_kernel(const sx_region* 
             }
         }
         else
-        for (uint32_t w = tid; w < nw; w += KQ_THREADS)
+        for (uint32_t w = tid; w < nw; w += THREADS)
         {
             const uint32_t s = seq32[w];
             uint32_t q;
@@ -316,7 +236,7 @@ __global__ void __launch_bounds__(KQ_THREADS) k1q_score_kernel(const sx_region* 
             // packed BAM codes -> one reference code per byte (two per packed byte, high nibble first)
             const uint8_t* rp = smem + L.refp;
             uint16_t* ref16 = reinterpret_cast<uint16_t*>(ref_s);
-            for (uint32_t i = tid; i < L.ref_bytes / 2; i += KQ_THREADS)
+            for (uint32_t i = tid; i < L.ref_bytes / 2; i += THREADS)
             {
                 const uint32_t b = i < L.refp_bytes ? rp[i] : 0xffu;
                 const uint32_t hi = b >> 4, lo = b & 15u;
@@ -326,13 +246,13 @@ __global__ void __launch_bounds__(KQ_THREADS) k1q_score_kernel(const sx_region* 
             }
         }
         else
-        for (uint32_t i = tid; i < L.ref_bytes / 4; i += KQ_THREADS)
+        for (uint32_t i = tid; i < L.ref_bytes / 4; i += THREADS)
         {
             const uint32_t v = ref32[i];
             ref32[i] = ref_code_of_char(v & 0xffu) | (ref_code_of_char((v >> 8) & 0xffu) << 8) | (ref_code_of_char((v >> 16) & 0xffu) << 16) |
                        (ref_code_of_char(v >> 24) << 24);
         }
-        for (uint32_t i = tid; i < L.ins_bytes; i += KQ_THREADS) ins_s[i] = static_cast<uint8_t>(ref_code_of_char(ins_s[i]));
+        for (uint32_t i = tid; i < L.ins_bytes; i += THREADS) ins_s[i] = static_cast<uint8_t>(ref_code_of_char(ins_s[i]));
     }
     __syncthreads();
 
@@ -343,11 +263,11 @@ __global__ void __launch_bounds__(KQ_THREADS) k1q_score_kernel(const sx_region* 
     // high address byte of a masked cell, in every byte lane: table page 2 (all zeros).  Bits 0-1 of tab_saddr >> 8 are clear, bit 7 too.
     const uint32_t k2 = ((tab_saddr >> 8) | PAGE_ZERO) * 0x01010101u;
 
-    for (uint32_t a = tid; a < L.n_alns; a += KQ_THREADS)
+    for (uint32_t a = tid; a < L.n_alns; a += THREADS)
     {
-        const uint4 h = aln_at(a);
+        const uint4 h = rd.aln_at(a);
         const uint32_t rl = h.x;
-        const uint32_t seg0 = h.z, seg1 = seg_end_of(a);
+        const uint32_t seg0 = h.z, seg1 = rd.seg_end(a);
         if (rl >= L.n_reads || seg1 > L.n_segs || seg0 > seg1)
         {
             atomicOr(status, SX_ST_TILE);
@@ -365,7 +285,7 @@ __global__ void __launch_bounds__(KQ_THREADS) k1q_score_kernel(const sx_region* 
             uint32_t rp = rec0, pre = 0;
             for (uint32_t s = seg0; s < seg1; ++s)
             {
-                const uint32_t seg = seg_at(s);
+                const uint32_t seg = rd.seg_at(s);
                 const int len = static_cast<int>(seg & 0xffffu);
                 const uint32_t kind = (seg >> 16) & 0xffu;
                 if (kind == SX_SEG_MATCH || kind == SX_SEG_INSERT || kind == SX_SEG_SOFTCLIP)
@@ -442,7 +362,7 @@ __global__ void __launch_bounds__(KQ_THREADS) k1q_score_kernel(const sx_region* 
                     int p0 = static_cast<int>(h.y);
                     for (uint32_t ss = seg0; ss < (rec.x >> 16); ++ss)
                     {
-                        const uint32_t sg = seg_at(ss), k = (sg >> 16) & 0xffu;
+                        const uint32_t sg = rd.seg_at(ss), k = (sg >> 16) & 0xffu;
                         if (k == SX_SEG_MATCH || k == SX_SEG_REFSKIP) p0 += static_cast<int>(sg & 0xffffu);
                     }
                     const uint32_t ea = rec.x & 0xffffu, len = rec.y & 0xffffu;
@@ -502,11 +422,11 @@ int sx_k1q_launch(sx_ctx* ctx, const sx_align_batch* d, uint32_t region_begin, u
 {
     if (region_end <= region_begin) return SX_OK;
     if (smem_bytes > 48 * 1024)
-        SX_CUDA(ctx, cudaFuncSetAttribute(k1q_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(k1q::KQ_MAX_SMEM)));
+        SX_CUDA(ctx, cudaFuncSetAttribute(k1q_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(k1::KQ_MAX_SMEM)));
     uint4 qd;
     memcpy(&qd, d->qual_dict, 16);
-    k1q_score_kernel<<<region_end - region_begin, k1q::KQ_THREADS, smem_bytes, st>>>(d->regions, d->read_len, d->seq4, d->qual, d->ref, d->alns, d->segs, d->ins,
-                                                                                    ctx->d_tables, region_begin, lnp_dev, ctx->d_status, static_cast<uint32_t>(smem_bytes), qd, d->format, d->qual_bits, d->exc_off, d->exc);
+    k1q_score_kernel<<<region_end - region_begin, k1::THREADS, smem_bytes, st>>>(d->regions, d->read_len, d->seq4, d->qual, d->ref, d->alns, d->segs, d->ins,
+                                                                                 ctx->d_tables, region_begin, lnp_dev, ctx->d_status, static_cast<uint32_t>(smem_bytes), qd, d->format, d->qual_bits, d->exc_off, d->exc);
     SX_CUDA(ctx, cudaGetLastError());
     return SX_OK;
 }

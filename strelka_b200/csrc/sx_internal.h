@@ -343,7 +343,7 @@ struct sx_call_timer
 // kernels' host launchers (each in its own .cu)
 int sx_k1_launch(sx_ctx* ctx, const sx_align_batch* dev, uint32_t region_begin, uint32_t region_end, double* lnp_dev, size_t smem_bytes, size_t smem_fast,
                  cudaStream_t st);
-size_t sx_k1_region_smem(const sx_region* r0, const sx_region* r1, const sx_aln* alns);
+int sx_k1q_launch(sx_ctx* ctx, const sx_align_batch* dev, uint32_t region_begin, uint32_t region_end, double* lnp_dev, size_t smem_bytes, cudaStream_t st);
 
 // The stage launchers, each beside its kernels and the only code that launches them.  A launcher enqueues its stage on ctx->s_compute
 // (device pointers in and out) and adds the stage's launches to *launches; it does no timing, reads no status word and leaves the device
