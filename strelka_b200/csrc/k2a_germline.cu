@@ -441,7 +441,9 @@ __global__ void __launch_bounds__(K2_WARPS * 32) k2a_germline_batch_kernel(const
 //   * the (strand x base) grouping takes 8 ballot rounds per site, each a loop over the calls;
 //   * the serial per-group phase has 32 (site, group) lanes, of which a homozygous site fills 2 of its 8.
 // Here the same arithmetic is laid out so that the lanes are full:
-//   * grouping: with <= 32 calls a lane holds one call and 8 ballots give every group's members and rank;
+//   * filter and grouping: the batch's 12 sites own one contiguous call block, copied once into shared memory and taken 32 calls at a
+//     time across site boundaries (a site's calls are a contiguous lane range of a chunk), three bit-plane ballots give every call its
+//     (site, group) members and rank, one scan per batch the group starts;
 //   * the serial phase takes a compacted list of the NON-EMPTY (site, group) pairs of 12 sites, one pair per lane;
 //   * accumulation and posteriors run for THREE sites at once, 10 lanes each (lanes 30, 31 idle): the `all' sums only; the two
 //     strand-specific sums of the called genotype are computed by two lanes, for SNP sites only.
@@ -473,6 +475,29 @@ __device__ __forceinline__ uint32_t k2_repack(uint32_t c)
 }
 // adjust_joint_eprob's group of a repacked call: is_fwd + 2*base_id for q >= 3 and base_id < 4, else 0xff (not in any group)
 __device__ __forceinline__ uint32_t k2_group(uint32_t r) { return (((r >> 3) & 63u) >= 3u && !(r & 0x400u)) ? (r & 1u) | ((r >> 13) & 6u) : 0xffu; }
+// the lanes of elements [beg, end) in the 32-element chunk starting at element b
+__device__ __forceinline__ uint32_t k2_lanes(uint32_t beg, uint32_t end, uint32_t b)
+{
+    const uint32_t lo = beg > b ? beg - b : 0u, hi = end > b ? end - b : 0u;
+    if (lo >= 32u || hi <= lo) return 0u;
+    return (hi >= 32u ? FULL : (1u << hi) - 1u) & (FULL << lo);
+}
+// the site of element b + lane of a twelve-site block: lane k <= 12 holds the block offset of site k's first element (lanes from the batch's
+// last site + 1 on: the block's end), so the site is the number of sites 1..12 that start at or before the element.  The sites starting
+// inside the chunk (about one per chunk) are taken one by one.
+__device__ __forceinline__ uint32_t k2_site_of(uint32_t my_off, uint32_t b, uint32_t lane)
+{
+    const bool bnd = lane - 1u < 12u;
+    uint32_t s = __popc(__ballot_sync(FULL, bnd && my_off <= b));
+    uint32_t inner = __ballot_sync(FULL, bnd && my_off > b && my_off < b + 32u);
+    while (inner)
+    {
+        const uint32_t o = __shfl_sync(FULL, my_off, __ffs(inner) - 1);
+        inner &= inner - 1u;
+        if (b + lane >= o) ++s;
+    }
+    return s;
+}
 constexpr int K2_CAP12 = 96;       // deepest site this kernel takes (shared memory: 12 sites x cap x 8 bytes per warp)
 constexpr int K2_SORT_STACK12 = 16; // sx_stdsort_desc's stack for groups of at most K2_CAP12 members: 2*floor(log2(96)) + 1 = 13 entries
 
@@ -517,9 +542,12 @@ __global__ void k2a_init_tables_kernel(sx_tables* __restrict__ t)
 __global__ void __launch_bounds__(K2_WARPS * 32, 8) k2a_germline12_kernel(const uint32_t* __restrict__ site_off, const uint16_t* __restrict__ calls_g,
                                                                        const char* __restrict__ ref_base, const uint8_t* __restrict__ ploidy,
                                                                        uint32_t n_sites, int is_always_test, const sx_tables* __restrict__ tables,
-                                                                       sx_digt_result* __restrict__ out, int* __restrict__ status, uint32_t cap)
+                                                                       sx_digt_result* __restrict__ out, int* __restrict__ status, uint32_t cap,
+                                                                       uint32_t ord_stride)
 {
     __shared__ germ12_tables T;
+    // per warp: 12 sites x `cap` cleaned calls (uint16) and their values (float); an `ord_stride`-slot region (uint16) that first holds the
+    // batch's raw calls as staged from global memory, then site s's per-group order at s * cap
     extern __shared__ __align__(16) unsigned char k2_dyn[];
     float* const s_val_all = reinterpret_cast<float*>(k2_dyn);
     uint16_t* const s_calls_all = reinterpret_cast<uint16_t*>(k2_dyn + (size_t)K2_WARPS * K2_B12 * cap * 4);
@@ -527,7 +555,14 @@ __global__ void __launch_bounds__(K2_WARPS * 32, 8) k2a_germline12_kernel(const 
     __shared__ uint16_t s_gstart[K2_WARPS][K2_B12][10];
     __shared__ uint16_t s_n[K2_WARPS][K2_B12];
     __shared__ uint8_t s_pair[K2_WARPS][K2_B12 * 8]; // site * 8 + group, | 0x80 if the group holds a neighbour-mismatch call
-    __shared__ float s_lh[K2_WARPS][K2_B12][10]; // ln P(column | genotype) of the batch's sites, phase C -> phase D
+    // ln P(column | genotype) of the batch's sites, phase C -> phase D; in phase A the running member count of each (site, group),
+    // site * 8 + group, | 0x80 once a member carries the neighbour-mismatch bit
+    __shared__ union
+    {
+        float lh[K2_B12][10];
+        uint32_t gcnt4[K2_B12 * 2];
+        uint8_t gcnt[K2_B12 * 8];
+    } s_ab[K2_WARPS];
     __shared__ float s_val12[2 * (SX_MAX_QSCORE + 1)]; // {val1[q], val2[q]} side by side: the two tables no longer share a bank
     for (int i = threadIdx.x; i <= SX_MAX_QSCORE; i += blockDim.x)
     {
@@ -558,171 +593,155 @@ __global__ void __launch_bounds__(K2_WARPS * 32, 8) k2a_germline12_kernel(const 
     for (uint32_t base = gwarp * K2_B12; base < n_sites; base += nwarps * K2_B12)
     {
         const uint32_t nb = min((uint32_t)K2_B12, n_sites - base);
-        uint32_t nonref_mask = 0, n_pairs = 0;
-        // ---- phase A, site by site: CleanPileupFilter, initial eprobs, grouping, the list of non-empty groups
-        for (uint32_t s = 0; s < nb; ++s)
+        uint32_t n_pairs = 0;
+        float* const w_val0 = s_val_all + warp * K2_B12 * cap;
+        uint16_t* const w_calls0 = s_calls_all + warp * K2_B12 * cap;
+        uint16_t* const w_ord0 = s_ord_all + warp * ord_stride;
+        // ---- phase A over the batch's call block [site_off[base], site_off[base + nb]), 32 calls at a time across site boundaries.
+        //      Lane k <= 12 holds site k's block offset (from nb on: the block's end); lane k < nb the site's reference genotype (0-4, bit 0-2),
+        //      haploid (bit 3) and "deeper than cap" (bit 4: status bit, and the site counts as empty).
+        uint32_t my_off = site_off[base + min(lane, nb)];
+        uint32_t my_info = 0;
+        if (lane < nb)
         {
-            uint16_t* w_calls = s_calls_all + (warp * K2_B12 + s) * cap;
-            float* w_val = s_val_all + (warp * K2_B12 + s) * cap;
-            uint16_t* w_ord = s_ord_all + (warp * K2_B12 + s) * cap;
-            const uint32_t site = base + s;
-            const uint32_t c0 = site_off[site], c1 = site_off[site + 1];
-            uint32_t n_raw = c1 - c0;
-            if (n_raw > cap) // the host sizes cap from the deepest site
+            const char rb = ref_base[base + lane];
+            my_info = (rb == 'A' ? 0u : rb == 'C' ? 1u : rb == 'G' ? 2u : rb == 'T' ? 3u : 4u) | ((ploidy != nullptr && ploidy[base + lane] == 1) ? 8u : 0u);
+        }
+        const uint32_t blk0 = __shfl_sync(FULL, my_off, 0);
+        my_off -= blk0;
+        const uint32_t n_blk = __shfl_sync(FULL, my_off, 12);
+        const uint32_t next_off = __shfl_down_sync(FULL, my_off, 1); // lane k < 12: site k's end
+        if (lane < nb && next_off - my_off > cap) // the host sizes cap from the deepest site
+        {
+            atomicOr(status, SX_ST_SITE_DEPTH);
+            my_info |= 16u;
+        }
+        // the raw block into the warp's order region: 16-byte loads from the 16-byte boundary at or below its first call, two in flight per lane
+        // (the host sizes ord_stride from the largest block; the last 16 bytes may run past the array's end, inside its allocation's granule)
+        {
+            const uintptr_t a = reinterpret_cast<uintptr_t>(calls_g + blk0);
+            const uint4* __restrict__ src = reinterpret_cast<const uint4*>(a & ~static_cast<uintptr_t>(15));
+            uint4* const dst = reinterpret_cast<uint4*>(w_ord0);
+            const uint32_t n_vec = (static_cast<uint32_t>(a & 15u) / 2u + n_blk + 7u) / 8u;
+            for (uint32_t v = lane; v < n_vec; v += 64)
             {
-                if (lane == 0) atomicOr(status, SX_ST_SITE_DEPTH);
-                n_raw = 0;
+                const uint4 x = src[v];
+                uint4 y;
+                if (v + 32u < n_vec) y = src[v + 32u];
+                dst[v] = x;
+                if (v + 32u < n_vec) dst[v + 32u] = y;
             }
-            const char rb = ref_base[site];
-            const uint32_t ref_gt = rb == 'A' ? 0u : rb == 'C' ? 1u : rb == 'G' ? 2u : rb == 'T' ? 3u : 4u;
-            uint32_t n = 0;
-            bool nonref = false;
-            for (uint32_t b = 0; b < n_raw; b += 32)
-            {
-                const uint32_t i = b + lane;
-                const uint32_t c = i < n_raw ? calls_g[c0 + i] : 0x1000u;
-                const bool keep = !((c >> 12) & 1u);
-                const uint32_t m = __ballot_sync(FULL, keep);
-                if (keep)
-                {
-                    // val0 of a call outside every group (q < 3, or no dependent model); phase B overwrites the grouped calls'
-                    const uint32_t at = n + __popc(m & lt_mask);
-                    w_calls[at] = static_cast<uint16_t>(k2_repack(c));
-                    w_val[at] = T.val0_plain[c & 63u];
-                    if (((c >> 6) & 15u) != ref_gt) nonref = true;
-                }
-                n += __popc(m);
-            }
-            if (__any_sync(FULL, nonref)) nonref_mask |= 1u << s;
-            __syncwarp();
-            if (lane == 0) s_n[warp][s] = static_cast<uint16_t>(n);
+        }
+        if (lane < 24) s_ab[warp].gcnt4[lane] = 0u;
+        __syncwarp();
+        const uint16_t* const stg = w_ord0 + (reinterpret_cast<uintptr_t>(calls_g + blk0) & 15u) / 2u;
+        // pass 1: CleanPileupFilter (the kept calls of site s, repacked, at w_calls[s * cap + k] in pileup order), val0_plain[q] as their value,
+        // nonref per site; with the dependent model each grouped call's rank in its (site, group), in pileup order, from the three bit-plane
+        // ballots of the group id ANDed with the site's lanes and the count of earlier chunks.  A grouped call's value slot holds its rank
+        // until pass 2; phase B gives every grouped call its value.
+        uint32_t my_cnt = 0; // lane k < 12: kept calls of site k so far
+        bool my_nonref = false;
+        for (uint32_t b = 0; b < n_blk; b += 32)
+        {
+            const uint32_t j = b + lane;
+            const uint32_t s = k2_site_of(my_off, b, lane);
+            const uint32_t site_m = k2_lanes(__shfl_sync(FULL, my_off, s), __shfl_sync(FULL, my_off, s + 1u), b);
+            const uint32_t info = __shfl_sync(FULL, my_info, s);
+            const uint32_t c = j < n_blk ? stg[j] : 0x1000u;
+            const bool keep = !((c >> 12) & 1u) && !(info & 16u);
+            const uint32_t km = __ballot_sync(FULL, keep);
+            const uint32_t nrm = __ballot_sync(FULL, keep && ((c >> 6) & 15u) != (info & 7u));
+            const uint32_t at = s * cap + __shfl_sync(FULL, my_cnt, s) + __popc(km & site_m & lt_mask);
+            const uint32_t r = k2_repack(c);
+            if (keep) w_calls0[at] = static_cast<uint16_t>(r);
+            const uint32_t mine = k2_lanes(my_off, next_off, b); // lane k < 12: site k's lanes in this chunk
+            my_cnt += __popc(km & mine);
+            my_nonref = my_nonref || (nrm & mine) != 0u;
+            uint32_t gi = 0xffu;
             if (is_dep)
             {
-                // group = is_fwd + 2*base_id over the calls with q >= 3, pileup order kept inside a group (adjust_joint_eprob.cpp:209-232)
-                uint32_t my_start = 0, my_size = 0;
-                bool my_dirty = false; // lane g < 8: group g holds a call with the neighbour-mismatch bit
-                if (n <= 64)
+                gi = keep ? k2_group(r) : 0xffu;
+                const uint32_t v = __ballot_sync(FULL, gi < 8u);
+                const uint32_t p0 = __ballot_sync(FULL, (gi & 1u) != 0u), p1 = __ballot_sync(FULL, (gi & 2u) != 0u), p2 = __ballot_sync(FULL, (gi & 4u) != 0u);
+                const uint32_t x = __ballot_sync(FULL, keep && (r & 0x200u));
+                const uint32_t same = v & site_m & ((gi & 1u) ? p0 : ~p0) & ((gi & 2u) ? p1 : ~p1) & ((gi & 4u) ? p2 : ~p2); // this call's (site, group)
+                const uint32_t slot = s * 8u + (gi & 7u);
+                const uint32_t prev = gi < 8u ? s_ab[warp].gcnt[slot] : 0u;
+                __syncwarp();
+                if (gi < 8u)
                 {
-                    // one or two chunks of 32 calls: the three bits of the group id as ballots; a group's members are an AND of the three (or their
-                    // complements), which gives lane g < 8 its group's size and every call its rank (a ballot + store loop was a visible share of the kernel
-                    // over the 8 groups here).  At 30x about four sites in ten hold 33-64 calls: they take the same path with a second set of ballots,
-                    // the second chunk's members ranked behind the first's (pileup order inside a group).
-                    uint32_t gi0 = 0xffu, cq0 = 0, gi1 = 0xffu, cq1 = 0, mm0 = 0, mm1 = 0;
-                    if (lane < n)
-                    {
-                        const uint32_t r = w_calls[lane];
-                        cq0 = (r >> 3) & 63u;
-                        gi0 = k2_group(r);
-                        mm0 = r & 0x200u;
-                    }
-                    const bool two = n > 32; // warp-uniform
-                    if (two && 32u + lane < n)
-                    {
-                        const uint32_t r = w_calls[32u + lane];
-                        cq1 = (r >> 3) & 63u;
-                        gi1 = k2_group(r);
-                        mm1 = r & 0x200u;
-                    }
-                    const uint32_t v0 = __ballot_sync(FULL, gi0 < 8u);
-                    const uint32_t p0 = __ballot_sync(FULL, (gi0 & 1u) != 0u), p1 = __ballot_sync(FULL, (gi0 & 2u) != 0u), p2 = __ballot_sync(FULL, (gi0 & 4u) != 0u);
-                    const uint32_t x0 = __ballot_sync(FULL, mm0 != 0u);
-                    const uint32_t of_lane0 = v0 & ((lane & 1u) ? p0 : ~p0) & ((lane & 2u) ? p1 : ~p1) & ((lane & 4u) ? p2 : ~p2);
-                    const uint32_t of_call0 = v0 & ((gi0 & 1u) ? p0 : ~p0) & ((gi0 & 2u) ? p1 : ~p1) & ((gi0 & 4u) ? p2 : ~p2);
-                    const uint32_t size0 = lane < 8u ? __popc(of_lane0) : 0u;
-                    uint32_t of_call1 = 0;
-                    my_size = size0;
-                    my_dirty = (of_lane0 & x0) != 0u;
-                    if (two)
-                    {
-                        const uint32_t v1 = __ballot_sync(FULL, gi1 < 8u);
-                        const uint32_t q0 = __ballot_sync(FULL, (gi1 & 1u) != 0u), q1 = __ballot_sync(FULL, (gi1 & 2u) != 0u), q2 = __ballot_sync(FULL, (gi1 & 4u) != 0u);
-                        const uint32_t x1 = __ballot_sync(FULL, mm1 != 0u);
-                        const uint32_t of_lane1 = v1 & ((lane & 1u) ? q0 : ~q0) & ((lane & 2u) ? q1 : ~q1) & ((lane & 4u) ? q2 : ~q2);
-                        of_call1 = v1 & ((gi1 & 1u) ? q0 : ~q0) & ((gi1 & 2u) ? q1 : ~q1) & ((gi1 & 4u) ? q2 : ~q2);
-                        if (lane < 8u)
-                        {
-                            my_size += __popc(of_lane1);
-                            my_dirty = my_dirty || (of_lane1 & x1) != 0u;
-                        }
-                    }
-                    uint32_t incl = my_size;
-#pragma unroll
-                    for (uint32_t d = 1; d < 8; d <<= 1)
-                    {
-                        const uint32_t t = __shfl_up_sync(FULL, incl, d);
-                        if (lane >= d) incl += t;
-                    }
-                    my_start = incl - my_size;
-                    const uint32_t st0 = __shfl_sync(FULL, my_start, gi0 & 7u);
-                    if (gi0 < 8u) w_ord[st0 + __popc(of_call0 & lt_mask)] = static_cast<uint16_t>((cq0 << 7) | lane); // (quality, call index): K2_CAP12 + 2 < 128
-                    if (two)
-                    {
-                        const uint32_t st1 = __shfl_sync(FULL, my_start + size0, gi1 & 7u);
-                        if (gi1 < 8u) w_ord[st1 + __popc(of_call1 & lt_mask)] = static_cast<uint16_t>((cq1 << 7) | (32u + lane));
-                    }
+                    const uint32_t rank = (prev & 127u) + __popc(same & lt_mask);
+                    w_val0[at] = __uint_as_float(rank);
+                    if ((same >> lane) == 1u) // the (site, group)'s last member in this chunk carries the count on
+                        s_ab[warp].gcnt[slot] = static_cast<uint8_t>((rank + 1u) | (prev & 0x80u) | ((same & x) ? 0x80u : 0u));
                 }
-                else
+                __syncwarp();
+            }
+            // val0 of a call outside every group (q < 3, or no dependent model)
+            if (keep && gi >= 8u) w_val0[at] = T.val0_plain[c & 63u];
+        }
+        const uint32_t nonref_mask = __ballot_sync(FULL, my_nonref) & 0xfffu;
+        if (lane < K2_B12) s_n[warp][lane] = static_cast<uint16_t>(my_cnt);
+        if (is_dep)
+        {
+            __syncwarp();
+            // the group starts of site `lane` (exclusive sums over its 8 groups) and the list of non-empty (site, group) pairs, site-major
+            uint32_t n_ne = 0, w0 = 0, w1 = 0; // w0, w1: the site's 8 count bytes
+            if (lane < K2_B12)
+            {
+                w0 = s_ab[warp].gcnt4[2 * lane];
+                w1 = s_ab[warp].gcnt4[2 * lane + 1];
+                uint32_t start = 0;
+#pragma unroll
+                for (uint32_t g = 0; g < 8; ++g)
                 {
-                    // deeper sites (every group goes to phase B): sizes first (every chunk's share of every group) ...
-                    for (uint32_t b = 0; b < n; b += 32)
-                    {
-                        const uint32_t i = b + lane;
-                        uint32_t gi = 0xffu;
-                        bool mm = false;
-                        if (i < n)
-                        {
-                            const uint32_t r = w_calls[i];
-                            gi = k2_group(r);
-                            mm = (r & 0x200u) != 0u;
-                        }
-                        const uint32_t x = __ballot_sync(FULL, mm);
-#pragma unroll
-                        for (uint32_t g = 0; g < 8; ++g)
-                        {
-                            const uint32_t m = __ballot_sync(FULL, gi == g);
-                            if (lane == g)
-                            {
-                                my_size += __popc(m);
-                                my_dirty = my_dirty || (m & x) != 0u;
-                            }
-                        }
-                    }
-                    // ... then the starts (exclusive prefix over the 8 groups) and the stable placement, chunk by chunk
-                    uint32_t run = 0;
-#pragma unroll
-                    for (uint32_t g = 0; g < 8; ++g)
-                    {
-                        const uint32_t sz = __shfl_sync(FULL, my_size, g);
-                        if (lane == g) my_start = run;
-                        run += sz;
-                    }
-                    uint32_t cursor = my_start; // lane g: next free slot of group g
-                    for (uint32_t b = 0; b < n; b += 32)
-                    {
-                        const uint32_t i = b + lane;
-                        uint32_t gi = 0xffu, cq = 0;
-                        if (i < n)
-                        {
-                            const uint32_t r = w_calls[i];
-                            cq = (r >> 3) & 63u;
-                            gi = k2_group(r);
-                        }
-#pragma unroll
-                        for (uint32_t g = 0; g < 8; ++g)
-                        {
-                            const uint32_t m = __ballot_sync(FULL, gi == g);
-                            const uint32_t cur = __shfl_sync(FULL, cursor, g);
-                            if (gi == g) w_ord[cur + __popc(m & lt_mask)] = static_cast<uint16_t>((cq << 7) | i);
-                            if (lane == g) cursor += __popc(m);
-                        }
-                    }
+                    const uint32_t e = ((g < 4 ? w0 : w1) >> (8 * (g & 3u))) & 0xffu;
+                    s_gstart[warp][lane][g] = static_cast<uint16_t>(start);
+                    start += e & 127u;
+                    if (e & 127u) ++n_ne;
                 }
-                if (lane < 8) s_gstart[warp][s][lane] = static_cast<uint16_t>(my_start);
-                const uint32_t total = __shfl_sync(FULL, my_start + my_size, 7);
-                if (lane == 8) s_gstart[warp][s][8] = static_cast<uint16_t>(total);
-                const uint32_t m8 = __ballot_sync(FULL, lane < 8 && my_size > 0);
-                if (lane < 8 && my_size > 0) s_pair[warp][n_pairs + __popc(m8 & lt_mask)] = static_cast<uint8_t>(s * 8u + lane + (my_dirty ? 0x80u : 0u));
-                n_pairs += __popc(m8);
+                s_gstart[warp][lane][8] = static_cast<uint16_t>(start);
+            }
+            uint32_t incl = n_ne;
+#pragma unroll
+            for (uint32_t d = 1; d < 16; d <<= 1)
+            {
+                const uint32_t t = __shfl_up_sync(FULL, incl, d);
+                if (lane >= d) incl += t;
+            }
+            n_pairs = __shfl_sync(FULL, incl, K2_B12 - 1);
+            if (lane < K2_B12)
+            {
+                uint32_t p = incl - n_ne;
+#pragma unroll
+                for (uint32_t g = 0; g < 8; ++g)
+                {
+                    const uint32_t e = ((g < 4 ? w0 : w1) >> (8 * (g & 3u))) & 0xffu;
+                    if (e & 127u) s_pair[warp][p++] = static_cast<uint8_t>(lane * 8u + g + (e & 0x80u));
+                }
+            }
+            // pass 2: every grouped call to gstart + rank in its site's order, (quality, call index): K2_CAP12 + 2 < 128.  Over the compacted calls,
+            // whose block offsets are the exclusive sums of the sites' counts.
+            uint32_t my_coff = lane < K2_B12 ? my_cnt : 0u;
+#pragma unroll
+            for (uint32_t d = 1; d < 16; d <<= 1)
+            {
+                const uint32_t t = __shfl_up_sync(FULL, my_coff, d);
+                if (lane >= d) my_coff += t;
+            }
+            my_coff -= lane < K2_B12 ? my_cnt : 0u;
+            const uint32_t n_kept = __shfl_sync(FULL, my_coff, K2_B12);
+            __syncwarp();
+            for (uint32_t b = 0; b < n_kept; b += 32)
+            {
+                const uint32_t s = k2_site_of(my_coff, b, lane);
+                const uint32_t k = b + lane - __shfl_sync(FULL, my_coff, s);
+                if (b + lane < n_kept)
+                {
+                    const uint32_t r = w_calls0[s * cap + k];
+                    const uint32_t gi = k2_group(r);
+                    if (gi < 8u) w_ord0[s * cap + s_gstart[warp][s][gi] + __float_as_uint(w_val0[s * cap + k])] = static_cast<uint16_t>((((r >> 3) & 63u) << 7) | k);
+                }
             }
         }
         __syncwarp();
@@ -739,7 +758,7 @@ __global__ void __launch_bounds__(K2_WARPS * 32, 8) k2a_germline12_kernel(const 
                 const uint16_t* w_calls = s_calls_all + (warp * K2_B12 + s) * cap;
                 float* w_val = s_val_all + (warp * K2_B12 + s) * cap;
                 const uint32_t g0 = s_gstart[warp][s][g], sz = s_gstart[warp][s][g + 1] - g0;
-                uint16_t* ic = s_ord_all + (warp * K2_B12 + s) * cap + g0;
+                uint16_t* ic = w_ord0 + s * cap + g0;
                 const PKey key{};
                 // the exponent chain: a clean group (mismatch_frac 0) has the tabulated one, a group with a mismatch call takes its vexp_frac
                 // from the weight sums; either way only the ranks before the clamp have their own de, every later member gets depmin[q]
@@ -855,8 +874,8 @@ __global__ void __launch_bounds__(K2_WARPS * 32, 8) k2a_germline12_kernel(const 
             const uint16_t* w_calls = s_calls_all + (warp * K2_B12 + (have ? s : 0)) * cap;
             const float* w_val = s_val_all + (warp * K2_B12 + (have ? s : 0)) * cap;
             const uint32_t n = have ? s_n[warp][s] : 0u;
-            const char rb = ref_base[site];
-            const uint32_t ref_gt = rb == 'A' ? 0u : rb == 'C' ? 1u : rb == 'G' ? 2u : rb == 'T' ? 3u : 4u;
+            const uint32_t info = __shfl_sync(FULL, my_info, have ? s : 0u);
+            const uint32_t ref_gt = info & 7u;
             const bool nonref = (nonref_mask >> (have ? s : 0)) & 1u;
             const bool computed = have && (ref_gt < 4u) && (is_always_test || nonref);
             sx_digt_result* res = out + site;
@@ -889,7 +908,7 @@ __global__ void __launch_bounds__(K2_WARPS * 32, 8) k2a_germline12_kernel(const 
                 const float v = lds_f32(k4 ? a_tab + (r & 0x1f8u) + k4 : a_v);
                 lh = f_add(lh, i < n_mine ? v : 0.f);
             }
-            const bool haploid = have && ploidy != nullptr && ploidy[site] == 1;
+            const bool haploid = have && (info & 8u);
             const uint32_t gtcount = haploid ? 4u : 10u;
             float lmax = __shfl_sync(FULL, lh, sbase);
             for (uint32_t g = 1; g < 10; ++g)
@@ -903,7 +922,7 @@ __global__ void __launch_bounds__(K2_WARPS * 32, 8) k2a_germline12_kernel(const 
             {
                 res->lhood[sl] = lh;
                 res->phredLoghood[sl] = pl;
-                s_lh[warp][s][sl] = lh; // the row phase D reads
+                s_ab[warp].lh[s][sl] = lh; // the row phase D reads
             }
             const uint32_t cm = __ballot_sync(FULL, computed && sl == 0u); // lanes 0, 10, 20
             computed_mask |= ((cm & 1u) | ((cm >> 9) & 2u) | ((cm >> 18) & 4u)) << s0;
@@ -917,8 +936,8 @@ __global__ void __launch_bounds__(K2_WARPS * 32, 8) k2a_germline12_kernel(const 
             const uint32_t ps = lane < 12u ? lane : lane - 12u;
             const bool pact = lane < 24u && ps < nb && ((computed_mask >> ps) & 1u);
             const uint32_t site = base + (pact ? ps : 0u);
-            const char rb = ref_base[site];
-            const uint32_t ref_gt = rb == 'A' ? 0u : rb == 'C' ? 1u : rb == 'G' ? 2u : rb == 'T' ? 3u : 0u;
+            const uint32_t info = __shfl_sync(FULL, my_info, pact ? ps : 0u);
+            const uint32_t ref_gt = info & 3u; // < 4 where it is used (pact)
             sx_digt_result* res = out + site;
             rs_out r;
             r.ref_pprob = 0.0;
@@ -927,9 +946,9 @@ __global__ void __launch_bounds__(K2_WARPS * 32, 8) k2a_germline12_kernel(const 
             r.max_gt_qphred = 0;
             if (pact)
             {
-                const bool haploid = ploidy != nullptr && ploidy[site] == 1;
+                const bool haploid = (info & 8u) != 0u;
                 const float* pri = T.lnprior[haploid ? 1 : 0][ref_gt][0] + (lane < 12u ? 0 : 10);
-                const float* lh10 = s_lh[warp][ps];
+                const float* lh10 = s_ab[warp].lh[ps];
                 double e[10];
                 double mx = 0.0;
 #pragma unroll
@@ -977,11 +996,10 @@ __global__ void __launch_bounds__(K2_WARPS * 32, 8) k2a_germline12_kernel(const 
                 const uint32_t tgt = __shfl_sync(FULL, r.max_gt, s);
                 const uint16_t* w_calls = s_calls_all + (warp * K2_B12 + s) * cap;
                 const float* w_val = s_val_all + (warp * K2_B12 + s) * cap;
+                const uint32_t ref_s = __shfl_sync(FULL, my_info, s) & 3u;
                 float ls = 0.f;
                 if (lane < 2u)
                 {
-                    const char rbs = ref_base[base + s];
-                    const uint32_t ref_s = rbs == 'A' ? 0u : rbs == 'C' ? 1u : rbs == 'G' ? 2u : 3u;
                     const uint32_t e2_t = expect2_pack(tgt), e2_ref = expect2_pack(ref_s);
                     const uint32_t n = s_n[warp][s];
                     for (uint32_t i = 0; i < n; ++i)
@@ -993,7 +1011,7 @@ __global__ void __launch_bounds__(K2_WARPS * 32, 8) k2a_germline12_kernel(const 
                         ls = f_add(ls, (k == 0u) ? w_val[i] : s_val12[2u * q + k - 1u]);
                     }
                 }
-                const float lf = __shfl_sync(FULL, ls, 0), lr = __shfl_sync(FULL, ls, 1), l0 = s_lh[warp][s][tgt];
+                const float lf = __shfl_sync(FULL, ls, 0), lr = __shfl_sync(FULL, ls, 1), l0 = s_ab[warp].lh[s][tgt];
                 if (lane == s) strand_bias = static_cast<double>(f_sub((lf < lr) ? lr : lf, l0));
             }
             if (pact && lane < 12u)
@@ -1009,15 +1027,36 @@ __global__ void __launch_bounds__(K2_WARPS * 32, 8) k2a_germline12_kernel(const 
     }
 }
 
+// out[0]: the deepest site; out[1]: the most raw calls of one twelve-site batch (the twelve-site kernel's batches start at multiples of K2_B12)
 __global__ void k2_max_site_kernel(const uint32_t* __restrict__ site_off, uint32_t n_sites, uint32_t* __restrict__ out)
 {
-    uint32_t m = 0;
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_sites; i += gridDim.x * blockDim.x) m = max(m, site_off[i + 1] - site_off[i]);
-    for (int d = 16; d; d >>= 1) m = max(m, __shfl_xor_sync(FULL, m, d));
+    uint32_t m = 0, mb = 0;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_sites; i += gridDim.x * blockDim.x)
+    {
+        const uint32_t o = site_off[i];
+        m = max(m, site_off[i + 1] - o);
+        if (i % K2_B12 == 0) mb = max(mb, site_off[min(i + K2_B12, n_sites)] - o);
+    }
+    for (int d = 16; d; d >>= 1)
+    {
+        m = max(m, __shfl_xor_sync(FULL, m, d));
+        mb = max(mb, __shfl_xor_sync(FULL, mb, d));
+    }
     if ((threadIdx.x & 31) == 0 && m) atomicMax(out, m);
+    if ((threadIdx.x & 31) == 0 && mb) atomicMax(out + 1, mb);
 }
 
-int germline_run(sx_ctx* ctx, const sx_pileup_batch* d, int is_always_test, sx_digt_result* out_dev, uint32_t* de_off_dev, float* de_dev, uint32_t max_site)
+// the same two numbers for a host batch
+void max_block_host(const sx_pileup_batch* b, uint32_t* max_block)
+{
+    uint32_t mb = 0;
+    for (uint32_t s = 0; s < b->n_sites; s += K2_B12) mb = std::max(mb, b->site_off[std::min<uint32_t>(s + K2_B12, b->n_sites)] - b->site_off[s]);
+    *max_block = mb;
+}
+
+// max_block: the most raw calls of one twelve-site batch (read only when the twelve-site kernel runs)
+int germline_run(sx_ctx* ctx, const sx_pileup_batch* d, int is_always_test, sx_digt_result* out_dev, uint32_t* de_off_dev, float* de_dev, uint32_t max_site,
+                 uint32_t max_block)
 {
     if (max_site > K2_CAP_BIG)
         return sx_fail(ctx, SX_ERR_UNSUPPORTED, "sx_site_gl_germline: a site holds %u calls; the kernel handles at most %d per site", max_site, K2_CAP_BIG);
@@ -1029,12 +1068,15 @@ int germline_run(sx_ctx* ctx, const sx_pileup_batch* d, int is_always_test, sx_d
         // a stride of 32 (64) slots put the three float (16-bit) words on one bank (most shared-memory wavefronts were then bank conflicts)
         uint32_t cap = std::max<uint32_t>(18, (max_site + 1) & ~1u);
         if (cap % 16 == 0) cap += 2;
-        const size_t smem = (size_t)per_cta * cap * 8;
+        // the order region also takes a batch's raw block with up to 7 calls before it and 7 after (whole 16-byte words): 12 * cap slots
+        // suffice unless nearly every site of a batch is the deepest; a multiple of 8 slots keeps every warp's region 16-byte aligned
+        const uint32_t ord_stride = std::max<uint32_t>(K2_B12 * cap, (max_block + 14 + 7) & ~7u);
+        const size_t smem = (size_t)K2_WARPS * (K2_B12 * cap * 6 + ord_stride * 2);
         int occ = 4;
         SX_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k2a_germline12_kernel, K2_WARPS * 32, smem));
         const int grid12 = static_cast<int>(std::min<uint32_t>((d->n_sites + per_cta - 1) / per_cta, (uint32_t)(ctx->sm_count * std::max(1, occ))));
         k2a_germline12_kernel<<<grid12, K2_WARPS * 32, smem, ctx->s_compute>>>(d->site_off, d->calls, d->ref_base, d->ploidy, d->n_sites, is_always_test, ctx->d_tables, out_dev,
-                                                                             ctx->d_status, cap);
+                                                                             ctx->d_status, cap, ord_stride);
         SX_CUDA(ctx, cudaGetLastError());
         return SX_OK;
     }
@@ -1064,14 +1106,15 @@ int germline_run(sx_ctx* ctx, const sx_pileup_batch* d, int is_always_test, sx_d
     return SX_OK;
 }
 
+// out[0]: the deepest site, out[1]: the largest twelve-site batch, in one round trip
 int max_site_dev(sx_ctx* ctx, const uint32_t* site_off_dev, uint32_t n_sites, uint32_t* out)
 {
     uint32_t* d = nullptr;
-    int rc = sx_take(ctx, SX_SLOT_K2A_MAX_SITE, 1, d, 0);
+    int rc = sx_take(ctx, SX_SLOT_K2A_MAX_SITE, 2, d, 0);
     if (rc) return rc;
-    SX_CUDA(ctx, cudaMemsetAsync(d, 0, sizeof(uint32_t), ctx->s_compute));
+    SX_CUDA(ctx, cudaMemsetAsync(d, 0, 2 * sizeof(uint32_t), ctx->s_compute));
     k2_max_site_kernel<<<std::min<uint32_t>((n_sites + 255) / 256, 1184), 256, 0, ctx->s_compute>>>(site_off_dev, n_sites, d);
-    SX_CUDA(ctx, cudaMemcpyAsync(out, d, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->s_compute));
+    SX_CUDA(ctx, cudaMemcpyAsync(out, d, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->s_compute));
     SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
     return SX_OK;
 }
@@ -1139,7 +1182,9 @@ extern "C" int sx_site_gl_germline(sx_ctx* ctx, const sx_pileup_batch* b, int is
     if (rc) return rc;
     sx_digt_result* d_out = nullptr;
     if ((rc = sx_take(ctx, sx_host_slot(15), b->n_sites, d_out, 0))) return rc;
-    if ((rc = germline_run(ctx, &d, is_always_test, d_out, nullptr, nullptr, max_site))) return rc;
+    uint32_t max_block = 0;
+    max_block_host(b, &max_block);
+    if ((rc = germline_run(ctx, &d, is_always_test, d_out, nullptr, nullptr, max_site, max_block))) return rc;
     if ((rc = sx_download(ctx, out_host, d_out, b->n_sites))) return rc;
     if ((rc = t.finish(1))) return rc; // (the deepest site was found on the host)
     return sx_check_status(ctx, "sx_site_gl_germline");
@@ -1172,7 +1217,7 @@ extern "C" int sx_dependent_eprob(sx_ctx* ctx, const sx_pileup_batch* b, uint32_
     float* d_de = nullptr;
     if ((rc = sx_upload(ctx, sx_host_slot(16), out_off_host, (size_t)b->n_sites + 1, d_off, 0))) return rc;
     if ((rc = sx_take(ctx, sx_host_slot(17), off, d_de, 16))) return rc;
-    if ((rc = germline_run(ctx, &d, 1, nullptr, d_off, d_de, max_site))) return rc;
+    if ((rc = germline_run(ctx, &d, 1, nullptr, d_off, d_de, max_site, 0))) return rc;
     if ((rc = sx_download(ctx, de_host, d_de, off))) return rc;
     SX_CUDA(ctx, cudaStreamSynchronize(ctx->s_compute));
     ctx->timing.launches = 1;
@@ -1180,14 +1225,14 @@ extern "C" int sx_dependent_eprob(sx_ctx* ctx, const sx_pileup_batch* b, uint32_
     return sx_check_status(ctx, "sx_dependent_eprob");
 }
 
-// K2a's launcher: one 4-byte round trip (the deepest column) picks the kernel
+// K2a's launcher: one 8-byte round trip (the deepest column, the largest twelve-site block) picks and sizes the kernel
 int sx_k2a_run(sx_ctx* ctx, const sx_pileup_batch* d, int is_always_test, sx_digt_result* out_dev, unsigned* launches)
 {
     if (d->n_sites == 0) return SX_OK;
-    uint32_t max_site = 0;
-    int rc = max_site_dev(ctx, d->site_off, d->n_sites, &max_site);
+    uint32_t max_site[2] = {0, 0};
+    int rc = max_site_dev(ctx, d->site_off, d->n_sites, max_site);
     if (rc) return rc;
-    rc = germline_run(ctx, d, is_always_test, out_dev, nullptr, nullptr, max_site);
+    rc = germline_run(ctx, d, is_always_test, out_dev, nullptr, nullptr, max_site[0], max_site[1]);
     *launches += 2;
     return rc;
 }
